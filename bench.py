@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the fake-quant hot path on B200.
+"""bench.py -- headline benchmark of the fake-quant hot path on H100.
 
 Workload (BASELINE.json configs[1]): the quantize->dequantize work of ONE ResNet-50 QAT forward at
 batch 256, 8w8a: the 55 activation quantizer sites (per-tensor 8-bit, fused QDQ + MinMax-observer
@@ -7,7 +7,7 @@ statistics kernel -- the kernel the 70 %-of-HBM-roofline target is quoted on) an
 quantizer sites (per-channel symmetric 8-bit).  A "step" is one pass over all 109 sites on
 synthetic tensors of exactly those shapes.  metric = fake-quant forward Gelem/s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 N > 1 is launched by torchrun (one rank per GPU); the path has no exchange step, so ranks are
 independent replicas (weak scaling) and only the timing barrier uses NCCL.
@@ -562,6 +562,34 @@ def run_reference_arm(args):
 
 
 # ------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 65536  # elements per site written by --dump-outputs (a fixed, seeded sample of each output tensor)
+
+
+def dump_outputs(out_dir, lib, acts, weights, mm_states, dev):
+    """What the timed step hands its caller: the 55 activation outputs with their MinMax-observer state and the 54 weight
+    outputs.  The full outputs are 22 GB, so each tensor is written as a seeded sample of DUMP_SAMPLE elements (all of it
+    when smaller); the per-site min / max are complete.  float32 .npy files, about 28 MB in all."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    g = torch.Generator(device="cpu").manual_seed(1234)
+    torch.cuda.synchronize()
+    for prefix, sites in (("act", acts), ("weight", weights)):
+        for i, site in enumerate(sites):
+            y = site[1].reshape(-1)
+            if y.numel() > DUMP_SAMPLE:
+                idx = torch.randint(0, y.numel(), (DUMP_SAMPLE,), generator=g).to(dev)
+                y = y[idx]
+            np.save(os.path.join(out_dir, f"{prefix}_out_{i:02d}.npy"), y.float().cpu().numpy())
+    mn = torch.empty(len(acts), device=dev)
+    mx = torch.empty(len(acts), device=dev)
+    from sparsebit_b200 import _lib
+
+    _lib.check(lib.sb200_minmax_read(mm_states.data_ptr(), len(acts), mn.data_ptr(), mx.data_ptr(), torch.cuda.current_stream(dev).cuda_stream),
+               "minmax_read")
+    np.save(os.path.join(out_dir, "act_minmax.npy"), torch.stack([mn, mx], 1).cpu().numpy())
+
+
 class ClockSampler:
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -617,6 +645,7 @@ def main():
     ap.add_argument("--no-gptq", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[0] / [2] / [3] blocks and the observer / sparser CPU baselines")
     ap.add_argument("--no-graphs", action="store_true", help="enqueue the 109 launches eagerly instead of replaying CUDA graphs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
     if args.impl == "reference":
@@ -746,6 +775,8 @@ def main():
     barrier()
     if os.environ.get("SB200_NCU_RANGE"):
         torch.cuda.profiler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, lib, acts, weights, mm_states, dev)
     launches = (_lib.launch_count() - launches0) + kernels_per_step * args.steps
     clocks = sampler.stop() if rank == 0 else None
     total_ms = ev0.elapsed_time(ev1)
@@ -767,7 +798,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "fallback (H100 SXM data sheet, HBM3)"
     act_launches = 55 * args.steps  # (+1 tiny minmax_init launch per step inside the same event pair)
     alg_bytes_per_launch = act_elems * 8.0 / 55
     avg_launch_s = act_ms * 1e-3 / act_launches
@@ -776,15 +807,6 @@ def main():
                 "kernel": "sb200::stream_kernel<MODE_TENSOR,VEC4,DOQ,STORE,STATS> (sb200_qdq_stats_pertensor_fwd)",
                 "algorithmic_bytes_per_launch": alg_bytes_per_launch, "avg_launch_us": avg_launch_s * 1e6,
                 "kernel_share_of_step": act_ms / (ms_per_step * args.steps), "peak_source": peak_src}
-    # DRAM traffic of this kernel: dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed
-    # `ncu --set full` capture of this command (profiles/r02_traffic.json, written by scripts/summarize_ncu.py);
-    # null when no capture of this round is present.
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))["qdq_stats_pertensor"]
-        roofline["traffic"] = float(tr["dram_bytes_per_algorithmic_byte"]) * alg_bytes_per_launch
-        roofline["traffic_note"] = tr.get("note")
-    except Exception:
-        pass
     # headline tensor alone: [256,3,224,224] (308 MB in+out > L2), 30 back-to-back launches
     a0 = (acts[0][0].data_ptr(), acts[0][2].data_ptr(), acts[0][3].data_ptr(), acts[0][1].data_ptr(), mm_states.data_ptr(),
           acts[0][0].numel(), 0, 255, 0, stream)
@@ -871,7 +893,7 @@ def main():
 
     # ---- secondary metric of BASELINE.json: GPTQ int4 g128 tok/s on the LLaMA-7B linear shapes ----------
     # `reference_cuda_kernel` below is a BASELINE leg like `cpu_baseline`: the reference's own CUDA kernel (built
-    # from /root/reference into oracle/_ref/gptq_ref.so by oracle/build_ref.py) timed next to ours, because the
+    # from the reference checkout into oracle/_ref/gptq_ref.so by oracle/build_ref.py, when present) timed next to ours, because the
     # north star states this target relative to it (>= 1.0x).  Nothing of ours runs through it.
     gptq = None
     if rank == 0 and world == 1 and not args.no_gptq:
@@ -881,7 +903,7 @@ def main():
 
             totals = bench_gptq.run([1, 2048], with_reference=True, quiet=True)
             peaks = json.load(open(peaks_path)) if os.path.exists(peaks_path) else {}
-            tf_peak = float(peaks.get("bf16_tflops", 1590.0))
+            tf_peak = float(peaks.get("bf16_tflops", 989.0))  # H100 SXM data sheet, dense FP16 / BF16
             flops_tok = 2 * 6_476_005_376
             t_pre = totals[(2048, "ours_auto")]
             t_dec = min(totals[(1, "ours_auto")], totals.get((1, "ours_fused_launches"), float("inf")))
@@ -894,9 +916,9 @@ def main():
                     "prefill_2048_useful_TFLOPs": flops_tok * 2048 / t_pre / 1e12,
                     "roofline_prefill": {"bound": "tensor", "achieved": flops_tok * 2048 / t_pre / 1e12, "peak": tf_peak, "unit": "TFLOP/s",
                                          "frac": flops_tok * 2048 / t_pre / 1e12 / tf_peak,
-                                         "kernel": "sb200::gptq4_ts_kernel (tcgen05.mma kind::f16, weight planes in TMEM)",
-                                         "note": "useful flops 2*M*K*N; the kernel issues two MMA passes (w_hi and w_lo fp16 planes) to keep "
-                                                 "fp32-level accuracy, so the tensor pipe does 2x this work"},
+                                         "kernel": "sb200::gptq4_tc_kernel (wgmma.m64n128k16 f16, exact int4 weights, per-128-K fp32 rescale)",
+                                         "note": "useful flops 2*M*K*N; fp16-exact activations take one MMA pass, fp32 activations two "
+                                                 "(x_hi and x_lo fp16 planes, for fp32-level accuracy)"},
                     "roofline_decode": {"bound": "hbm", "achieved": dec_bytes / t_dec / 1e9, "peak": peak, "unit": "GB/s",
                                         "frac": dec_bytes / t_dec / 1e9 / peak, "algorithmic_bytes_per_token": dec_bytes}}
             try:  # the model path: QuantLinear.forward with fp16 activations (sb200_gptq4_linear_f16_ex), one launch per linear

@@ -1,5 +1,5 @@
 /*
- * sparsebit_b200.h -- C-ABI of the B200-native (sm_100a) fake-quantization / observer / sparser /
+ * sparsebit_b200.h -- C-ABI of the H100-native (sm_90a) fake-quantization / observer / sparser /
  * GPTQ-int4 hot path.  This is the drop-in boundary: plain pointers and sizes, no torch types.
  *
  * Every entry point cites the reference interface it replaces (paths relative to the
@@ -325,20 +325,20 @@ int sb200_dorefa_bwd(const float* x, const float* absmax, const float* scale, co
  * (utils/quant.py:220-225); out: [M, N] fp32, PRE-INITIALISED (bias) and accumulated in place;
  * scales / zeros (= zero*scale, utils/quant.py:188): fp32 [N, G], G = ceil(K / group_size).
  * group_size == 0 means one group (= K), like vecquant4matmul; otherwise it must be a multiple of
- * 128 (cuda_kernel_4bit.cu:60).  Large-M problems with TMA-compatible shapes run on tcgen05
- * tensor cores (split-fp16 activations, exact int4 operands, fp32 TMEM accumulation, per-group
- * scale/zero applied in the epilogue); everything else runs the HBM-bound SIMT path.
+ * 128 (cuda_kernel_4bit.cu:60).  Large-M problems with TMA-compatible shapes run on wgmma
+ * tensor cores (split-fp16 activations, exact int4 operands, fp32 register accumulation, per-group
+ * scale/zero applied on the accumulator); everything else runs the HBM-bound SIMT path.
  * `workspace` from sb200_gptq4_workspace_bytes (may be 0 bytes / NULL for the SIMT path). */
 size_t sb200_gptq4_workspace_bytes(int64_t m, int64_t k, int64_t n, int group_size);
 int sb200_gptq4_matmul(const float* x, const int32_t* qweight, float* out, const float* scales,
                        const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows,
                        int group_size, void* workspace, size_t workspace_bytes, void* stream);
-/* Per-call options instead of process-global switches.  impl: 0 = auto (M >= 768 -> 3, M >= 32 -> 2, else 1),
+/* Per-call options instead of process-global switches.  impl: 0 = auto (M >= 32 -> 2, else 1),
  * 1 = small-M path (warp-level HMMA streaming kernel when N % 4 == 0, scalar kernel otherwise), 4 = scalar kernel,
- * 2 = tcgen05 with exact int4 operands and a per-128-K-group fp32 rescale of the accumulator,
- * 3 = tcgen05 with the scaled weights as two fp16 planes written to tensor memory (A operand) and whole-K
- * accumulation, drained into fp32 registers every chunk_k K (multiple of 64; 0 = default 512) to bound the
- * tensor core's truncating accumulation. */
+ * 2 = wgmma with exact int4 operands and a per-128-K-group fp32 rescale of the register accumulator,
+ * 3 = wgmma with the scaled weights as two fp16 planes in the register operand and whole-K accumulation, restarted
+ * into a second fp32 register accumulator every chunk_k K (multiple of 64; 0 = default 512) to bound the tensor
+ * core's truncating accumulation. */
 /* flags: SB200_GPTQ4_STATIC_WEIGHTS -- the caller guarantees that qweight / scales / zeros are constants of the model,
  * i.e. NOT written by the kernel immediately in front of this call on the stream.  The decode kernel (M <= 32) is
  * launched programmatically dependent (it may begin while its predecessor drains); with this flag it requests the
@@ -374,8 +374,8 @@ int sb200_gptq4_matmul_batch_ex(const sb200_gptq4_problem* problems, int count, 
 /* fp16 activations in, fp16 result out, WITHOUT the per-call casts of QuantLinear.forward (utils/quant.py:262-278 casts
  * x / scales / zeros / bias to fp32, materialises y = bias, and casts the result back):
  *   out_f16[m, n] = fp16( bias[n] + sum_k (scales * q - zeros) * x_f16[m, k] )          (overwrites out_f16)
- * bias may be NULL; scales / zeros are the fp32 [N, G] tables.  Prefill-sized M runs the tensor-memory-operand
- * tcgen05 kernel directly on the fp16 activations (their hi plane, no lo pass) and writes fp16 from the epilogue;
+ * bias may be NULL; scales / zeros are the fp32 [N, G] tables.  Prefill-sized M runs the weight-plane
+ * wgmma kernel (impl 3) directly on the fp16 activations (their hi plane, no lo pass) and writes fp16 from the epilogue;
  * smaller M is staged through fp32 inside the library (cast, bias, kernel, cast) -- or runs as ONE launch through
  * sb200_gptq4_linear_f16_ex below.  Same accuracy as the fp32 entry point before the final rounding to fp16.  workspace: sb200_gptq4_linear_f16_workspace_bytes(...) bytes. */
 size_t sb200_gptq4_linear_f16_workspace_bytes(int64_t m, int64_t k, int64_t n, int group_size);
@@ -404,12 +404,11 @@ int sb200_gptq_matmul(const float* x, const int32_t* qweight, float* out, const 
                       const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows,
                       int bits, int group_size, void* workspace, size_t workspace_bytes, void* stream);
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
- * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 / 3 = the two tcgen05 kernels, 4 = scalar kernel. */
+ * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 / 3 = the two wgmma kernels, 4 = scalar kernel. */
 int sb200_gptq4_set_impl(int impl);
 
-/* Tuning knob of the tcgen05 kernel: nanoseconds its mostly-waiting roles (TMA producer, MMA issuer waiting for a
- * drained accumulator, unpack warps waiting for a stage) sleep between mbarrier polls.  0 (default) = poll
- * continuously. */
+/* Tuning knob of the wgmma kernels: nanoseconds their TMA producer sleeps between polls of a stage's mbarrier while it
+ * waits for the consumers to free the stage.  0 (default) = poll continuously. */
 int sb200_gptq4_set_wait_backoff(int nanoseconds);
 
 /* Variant of the decode kernel (M <= 32; process-wide, tests / benchmarking only), a bit mask:
@@ -425,15 +424,6 @@ int sb200_gptq4_set_wait_backoff(int nanoseconds);
  * Default 6 (measured best at M = 1, profiles/r02_ab_decode.jsonl).  Results are identical in every mode up to the
  * order of the fp32 atomic adds across K slices. */
 int sb200_gptq4_set_decode(int mode);
-
-/* Tuning knob of the per-group tcgen05 kernel (impl 2): how its epilogue warps drain the accumulator out of tensor
- * memory.  1 (default) = pairs of tcgen05.ld.32x32b.x8, 0 = one .x16 per batch (round 1's form).  Same values either
- * way; benchmarking only. */
-int sb200_gptq4_set_tc_drain(int narrow);
-
-/* Debug aid: when non-NULL, the tcgen05 kernel's CTA (0,0) writes clock64() stamps of its pipeline
- * handoffs into device_buffer[13][256] (event-major).  NULL disables tracing. */
-int sb200_gptq4_set_trace(int64_t* device_buffer);
 
 /* Number of kernels this library launched since load (bench.py's `gpu_launches`). */
 int64_t sb200_launch_count(void);

@@ -24,7 +24,7 @@ def main():
     if not os.path.isdir(REF):
         print("reference tree not present; nothing to build")
         return 0
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "6")
     from torch.utils.cpp_extension import load
 

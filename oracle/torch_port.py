@@ -2,9 +2,8 @@
 ATen elementwise ops (sparsebit/quantization/quantizers/quant_tensor.py:181-184), torch.min/max
 (observers/minmax.py:22) and ``weight * w_mask`` (sparse/modules/conv.py:40).
 
-TEST / BASELINE INFRASTRUCTURE ONLY: ``bench.py`` times these functions on the GPU box's host
-cores (``cpu_baseline`` and ``--impl reference``); the reference itself (``/root/reference``) cannot
-travel to the GPU box.  Validated bit-for-bit against the unmodified reference through the
+TEST / BASELINE INFRASTRUCTURE ONLY: ``bench.py`` times these functions on the GPU machine's host
+cores (``cpu_baseline`` and ``--impl reference``), where the reference itself need not be installed.  Validated bit-for-bit against the unmodified reference through the
 golden vectors (tests/test_oracle_golden.py::test_torch_port_matches_reference).
 """
 import torch

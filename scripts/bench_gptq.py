@@ -1,9 +1,9 @@
-"""GPTQ int4 g128 on the LLaMA-7B linear shapes: this repo (SIMT decode path, tcgen05 prefill path)
-vs the REFERENCE's own CUDA kernel built from /root/reference into oracle/_ref/gptq_ref.so
-(oracle/build_ref.py).  Benchmark infrastructure; prints one JSON line per (shape, M, impl).
+"""GPTQ int4 g128 on the LLaMA-7B linear shapes: this repo (SIMT decode path, wgmma prefill path)
+vs the REFERENCE's own CUDA kernel, built from the reference checkout into oracle/_ref/gptq_ref.so
+(oracle/build_ref.py) when that is present.  Benchmark infrastructure; prints one JSON line per (shape, M, impl).
 
 Timing: CUDA events, >= 3 warm-ups, rotating over enough distinct weight copies that the packed
-weights of consecutive launches exceed L2 (126 MB) at decode sizes.
+weights of consecutive launches exceed L2 (50 MB on an H100) at decode sizes.
 """
 import importlib.util
 import json
@@ -93,9 +93,9 @@ def run(ms, with_reference=True, quiet=False):
                 # the reference's model path: fp16 activations cast to fp32 (utils/quant.py:262-277, SURVEY 8d)
                 x = x.half().float()
             y = torch.zeros(m, n, device=dev)
-            impls = [("ours_auto", 0, 0)] + ([("ours_simt", 1, 0)] if m <= 64 else []) + [("ours_tcgen05_group", 2, 0)]
-            if m >= 32:  # the tensor-memory-operand kernel, accumulator drained every chunk_k K
-                impls += [(f"ours_tcgen05_ts_c{c}", 3, c) for c in TS_CHUNKS]
+            impls = [("ours_auto", 0, 0)] + ([("ours_simt", 1, 0)] if m <= 64 else []) + [("ours_wgmma_group", 2, 0)]
+            if m >= 32:  # the weight-plane kernel, accumulator restarted every chunk_k K
+                impls += [(f"ours_wgmma_ts_c{c}", 3, c) for c in TS_CHUNKS]
             for label, impl, chunk in impls:
                 try:
                     t = timeit(lambda i: ops.gptq4_matmul(x, *ws[i % copies][:1], y, *ws[i % copies][1:], 128, impl=impl, chunk_k=chunk, static_weights=STATIC),

@@ -1,4 +1,4 @@
-"""sparsebit_b200 -- B200-native (sm_100a) fake-quantisation / observer / sparser / GPTQ-int4 hot
+"""sparsebit_b200 -- H100-native (sm_90a) fake-quantisation / observer / sparser / GPTQ-int4 hot
 path behind Sparsebit's own plugin and kernel-module interfaces.
 
 Layout
@@ -20,7 +20,7 @@ __version__ = "0.1.0"
 
 def install():
     """Drop-in mode for an importable, unmodified ``sparsebit``: rebind its native fake-quant
-    module to the sm_100a kernels and register the streaming observers / radix-select sparser
+    module to the sm_90a kernels and register the streaming observers / radix-select sparser
     under their reference TYPE / STRATEGY names.  See INTEGRATION.md."""
     import importlib
 

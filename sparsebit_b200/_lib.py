@@ -85,9 +85,7 @@ PROTOTYPES = {
     "sb200_gptq4_linear_f16_ex": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_sz, c_vp]),
     "sb200_gptq_matmul": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_sz, c_vp]),
     "sb200_gptq4_set_impl": (c_int, [c_int]),
-    "sb200_gptq4_set_trace": (c_int, [c_vp]),
     "sb200_gptq4_set_wait_backoff": (c_int, [c_int]),
-    "sb200_gptq4_set_tc_drain": (c_int, [c_int]),
     "sb200_gptq4_set_decode": (c_int, [c_int]),
 }
 
@@ -105,7 +103,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise SparsebitB200Error(
             f"native library not found: {LIB_PATH}. sparsebit_b200 has no CPU / eager fallback -- build it "
-            "with `make -C sparsebit_b200/csrc` (nvcc, sm_100a) or `python -c 'import __graft_entry__ as g; g.build()'`."
+            "with `make -C sparsebit_b200/csrc` (nvcc, sm_90a) or `python -c 'import __graft_entry__ as g; g.build()'`."
         )
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in PROTOTYPES.items():

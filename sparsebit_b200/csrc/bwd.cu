@@ -1,4 +1,4 @@
-// bwd.cu -- STE backward of the fake-quant op for sm_100a.
+// bwd.cu -- STE backward of the fake-quant op for sm_90a.
 //
 // Replaces (reference, megvii-research/Sparsebit):
 //   sparsebit/quantization/torch_extensions/fake_quant_tensor.cu:97-167   per-tensor backward

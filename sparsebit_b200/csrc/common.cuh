@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the sm_100a kernels behind include/sparsebit_b200.h.
+// common.cuh -- shared device/host helpers for the sm_90a kernels behind include/sparsebit_b200.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

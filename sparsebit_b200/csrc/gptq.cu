@@ -1,4 +1,4 @@
-// gptq.cu -- C-ABI entry points of the GPTQ int4 dequant-matmul and the SIMT / tcgen05 dispatch.
+// gptq.cu -- C-ABI entry points of the GPTQ int4 dequant-matmul and the SIMT / tensor-core dispatch.
 //
 // Boundary replaced: cuda_kernel.vecquant4matmul / vecgroupquant4matmul
 // (large_language_models/llama/quantization/cuda/cuda_kernel.cpp:10-23,70,73) and their argument
@@ -27,9 +27,7 @@ int gptq4_decode_f16(const __half* x_h, const int32_t* qweight, __half* out_h, c
                      const float* zeros, long long M, long long K, long long N, long long KW, int group_size, float* partial,
                      int* counters, int flags, cudaStream_t st);
 bool gptq4_decode_supported(const int32_t* qweight, long long N);
-void gptq4_tc_set_trace(long long* p);
 void gptq4_tc_set_backoff(int ns);
-void gptq4_tc_set_drain(int narrow);
 void gptq4_decode_set_mode(int mode);
 int gptq_lowbit(int bits, const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                 long long M, long long K, long long N, long long KW, int group_size, cudaStream_t st);
@@ -73,17 +71,6 @@ int sb200_gptq4_set_decode(int mode) {
   return SB200_OK;
 }
 
-int sb200_gptq4_set_tc_drain(int narrow) {
-  SB_REQUIRE(narrow == 0 || narrow == 1, "sb200_gptq4_set_tc_drain: 0 (tcgen05.ld .x16) or 1 (pairs of .x8) (got %d)", narrow);
-  gptq4_tc_set_drain(narrow);
-  return SB200_OK;
-}
-
-int sb200_gptq4_set_trace(int64_t* device_buffer) {
-  gptq4_tc_set_trace(reinterpret_cast<long long*>(device_buffer));
-  return SB200_OK;
-}
-
 size_t sb200_gptq4_workspace_bytes(int64_t m, int64_t k, int64_t n, int group_size) {
   if (m <= 0 || k <= 0 || n <= 0) return 0;
   if (group_size <= 0) group_size = (int)k;
@@ -101,7 +88,7 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
   SB_REQUIRE(qweight_rows >= (k + 7) / 8,
              "sb200_gptq4_matmul: qweight has %lld rows, need ceil(K/8) = %lld", (long long)qweight_rows,
              (long long)((k + 7) / 8));
-  SB_REQUIRE(impl >= 0 && impl <= 4, "sb200_gptq4_matmul: impl must be 0 (auto), 1 (small-M), 2 or 3 (tcgen05), 4 (scalar) (got %d)", impl);
+  SB_REQUIRE(impl >= 0 && impl <= 4, "sb200_gptq4_matmul: impl must be 0 (auto), 1 (small-M), 2 or 3 (tensor core), 4 (scalar) (got %d)", impl);
   SB_REQUIRE(chunk_k >= 0 && chunk_k % 64 == 0, "sb200_gptq4_matmul: chunk_k must be a multiple of 64 (got %d)", chunk_k);
   if (group_size != 0) {
     // cuda_kernel_4bit.cu:60
@@ -112,8 +99,8 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
   }
   cudaStream_t st = (cudaStream_t)stream;
   // 1 = small-M path: warp-level HMMA streaming kernel (gptq_decode.cu) when N % 4 == 0, else the scalar kernel;
-  // 4 = scalar SIMT kernel (gptq_simt.cu, any shape);  2 = tcgen05, exact int4 operands + per-128-K-group fp32 rescale (gptq_tc.cu);
-  // 3 = tcgen05, scaled fp16 weight planes written to tensor memory, whole-K accumulation (gptq_ts.cu).
+  // 4 = scalar SIMT kernel (gptq_simt.cu, any shape);  2 = wgmma, exact int4 operands + per-128-K-group fp32 rescale (gptq_tc.cu);
+  // 3 = wgmma, scaled fp16 weight planes as the register operand, whole-K accumulation (gptq_ts.cu).
   int use = 1;
   if (impl != 1 && impl != 4) {
     const bool shape_ok = gptq4_tc_supported(x, qweight, out, m, k, n, qweight_rows, group_size) && workspace;
@@ -121,14 +108,12 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
     const bool ok3 = shape_ok && workspace_bytes >= gptq4_ts_workspace(m, k, n, group_size);
     if (impl == 2 || impl == 3) {
       if (!(impl == 2 ? ok2 : ok3)) {
-        set_error("sb200_gptq4_matmul: tcgen05 path forced but shape/workspace unsupported (M=%lld K=%lld N=%lld gs=%d ws=%zu)",
+        set_error("sb200_gptq4_matmul: tensor-core path forced but shape/workspace unsupported (M=%lld K=%lld N=%lld gs=%d ws=%zu)",
                   (long long)m, (long long)k, (long long)n, group_size, workspace_bytes);
         return SB200_E_UNSUPPORTED;
       }
       use = impl;
-    } else if (ok3 && m >= 768) {  // below that a 256-token tile leaves most SMs without a CTA (measured cross-over)
-      use = 3;
-    } else if (ok2 && m >= 32) {
+    } else if (ok2 && m >= 32) {  // on the H100 the per-group kernel is faster than impl 3 at every M (DESIGN.md section 7)
       use = 2;
     }
   }

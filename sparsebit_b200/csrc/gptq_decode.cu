@@ -6,7 +6,7 @@
 //
 // The scalar path (gptq_simt.cu) needs 3 instructions per weight (LOP3, FADD, FFMA) and is issue-bound at 0.27 of the
 // HBM roofline.  Here the multiply-accumulate goes to the tensor cores through the warp-level mma.sync.m16n8k16
-// (HMMA; tcgen05 needs 128-row tiles and TMEM, pointless for 1..32 tokens):
+// (HMMA; wgmma needs 64-row warpgroup tiles, pointless for 1..32 tokens):
 //   A (16 features x 16 K)  = the int4 values as EXACT fp16 integers (q in [0, 15])
 //   B (16 K x 8 tokens)     = the activations x * 2^-e as fp16 hi (+ lo) planes, staged once per CTA in shared memory
 //   D (16 x 8 fp32)         = integer dot products of one 128-K group; the group's scale / zero are applied in fp32:

@@ -1,4 +1,4 @@
-// gptq_tc.cu -- GPTQ int4 group-wise dequant-matmul on tcgen05 tensor cores (sm_100a).
+// gptq_tc.cu -- GPTQ int4 group-wise dequant-matmul on Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the M-serial SIMT loop of VecQuant4MatMulKernel
 // (large_language_models/llama/quantization/cuda/cuda_kernel_4bit.cu:88-180) for prefill-sized M:
@@ -8,75 +8,28 @@
 // single fp16/bf16 tensor-core pass cannot meet.  Here the 4-bit integers q in [0, 15] enter the MMA
 // EXACTLY (they are fp16 integers), the fp32 activations are split x * 2^-e = hi + lo into two fp16
 // operands (e = per-row power of two so that hi never overflows; 22 significant bits survive), both
-// products accumulate in fp32 in TMEM, and the affine part is applied per 128-wide K group on the
+// products accumulate in fp32 registers, and the affine part is applied per 128-wide K group on the
 // integer dot product:   sum_k (s q - z) x  =  s * (sum_k q x) - z * (sum_k x).
 // The reference's group_size is a multiple of 128 (cuda_kernel_4bit.cu:60), so one (s, z) pair per
 // 128-K block -- the same blocking the reference uses (BLOCKLEN = 128).
 //
-// Pipeline (one CTA = one 128 x 128 output tile, 16 warps, 1 CTA / SM):
-//   warp 0      TMA producer: per 64-K stage one bulk-tensor load each for A_hi, A_lo (128x64 fp16,
-//               SWIZZLE_128B) and for the PACKED weight tile (8 x 128 int32 = 4 KB)
-//   warps 12-19 unpack (two sets of 4 warps alternating stages, so one set's proxy fence / load
-//               latency overlaps the other's ALU work): packed words (shared) -> fp16 B tile in the
-//               canonical K-major SWIZZLE_128B UMMA layout (one int32 = 8 nibbles = one 16-byte chunk);
-//               one (x & mask) | bias LOP3 per nibble pair, the group's integer zero point prefetched as
-//               raw fp16 bits two stages ahead
-//   warp 1      MMA issuer: 4 x (hi, lo) tcgen05.mma.kind::f16 128x128x16 per stage, fp32 accumulators
-//               in TMEM, four buffers (all 512 columns) so the MMA runs up to 3 K groups ahead of the drain --
-//               the drain is the paced resource: 64 KB of tcgen05.ld per group at 64 B/clk = 1024 cycles
-//               against 512 cycles of tensor-core work; tcgen05.commit releases stages / publishes groups
-//   warps 4-11  epilogue: drain the group's 128x128 partial sums with software-pipelined tcgen05.ld.x16, fold
-//               in scale / zero / row sums into register accumulators, finally out += acc.  Every warp stages
-//               its own 64 scales one group ahead in a private double buffer (__syncwarp only, no CTA barrier)
-// Measured pacing (clock64 trace, scripts/gpu_tc_trace.py, DESIGN.md section 7): per 128-K group the tensor core
-// needs 512 cycles, the drain chain of an epilogue warp ~2200 (tcgen05.ld.x16 round trips of ~350 cycles with 8
-// warps draining; TMEM read bandwidth is 64 B/clk = 1024 cycles per group at best), the unpack ~670 per stage.
-//   warp 2      TMEM allocator.
+// Pipeline (tc_common.cuh): one CTA = 128 features x 128 tokens, a 5-stage TMA ring of 64-K stages.  Each consumer
+// thread unpacks its own A fragments (q - zero for two feature rows) from the packed words of the stage, issues
+// 4 (+4 lo) wgmma.m64n128k16 into a per-group partial accumulator, and after every 128 K folds
+// acc += scale * partial (- zero * xsum) in fp32 registers -- the per-group rescale costs one FMA per accumulator,
+// since the accumulator never leaves the registers.
 // A prologue kernel splits x into (hi, lo), computes the per-(row, 128-K) sums and the row scales.
 #include "tc_common.cuh"
 
 namespace sb200 {
 
-constexpr int kTileM = 128;
-constexpr int kTileN = 128;
-constexpr int kBlockK = 64;   // fp16 elements per stage = one 128-byte swizzle atom
-constexpr int kStages = 4;
-constexpr int kGroupK = 128;  // epilogue granularity (= the reference's BLOCKLEN)
-constexpr int kUnpackSets = 2;   // 4-warp unpack sets taking stages round-robin
-constexpr int kTcThreads = (12 + 4 * kUnpackSets) * 32;  // warpgroups: control | epilogue x2 | unpack x kUnpackSets
-constexpr int kAccBufs = 4;           // accumulator buffers in TMEM: the MMA runs up to 3 K groups ahead of the drain
-constexpr uint32_t kTmemCols = kAccBufs * kTileN;  // 4 x 128 fp32 columns = all of TMEM (1 CTA / SM)
-
-constexpr int kABytes = kTileM * kBlockK * 2;      // 16 KB  (hi or lo)
-constexpr int kBBytes = kTileN * kBlockK * 2;      // 16 KB  unpacked fp16 B tile
-constexpr int kBqBytes = (kBlockK / 8) * kTileN * 4;  // 4 KB packed words
-constexpr int kStageBytes = 2 * kABytes + kBBytes + kBqBytes;  // 52 KB
-constexpr int kTxBytes = 2 * kABytes + kBqBytes;               // bytes TMA delivers per stage
+constexpr int kTcStages = 5;
+constexpr int kGroupK = 128;  // fold granularity (= the reference's BLOCKLEN)
 
 struct TcSmem {
-  // dynamic shared memory, 1024-byte aligned: [stage][A_hi | A_lo | B | Bq]
-  uint64_t full[kStages];
-  uint64_t bready[kStages];
-  uint64_t empty[kStages];
-  uint64_t tmem_full[kAccBufs];
-  uint64_t tmem_empty[kAccBufs];
-  uint32_t tmem_base;
-  uint32_t pad;
-  // per epilogue warp, double buffered: scales / zeros of the warp's 64 columns for one 128-K group
-  alignas(16) float scw[8][2][64];
-  alignas(16) float zrw[8][2][64];
+  uint64_t full[kTcStages];   // TMA data of the stage landed
+  uint64_t empty[kTcStages];  // the 8 consumer warps' wgmmas reading the stage completed
 };
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 (ignored for swizzled K-major) | [32,46) SBO >> 4 = 1024 B
-//   (8 rows x 128 B) | [46,48) version = 1 | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor) for kind::f16: D = F32 (bit 4), A = B = F16 (0),
-// both K-major, N >> 3 at [17,23), M >> 4 at [24,29).
-constexpr uint32_t kIdesc = (1u << 4) | ((uint32_t)(kTileN >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
 
 // ---------------------------------------------------------------------------------- prologue kernel
 // Row m of x -> A_hi[m, :], A_lo[m, :] (fp16, K order permuted inside every 8 as 0,4,1,5,2,6,3,7 to
@@ -155,333 +108,113 @@ __global__ void gptq_zero_probe_kernel(const float* __restrict__ scales, const f
 }
 
 // ---------------------------------------------------------------------------------- main kernel
-__global__ void __launch_bounds__(kTcThreads, 1)
+__global__ void __launch_bounds__(kWgThreads, 1)
 gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                 const __grid_constant__ CUtensorMap map_q, float* __restrict__ out, const float* __restrict__ scales,
                 const float* __restrict__ zeros, const float* __restrict__ xsum, const float* __restrict__ rowscale,
                 const __half* __restrict__ zint, const int* __restrict__ int_zero_flag, int M, int K, int N, int Gq,
-                int G128, int group_size, long long* __restrict__ trace, int backoff_ns, int narrow_drain) {
+                int G128, int group_size, int backoff_ns) {
   extern __shared__ unsigned char smem_raw[];
   // stage buffers first (1024-byte aligned for SWIZZLE_128B), bookkeeping after them
   unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  TcSmem* sm = reinterpret_cast<TcSmem*>(stage_base + (size_t)kStages * kStageBytes);
+  TcSmem* sm = reinterpret_cast<TcSmem*>(stage_base + (size_t)kTcStages * kWgStageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * kTileM, n0 = blockIdx.y * kTileN;
-  const int num_kb = (K + kBlockK - 1) / kBlockK;
-  const int num_g = (num_kb + 1) / 2;  // 128-K groups
+  const int tiles_m = (M + kWgTok - 1) / kWgTok;
+  const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kWgTok, n0 = (int)(blockIdx.x / (unsigned)tiles_m) * kWgFeat;
+  const int num_kb = (K + kWgBK - 1) / kWgBK;
   const bool int_zero = int_zero_flag[0] != 0;  // uniform: every zeros[n,g] is an integer multiple of scales[n,g]
   const bool need_lo = int_zero_flag[1] != 0;   // uniform: some activation has a non-zero fp16 low part
-  // optional pipeline trace (sb200_gptq4_set_trace): CTA (0,0) stamps clock64() at each handoff, [event][stage]
-  long long* tr = (trace && blockIdx.x == 0 && blockIdx.y == 0) ? trace : nullptr;
-#define SB_TRACE(ev, idx) do { if (tr && (idx) < 256) tr[(ev) * 256 + (idx)] = clock64(); } while (0)
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) {
+    for (int s = 0; s < kTcStages; ++s) {
       mbar_init(&sm->full[s], 1);
-      mbar_init(&sm->bready[s], 4);  // one arrive per warp of the unpack set that owns the stage
-      mbar_init(&sm->empty[s], 1);
-    }
-    for (int b = 0; b < kAccBufs; ++b) {
-      mbar_init(&sm->tmem_full[b], 1);
-      mbar_init(&sm->tmem_empty[b], 8);  // one arrive per epilogue warp
+      mbar_init(&sm->empty[s], 8);  // one arrival per consumer warp
     }
     mbar_fence_init();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm->tmem_base)),
-                 "r"(kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sm->tmem_base;
 
-  if (warp < 4) reg_dec<40>();
-  if (warp == 0) {
+  if (warp < 4) {
     // ================================================================== TMA producer
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (uint32_t)(kb / kStages) & 1u;
-        mbar_wait_relaxed(&sm->empty[s], ph ^ 1u, backoff_ns);
-        SB_TRACE(0, kb);
-        unsigned char* st = stage_base + (size_t)s * kStageBytes;
-        mbar_expect_tx(&sm->full[s], need_lo ? kTxBytes : kTxBytes - kABytes);
-        tma_load_2d(st, &map_hi, kb * kBlockK, m0, &sm->full[s]);
-        if (need_lo) tma_load_2d(st + kABytes, &map_lo, kb * kBlockK, m0, &sm->full[s]);
-        tma_load_2d(st + 2 * kABytes + kBBytes, &map_q, n0, kb * (kBlockK / 8), &sm->full[s]);
-      }
-      // drain the asynchronous tcgen05.commit arrivals on empty[] of the last stages before the CTA may exit
-      for (int kb = num_kb; kb < num_kb + kStages; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (uint32_t)(kb / kStages) & 1u;
-        mbar_wait_relaxed(&sm->empty[s], ph ^ 1u, backoff_ns);
-      }
+    reg_dec<40>();
+    if (threadIdx.x == 0)
+      wg_produce(stage_base, sm->full, sm->empty, kTcStages, &map_hi, &map_lo, &map_q, m0, n0, num_kb, need_lo, backoff_ns);
+    return;
+  }
+  // ==================================================================== consumers: 64 features x 128 tokens each
+  reg_inc<232>();
+  const int q = lane & 3;
+  const int f0 = ((warp - 4) >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);  // feature rows f0, f0 + 8 of the tile
+  const int na = n0 + f0, nb = na + 8;
+  const bool live_a = na < N, live_b = nb < N;
+  const NibblePair unpack(q);
+  const uint32_t stage0 = smem_u32(stage_base);
+  float acc[64], part[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % kTcStages;
+    const uint32_t ph = (uint32_t)(kb / kTcStages) & 1u;
+    const int g = kb >> 1;                                            // 128-K group
+    const int gq = (int)((long long)g * kGroupK / group_size);        // quantisation group
+    // this group's parameters, requested before the wait for the stage
+    const float sa = live_a ? __ldg(scales + (size_t)na * Gq + gq) : 0.f;
+    const float sb = live_b ? __ldg(scales + (size_t)nb * Gq + gq) : 0.f;
+    const float zfa = (!int_zero && live_a) ? __ldg(zeros + (size_t)na * Gq + gq) : 0.f;
+    const float zfb = (!int_zero && live_b) ? __ldg(zeros + (size_t)nb * Gq + gq) : 0.f;
+    // integer-zero mode: (q - zero) enters the MMA and the fold is one FMA; otherwise q alone and zeros * xsum
+    const float za = (int_zero && live_a) ? __half2float(zint[(size_t)na * Gq + gq]) : 0.f;
+    const float zb = (int_zero && live_b) ? __half2float(zint[(size_t)nb * Gq + gq]) : 0.f;
+    const __half2 offa = unpack.offset(za), offb = unpack.offset(zb);
+    mbar_wait_relaxed(&sm->full[s], ph, 0);
+    const uint32_t* bq = reinterpret_cast<const uint32_t*>(stage_base + (size_t)s * kWgStageBytes + 2 * kWgXBytes);
+    uint32_t a[4][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {  // 16 K = packed rows 2j (K 0..7) and 2j + 1 (K 8..15)
+      a[j][0] = h2u(unpack(bq[(2 * j) * kWgFeat + f0], offa));
+      a[j][1] = h2u(unpack(bq[(2 * j) * kWgFeat + f0 + 8], offb));
+      a[j][2] = h2u(unpack(bq[(2 * j + 1) * kWgFeat + f0], offa));
+      a[j][3] = h2u(unpack(bq[(2 * j + 1) * kWgFeat + f0 + 8], offb));
     }
-  } else if (warp == 1) {
-    // ================================================================== MMA issuer
-    // (Measured with the clock64 trace: a `lane == 0` issue region cost 550-750 cycles of issue overhead
-    // per stage against 256-512 cycles of tensor-core work.)
-    // The whole warp runs the (uniform) control flow and descriptor arithmetic; one elected lane issues.
-    // bready[s] is only completed by warps that already observed full[s], so it implies the TMA data landed.
-    {
-      const uint32_t stage0 = smem_u32(stage_base);
-      const uint64_t dconst = (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (uint32_t)(kb / kStages) & 1u;
-        const int g = kb >> 1, b = g & (kAccBufs - 1);
-        if ((kb & 1) == 0) {  // first stage of a K group: the accumulator buffer must have been drained
-          mbar_wait_relaxed(&sm->tmem_empty[b], (((uint32_t)(g / kAccBufs)) & 1u) ^ 1u, backoff_ns);
-        }
-        mbar_wait(&sm->bready[s], ph);
-        tc_fence_after();
-        const uint32_t a_hi = stage0 + (uint32_t)s * kStageBytes;
-        const uint64_t da = dconst | (uint64_t)((a_hi >> 4) & 0x3FFFu);
-        const uint64_t dl = dconst | (uint64_t)(((a_hi + kABytes) >> 4) & 0x3FFFu);
-        const uint64_t db = dconst | (uint64_t)(((a_hi + 2 * kABytes) >> 4) & 0x3FFFu);
-        const uint32_t d = tmem_base + (uint32_t)(b * kTileN);
-        if (elect_one()) {
-          SB_TRACE(3, kb);
-          if (need_lo) {
+    const uint32_t xh = stage0 + (uint32_t)s * kWgStageBytes;
+    const uint64_t dh = gmma_desc_sw128(xh), dl = gmma_desc_sw128(xh + kWgXBytes);
+    wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {  // +2 in the address field = 32 bytes = 16 fp16 along K
-              tc_mma_f16(d, da + 2 * k, db + 2 * k, kIdesc, !((kb & 1) == 0 && k == 0));
-              tc_mma_f16(d, dl + 2 * k, db + 2 * k, kIdesc, true);
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k)
-              tc_mma_f16(d, da + 2 * k, db + 2 * k, kIdesc, !((kb & 1) == 0 && k == 0));
-          }
-          SB_TRACE(4, kb);
-          tc_commit(&sm->empty[s]);                                            // stage reusable when these MMAs finish
-          if ((kb & 1) == 1 || kb == num_kb - 1) tc_commit(&sm->tmem_full[b]);  // group complete
-        }
-        __syncwarp();
-      }
+    for (int j = 0; j < 4; ++j) {
+      wgmma_m64n128k16_rs(part, a[j], dh + 2 * j, !((kb & 1) == 0 && j == 0));
+      if (need_lo) wgmma_m64n128k16_rs(part, a[j], dl + 2 * j, 1);
     }
-  } else if (warp >= 12) {
-    // ================================================================== unpack: packed int4 -> fp16 UMMA tile
-    if (kUnpackSets == 2) reg_dec<64>();  // room for all 8 output chunks: no STS source register is recycled early
-    const int t = (threadIdx.x - 12 * 32) & 127;  // column of the tile
-    const int uset = (warp - 12) >> 2;             // this set handles stages kb with kb % kUnpackSets == uset
-    uint32_t bias;
-    asm volatile("mov.b32 %0, 0x64006400;" : "=r"(bias));  // opaque to constant propagation
-    // integer zero point of this column per K stage, fetched one iteration (two stages) ahead of its use;
-    // the group index is advanced incrementally (no division in the loop)
-    int gq_next = (uset * kBlockK) / group_size;
-    int koff_next = uset * kBlockK;
-    // (the raw fp16 bits are carried to the next iteration: converting at the fetch site would stall this
-    // warp on the global load right here -- 21 % of the unpack warps' samples in the ncu source view)
-    auto zint_fetch = [&](int kb) -> unsigned short {
-      if (!int_zero || n0 + t >= N || kb >= num_kb) return (unsigned short)0;
-      return __ldg(reinterpret_cast<const unsigned short*>(zint) + (size_t)(n0 + t) * Gq + gq_next);
-    };
-    unsigned short z_cur = zint_fetch(uset);
-    for (int kb = uset; kb < num_kb; kb += kUnpackSets) {
-      const int s = kb % kStages;
-      const uint32_t ph = (uint32_t)(kb / kStages) & 1u;
-      koff_next += kUnpackSets * kBlockK;
-      while (koff_next >= (gq_next + 1) * group_size) ++gq_next;
-      const unsigned short z_next = zint_fetch(kb + kUnpackSets);
-      mbar_wait_relaxed(&sm->full[s], ph, backoff_ns);
-      if (t == 0 && (warp & 3) == 0) SB_TRACE(1, kb);
-      unsigned char* st = stage_base + (size_t)s * kStageBytes;
-      const uint32_t* bq = reinterpret_cast<const uint32_t*>(st + 2 * kABytes + kBBytes);
-      unsigned char* brow = st + 2 * kABytes + (size_t)t * 128;  // row t of the B tile (64 fp16 = 128 B)
-      // all 8 packed words first: the loads must not be interleaved with the stores below (both are
-      // shared-memory accesses the compiler cannot disambiguate, which serialised 8 LDS->ALU->STS chains)
-      uint32_t w[kBlockK / 8];
+    wgmma_commit();
+    wgmma_wait_all(part);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&sm->empty[s]);
+    if ((kb & 1) == 1 || kb == num_kb - 1) {
+      // acc[n, m] += s[n] * part (- z[n] * xsum[m, g]);  d[j]: feature f0 + 8 * ((j >> 1) & 1), token 8 (j >> 2) + 2q + (j & 1)
+      if (int_zero) {
 #pragma unroll
-      for (int r = 0; r < kBlockK / 8; ++r) w[r] = bq[r * kTileN + t];
-      if (tr && t == 0 && (warp & 3) == 0) { asm volatile("" ::"r"(w[0] ^ w[7])); SB_TRACE(7, kb); }
-      // subtrahend: 1024 (the 0x6400 bias) plus, in integer-zero mode, the group's zero point
-      const float zsub = 1024.f + __half2float(__ushort_as_half(z_cur));
-      z_cur = z_next;
-      const __half2 sub = __float2half2_rn(zsub);
-      const __half2 k16 = __float2half2_rn(0.0625f);
-#pragma unroll
-      for (int r = 0; r < kBlockK / 8; ++r) {
-        // halves (n0,n4) (n1,n5) (n2,n6) (n3,n7).  0x6400 | q is the fp16 number 1024 + q; for the odd
-        // nibbles the mask is applied in place (bits 4..7): 0x6400 | (q << 4) = 1024 + 16 q, brought back by
-        // one exact HFMA2: (1024 + 16 q) / 16 - (64 + zero) ... folded as v * 1/16 + (64 - zsub) - 64 below.
-        // (x & mask) | bias as ONE LOP3 (immLut 0xEA): the bias sits in a register because a LOP3 takes a
-        // single immediate (with two the compiler emits an AND and an OR)
-        const uint32_t lo = w[r], hi = w[r] >> 8;
-        const uint32_t v0 = and_or<0x000F000Fu>(lo, bias);  // (n0, n4)
-        const uint32_t v1 = and_or<0x00F000F0u>(lo, bias);  // 1024 + 16 * (n1, n5)
-        const uint32_t v2 = and_or<0x000F000Fu>(hi, bias);  // (n2, n6)
-        const uint32_t v3 = and_or<0x00F000F0u>(hi, bias);  // 1024 + 16 * (n3, n7)
-        // (1024 + 16 q) * 1/16 = 64 + q exactly;  64 + q - (zsub - 960) = q - (zsub - 1024)
-        const __half2 off = __hsub2(sub, __float2half2_rn(960.f));
-        const __half2 h0 = __hsub2(*reinterpret_cast<const __half2*>(&v0), sub);
-        const __half2 h1 = __hfma2(*reinterpret_cast<const __half2*>(&v1), k16, __hneg2(off));
-        const __half2 h2 = __hsub2(*reinterpret_cast<const __half2*>(&v2), sub);
-        const __half2 h3 = __hfma2(*reinterpret_cast<const __half2*>(&v3), k16, __hneg2(off));
-        *reinterpret_cast<uint4*>(brow + ((r ^ (t & 7)) << 4)) =
-            make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
-                       *reinterpret_cast<const uint32_t*>(&h2), *reinterpret_cast<const uint32_t*>(&h3));
-      }
-      if (t == 0 && (warp & 3) == 0) SB_TRACE(8, kb);
-      fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
-      if (t == 0 && (warp & 3) == 0) SB_TRACE(9, kb);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm->bready[s]);
-      if (t == 0 && (warp & 3) == 0) SB_TRACE(2, kb);
-    }
-  } else if (warp >= 4) {
-    // ================================================================== epilogue (8 warps)
-    // two sets (640 threads, 96 regs at launch): (152-96)*256 <= (96-40)*128 + (96-64)*256
-    // one set  (512 threads, 128 at launch):     (152-128)*256 <= (128-24)*128
-    reg_inc<152>();
-    const int e = threadIdx.x - 4 * 32;           // 0..255
-    const int quarter = warp & 3;                  // TMEM lane quarter this warp may read
-    const int half = (warp - 4) >> 2;              // which 64 columns
-    const int row = quarter * 32 + lane;           // accumulator row == TMEM lane
-    const int m = m0 + row;
-    const int col0 = half * 64;
-    float acc[64];
-#pragma unroll
-    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-    // Every epilogue warp stages the scales (zeros) of its own 64 columns, one group ahead, in its private
-    // double buffer: the warps only __syncwarp, never meet at a CTA barrier, and so drift apart -- one warp's
-    // bookkeeping overlaps the other warps' TMEM drains (the drain is the paced resource; with a per-group
-    // bar.sync all 8 warps left the TMEM pipe idle together for ~900 of every ~2300 cycles).
-    float* my_sc = &sm->scw[warp - 4][0][0];
-    float* my_zr = &sm->zrw[warp - 4][0][0];
-    auto fetch = [&](int g, int gq, float (&v)[4], float& xs_out) {
-      const int na = n0 + col0 + lane, nb = na + 32;  // lane stages columns col0 + lane and col0 + 32 + lane
-      v[0] = (na < N) ? __ldg(scales + (size_t)na * Gq + gq) : 0.f;
-      v[1] = (nb < N) ? __ldg(scales + (size_t)nb * Gq + gq) : 0.f;
-      v[2] = (!int_zero && na < N) ? __ldg(zeros + (size_t)na * Gq + gq) : 0.f;
-      v[3] = (!int_zero && nb < N) ? __ldg(zeros + (size_t)nb * Gq + gq) : 0.f;
-      xs_out = (m < M) ? __ldg(xsum + (size_t)m * G128 + g) : 0.f;
-    };
-    auto stage = [&](int b, const float (&v)[4]) {
-      my_sc[b * 64 + lane] = v[0];
-      my_sc[b * 64 + 32 + lane] = v[1];
-      if (!int_zero) {
-        my_zr[b * 64 + lane] = v[2];
-        my_zr[b * 64 + 32 + lane] = v[3];
-      }
-      __syncwarp();
-    };
-    float v_next[4], xs_next;
-    fetch(0, 0, v_next, xs_next);
-    stage(0, v_next);
-    float xs = xs_next;
-    // quantisation group of the NEXT 128-K block, advanced incrementally (a 64-bit division here cost ~600
-    // cycles per group: the clock64 trace showed that gap between one group's drain and the next)
-    int gq_next = 0;
-    long long kend_next = group_size;  // first k that belongs to group gq_next + 1
-    for (int g = 0; g < num_g; ++g) {
-      const int b = g & 1;                   // scale / zero staging buffer
-      const int tb = g & (kAccBufs - 1);     // accumulator buffer
-      if (g + 1 < num_g) {
-        const long long k_next = (long long)(g + 1) * kGroupK;
-        while (k_next >= kend_next) { ++gq_next; kend_next += group_size; }
-        fetch(g + 1, gq_next, v_next, xs_next);
-      }
-      mbar_wait(&sm->tmem_full[tb], ((uint32_t)(g / kAccBufs)) & 1u);
-      if (e == 0) SB_TRACE(5, g);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(tb * kTileN + col0);
-      const float4* sc4 = reinterpret_cast<const float4*>(my_sc + b * 64);
-      const float4* zr4 = reinterpret_cast<const float4*>(my_zr + b * 64);
-      const float nxs = int_zero ? 0.f : -xs;  // integer-zero mode: the zero point is already inside the MMA
-      // 16 columns of this thread's row: acc += scale * partial (- zero * xsum)
-      auto fold = [&](int c, const uint32_t (&p)[16]) {
-        if (int_zero) {
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 s4 = sc4[4 * c + j4];
-            const int o = 16 * c + 4 * j4;
-            acc[o + 0] = fmaf(s4.x, __uint_as_float(p[4 * j4 + 0]), acc[o + 0]);
-            acc[o + 1] = fmaf(s4.y, __uint_as_float(p[4 * j4 + 1]), acc[o + 1]);
-            acc[o + 2] = fmaf(s4.z, __uint_as_float(p[4 * j4 + 2]), acc[o + 2]);
-            acc[o + 3] = fmaf(s4.w, __uint_as_float(p[4 * j4 + 3]), acc[o + 3]);
-          }
-        } else {
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 s4 = sc4[4 * c + j4], z4 = zr4[4 * c + j4];
-            const int o = 16 * c + 4 * j4;
-            acc[o + 0] = fmaf(s4.x, __uint_as_float(p[4 * j4 + 0]), fmaf(z4.x, nxs, acc[o + 0]));
-            acc[o + 1] = fmaf(s4.y, __uint_as_float(p[4 * j4 + 1]), fmaf(z4.y, nxs, acc[o + 1]));
-            acc[o + 2] = fmaf(s4.z, __uint_as_float(p[4 * j4 + 2]), fmaf(z4.z, nxs, acc[o + 2]));
-            acc[o + 3] = fmaf(s4.w, __uint_as_float(p[4 * j4 + 3]), fmaf(z4.w, nxs, acc[o + 3]));
-          }
-        }
-      };
-      // Software-pipelined drain: while 16 columns are folded, the next 16 are already on their way out of
-      // TMEM (the drain is the paced resource of this kernel: 64 KB per group at 64 B/clk).  tcgen05.wait::ld
-      // covers every outstanding load, so each load is issued right after the wait for the previous one.
-      uint32_t pa[16], pb[16];
-      auto ld16 = [&](uint32_t addr, uint32_t (&p)[16]) {  // warp-uniform choice: .x16, or the same columns as two .x8
-        if (narrow_drain) tc_ld16_narrow(addr, p);
-        else tc_ld16(addr, p);
-      };
-      ld16(taddr, pa);
-      tc_wait_ld16(pa);
-      if (e == 0) SB_TRACE(10, g);
-      ld16(taddr + 16, pb);
-      fold(0, pa);
-      tc_wait_ld16(pb);
-      ld16(taddr + 32, pa);
-      fold(1, pb);
-      tc_wait_ld16(pa);
-      ld16(taddr + 48, pb);
-      fold(2, pa);
-      tc_wait_ld16(pb);
-      if (e == 0) SB_TRACE(11, g);
-      // all 64 columns are in registers: the buffer may be overwritten by group g + kAccBufs
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm->tmem_empty[tb]);
-      fold(3, pb);
-      if (e == 0) SB_TRACE(12, g);
-      if (g + 1 < num_g) {
-        stage(b ^ 1, v_next);
-        xs = xs_next;
-      }
-      if (e == 0) SB_TRACE(6, g);
-    }
-    // out[m, n] += rowscale[m] * acc   (out is pre-initialised with the bias by the caller)
-    if (m < M) {
-      const float rs = __ldg(rowscale + m);
-      float* orow = out + (size_t)m * N + n0 + col0;
-      if ((N & 3) == 0 && ((reinterpret_cast<uintptr_t>(out) & 15u) == 0)) {
-#pragma unroll
-        for (int j4 = 0; j4 < 16; ++j4) {
-          if (n0 + col0 + 4 * j4 < N) {
-            float4 o = *reinterpret_cast<float4*>(orow + 4 * j4);
-            o.x = fmaf(rs, acc[4 * j4 + 0], o.x);
-            o.y = fmaf(rs, acc[4 * j4 + 1], o.y);
-            o.z = fmaf(rs, acc[4 * j4 + 2], o.z);
-            o.w = fmaf(rs, acc[4 * j4 + 3], o.w);
-            *reinterpret_cast<float4*>(orow + 4 * j4) = o;
-          }
-        }
+        for (int j = 0; j < 64; ++j) acc[j] = fmaf((j & 2) ? sb : sa, part[j], acc[j]);
       } else {
 #pragma unroll
-        for (int j = 0; j < 64; ++j)
-          if (n0 + col0 + j < N) orow[j] = fmaf(rs, acc[j], orow[j]);
+        for (int j = 0; j < 64; ++j) {
+          const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
+          const float nxs = (m < M) ? -__ldg(xsum + (size_t)m * G128 + g) : 0.f;
+          acc[j] = fmaf((j & 2) ? sb : sa, part[j], fmaf((j & 2) ? zfb : zfa, nxs, acc[j]));
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
+  // out[m, n] += rowscale[m] * acc   (out is pre-initialised with the bias by the caller)
+#pragma unroll
+  for (int j = 0; j < 64; ++j) {
+    const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
+    const int n = (j & 2) ? nb : na;
+    if (m < M && n < N) {
+      float* o = out + (size_t)m * N + n;
+      *o = fmaf(__ldg(rowscale + m), acc[j], *o);
+    }
   }
 }
 
@@ -509,12 +242,9 @@ int gptq_launch_split(const float* x, __half* a_hi, __half* a_lo, float* xsum, f
   return SB200_OK;
 }
 
-static long long* g_tc_trace = nullptr;
-void gptq4_tc_set_trace(long long* p) { g_tc_trace = p; }
 static int g_tc_backoff_ns = 0;
 void gptq4_tc_set_backoff(int ns) { g_tc_backoff_ns = ns; }
-static int g_tc_narrow_drain = 1;
-void gptq4_tc_set_drain(int narrow) { g_tc_narrow_drain = narrow; }
+int gptq4_tc_backoff() { return g_tc_backoff_ns; }
 
 bool gptq4_tc_supported(const float* x, const int32_t* qweight, const float* out, long long M, long long K, long long N,
                         long long KW, int group_size) {
@@ -559,23 +289,18 @@ int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* sc
   SB_LAUNCHED();
 
   CUtensorMap map_hi, map_lo, map_q;
-  const bool ok = make_map_2d(&map_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a_hi, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2,
-                              kBlockK, kTileM, CU_TENSOR_MAP_SWIZZLE_128B) &&
-                  make_map_2d(&map_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a_lo, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2,
-                              kBlockK, kTileM, CU_TENSOR_MAP_SWIZZLE_128B) &&
-                  make_map_2d(&map_q, CU_TENSOR_MAP_DATA_TYPE_INT32, qweight, (uint64_t)N, (uint64_t)KW, (uint64_t)N * 4,
-                              kTileN, kBlockK / 8, CU_TENSOR_MAP_SWIZZLE_NONE);
-  if (!ok) {
+  if (!make_wg_maps(&map_hi, &map_lo, &map_q, a_hi, a_lo, qweight, M, K, N, KW)) {
     set_error("gptq4_tc: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", M, K, N);
     return SB200_E_CUDA;
   }
-  const size_t smem = (size_t)kStages * kStageBytes + sizeof(TcSmem) + 1024;
+  const size_t smem = (size_t)kTcStages * kWgStageBytes + sizeof(TcSmem) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(gptq4_tc_kernel, (int)smem, attr_done));
-  const dim3 grid((unsigned)((M + kTileM - 1) / kTileM), (unsigned)((N + kTileN - 1) / kTileN));
-  gptq4_tc_kernel<<<grid, kTcThreads, smem, st>>>(map_hi, map_lo, map_q, out, scales, zeros, xsum, rowscale, zint, flag,
-                                                  (int)M, (int)K, (int)N, Gq, G128, group_size, g_tc_trace,
-                                                  g_tc_backoff_ns, g_tc_narrow_drain);
+  // one CTA per tile, token tile fastest: CTAs running side by side share the packed weight tile through L2
+  const long long tiles = ((M + kWgTok - 1) / kWgTok) * ((N + kWgFeat - 1) / kWgFeat);
+  gptq4_tc_kernel<<<(unsigned)tiles, kWgThreads, smem, st>>>(map_hi, map_lo, map_q, out, scales, zeros, xsum, rowscale,
+                                                            zint, flag, (int)M, (int)K, (int)N, Gq, G128, group_size,
+                                                            g_tc_backoff_ns);
   SB_LAUNCHED();
   return SB200_OK;
 }

@@ -1,65 +1,35 @@
-// gptq_ts.cu -- GPTQ int4 group-wise dequant-matmul on tcgen05 with the WEIGHTS as the tensor-memory operand.
+// gptq_ts.cu -- GPTQ int4 group-wise dequant-matmul on wgmma with the SCALED weights as the register operand.
 //
 // Replaces VecQuant4MatMulKernel (large_language_models/llama/quantization/cuda/cuda_kernel_4bit.cu:88-180) for
 // prefill-sized M:   out[m, n] += sum_k (scales[n, k/gs] * q[k, n] - zeros[n, k/gs]) * x[m, k]
 //
-// Why a second tensor-core kernel.  gptq_tc.cu keeps the int4 values exact in the MMA and applies the per-group
-// fp32 scale on the accumulator, which costs a 64 KB TMEM drain for every 512 cycles of MMA work (measured: 17.5 %
-// tensor-pipe utilisation, profiles/r01_prof_gptq_tc.txt).  Here the scale goes INTO the operand instead:
+// Why a second tensor-core kernel.  gptq_tc.cu keeps the int4 values exact in the MMA and applies the per-group fp32
+// scale on the accumulator every 128 K.  Here the scale goes INTO the operand instead:
 //   w'[n, k] = 2^e[n] * scales[n, g] * (q[k, n] - zero[n, g])  =  w_hi + w_lo     (two fp16 planes, 22 bits)
 // built with error-free half2 arithmetic (hi = s_hi * d rounded, t = fma(s_hi, d, -hi) exact, lo = fma(s_lo, d, t)),
 // so the accumulator runs over the whole K with no per-group epilogue.  The transposed problem is computed,
 //   D[n, m] = sum_k w'[n, k] * x'[m, k],
-// the weight planes are the A operand and are written by the unpack warps straight into TENSOR MEMORY with
-// tcgen05.st (no shared-memory round trip, no bank conflicts, half the MMA's shared-memory operand reads); the
-// activations x' = x * 2^-ex[m] = x_hi + x_lo (fp16 planes from gptq_split_kernel) are the B operand, TMA-loaded
-// as 256-token x 64-K SWIZZLE_128B tiles.  MMAs per 64-K stage: w_hi x_hi, w_lo x_hi (+ w_hi x_lo unless the
-// activations are fp16-exact, which is the reference's model path, utils/quant.py:262-277), all 128 x 256 x 16 into
-// ONE 128 x 256 fp32 accumulator (a dependent chain of N = 256 MMAs runs at 138 cycles each against the 128-cycle
-// floor; N = 128 would run at 94 against 64 -- profiles/r02_tmem_probe*.jsonl).
+// the weight planes are the A operand, built by every consumer thread in its own wgmma register fragment; the
+// activations x' = x * 2^-ex[m] = x_hi + x_lo (fp16 planes from gptq_split_kernel) are the B operand (tc_common.cuh).
+// wgmmas per 64-K stage: w_hi x_hi, w_lo x_hi (+ w_hi x_lo unless the activations are fp16-exact, which is the
+// reference's model path, utils/quant.py:262-277), all m64n128k16 into one fp32 register accumulator.
 //
-// Accumulator rounding.  The tensor core truncates when it accumulates (measured with positive operands: -1.0e-7
-// relative per MMA, profiles/r02_tmem_probe*.jsonl), so a K = 4096 chain of 512 MMAs would lose ~1e-5.  The
-// accumulator is therefore drained every `chunk` 64-K stages (default 8 = 512 K = 64 / 96 MMAs) into fp32 registers
-// that add with round-to-nearest; the drain moves 128 KB out of TMEM with tcgen05.ld.x8 (256 B/clk) while the
-// producers keep running ahead through the 3-stage ring.
-//
-// Roles (640 threads, one persistent CTA per SM; a tile = 128 features x 256 tokens over all of K):
-//   warp 0      TMA producer: x_hi (+ x_lo) tile and the packed 8 x 128 int32 weight tile per stage
-//   warp 1      MMA issuer (elect.sync lane), tcgen05.commit -> stage empty / chunk complete
-//   warp 2      TMEM allocator (512 columns: 256 accumulator + 3 stages x (32 hi + 32 lo) operand columns)
-//   warps 4-11  epilogue: each thread = one feature row (TMEM lane) x 128 tokens, fp32 register accumulators
-//   warps 12-19 unpack (two 4-warp sets, each on one half of every stage's 64 K): packed words -> (q - zero) integers ->
-//               scaled hi / lo planes -> tcgen05.st.x8 into the stage's operand columns
+// Accumulator rounding.  The tensor core does not round to nearest when it accumulates, so a K = 4096 chain of 512
+// MMAs could lose ~1e-5.  The accumulator is therefore restarted every `chunk` 64-K stages (default 8 = 512 K) and
+// added into a second fp32 register accumulator with round-to-nearest.
 // Zero points.  GPTQ checkpoints store zeros = zero * scale with an integer zero (utils/quant.py:188); the prepare
-// kernel verifies that on the device.  If it does not hold, the MMA runs on q alone and the epilogue subtracts
-// zeros[n, g] * sum_k x'[m, k in g] (the per-128-K row sums gptq_split_kernel already produces).
+// kernel verifies that on the device.  If it does not hold, the MMA runs on q - rint(zero) and the epilogue subtracts
+// the residual times sum_k x'[m, k in g] (the per-128-K row sums gptq_split_kernel already produces).
 #include "tc_common.cuh"
 
 namespace sb200 {
 
-constexpr int kWRows = 128;                              // output features per CTA = MMA M = TMEM lanes
-constexpr int kTok = 256;                                // tokens per CTA = MMA N (at most)
-constexpr int kTsBK = 64;                                // K per stage (one 128-byte swizzle atom of fp16)
-constexpr int kTsStages = 3;
-constexpr int kXBytes = kTok * kTsBK * 2;                // 32 KB  x_hi or x_lo tile
-constexpr int kQBytes = (kTsBK / 8) * kWRows * 4;        // 4 KB   packed words
-constexpr int kTsStageBytes = 2 * kXBytes + kQBytes;     // 68 KB
-constexpr uint32_t kAccCols = 256;
-constexpr uint32_t kAStageCols = 64;                     // 32 columns (64 fp16) hi plane + 32 lo plane
-constexpr uint32_t kTsTmemCols = 512;
-constexpr int kTsThreads = 640;
+constexpr int kTsStages = 5;
 constexpr int kGroup128 = 128;
 
 struct TsSmem {
   uint64_t full[kTsStages];   // TMA data of the stage landed
-  uint64_t ready[kTsStages];  // the stage's weight planes are in TMEM (8 warp arrivals)
-  uint64_t empty[kTsStages];  // the MMAs reading the stage completed (tcgen05.commit)
-  uint64_t acc_full;          // a chunk's MMAs completed
-  uint64_t acc_empty;         // the 8 epilogue warps drained the accumulator
-  uint32_t tmem_base;
-  uint32_t pad;
-  float rs[kTok];             // 2^ex[m] of the tile's tokens (0 beyond M)
+  uint64_t empty[kTsStages];  // the 8 consumer warps' wgmmas reading the stage completed
 };
 
 // ---------------------------------------------------------------------------------- weight-side prepare kernel
@@ -107,298 +77,155 @@ __global__ void gptq_ts_prepare_kernel(const float* __restrict__ scales, const f
   }
 }
 
-__device__ __forceinline__ __half2 u2h2(uint32_t v) { return *reinterpret_cast<const __half2*>(&v); }
-__device__ __forceinline__ uint32_t h22u(__half2 v) { return *reinterpret_cast<const uint32_t*>(&v); }
-
 // ---------------------------------------------------------------------------------- main kernel
-// Persistent: one CTA per SM walks the output tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (token tile fastest,
-// so CTAs running side by side share the packed weight tile through L2).  Stage and accumulator phases run on
-// counters that continue across tiles, so the producers start the next tile while the epilogue still writes the
-// previous one to global memory.
-__global__ void __launch_bounds__(kTsThreads, 1)
+// One CTA per 128-feature x 128-token tile (token tile fastest, so CTAs running side by side share the packed weight
+// tile through L2).
+__global__ void __launch_bounds__(kWgThreads, 1)
 gptq4_ts_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                 const __grid_constant__ CUtensorMap map_q, float* __restrict__ out, const float* __restrict__ scales,
                 const float* __restrict__ zeros,
                 const float* __restrict__ xsum, const float* __restrict__ rowscale, const uint2* __restrict__ sz,
                 const float* __restrict__ colscale, const int* __restrict__ flags, int M, int K, int N, int Gq, int G128,
-                int group_size, int chunk_kb, __half* __restrict__ out_h, const float* __restrict__ bias) {
+                int group_size, int chunk_kb, __half* __restrict__ out_h, const float* __restrict__ bias, int backoff_ns) {
   // out_h != nullptr: fp16 result  out_h[m, n] = bias[n] + x @ W  (overwrite, no read of `out`); otherwise the fp32
   // accumulate-in-place contract of the reference kernel, out[m, n] += x @ W.
   extern __shared__ unsigned char smem_raw[];
   unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  TsSmem* sm = reinterpret_cast<TsSmem*>(stage_base + (size_t)kTsStages * kTsStageBytes);
+  TsSmem* sm = reinterpret_cast<TsSmem*>(stage_base + (size_t)kTsStages * kWgStageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = (K + kTsBK - 1) / kTsBK;
-  const int num_chunks = (num_kb + chunk_kb - 1) / chunk_kb;
-  const int tiles_m = (M + kTok - 1) / kTok;
-  const int num_tiles = tiles_m * ((N + kWRows - 1) / kWRows);
+  const int tiles_m = (M + kWgTok - 1) / kWgTok;
+  const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kWgTok, n0 = (int)(blockIdx.x / (unsigned)tiles_m) * kWgFeat;
+  const int num_kb = (K + kWgBK - 1) / kWgBK;
   const bool int_zero = flags[0] != 0;  // uniform: every zeros[n, g] is an integer multiple of scales[n, g] (no residual)
   const bool need_lo = flags[1] != 0;   // uniform: some activation has a non-zero fp16 low part
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kTsStages; ++s) {
       mbar_init(&sm->full[s], 1);
-      mbar_init(&sm->ready[s], 8);  // one arrival per unpack warp (both sets work on every stage)
-      mbar_init(&sm->empty[s], 1);
+      mbar_init(&sm->empty[s], 8);  // one arrival per consumer warp
     }
-    mbar_init(&sm->acc_full, 1);
-    mbar_init(&sm->acc_empty, 8);
     mbar_fence_init();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm->tmem_base)),
-                 "r"(kTsTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sm->tmem_base;
 
-  if (warp < 4) reg_dec<40>();
-  if (warp == 0) {
+  if (warp < 4) {
     // ================================================================== TMA producer
-    if (lane == 0) {
-      const uint32_t tx = (uint32_t)(kXBytes + kQBytes + (need_lo ? kXBytes : 0));
-      uint32_t it = 0;  // stage counter, continues across tiles
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile % tiles_m) * kTok, n0 = (tile / tiles_m) * kWRows;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % kTsStages, ph = (it / kTsStages) & 1u;
-          mbar_wait_relaxed(&sm->empty[s], ph ^ 1u, 0);
-          unsigned char* st = stage_base + (size_t)s * kTsStageBytes;
-          mbar_expect_tx(&sm->full[s], tx);
-          tma_load_2d(st, &map_hi, kb * kTsBK, m0, &sm->full[s]);
-          if (need_lo) tma_load_2d(st + kXBytes, &map_lo, kb * kTsBK, m0, &sm->full[s]);
-          tma_load_2d(st + 2 * kXBytes, &map_q, n0, kb * (kTsBK / 8), &sm->full[s]);
+    reg_dec<40>();
+    if (threadIdx.x == 0)
+      wg_produce(stage_base, sm->full, sm->empty, kTsStages, &map_hi, &map_lo, &map_q, m0, n0, num_kb, need_lo, backoff_ns);
+    return;
+  }
+  // ==================================================================== consumers: 64 features x 128 tokens each
+  reg_inc<232>();
+  const int q = lane & 3;
+  const int f0 = ((warp - 4) >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);  // feature rows f0, f0 + 8 of the tile
+  const int na = n0 + f0, nb = na + 8;
+  const bool live_a = na < N, live_b = nb < N;
+  const NibblePair unpack(q);
+  const uint32_t stage0 = smem_u32(stage_base);
+  float acc[64], c[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+  for (int kb = 0; kb < num_kb;) {
+    const int kb_end = min(num_kb, kb + chunk_kb);
+    for (bool first = true; kb < kb_end; ++kb, first = false) {
+      const int s = kb % kTsStages;
+      const uint32_t ph = (uint32_t)(kb / kTsStages) & 1u;
+      const int gq = (int)((long long)kb * kWgBK / group_size);
+      // {fp16 hi | fp16 lo << 16 of 2^e * scale, fp16 bits of the integer zero} of both rows for this stage's group
+      const uint2 pa = live_a ? __ldg(sz + (size_t)na * Gq + gq) : make_uint2(0u, 0u);
+      const uint2 pb = live_b ? __ldg(sz + (size_t)nb * Gq + gq) : make_uint2(0u, 0u);
+      const __half2 sha = __half2half2(__ushort_as_half((unsigned short)(pa.x & 0xFFFFu)));
+      const __half2 sla = __half2half2(__ushort_as_half((unsigned short)(pa.x >> 16)));
+      const __half2 shb = __half2half2(__ushort_as_half((unsigned short)(pb.x & 0xFFFFu)));
+      const __half2 slb = __half2half2(__ushort_as_half((unsigned short)(pb.x >> 16)));
+      const __half2 offa = unpack.offset(__half2float(__ushort_as_half((unsigned short)pa.y)));
+      const __half2 offb = unpack.offset(__half2float(__ushort_as_half((unsigned short)pb.y)));
+      mbar_wait_relaxed(&sm->full[s], ph, 0);
+      const uint32_t* bq = reinterpret_cast<const uint32_t*>(stage_base + (size_t)s * kWgStageBytes + 2 * kWgXBytes);
+      uint32_t H[4][4], L[4][4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {  // 16 K = packed rows 2j (K 0..7) and 2j + 1 (K 8..15)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {  // fragment register r: row f0 / f0 + 8 (r & 1), K half (r >> 1)
+          const bool rb = (r & 1) != 0;
+          const __half2 d = unpack(bq[(2 * j + (r >> 1)) * kWgFeat + f0 + (rb ? 8 : 0)], rb ? offb : offa);  // q - zero
+          const __half2 sh = rb ? shb : sha, sl = rb ? slb : sla;
+          const __half2 hi = __hmul2(sh, d);               // RN16(s_hi * d)
+          const __half2 tt = __hfma2(sh, d, __hneg2(hi));  // s_hi * d - hi, exact
+          H[j][r] = h2u(hi);
+          L[j][r] = h2u(__hfma2(sl, d, tt));               // + s_lo * d
         }
       }
-      // Drain: the tcgen05.commit arrivals on empty[] of the last stages are asynchronous and nobody else waits for
-      // them.  The CTA must not exit while one is in flight (with a handful of tokens the epilogue finishes within
-      // nanoseconds of the last MMA): wait for each stage exactly as if one more load were to be issued into it.
-      for (int d = 0; d < kTsStages; ++d, ++it) {
-        const uint32_t s = it % kTsStages, ph = (it / kTsStages) & 1u;
-        mbar_wait_relaxed(&sm->empty[s], ph ^ 1u, 0);
+      const uint32_t xh = stage0 + (uint32_t)s * kWgStageBytes;
+      const uint64_t dh = gmma_desc_sw128(xh), dl = gmma_desc_sw128(xh + kWgXBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) wgmma_m64n128k16_rs(c, H[j], dh + 2 * j, !(first && j == 0));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) wgmma_m64n128k16_rs(c, L[j], dh + 2 * j, 1);
+      if (need_lo) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wgmma_m64n128k16_rs(c, H[j], dl + 2 * j, 1);
       }
+      wgmma_commit();
+      wgmma_wait_all(c);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&sm->empty[s]);
     }
-  } else if (warp == 1) {
-    // ================================================================== MMA issuer
-    const uint32_t stage0 = smem_u32(stage_base);
-    const uint64_t dconst = (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-    uint32_t it = 0, cc = 0;  // stage / chunk counters, continue across tiles
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile % tiles_m) * kTok;
-      // tokens this tile really has, rounded up to the MMA's N granularity (TMA zero-fills the rows beyond M)
-      const int tok_n = min(kTok, ((M - m0 + 15) >> 4) << 4);
-      // instruction descriptor: D = F32, A = B = F16, K-major, N = tok_n, M = 128
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(tok_n >> 3) << 17) | ((uint32_t)(kWRows >> 4) << 24);
-      int kb = 0;
-      for (int c = 0; c < num_chunks; ++c, ++cc) {
-        if (cc > 0) mbar_wait(&sm->acc_empty, (cc - 1) & 1u);  // the previous chunk left the accumulator
-        const int kb_end = min(num_kb, kb + chunk_kb);
-        for (bool first = true; kb < kb_end; ++kb, ++it, first = false) {
-          const uint32_t s = it % kTsStages, ph = (it / kTsStages) & 1u;
-          mbar_wait(&sm->ready[s], ph);  // implies full[s]: the unpack warps waited for it
-          tc_fence_after();
-          const uint32_t xh = stage0 + s * kTsStageBytes;
-          const uint64_t dbh = dconst | (uint64_t)((xh >> 4) & 0x3FFFu);
-          const uint64_t dbl = dconst | (uint64_t)(((xh + kXBytes) >> 4) & 0x3FFFu);
-          const uint32_t a_hi = tmem_base + kAccCols + s * kAStageCols;
-          const uint32_t a_lo = a_hi + 32;
-          if (elect_one()) {
 #pragma unroll
-            for (int k = 0; k < kTsBK / 16; ++k)  // 16 K = 8 TMEM columns of A, 32 bytes of B
-              tc_mma_f16_ts(tmem_base, a_hi + 8 * k, dbh + 2 * k, idesc, !(first && k == 0));
+    for (int j = 0; j < 64; ++j) acc[j] += c[j];
+  }
+  // d[j]: feature f0 + 8 * ((j >> 1) & 1), token m0 + 8 (j >> 2) + 2q + (j & 1)
+  const float csa = live_a ? __ldg(colscale + na) : 0.f, csb = live_b ? __ldg(colscale + nb) : 0.f;
 #pragma unroll
-            for (int k = 0; k < kTsBK / 16; ++k) tc_mma_f16_ts(tmem_base, a_lo + 8 * k, dbh + 2 * k, idesc, true);
-            if (need_lo) {
+  for (int j = 0; j < 64; ++j) acc[j] *= (j & 2) ? csb : csa;
+  if (!int_zero) {
+    // zero points with a fractional part: the MMA used q - rint(zero); subtract the residual
+    //   out = rs * (cs * acc - sum_g (zeros[n, g] - rint(zero) * scales[n, g]) * xsum[m, g])
+    for (int g = 0; g < G128; ++g) {
+      const int gq = (int)((long long)g * kGroup128 / group_size);
+      float zr[2] = {0.f, 0.f};
 #pragma unroll
-              for (int k = 0; k < kTsBK / 16; ++k) tc_mma_f16_ts(tmem_base, a_hi + 8 * k, dbl + 2 * k, idesc, true);
-            }
-            tc_commit(&sm->empty[s]);
-            if (kb == kb_end - 1) tc_commit(&sm->acc_full);
-          }
-          __syncwarp();
+      for (int h = 0; h < 2; ++h) {
+        const int n = h ? nb : na;
+        if (n < N) {
+          const float zi = __half2float(__ushort_as_half((unsigned short)__ldg(&sz[(size_t)n * Gq + gq].y)));
+          zr[h] = -fmaf(-zi, __ldg(scales + (size_t)n * Gq + gq), __ldg(zeros + (size_t)n * Gq + gq));
         }
       }
-    }
-  } else if (warp >= 12) {
-    // ================================================================== unpack: packed int4 -> scaled fp16 planes in TMEM
-    reg_dec<56>();
-    const int t = (threadIdx.x - 12 * 32) & 127;  // feature row of the tile = TMEM lane
-    const uint32_t uset = (uint32_t)(warp - 12) >> 2;
-    uint32_t bias;
-    asm volatile("mov.b32 %0, 0x64006400;" : "=r"(bias));  // half2(1024, 1024); opaque to constant propagation
-    const uint32_t lane_base = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + kAccCols;
-    const __half2 k16 = __float2half2_rn(0.0625f);
-    // Both 4-warp sets work on EVERY stage, each on one half of its 64 K (set 0: packed rows 0-3 = MMA K steps 0, 1;
-    // set 1: rows 4-7 = K steps 2, 3).  (Alternating whole stages between the sets would make each set see only every
-    // other phase of full[s] -- 3 stages, 2 sets -- and a parity wait cannot tell "my phase completed" from "the
-    // barrier is still a phase behind me": with tiny MMAs a set that ran ahead of the TMA frontier unpacked stale words.)
-    uint32_t it = 0;  // stage counter, continues across tiles
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int n = (tile / tiles_m) * kWRows + t;
-      const bool live = n < N;
-      // quantisation group of the stage, advanced incrementally; its parameters are fetched one stage ahead
-      int gq_next = 0;
-      long long koff_next = 0;
-      auto fetch = [&](int kb) -> uint2 {
-        if (!live || kb >= num_kb) return make_uint2(0u, 0u);
-        return __ldg(sz + (size_t)n * Gq + gq_next);
-      };
-      uint2 p_cur = fetch(0);
-      for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const uint32_t s = it % kTsStages, ph = (it / kTsStages) & 1u;
-        koff_next += kTsBK;
-        while (koff_next >= (long long)(gq_next + 1) * group_size) ++gq_next;
-        const uint2 p_next = fetch(kb + 1);
-        // scale planes and zero point of this stage's group
-        const __half2 sh2 = __half2half2(__ushort_as_half((unsigned short)(p_cur.x & 0xFFFFu)));
-        const __half2 sl2 = __half2half2(__ushort_as_half((unsigned short)(p_cur.x >> 16)));
-        const float zf = __half2float(__ushort_as_half((unsigned short)p_cur.y));
-        const __half2 zsub = __float2half2_rn(1024.f + zf);  // exact: |zero| <= 1024
-        const __half2 noff = __float2half2_rn(-(64.f + zf));
-        p_cur = p_next;
-        mbar_wait_relaxed(&sm->full[s], ph, 0);
-        const uint32_t* bq = reinterpret_cast<const uint32_t*>(stage_base + (size_t)s * kTsStageBytes + 2 * kXBytes);
-        uint32_t w[kTsBK / 16];
 #pragma unroll
-        for (int r = 0; r < kTsBK / 16; ++r) w[r] = bq[(uset * (kTsBK / 16) + r) * kWRows + t];
-        const uint32_t abase = lane_base + s * kAStageCols;
-#pragma unroll
-        for (int pp = 0; pp < kTsBK / 32; ++pp) {  // two packed words = 16 K = one MMA K step = 8 TMEM columns per plane
-          const int p = (int)uset * (kTsBK / 32) + pp;
-          uint32_t H[8], L[8];
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const uint32_t lo32 = w[2 * pp + i], hi32 = lo32 >> 8;
-            // 0x6400 | q = fp16(1024 + q);  0x6400 | (q << 4) = fp16(1024 + 16 q)
-            const __half2 v0 = u2h2(and_or<0x000F000Fu>(lo32, bias));  // k = 8r + (0, 4)
-            const __half2 v1 = u2h2(and_or<0x00F000F0u>(lo32, bias));  // k = 8r + (1, 5), times 16
-            const __half2 v2 = u2h2(and_or<0x000F000Fu>(hi32, bias));  // k = 8r + (2, 6)
-            const __half2 v3 = u2h2(and_or<0x00F000F0u>(hi32, bias));  // k = 8r + (3, 7), times 16
-            __half2 d[4];
-            d[0] = __hsub2(v0, zsub);        // (1024 + q) - (1024 + zero)           = q - zero, exact
-            d[1] = __hfma2(v1, k16, noff);   // (1024 + 16 q) / 16 - (64 + zero)     = q - zero, exact
-            d[2] = __hsub2(v2, zsub);
-            d[3] = __hfma2(v3, k16, noff);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const __half2 hi = __hmul2(sh2, d[j]);                  // RN16(s_hi * d)
-              const __half2 tt = __hfma2(sh2, d[j], __hneg2(hi));     // s_hi * d - hi, exact
-              const __half2 lo = __hfma2(sl2, d[j], tt);              // + s_lo * d
-              H[4 * i + j] = h22u(hi);
-              L[4 * i + j] = h22u(lo);
-            }
-          }
-          tc_st8(abase + 8 * p, H);
-          tc_st8(abase + 32 + 8 * p, L);
-        }
-        tc_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm->ready[s]);
-      }
-    }
-  } else if (warp >= 4) {
-    // ================================================================== epilogue (8 warps)
-    reg_inc<160>();
-    const int e = threadIdx.x - 4 * 32;     // 0..255
-    const int quarter = warp & 3;           // TMEM lane quarter this warp may read
-    const int half = (warp - 4) >> 2;       // which 128 token columns
-    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(half * 128);
-    uint32_t cc = 0;  // chunk counter, continues across tiles
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile % tiles_m) * kTok;
-      const int n = (tile / tiles_m) * kWRows + quarter * 32 + lane;  // this thread's output feature
-      asm volatile("bar.sync 1, 256;" ::: "memory");  // every epilogue warp finished reading rs[] of the previous tile
-      sm->rs[e] = (m0 + e < M) ? __ldg(rowscale + m0 + e) : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      float acc[128];
-#pragma unroll
-      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
-      for (int c = 0; c < num_chunks; ++c, ++cc) {
-        mbar_wait(&sm->acc_full, cc & 1u);
-        tc_fence_after();
-#pragma unroll
-        for (int g = 0; g < 16; g += 2) {
-          uint32_t a[8], b[8];
-          tc_ld8(taddr + 8 * g, a);
-          tc_ld8(taddr + 8 * g + 8, b);
-          tc_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            acc[8 * g + j] += __uint_as_float(a[j]);
-            acc[8 * g + 8 + j] += __uint_as_float(b[j]);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm->acc_empty);
-      }
-      // the accumulator is free again: the MMAs of the next tile run while this tile is written out
-      if (n < N) {
-        const float cs = __ldg(colscale + n);
-#pragma unroll
-        for (int j = 0; j < 128; ++j) acc[j] *= cs;
-        if (!int_zero) {
-          // zero points with a fractional part: the MMA used q - rint(zero); subtract the residual
-          //   out = rs * (cs * acc - sum_g (zeros[n, g] - rint(zero) * scales[n, g]) * xsum[m, g])
-          int gq = 0;
-          long long kend = group_size;
-          for (int g = 0; g < G128; ++g) {
-            while ((long long)g * kGroup128 >= kend) { ++gq; kend += group_size; }
-            const float zi = __half2float(__ushort_as_half((unsigned short)__ldg(&sz[(size_t)n * Gq + gq].y)));
-            const float zr = -fmaf(-zi, __ldg(scales + (size_t)n * Gq + gq), __ldg(zeros + (size_t)n * Gq + gq));
-#pragma unroll
-            for (int j = 0; j < 128; ++j) {
-              const int m = m0 + half * 128 + j;
-              if (m < M) acc[j] = fmaf(zr, __ldg(xsum + (size_t)m * G128 + g), acc[j]);
-            }
-          }
-        }
-        // out[m, n] += rs[m] * acc: 16 independent loads in flight, then 16 stores (a load-modify-store per element
-        // would serialise 128 global round trips: the compiler cannot prove that row j + 1 does not alias row j)
-        const float* rsv = sm->rs + half * 128;
-        const int rows_here = min(128, M - (m0 + half * 128));
-        if (out_h) {
-          const float bn = bias ? __ldg(bias + n) : 0.f;
-          __half* hcol = out_h + (size_t)(m0 + half * 128) * N + n;
-#pragma unroll
-          for (int j = 0; j < 128; ++j)
-            if (j < rows_here) hcol[(size_t)j * N] = __float2half_rn(fmaf(rsv[j], acc[j], bn));
-          continue;
-        }
-        float* ocol = out + (size_t)(m0 + half * 128) * N + n;
-#pragma unroll
-        for (int j0 = 0; j0 < 128; j0 += 16) {
-          float o[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) o[j] = (j0 + j < rows_here) ? __ldcg(ocol + (size_t)(j0 + j) * N) : 0.f;
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (j0 + j < rows_here) __stcg(ocol + (size_t)(j0 + j) * N, fmaf(rsv[j0 + j], acc[j0 + j], o[j]));
-        }
+      for (int j = 0; j < 64; ++j) {
+        const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
+        if (m < M) acc[j] = fmaf(zr[(j >> 1) & 1], __ldg(xsum + (size_t)m * G128 + g), acc[j]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTsTmemCols) : "memory");
+  const float bna = (out_h && bias && live_a) ? __ldg(bias + na) : 0.f;
+  const float bnb = (out_h && bias && live_b) ? __ldg(bias + nb) : 0.f;
+#pragma unroll
+  for (int j = 0; j < 64; ++j) {
+    const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
+    const int n = (j & 2) ? nb : na;
+    if (m < M && n < N) {
+      const float rs = __ldg(rowscale + m);
+      if (out_h) {
+        out_h[(size_t)m * N + n] = __float2half_rn(fmaf(rs, acc[j], (j & 2) ? bnb : bna));
+      } else {
+        float* o = out + (size_t)m * N + n;
+        *o = fmaf(rs, acc[j], *o);
+      }
+    }
   }
 }
 
 // ---------------------------------------------------------------------------------- host side
 int gptq_launch_split(const float* x, __half* a_hi, __half* a_lo, float* xsum, float* rowscale, int* need_lo, long long M,
                       int K, int G, cudaStream_t st);  // gptq_tc.cu
+int gptq4_tc_backoff();                                // gptq_tc.cu
 
 struct TsWorkspace {
   size_t off_hi, off_lo, off_xsum, off_rs, off_sz, off_cs, off_flag, total;
@@ -482,23 +309,17 @@ int gptq4_ts(const float* x, const int32_t* qweight, float* out, const float* sc
   }
 
   CUtensorMap map_hi, map_lo, map_q;
-  const bool ok = make_map_2d(&map_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a_hi, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2,
-                              kTsBK, kTok, CU_TENSOR_MAP_SWIZZLE_128B) &&
-                  make_map_2d(&map_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a_lo, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2,
-                              kTsBK, kTok, CU_TENSOR_MAP_SWIZZLE_128B) &&
-                  make_map_2d(&map_q, CU_TENSOR_MAP_DATA_TYPE_INT32, qweight, (uint64_t)N, (uint64_t)KW, (uint64_t)N * 4,
-                              kWRows, kTsBK / 8, CU_TENSOR_MAP_SWIZZLE_NONE);
-  if (!ok) {
+  if (!make_wg_maps(&map_hi, &map_lo, &map_q, a_hi, a_lo, qweight, M, K, N, KW)) {
     set_error("gptq4_ts: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", M, K, N);
     return SB200_E_CUDA;
   }
-  const size_t smem = (size_t)kTsStages * kTsStageBytes + sizeof(TsSmem) + 1024;
+  const size_t smem = (size_t)kTsStages * kWgStageBytes + sizeof(TsSmem) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(gptq4_ts_kernel, (int)smem, attr_done));
-  const long long num_tiles = ((M + kTok - 1) / kTok) * ((N + kWRows - 1) / kWRows);
-  const unsigned grid = (unsigned)(num_tiles < sm_count() ? num_tiles : sm_count());  // persistent: one CTA per SM
-  gptq4_ts_kernel<<<grid, kTsThreads, smem, st>>>(map_hi, map_lo, map_q, out, scales, zeros, xsum, rowscale, sz, cs, flag, (int)M,
-                                                  (int)K, (int)N, Gq, G128, group_size, chunk_kb, out_h, bias);
+  const long long tiles = ((M + kWgTok - 1) / kWgTok) * ((N + kWgFeat - 1) / kWgFeat);
+  gptq4_ts_kernel<<<(unsigned)tiles, kWgThreads, smem, st>>>(map_hi, map_lo, map_q, out, scales, zeros, xsum, rowscale, sz, cs,
+                                                            flag, (int)M, (int)K, (int)N, Gq, G128, group_size, chunk_kb,
+                                                            out_h, bias, gptq4_tc_backoff());
   SB_LAUNCHED();
   return SB200_OK;
 }

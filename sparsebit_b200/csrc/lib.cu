@@ -21,11 +21,11 @@ int sm_count() {
   // Cached per device ordinal (up to 64 devices per process).
   static std::atomic<int> cache[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   int v = cache[dev].load(std::memory_order_relaxed);
   if (v > 0) return v;
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   cache[dev].store(n, std::memory_order_relaxed);
   return n;
 }

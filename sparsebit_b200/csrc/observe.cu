@@ -1,4 +1,4 @@
-// observe.cu -- Observer calibration reductions for sm_100a.
+// observe.cu -- Observer calibration reductions for sm_90a.
 //
 // Replaces the ATen op chains inside the reference observers (megvii-research/Sparsebit):
 //   observers/minmax.py:14-25        torch.cat + min/max                  -> minmax_* kernels

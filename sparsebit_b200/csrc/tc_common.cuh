@@ -1,5 +1,12 @@
-// tc_common.cuh -- PTX wrappers shared by the tcgen05 GPTQ kernels (gptq_tc.cu, gptq_ts.cu): mbarrier / TMA /
-// tcgen05 (mma, commit, ld, st, fences), elect.sync, setmaxnreg, cuTensorMapEncodeTiled lookup.
+// tc_common.cuh -- pieces shared by the wgmma GPTQ kernels (gptq_tc.cu, gptq_ts.cu): mbarrier / TMA / wgmma PTX
+// wrappers, setmaxnreg, the in-register int4 -> fp16 fragment unpack, the TMA producer role, cuTensorMapEncodeTiled.
+//
+// Both kernels compute the transposed product D[n, m] = sum_k W[n, k] * x'[m, k] with one warpgroup-wide
+// wgmma.m64n128k16 per 16 K: the weights are the A operand, unpacked by every consumer thread straight into its own
+// register fragment (no shared-memory round trip for the fp16 weights), the activations x' (fp16 planes, every 8 K
+// permuted as 0,4,1,5,2,6,3,7) are the B operand, TMA-loaded as 128-token x 64-K SWIZZLE_128B tiles.
+// CTA = one 128-feature x 128-token output tile: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = 64
+// features each.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -9,6 +16,14 @@
 #include "common.cuh"
 
 namespace sb200 {
+
+constexpr int kWgFeat = 128;                                 // features per CTA (two consumer warpgroups x 64)
+constexpr int kWgTok = 128;                                  // tokens per CTA = wgmma N
+constexpr int kWgBK = 64;                                    // K per stage = one 128-byte swizzle atom of fp16
+constexpr int kWgThreads = 384;                              // producer warpgroup + two consumer warpgroups
+constexpr int kWgXBytes = kWgTok * kWgBK * 2;                // 16 KB  x_hi or x_lo tile
+constexpr int kWgQBytes = (kWgBK / 8) * kWgFeat * 4;         // 4 KB   packed words [8][128]
+constexpr int kWgStageBytes = 2 * kWgXBytes + kWgQBytes;     // 36 KB  (a multiple of 1024: every tile stays aligned)
 
 // ---------------------------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -21,24 +36,7 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"((uint32_t)accum)
-      : "memory");
-}
-// mbarrier wait with an optional back-off between polls: the producer / issuer / unpack roles spend most of their
-// time waiting, and every poll is an MIO operation competing with the LDS / STS / tcgen05.ld traffic of the
-// roles that are busy (sb200_gptq4_set_wait_backoff; 0 = poll continuously like mbar_wait).
+// mbarrier wait with an optional back-off between polls (sb200_gptq4_set_wait_backoff; 0 = poll continuously)
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, int backoff_ns) {
   for (;;) {
     uint32_t done;
@@ -53,100 +51,89 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity
     if (backoff_ns > 0) __nanosleep((unsigned)backoff_ns);
   }
 }
-// elect.sync: exactly one lane of a converged warp gets `true`.  Unlike `lane == 0` the compiler knows the
-// guarded code runs on a single lane of a uniform warp and keeps tcgen05 operands in uniform registers
-// (no per-instruction ELECT / R2UR.BROADCAST / BRA.U.ANY lane loop).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-      "elect.sync rx|px, %1;\n\t"
-      "@px mov.s32 %0, 1;\n\t}"
-      : "+r"(pred)
-      : "r"(0xFFFFFFFFu));
-  return pred != 0;
-}
-template <uint32_t MASK>
-__device__ __forceinline__ uint32_t and_or(uint32_t x, uint32_t c) {
-  uint32_t r;
-  asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(r) : "r"(x), "n"(MASK), "r"(c));
-  return r;
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// the same 16 columns as two .x8 loads issued back to back (the narrow forms pipeline through the TMEM read port far
-// better than the wide ones: 256 B/clk/SM for .x8 pairs against 52 for .x16, profiles/r02_tmem_probe*.jsonl)
-__device__ __forceinline__ void tc_ld16_narrow(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%16];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%8,%9,%10,%11,%12,%13,%14,%15}, [%17];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr), "r"(taddr + 8)
-      : "memory");
-}
-// wait for the outstanding tcgen05.ld; the registers are threaded through the statement so that no use of them
-// can be scheduled above the wait
-__device__ __forceinline__ void tc_wait_ld16(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
 
-// Register re-balancing between warpgroups (the kernel is launched with 65536 / 640 -> 96 registers per
-// thread; the epilogue needs ~130 for its 64 accumulators, the other roles far fewer).
+// Register re-balancing between warpgroups (384 threads launch with 168 registers each; the producer needs few, the
+// consumers hold two 64-float accumulators plus the weight fragments).
 template <int N>
 __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N>
 __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait for every outstanding wgmma of this warpgroup; the accumulators are threaded through the statement so that no
+// use of them can be scheduled above the wait
+__device__ __forceinline__ void wgmma_wait_all(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// A operand read from TENSOR MEMORY (the "TS" form): D[tmem] += A[tmem] * B[smem]
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, bool accum) {
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA form): [0,14) start address >> 4 | [16,30) LBO >> 4
+// (unused for swizzled K-major, 1) | [32,46) SBO >> 4 = 1024 B between 8-row groups | [62,64) layout 1 = SWIZZLE_128B.
+// Advancing 16 K inside the 128-byte atom adds 32 bytes (2) to the start address field.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128]: A = fp16 fragments in registers (the m16n8k16 layout per warp, warp w of the
+// warpgroup holding rows 16w..16w+15), B = 128 x 16 fp16 K-major in shared memory (SWIZZLE_128B descriptor), fp32 D in
+// registers.  accumulate == 0 overwrites D.
+__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"((uint32_t)accum)
-      : "memory");
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "{%64,%65,%66,%67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
-// 32 lanes x 8 consecutive 32-bit columns (the narrow forms pipeline far better than .x32: measured 256 B/clk/SM
-// with four .x8 loads in flight against 57 B/clk/SM for one .x32, profiles/r02_tmem_probe*.jsonl)
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
+
+// ---------------------------------------------------------------------------------- int4 -> fp16 fragment unpack
+// One packed word = 8 nibbles along K.  With the activations permuted inside every 8 K as 0,4,1,5,2,6,3,7, the two
+// fp16 values a thread with (lane & 3) == q needs from a word (K positions 2q, 2q+1 of the fragment layout) are the
+// nibbles q and q + 4: one shift, one (x & mask) | bias, one HFMA2.  0x6400 | v is the fp16 number 1024 + v; the odd
+// pairs are extracted in place (bits 4..7, i.e. 1024 + 16 q) and brought back by the multiplier 1/16.
+struct NibblePair {
+  uint32_t shift, mask;
+  __half2 mul;
+  float base;  // 1024 or 64: the bias the extraction leaves after the multiplier
+  __device__ __forceinline__ explicit NibblePair(int q) {
+    shift = (uint32_t)(q >> 1) * 8u;
+    mask = (q & 1) ? 0x00F000F0u : 0x000F000Fu;
+    mul = __float2half2_rn((q & 1) ? 0.0625f : 1.f);
+    base = (q & 1) ? 64.f : 1024.f;
+  }
+  // -(base + zero) for an integer zero point |zero| <= 1024 (exact in fp16)
+  __device__ __forceinline__ __half2 offset(float zero) const { return __float2half2_rn(-(base + zero)); }
+  // (q - zero) for the two nibbles, exact
+  __device__ __forceinline__ __half2 operator()(uint32_t w, __half2 off) const {
+    const uint32_t v = ((w >> shift) & mask) | 0x64006400u;
+    return __hfma2(*reinterpret_cast<const __half2*>(&v), mul, off);
+  }
+};
+__device__ __forceinline__ uint32_t h2u(__half2 v) { return *reinterpret_cast<const uint32_t*>(&v); }
+
+// ---------------------------------------------------------------------------------- TMA producer role
+// Stage s of a tile: x_hi [128 tok][64 K] | x_lo [128 tok][64 K] (only when need_lo) | packed words [8][128 features].
+__device__ __forceinline__ void wg_produce(unsigned char* stage_base, uint64_t* full, uint64_t* empty, int stages,
+                                           const CUtensorMap* map_hi, const CUtensorMap* map_lo, const CUtensorMap* map_q,
+                                           int m0, int n0, int num_kb, bool need_lo, int backoff_ns) {
+  const uint32_t tx = (uint32_t)(kWgXBytes + kWgQBytes + (need_lo ? kWgXBytes : 0));
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % stages;
+    const uint32_t ph = (uint32_t)(kb / stages) & 1u;
+    mbar_wait_relaxed(&empty[s], ph ^ 1u, backoff_ns);
+    unsigned char* st = stage_base + (size_t)s * kWgStageBytes;
+    mbar_expect_tx(&full[s], tx);
+    tma_load_2d(st, map_hi, kb * kWgBK, m0, &full[s]);
+    if (need_lo) tma_load_2d(st + kWgXBytes, map_lo, kb * kWgBK, m0, &full[s]);
+    tma_load_2d(st + 2 * kWgXBytes, map_q, n0, kb * (kWgBK / 8), &full[s]);
+  }
 }
-__device__ __forceinline__ void tc_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%8], {%0,%1,%2,%3,%4,%5,%6,%7};" ::"r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------- tensor maps (host)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -176,6 +163,17 @@ static inline bool make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const v
   const cuuint32_t estr[2] = {1, 1};
   return enc(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// the three maps of a launch: activation planes (128-token x 64-K boxes, SWIZZLE_128B) and packed words (128 x 8)
+static inline bool make_wg_maps(CUtensorMap* hi, CUtensorMap* lo, CUtensorMap* q, const __half* a_hi, const __half* a_lo,
+                                const int32_t* qweight, long long M, long long K, long long N, long long KW) {
+  return make_map_2d(hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a_hi, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2, kWgBK, kWgTok,
+                     CU_TENSOR_MAP_SWIZZLE_128B) &&
+         make_map_2d(lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a_lo, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2, kWgBK, kWgTok,
+                     CU_TENSOR_MAP_SWIZZLE_128B) &&
+         make_map_2d(q, CU_TENSOR_MAP_DATA_TYPE_INT32, qweight, (uint64_t)N, (uint64_t)KW, (uint64_t)N * 4, kWgFeat,
+                     kWgBK / 8, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }

@@ -1,6 +1,6 @@
 """Drop-in for the reference's JIT-built pybind module ``fake_quant``
 (sparsebit/quantization/torch_extensions/export.cc:3-8): same four names, argument order and
-return conventions, backed by the sm_100a C-ABI library instead of the PPQ-derived kernels.
+return conventions, backed by the sm_90a C-ABI library instead of the PPQ-derived kernels.
 
     import sparsebit_b200.fake_quant as fake_quant_kernel
     y = fake_quant_kernel.quant_pertensor_forward(x, scale, zero_point, qmin, qmax, 0)

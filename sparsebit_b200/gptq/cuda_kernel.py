@@ -1,6 +1,6 @@
 """Drop-in for the reference's JIT-built pybind module ``cuda_kernel``
 (large_language_models/llama/quantization/cuda/cuda_kernel.cpp:10-73): same six names, argument order
-and in-place-accumulate contract, backed by ``sb200_gptq4_matmul`` (4-bit: tcgen05 / SIMT) and
+and in-place-accumulate contract, backed by ``sb200_gptq4_matmul`` (4-bit: wgmma / SIMT) and
 ``sb200_gptq_matmul`` (3-bit, 2-bit: SIMT)."""
 from .. import ops
 

@@ -1,7 +1,7 @@
 """``QuantLinear`` for 2 / 3 / 4-bit GPTQ checkpoints (large_language_models/llama/quantization/utils/
 quant.py:147-420): same buffers (``qweight`` int32 [rows, N], ``scales`` / ``zeros`` [N, G, 1] with
 zeros = zero * scale, ``bias``), same packed layouts, same forward contract -- the 4-bit matmul runs in
-``sb200_gptq4_matmul`` (tcgen05 tensor cores for prefill-sized M, HBM-bound SIMT for decode), 3 / 2-bit in
+``sb200_gptq4_matmul`` (wgmma tensor cores for prefill-sized M, HBM-bound SIMT for decode), 3 / 2-bit in
 ``sb200_gptq_matmul`` (SIMT)."""
 import torch
 import torch.nn as nn

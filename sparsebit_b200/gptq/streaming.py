@@ -9,8 +9,8 @@ What differs from the reference:
 * the host copies are pinned once, so the H2D copies are truly asynchronous (``.to(cuda)`` from pageable memory, as
   the reference does it, serialises with the host);
 * readiness / reuse is tracked with CUDA events per slot instead of three new streams per layer.
-scales / zeros / bias stay resident like in the reference (they are 1/8 of the packed weights).  On a 180 GB B200 a
-7B ... 65B int4 model fits entirely, so this is for models beyond HBM or for sharing the GPU; it is part of the
+scales / zeros / bias stay resident like in the reference (they are 1/8 of the packed weights).  On an 80 GB H100 a
+7B ... 65B int4 model fits entirely (65B: 33 GB of packed weights), so this is for models beyond HBM or for sharing the GPU; it is part of the
 reference's inference path (SURVEY 8f #3) and kept behaviour-compatible: same outputs as the resident execution."""
 import torch
 

@@ -3,7 +3,7 @@
 scale is an ``nn.Parameter`` initialised from calibration data as 2 * mean(|x|) / sqrt(qmax)
 (per tensor or per channel, lsq.py:32-51); the forward is the same fake-quant op as ``uniform`` with
 the scale's gradient damped by 1 / sqrt(numel * qmax) (lsq.py:68-76).  Forward and backward run in
-the sm_100a kernels through ``STE`` (the scale gradient is the kernels' deterministic ``gs``).
+the sm_90a kernels through ``STE`` (the scale gradient is the kernels' deterministic ``gs``).
 """
 import math
 import warnings

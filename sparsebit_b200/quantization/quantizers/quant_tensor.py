@@ -16,7 +16,7 @@ from ..common import Backend
 
 
 def _host_forward(x_f, scale, zero_point, qdesc):
-    """CPU tensors: sb200_qdq_*_fwd_host (H2D -> sm_100a kernel -> D2H inside the library)."""
+    """CPU tensors: sb200_qdq_*_fwd_host (H2D -> sm_90a kernel -> D2H inside the library)."""
     lib = _lib.load()
     x = x_f.detach().float().contiguous()
     out = torch.empty_like(x)

@@ -96,7 +96,6 @@ def test_widened_entry_points_validate_before_launching():
     assert lib.sb200_gptq4_set_wait_backoff(-1) == -1
     assert lib.sb200_gptq4_set_wait_backoff(0) == 0
     assert lib.sb200_gptq4_set_decode(256) == -1 and lib.sb200_gptq4_set_decode(6) == 0
-    assert lib.sb200_gptq4_set_tc_drain(2) == -1 and lib.sb200_gptq4_set_tc_drain(1) == 0
     assert lib.sb200_gptq4_matmul_batch_ex(p, 1, 1, 2, None) == -1 and b"flags" in lib.sb200_last_error()
     assert lib.sb200_gptq4_linear_f16_state_bytes() >= 4 * 16384
     assert lib.sb200_gptq4_linear_f16_ex(p, p, p, None, p, p, 1, 128, 128, 16, 128, p, 4, p, 1 << 20, None) == -1 and b"flags" in lib.sb200_last_error()

@@ -66,7 +66,7 @@ def test_vs_fp64_oracle(bshape, k, n, gs, impl):
     np.testing.assert_allclose(y, exp, **TOL)
 
 
-# tcgen05 path forced (sb200_gptq4_set_impl(2)): ragged M / N tiles, odd number of 64-K stages,
+# per-group wgmma path forced (sb200_gptq4_set_impl(2)): ragged M / N tiles, odd number of 64-K stages,
 # group sizes 128 / 256 / 384, a single row, outlier activations (per-row power-of-two scaling).
 TC_CASES = [
     ((1,), 128, 128, 128), ((128,), 256, 128, 128), ((130,), 512, 264, 128), ((29,), 8192, 1024, 128),
@@ -152,8 +152,8 @@ def test_decode_hmma_path_vs_fp64_oracle(m, k, n, gs, fp16_acts, mode, decode_mo
         np.testing.assert_array_less(np.abs(y[0] - exp[0]), 1e-5 + 1e-5 * max(1.0, np.abs(exp[0]).max()))
 
 
-# tensor-memory-operand kernel (impl 3, gptq_ts.cu): ragged token / feature tiles, odd numbers of 64-K stages,
-# several chunks, group sizes 128 / 256 / 384, a single row, tiles of exactly 256 tokens and one more
+# weight-plane wgmma kernel (impl 3, gptq_ts.cu): ragged token / feature tiles, odd numbers of 64-K stages,
+# several chunks, group sizes 128 / 256 / 384, a single row, several 128-token tiles and ragged last tiles
 TS_CASES = [
     ((1,), 128, 128, 128), ((128,), 256, 128, 128), ((130,), 512, 264, 128), ((29,), 8192, 1024, 128),
     ((4,), 6144, 768, 384), ((300,), 1024, 512, 256), ((2, 130), 512, 260, 128), ((257,), 192 * 2, 132, 128),
@@ -289,7 +289,7 @@ def test_linear_f16_decode_sized_is_one_launch(m, k, n, gs):
     y_c = ops.gptq4_linear_f16(*args)
     before = launch_count()
     y_staged = ops.gptq4_linear_f16(*args, single_launch=False)
-    assert launch_count() - before >= 4  # cast, bias, kernel(s), cast (M = 32 runs the per-group tcgen05 kernel: two more)
+    assert launch_count() - before >= 4  # cast, bias, kernel(s), cast (M = 32 runs the per-group wgmma kernel: two more)
     a = y_a.cpu().numpy()
     assert a.dtype == np.float16 and a.shape == (m, n)
     assert np.array_equal(a, y_b.cpu().numpy()) and np.array_equal(a, y_c.cpu().numpy())  # fixed summation order
@@ -383,7 +383,7 @@ def test_linearity_and_accumulate_contract_at_llama_shape():
     rows = [0, 255, 256, 777, 2047]
     exp = ogptq.dequant_matmul(x[rows], qw, np.broadcast_to(bias, (len(rows), n)), scales, zeros, 128)
     np.testing.assert_allclose(y1[rows], exp, **TOL)
-    for impl in (2, 3):  # both tcgen05 kernels at the full shape
+    for impl in (2, 3):  # both wgmma kernels at the full shape
         np.testing.assert_allclose(_run_impl(x, qw, bias, scales, zeros, 128, impl=impl)[rows], exp, **TOL)
 
 

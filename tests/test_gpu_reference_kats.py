@@ -3,7 +3,7 @@ test_cuda_kernel.py:21-126, all thirteen 4-bit cases incl. M=6661 / N=25163, 122
 ``QuantLinear(x)`` against a dense ``nn.Linear`` holding the dequantised weights, fp32 with TF32 off, elementwise
 ``rtol = atol = 1e-5`` (test_cuda_kernel.py:47).  Construction follows run_case line by line, on the GPU
 (Quantizer.find_params -> quantize -> QuantLinear.pack -> forward); every case runs the dispatcher's choice
-(impl 0), the small-M paths (impl 1: HMMA streaming kernel, impl 4: scalar kernel) and, where the shape is TMA-compatible, both tcgen05 kernels (impl 2, 3)."""
+(impl 0), the small-M paths (impl 1: HMMA streaming kernel, impl 4: scalar kernel) and, where the shape is TMA-compatible, both wgmma kernels (impl 2, 3)."""
 import pytest
 import torch
 import torch.nn as nn

@@ -347,7 +347,7 @@ def test_kl_entropy_screen_equals_index_exact_search():
 
 
 def test_tcgen05_numeric_scheme_meets_the_reference_tolerance():
-    """CPU emulation of the arithmetic the tcgen05 GPTQ kernel performs (gptq_tc.cu header): activations scaled
+    """CPU emulation of the arithmetic the per-group wgmma GPTQ kernel performs (gptq_tc.cu header): activations scaled
     by a per-row power of two and split into fp16 hi + lo, exact int4 (minus integer zero) fp16 operands, fp32
     accumulation per 128-K group, fp32 fold `acc += scale * partial`, final `out += rowscale * acc`.  The
     scheme -- not a particular GPU -- must stay inside the reference's rtol = atol = 1e-5 (test_cuda_kernel.py:47)
