@@ -175,7 +175,10 @@ int sb200_minmax_qparams_multi(const sb200_minmax_qparams_desc* descs, int count
  * accumulated in place.  `range` = device {lo, hi}.  Bin rule = ATen's CPU histc
  * (HistogramKernel.cpp, linear interpolation): pos = (int64)(((x - lo) * bins) / (hi - lo)) in
  * fp32 with IEEE division, pos == bins folded into the last bin, x outside [lo, hi] and NaN
- * ignored. */
+ * ignored.  An empty range (lo == hi) is widened to [lo - 1, hi + 1].  ATen widens it to the
+ * data's own min and max first, so the two agree when every element of the data equals lo (for
+ * range [0, 0] and data {0, 5} ATen counts both in [0, 5], this kernel drops 5).  The KL observer's
+ * range [-absmax, absmax] is empty only when absmax == 0, i.e. for all-zero data. */
 int sb200_observe_hist(const float* x, int64_t n, const float* range, int bins, int64_t* counts,
                        void* stream);
 

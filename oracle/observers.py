@@ -109,10 +109,19 @@ def histc(x, bins, lo, hi):
     (aten/src/ATen/native/cpu/HistogramKernel.cpp, linear interpolation without local search):
         pos = int64(((x - lo) * bins) / (hi - lo))   in fp32;   pos == bins -> bins - 1
     elements outside [lo, hi] (and NaN) are dropped.  Verified against torch.histc on 6e6 random
-    and on-edge values (tests/golden/make_golden.py, tests/test_oracle_golden.py)."""
+    and on-edge values (tests/golden/make_golden.py, tests/test_oracle_golden.py).
+    An empty range (lo == hi) is widened first, as ATen's histc_select_outer_bin_edges does: to the
+    data's own min and max, and if those are equal too, to [lo - 1, hi + 1].  Like ATen, a range
+    that is not finite after this (an infinite bound, or NaN data in an empty range) raises."""
     x = np.asarray(x, dtype=F32).reshape(-1)
     lo = F32(lo)
     hi = F32(hi)
+    if lo == hi and x.size:
+        lo, hi = x.min(), x.max()
+    if lo == hi:
+        lo, hi = F32(lo - F32(1)), F32(hi + F32(1))
+    if not (np.isfinite(lo) and np.isfinite(hi)):
+        raise ValueError(f"histc: range of [{lo}, {hi}] is not finite")
     xs = x[(x >= lo) & (x <= hi)]
     with np.errstate(all="ignore"):
         pos = (((xs - lo).astype(F32) * F32(bins)).astype(F32) / F32(hi - lo)).astype(F32).astype(np.int64)

@@ -169,14 +169,19 @@ __global__ void __launch_bounds__(128) minmax_cols_kernel(const float* __restric
 // histc-compatible histogram
 // =========================================================================================
 // ATen CPU histc rule: pos = (int64)(((x - lo) * bins) / (hi - lo)) in fp32 (IEEE division),
-// pos == bins -> bins - 1, x outside [lo, hi] (or NaN) dropped.
+// pos == bins -> bins - 1, x outside [lo, hi] (or NaN) dropped.  An empty range lo == hi becomes
+// [lo - 1, hi + 1], which is what ATen does when every element equals lo (see sb200_observe_hist).
 __global__ void __launch_bounds__(kThreads) hist_kernel(const float* __restrict__ x, long long n,
                                                         const float* __restrict__ range, int bins,
                                                         unsigned long long* __restrict__ counts) {
   extern __shared__ unsigned int s_cnt[];  // bins
   for (int i = threadIdx.x; i < bins; i += blockDim.x) s_cnt[i] = 0;
   __syncthreads();
-  const float lo = __ldg(range), hi = __ldg(range + 1);
+  float lo = __ldg(range), hi = __ldg(range + 1);
+  if (lo == hi) {
+    lo = __fsub_rn(lo, 1.f);
+    hi = __fadd_rn(hi, 1.f);
+  }
   const float fb = (float)bins;
   QP dv;
   dv.set(__fsub_rn(hi, lo), 0.f);
@@ -474,7 +479,10 @@ __global__ void __launch_bounds__(kThreads) select_scan_kernel(unsigned long lon
     if (threadIdx.x == 0) {
       unsigned long long b = s_found[0];
       unsigned long long below = s_found[1];
-      if (b == 0xFFFFFFFFFFFFFFFFull) {  // rank beyond the population: clamp to the last non-empty bin
+      // Rank beyond the population: only a rank set directly (sb200_select_init / RadixSelect.set_ranks) >= the row's
+      // element count gets here; sb200_percentile_ranks clamps into range.  Bucket 0 is taken.  No key lies in it (its
+      // keys would be negative NaNs, which sel_key maps to the top), so the later passes miss too and the read-out is NaN.
+      if (b == 0xFFFFFFFFFFFFFFFFull) {
         b = 0;
         below = 0;
       }

@@ -66,6 +66,35 @@ def test_histc_matches_aten(golden):
     assert np.array_equal(h, g["histc_counts"].astype(np.int64))
 
 
+@pytest.mark.parametrize("x,lo", [
+    (np.zeros(5, np.float32), 0.0),                                 # all-zero channel: range [0, 0] -> [-1, 1]
+    (np.float32([0.0, -0.0, 0.0, -0.0]), -0.0),                     # [-0, +0] is empty too
+    (np.full(7, 0.3, np.float32), 0.3),                             # constant data: [0.3 - 1, 0.3 + 1] in fp32
+    (np.full(3, -1e-3, np.float32), 5.0),                           # constant data outside the range
+    (np.float32([1, 2, 3, 2.5, -0.5]), 5.0),                        # otherwise the data's own min and max
+    (np.float32([1e30, -2.0, 7.0, 3.25, 3.25]), 3.25),
+])
+@pytest.mark.parametrize("bins", [1, 4, 7, 2048])
+def test_histc_empty_range_matches_aten(x, lo, bins):
+    """torch.histc with min == max widens the range (ATen histc_select_outer_bin_edges); the oracle restates it."""
+    torch = pytest.importorskip("torch")
+    exp = torch.histc(torch.from_numpy(x), bins, min=lo, max=lo).numpy().astype(np.int64)
+    assert np.array_equal(oobs.histc(x, bins, lo, lo), exp)
+
+
+@pytest.mark.parametrize("x,lo,hi", [
+    (np.float32([np.nan, 1.0]), 0.0, 0.0),      # empty range widened to the data's [NaN, NaN]
+    (np.float32([np.inf, 1.0]), 0.0, 0.0),      # ... or to [1, inf]
+    (np.float32([1.0, 2.0]), 0.0, np.inf),      # an infinite bound given directly
+])
+def test_histc_nonfinite_range_raises_like_aten(x, lo, hi):
+    torch = pytest.importorskip("torch")
+    with pytest.raises(RuntimeError, match="is not finite"):
+        torch.histc(torch.from_numpy(x), 4, min=lo, max=hi)
+    with pytest.raises(ValueError, match="is not finite"):
+        oobs.histc(x, 4, lo, hi)
+
+
 def test_sparse_matches_reference(golden):
     g = golden("sparse")
     for name in g["cases"]:
