@@ -16,6 +16,8 @@
 // once, then carries (channel, position-in-row) forward with precomputed per-step increments.
 // Statistics are reduced with warp shuffles -> one shared-memory hop -> ONE atomic pair per CTA on
 // an order-preserving integer key, so the result is exact and independent of scheduling order.
+// The per-tensor QDQ entry points run chunk_kernel instead: the same per-thread work, but one CTA
+// per 16 KB chunk rather than a persistent grid (see there for why).
 #include "common.cuh"
 
 namespace sb200 {
@@ -235,7 +237,66 @@ stream_kernel(const float* __restrict__ x, const uint8_t* __restrict__ mask, flo
 }
 
 // ------------------------------------------------------------------------------------------
-// TMA variant of the per-tensor kernel.  The LDG version above is latency bound (ncu: ~all stalls
+// Per-tensor QDQ (+ MinMax) as a non-persistent launch: one CTA per contiguous chunk of kChunkVecs
+// vectors per thread (4096 floats = 16 KB on the 128-bit path), no grid-stride loop.  Every thread
+// issues all its loads of the chunk before using any of them, then computes and writes streaming
+// stores; the hardware block scheduler hands the next chunk to whichever SM frees a slot first.  The
+// persistent grid-stride split that stream_kernel uses gives every CTA the same share up front, and on
+// an H100 its CTAs finish far apart: on [256,3,224,224] the first finishes at 73 us and the last at
+// 112 us of the launch, so SMs sit idle for about a third of it.  Chunks of 8 KB lose on the 205 M
+// element sites and chunks of 32 or 64 KB on the 38 M, 205 M and 12.8 M element sites; write-back
+// stores are slower than st.global.cs, and L2 evict-first stores or a cp.async.bulk store from shared
+// memory are no faster (H100 80GB HBM3, 400 W power limit).  40 registers on the
+// 128-bit round-half-even paths: 6 CTAs = 96 KB of loads in flight per SM.  MinMax: one atomic pair
+// per CTA on the order-preserving keys, exact and independent of the order the chunks run in.
+// Nothing is carried between launches.
+constexpr int kChunkVecs = 4;
+
+template <int VEC, bool STATS, int ROUNDING>
+__global__ void __launch_bounds__(kThreads)
+chunk_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ scale,
+             const float* __restrict__ zero_point, long long n, float qmin, float qmax, int rounding,
+             uint32_t* __restrict__ mm) {
+  const long long nvec = (VEC == 4) ? (n >> 2) : n;
+  const long long v0 = (long long)blockIdx.x * (kChunkVecs * kThreads) + threadIdx.x;
+  float a[kChunkVecs][VEC];
+#pragma unroll
+  for (int u = 0; u < kChunkVecs; ++u) {
+    if (v0 + u * kThreads < nvec) load_vec<VEC>(x, v0 + u * kThreads, a[u]);
+  }
+  QP p;
+  p.qmin = qmin;
+  p.qmax = qmax;
+  p.set(__ldg(scale), __ldg(zero_point));
+  MinMaxAcc acc;
+  if (STATS) acc.init();
+#pragma unroll
+  for (int u = 0; u < kChunkVecs; ++u) {
+    if (v0 + u * kThreads < nvec) {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) {
+        if (STATS) acc.add(a[u][j]);
+        a[u][j] = qdq1<ROUNDING>(a[u][j], p, rounding);
+      }
+      store_vec<VEC>(out, v0 + u * kThreads, a[u]);
+    }
+  }
+  // Scalar tail (n % 4 elements) for the vector instantiation, in the last chunk.
+  if (VEC == 4 && blockIdx.x == gridDim.x - 1 && threadIdx.x < (n & 3)) {
+    const long long e = (nvec << 2) + threadIdx.x;
+    const float val = ld_stream1(x + e);
+    if (STATS) acc.add(val);
+    st_stream1(out + e, qdq1<ROUNDING>(val, p, rounding));
+  }
+  if (STATS) {
+    __shared__ float red[64];
+    block_reduce_minmax(acc, red);
+    if (threadIdx.x == 0) acc.publish(mm);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// TMA variant of the per-tensor kernel.  The grid-stride LDG version (stream_kernel) is latency bound (ncu: ~all stalls
 // are long_scoreboard with DRAM ~70 % busy) because the bytes in flight are capped by registers
 // (1024 threads x 4 x 16 B = 64 KB / SM).  Here the loads do not touch registers at all: one elected
 // thread keeps a ring of kTmaStages x 16 KB bulk copies (cp.async.bulk -> shared memory, completion
@@ -355,13 +416,36 @@ static int launch_stream_tma(const float* x, float* out, const float* scale, con
   return SB200_OK;
 }
 
-// Which implementation serves a per-tensor QDQ: sb200_set_variant 1 = LDG, 2 = TMA, 0 = auto.
+// Per-tensor QDQ launch: one chunk_kernel CTA per kChunkVecs x kThreads vectors.
+template <bool STATS>
+static int launch_chunks(const float* x, float* out, const float* scale, const float* zp, long long n, int qmin,
+                         int qmax, int rounding, uint32_t* mm, cudaStream_t st) {
+  const bool vec = aligned16(x) && aligned16(out) && n >= 4;
+  const long long nvec = vec ? (n >> 2) : n;
+  const long long per_cta = (long long)kChunkVecs * kThreads;
+  const long long grid = (nvec + per_cta - 1) / per_cta;
+  SB_REQUIRE(grid <= 0x7FFFFFFFLL, "per-tensor QDQ: %lld elements exceed the launch limit", n);
+#define SB_GO(VEC_, R_)                                                                                    \
+  chunk_kernel<VEC_, STATS, R_><<<(unsigned)grid, kThreads, 0, st>>>(x, out, scale, zp, n, (float)qmin, \
+                                                                     (float)qmax, rounding, mm)
+  if (vec) {
+    if (rounding == 0) SB_GO(4, 0); else SB_GO(4, -1);
+  } else {
+    if (rounding == 0) SB_GO(1, 0); else SB_GO(1, -1);
+  }
+#undef SB_GO
+  SB_LAUNCHED();
+  return SB200_OK;
+}
+
+// Which implementation serves a per-tensor QDQ: sb200_set_variant 1 = LDG chunks, 2 = TMA, 0 = auto.
 static inline bool use_tma(const float* x, const float* out, long long n) {
   if (g_variant == 1) return false;
   const bool ok = aligned16(x) && aligned16(out) && n >= 4 * kTmaTile;
   if (g_variant == 2) return ok;
-  // auto: measured on an H100 (400 W limit) the LDG register pipeline and the TMA ring take the same 115 us on the
-  // 154 MB headline tensor (0.80 of the 3.35 TB/s data-sheet bandwidth) -> the simpler LDG path unless selected.
+  // auto: the LDG chunks.  Measured on an H100 80GB HBM3 at a 400 W power limit (scripts/hbm_ceiling.py),
+  // the TMA ring is slower than them at every activation-site size of the ResNet-50 bench; on the 154 MB
+  // headline tensor [256,3,224,224] it takes 117 us against 106 us (a device-to-device copy: 104 us).
   return false;
 }
 
@@ -565,9 +649,7 @@ int sb200_qdq_pertensor_fwd(const float* x, const float* scale, const float* zer
   if (rc) return rc;
   if (use_tma(x, out, n))
     return launch_stream_tma<false>(x, out, scale, zero_point, n, qmin, qmax, rounding, nullptr, (cudaStream_t)stream);
-  return launch_stream<MODE_TENSOR, true, true, false, false>(x, nullptr, out, scale, zero_point, n, 1, 1,
-                                                              n, qmin, qmax, rounding, nullptr,
-                                                              (cudaStream_t)stream);
+  return launch_chunks<false>(x, out, scale, zero_point, n, qmin, qmax, rounding, nullptr, (cudaStream_t)stream);
 }
 
 int sb200_qdq_stats_pertensor_fwd(const float* x, const float* scale, const float* zero_point,
@@ -578,9 +660,7 @@ int sb200_qdq_stats_pertensor_fwd(const float* x, const float* scale, const floa
   SB_REQUIRE(minmax_state, "sb200_qdq_stats_pertensor_fwd: null minmax_state");
   if (use_tma(x, out, n))
     return launch_stream_tma<true>(x, out, scale, zero_point, n, qmin, qmax, rounding, minmax_state, (cudaStream_t)stream);
-  return launch_stream<MODE_TENSOR, true, true, true, false>(x, nullptr, out, scale, zero_point, n, 1, 1, n,
-                                                             qmin, qmax, rounding, minmax_state,
-                                                             (cudaStream_t)stream);
+  return launch_chunks<true>(x, out, scale, zero_point, n, qmin, qmax, rounding, minmax_state, (cudaStream_t)stream);
 }
 
 int sb200_qdq_perchannel_fwd(const float* x, const float* scale, const float* zero_point, float* out,
