@@ -406,6 +406,20 @@ int sb200_gptq4_linear_f16(const void* x_f16, const int32_t* qweight, void* out_
 int sb200_gptq_matmul(const float* x, const int32_t* qweight, float* out, const float* scales,
                       const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows,
                       int bits, int group_size, void* workspace, size_t workspace_bytes, void* stream);
+/* Input gradient of the dequant-matmul above (the backward of QuantLinear with respect to its input), any bit width:
+ *   grad_in[m, k] += sum_n grad_out[m, n] * (scales[n, k/gs] * q(k, n) - zeros[n, k/gs])
+ * grad_out: [M, N] fp32; grad_in: [M, K] fp32, accumulated in place; qweight / scales / zeros / group_size / bits: the
+ * tensors and values the forward takes, with the same argument checks (all before any CUDA call).  Results are
+ * deterministic: two identical calls are bit-identical.
+ * impl (per call): 0 = auto, 1 = SIMT kernel (any bits, any shape), 2 = wgmma kernel (bits = 4, N % 8 == 0, K % 4 == 0,
+ * 16-byte aligned grad_out; the weights are repacked along N into the workspace for the call, the scaled weights enter
+ * the MMA as two fp16 planes); forcing 2 on anything else returns SB200_E_UNSUPPORTED.  Auto takes the wgmma kernel for
+ * the shapes it supports from a measured M on (gptq.cu).
+ * workspace: sb200_gptq_dgrad_workspace_bytes(...) bytes (a pure function of its arguments). */
+size_t sb200_gptq_dgrad_workspace_bytes(int64_t m, int64_t k, int64_t n, int bits, int group_size);
+int sb200_gptq_matmul_dgrad(const float* grad_out, const int32_t* qweight, float* grad_in, const float* scales,
+                            const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int bits,
+                            int group_size, int impl, void* workspace, size_t workspace_bytes, void* stream);
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 / 3 = the two wgmma kernels, 4 = scalar kernel. */
 int sb200_gptq4_set_impl(int impl);

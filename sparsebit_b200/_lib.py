@@ -84,6 +84,8 @@ PROTOTYPES = {
     "sb200_gptq4_linear_f16_state_bytes": (c_sz, []),
     "sb200_gptq4_linear_f16_ex": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_sz, c_vp]),
     "sb200_gptq_matmul": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_sz, c_vp]),
+    "sb200_gptq_dgrad_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_int, c_int]),
+    "sb200_gptq_matmul_dgrad": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_vp, c_sz, c_vp]),
     "sb200_gptq4_set_impl": (c_int, [c_int]),
     "sb200_gptq4_set_wait_backoff": (c_int, [c_int]),
     "sb200_gptq4_set_decode": (c_int, [c_int]),

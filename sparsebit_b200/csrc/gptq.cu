@@ -31,6 +31,15 @@ void gptq4_tc_set_backoff(int ns);
 void gptq4_decode_set_mode(int mode);
 int gptq_lowbit(int bits, const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                 long long M, long long K, long long N, long long KW, int group_size, cudaStream_t st);
+size_t gptq_dgrad_simt_workspace(long long M, long long K, long long N, int group_size);
+size_t gptq_dgrad_tc_workspace(long long M, long long K, long long N, int group_size);
+bool gptq_dgrad_tc_supported(const float* grad_out, long long K, long long N, int group_size);
+int gptq_dgrad_simt(int bits, const float* go, const int32_t* qweight, float* grad_in, const float* scales, const float* zeros,
+                    long long M, long long K, long long N, long long KW, int group_size, void* workspace,
+                    size_t workspace_bytes, cudaStream_t st);
+int gptq4_dgrad_tc(const float* go, const int32_t* qweight, float* grad_in, const float* scales, const float* zeros,
+                   long long M, long long K, long long N, long long KW, int group_size, void* workspace, size_t workspace_bytes,
+                   cudaStream_t st);
 static int g_gptq_impl = 0;
 
 // fp16 <-> fp32 staging for the paths of sb200_gptq4_linear_f16 that run the fp32 kernels (small M)
@@ -237,6 +246,54 @@ int sb200_gptq_matmul(const float* x, const int32_t* qweight, float* out, const 
     group_size = (int)k;
   }
   return gptq_lowbit(bits, x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, (cudaStream_t)stream);
+}
+
+// Auto dispatch of the input gradient: the tensor-core kernel from this many rows of grad_out on (4-bit shapes it takes).
+// Measured crossover (scripts/bench_gptq_dgrad.py, H100 80GB HBM3 at a 700 W power limit, LLaMA-7B g128 shapes): at
+// M = 32 the SIMT kernel wins on 4096x4096 and 4096x11008 (84 vs 119 us, 223 vs 308 us), at M = 48 the two tie there
+// (120 vs 120 us, 317 vs 314 us), from M = 64 on the tensor-core kernel wins on every shape (11008x4096: from M = 32).
+constexpr int64_t kDgradTcMinM = 48;
+
+size_t sb200_gptq_dgrad_workspace_bytes(int64_t m, int64_t k, int64_t n, int bits, int group_size) {
+  if (m <= 0 || k <= 0 || n <= 0) return 0;
+  if (group_size <= 0) group_size = (int)k;
+  const size_t a = gptq_dgrad_simt_workspace(m, k, n, group_size);
+  const size_t b = bits == 4 ? gptq_dgrad_tc_workspace(m, k, n, group_size) : 0;
+  return a > b ? a : b;
+}
+
+int sb200_gptq_matmul_dgrad(const float* grad_out, const int32_t* qweight, float* grad_in, const float* scales,
+                            const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int bits,
+                            int group_size, int impl, void* workspace, size_t workspace_bytes, void* stream) {
+  SB_REQUIRE(bits == 2 || bits == 3 || bits == 4, "sb200_gptq_matmul_dgrad: only support 2/3/4 bit now (got %d)", bits);
+  SB_REQUIRE(grad_out && qweight && grad_in && scales && zeros, "sb200_gptq_matmul_dgrad: null pointer argument");
+  SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_gptq_matmul_dgrad: empty operand (M=%lld K=%lld N=%lld)", (long long)m,
+             (long long)k, (long long)n);
+  SB_REQUIRE(m < (1LL << 31) && k < (1LL << 31) && n < (1LL << 31), "sb200_gptq_matmul_dgrad: dimension too large");
+  const int64_t need = bits == 4 ? (k + 7) / 8 : (bits == 2 ? (k + 15) / 16 : ((k * 3 + 95) / 96) * 3);
+  SB_REQUIRE(qweight_rows >= need, "sb200_gptq_matmul_dgrad: qweight has %lld rows, %d-bit K=%lld needs %lld",
+             (long long)qweight_rows, bits, (long long)k, (long long)need);
+  SB_REQUIRE(impl >= 0 && impl <= 2, "sb200_gptq_matmul_dgrad: impl must be 0 (auto), 1 (SIMT) or 2 (tensor core) (got %d)", impl);
+  const int min_group = bits == 2 ? 64 : 128;
+  if (group_size != 0) {
+    SB_REQUIRE(group_size > 0 && group_size % min_group == 0,
+               "only group_size divisible by %d is supported in %d-bit quantization (got %d)", min_group, bits, group_size);
+  } else {
+    group_size = (int)k;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool tc_ok = bits == 4 && gptq_dgrad_tc_supported(grad_out, k, n, group_size) && workspace &&
+                     workspace_bytes >= gptq_dgrad_tc_workspace(m, k, n, group_size);
+  if (impl == 2 && !tc_ok) {
+    set_error("sb200_gptq_matmul_dgrad: tensor-core path forced but shape/workspace unsupported (bits=%d M=%lld K=%lld N=%lld gs=%d ws=%zu)",
+              bits, (long long)m, (long long)k, (long long)n, group_size, workspace_bytes);
+    return SB200_E_UNSUPPORTED;
+  }
+  if (impl == 2 || (impl == 0 && tc_ok && m >= kDgradTcMinM))
+    return gptq4_dgrad_tc(grad_out, qweight, grad_in, scales, zeros, m, k, n, qweight_rows, group_size, workspace,
+                          workspace_bytes, st);
+  return gptq_dgrad_simt(bits, grad_out, qweight, grad_in, scales, zeros, m, k, n, qweight_rows, group_size, workspace,
+                         workspace_bytes, st);
 }
 
 }  // extern "C"

@@ -17,6 +17,7 @@
 // block's words are in flight while the current one is decoded, and the per-group affine is applied once
 // per block:  sum_k (s q - z) x = s * (sum_k q x) - z * (sum_k x).
 #include "common.cuh"
+#include "gptq_unpack.cuh"
 
 namespace sb200 {
 namespace {
@@ -33,33 +34,6 @@ template <>
 struct Fmt<3> {
   static constexpr int kUnitWords = 3, kUnits = 4;  // block = 128 k, 12 words
 };
-
-// integer 0..7 -> float without I2F: OR the bits into the mantissa of 2^23 and subtract 2^23
-__device__ __forceinline__ float small_to_float(uint32_t v) { return __uint_as_float(0x4B000000u | v) - 8388608.0f; }
-
-template <int BITS>
-__device__ __forceinline__ void decode_unit(const uint32_t* w, float (&q)[32]);
-
-template <>
-__device__ __forceinline__ void decode_unit<2>(const uint32_t* w, float (&q)[32]) {
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    q[j] = small_to_float((w[0] >> (2 * j)) & 3u);
-    q[16 + j] = small_to_float((w[1] >> (2 * j)) & 3u);
-  }
-}
-
-template <>
-__device__ __forceinline__ void decode_unit<3>(const uint32_t* w, float (&q)[32]) {
-#pragma unroll
-  for (int j = 0; j < 10; ++j) {
-    q[j] = small_to_float((w[0] >> (3 * j)) & 7u);
-    q[11 + j] = small_to_float((w[1] >> (3 * j + 1)) & 7u);
-    q[22 + j] = small_to_float((w[2] >> (3 * j + 2)) & 7u);
-  }
-  q[10] = small_to_float((w[0] >> 30) | ((w[1] & 1u) << 2));
-  q[21] = small_to_float((w[1] >> 31) | ((w[2] & 3u) << 1));
-}
 
 // Dynamic shared memory: xs[MT][S * BK] activations of the CTA's K slice, then xsum[MT][S].
 template <int BITS, int MT>

@@ -81,15 +81,35 @@ def find_params_int4(weight, groupsize=-1):
     return find_params(weight, 4, groupsize)
 
 
+def _input_grad(ctx, grad):
+    """dL/dinput = grad @ dequant(qweight) through sb200_gptq_matmul_dgrad; None (and no launch) when the input does not
+    need it.  qweight / scales / zeros are frozen buffers: they never get a gradient."""
+    if not ctx.needs_input_grad[0]:
+        return None
+    from .. import ops
+
+    qweight, scales, zeros = ctx.saved_tensors
+    dev = ctx.dev
+    g = grad.to(device=dev, dtype=torch.float32).contiguous()
+    gi = torch.zeros(ctx.in_shape, dtype=torch.float32, device=dev)
+    ops.gptq_matmul_dgrad(g, qweight.to(dev), gi, scales.to(dev).contiguous(), zeros.to(dev).contiguous(), ctx.bit,
+                          0 if ctx.groupsize == -1 else int(ctx.groupsize))
+    return gi.to(device=ctx.in_device, dtype=ctx.in_dtype)
+
+
 class QuantMatmul(torch.autograd.Function):
     """Quant{2,3,4}Matmul (utils/quant.py:281-420): y = bias broadcast, then the kernel accumulates
-    x @ W^T in place."""
+    x @ W^T in place.  The backward returns the input gradient (sb200_gptq_matmul_dgrad); the weights are frozen."""
 
     @staticmethod
     def forward(ctx, input, qweight, scales, zeros, bias, groupsize=-1, bit=4):
         lead = list(input.shape[:-1])
         was_cuda = input.is_cuda
         dev = input.device if was_cuda else torch.device("cuda")
+        # references, not copies: a weight overwritten in place before backward raises autograd's version-counter error
+        ctx.save_for_backward(qweight, scales, zeros)
+        ctx.dev, ctx.in_shape, ctx.in_device, ctx.in_dtype = dev, input.shape, input.device, input.dtype
+        ctx.groupsize, ctx.bit = groupsize, bit
         x = input.to(dev).contiguous()
         # a private copy (the reference uses .repeat): expand(...).contiguous() of a [1, N] view would alias the
         # bias buffer itself and the in-place accumulation below would corrupt it
@@ -106,7 +126,7 @@ class QuantMatmul(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad):
-        return (None,) * 7
+        return (_input_grad(ctx, grad),) + (None,) * 6
 
 
 class Quant4Matmul(QuantMatmul):
@@ -116,7 +136,7 @@ class Quant4Matmul(QuantMatmul):
 
     @staticmethod
     def backward(ctx, grad):
-        return (None,) * 6
+        return (_input_grad(ctx, grad),) + (None,) * 5
 
 
 class QuantLinear(nn.Module):

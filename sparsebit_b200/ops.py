@@ -648,3 +648,33 @@ def gptq_matmul(x, qweight, out, scales, zeros, bits, group_size=0):
         check(lib.sb200_gptq_matmul(x.data_ptr(), qweight.data_ptr(), out.data_ptr(), scales.data_ptr(), zeros.data_ptr(),
                                     m, k, n, qweight.shape[0], int(bits), int(group_size), None, 0, _stream(x)))
     return out
+
+
+def gptq_matmul_dgrad(grad_out, qweight, grad_in, scales, zeros, bits, group_size=0, impl=None):
+    """In-place ``grad_in += grad_out @ dequant(qweight).T``: the input gradient of ``gptq_matmul`` for 2 / 3 / 4-bit
+    weights (sb200_gptq_matmul_dgrad).  ``grad_out`` [..., N], ``grad_in`` [..., K] fp32.  ``impl``: per-call kernel
+    selection, None / 0 = auto, 1 = SIMT, 2 = 4-bit wgmma kernel (an error on shapes it does not take).
+    Deterministic: identical calls give bit-identical results."""
+    lib = _lib.load()
+    _req(grad_out, "grad_out"), _req(grad_in, "grad_in"), _req(scales, "scales"), _req(zeros, "zeros")
+    _req(qweight, "qweight", torch.int32)
+    if qweight.dim() != 2:
+        raise SparsebitB200Error("qweight must be with dimension == 2")
+    n = qweight.shape[1]
+    if grad_out.shape[-1] != n:
+        raise SparsebitB200Error(f"grad_out has {grad_out.shape[-1]} features, qweight {n}")
+    k = grad_in.shape[-1]
+    m = grad_out.numel() // n
+    if grad_in.numel() // k != m:
+        raise SparsebitB200Error("grad_in and grad_out must have the same number of rows")
+    ws_bytes = int(lib.sb200_gptq_dgrad_workspace_bytes(m, k, n, int(bits), int(group_size)))
+    key = (grad_out.device, torch.cuda.current_stream(grad_out.device).cuda_stream, "dgrad")
+    ws = _gptq_ws.get(key)
+    if ws is None or ws.numel() < ws_bytes:
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=grad_out.device)
+        _gptq_ws[key] = ws
+    with torch.cuda.device(grad_out.device):
+        check(lib.sb200_gptq_matmul_dgrad(grad_out.data_ptr(), qweight.data_ptr(), grad_in.data_ptr(), scales.data_ptr(),
+                                          zeros.data_ptr(), m, k, n, qweight.shape[0], int(bits), int(group_size), int(impl or 0),
+                                          ws.data_ptr(), ws_bytes, _stream(grad_out)))
+    return grad_in
