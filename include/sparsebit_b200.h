@@ -420,6 +420,38 @@ size_t sb200_gptq_dgrad_workspace_bytes(int64_t m, int64_t k, int64_t n, int bit
 int sb200_gptq_matmul_dgrad(const float* grad_out, const int32_t* qweight, float* grad_in, const float* scales,
                             const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int bits,
                             int group_size, int impl, void* workspace, size_t workspace_bytes, void* stream);
+/* ---- (5) Integer-grid inference of a calibrated QLinear (int8 wgmma, sm_90a) -----------------
+ * New; the reference's QLinear (modules/linear.py) fake-quantises x and W and runs an fp32 matmul.  With
+ * v = clamp(round(x / s) + Z, qmin, qmax) - Z and Z = rint(zero_point) the fake-quant product is
+ *   y[m, n] = s_x * s_w[n] * sum_k v_x[m, k] * v_w[n, k] + bias[n]
+ * whose sum is an integer, computed exactly here on the int8 tensor cores.
+ *
+ * Stored grid.  Integer ranges are stored as s8: g - 128 for unsigned ranges (qmin >= 0, at most [0, 255]), g itself
+ * for signed ones (within [-128, 127]); the zero points on the stored grid are shifted by the same amount.  Rows are
+ * Kp = round_up(K, 16) bytes long, the padding is zero.  K < 2^17 (|sum| <= K * 2^14 fits int32), else
+ * SB200_E_UNSUPPORTED.  qmax - qmin > 255, or a range that fits neither form, is SB200_E_INVALID.
+ *
+ * sb200_int8_quantize_rows: x [rows, K] fp32 -> q [rows, Kp] s8 (16-byte aligned) holding the grid values
+ * clamp(round(x / s) + Z, qmin, qmax) on the stored grid, bit-identical to the QDQ kernels (half-to-even);
+ * row_sum[rows] int32 = sum of the stored row; nan_flag[rows] uint8 = 1 if the row holds a NaN (stored as 0).
+ * +-inf clamp to qmin / qmax.  scale / zero_point: device, 1 float each (per_row = 0) or one per row (per_row = 1).
+ *
+ * sb200_int8_linear: out[M, N] fp32 (overwritten) for x [M, K] fp32 with per-tensor device scalars x_scale /
+ * x_zero_point and the integer range [qmin_x, qmax_x]; the weights as sb200_int8_quantize_rows stored them:
+ * w_q [N, Kp] s8 (16-byte aligned), w_rowsum [N] int32, w_scale [N] fp32, w_zero [N] int32 = rint(zero_point) on the
+ * stored grid; bias [N] fp32 or NULL.  The zero points must lie in their integer ranges.  Epilogue: the zero points are
+ * removed exactly in int64, I = sum a b - Z_w sum a - Z_x sum b + K Z_x Z_w, then y = fp32(fp64(I * s_x * s_w[n])) and
+ * fp32 + bias[n]; a row of x holding a NaN gives a NaN row (a weight row holding a NaN is marked by w_scale[n] = NaN,
+ * which gives a NaN column).  Deterministic, no state between calls (graph-capturable).
+ * workspace: sb200_int8_linear_workspace_bytes(m, k) bytes (a pure function; too small -> SB200_E_WORKSPACE). */
+int sb200_int8_quantize_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax,
+                             int8_t* q, int32_t* row_sum, uint8_t* nan_flag, int64_t rows, int64_t k, void* stream);
+size_t sb200_int8_linear_workspace_bytes(int64_t m, int64_t k);
+int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_point, int qmin_x, int qmax_x,
+                      const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero,
+                      const float* bias, float* out, int64_t m, int64_t k, int64_t n, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 / 3 = the two wgmma kernels, 4 = scalar kernel. */
 int sb200_gptq4_set_impl(int impl);

@@ -86,6 +86,10 @@ PROTOTYPES = {
     "sb200_gptq_matmul": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_sz, c_vp]),
     "sb200_gptq_dgrad_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_int, c_int]),
     "sb200_gptq_matmul_dgrad": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_vp, c_sz, c_vp]),
+    "sb200_int8_quantize_rows": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
+    "sb200_int8_linear_workspace_bytes": (c_sz, [c_i64, c_i64]),
+    "sb200_int8_linear": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp,
+                                  c_sz, c_vp]),
     "sb200_gptq4_set_impl": (c_int, [c_int]),
     "sb200_gptq4_set_wait_backoff": (c_int, [c_int]),
     "sb200_gptq4_set_decode": (c_int, [c_int]),

@@ -650,6 +650,72 @@ def gptq_matmul(x, qweight, out, scales, zeros, bits, group_size=0):
     return out
 
 
+def int8_grid_offset(qmin):
+    """What the integer path subtracts from a grid value to store it as s8: 128 for unsigned ranges, else 0."""
+    return 128 if int(qmin) >= 0 else 0
+
+
+def int8_padded_k(k):
+    return (int(k) + 15) // 16 * 16
+
+
+def int8_quantize_rows(x, scale, zero_point, qmin, qmax):
+    """Integer grid of every row of ``x`` [rows, K] (sb200_int8_quantize_rows): returns ``(q, row_sum, nan)`` with
+    q int8 [rows, Kp] = clamp(round(x / s) + rint(zp), qmin, qmax) - int8_grid_offset(qmin), the padding to
+    Kp = round_up(K, 16) zero; row_sum int32 [rows]; nan bool [rows].  ``scale`` / ``zero_point``: one value for all
+    rows or one per row."""
+    lib = _lib.load()
+    _req(x, "data"), _req(scale, "scale"), _req(zero_point, "zero_point")
+    if x.dim() != 2:
+        raise SparsebitB200Error("int8_quantize_rows: data must be [rows, K]")
+    rows, k = x.shape
+    if scale.numel() != zero_point.numel() or scale.numel() not in (1, rows):
+        raise SparsebitB200Error(f"int8_quantize_rows: qparams need 1 or {rows} elements (got {scale.numel()}, {zero_point.numel()})")
+    q = torch.empty(rows, int8_padded_k(k), dtype=torch.int8, device=x.device)
+    row_sum = torch.empty(rows, dtype=torch.int32, device=x.device)
+    nan = torch.empty(rows, dtype=torch.bool, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_quantize_rows(x.data_ptr(), scale.data_ptr(), zero_point.data_ptr(), int(scale.numel() > 1),
+                                           int(qmin), int(qmax), q.data_ptr(), row_sum.data_ptr(), nan.data_ptr(), rows, k,
+                                           _stream(x)))
+    return q, row_sum, nan
+
+
+_int8_ws = {}
+
+
+def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias=None, k=None):
+    """``y = s_x s_w[n] sum_k v_x v_w + bias`` on the int8 tensor cores (sb200_int8_linear): the fake-quant linear of
+    per-tensor activations [qmin, qmax] with the weights stored by ``int8_quantize_rows`` (w_q int8 [N, Kp], w_rowsum
+    int32 [N], w_scale fp32 [N], w_zero int32 [N] = rint(zero point) - int8_grid_offset).  ``x`` [..., K] fp32; returns
+    fp32 [..., N].  ``k`` defaults to x.shape[-1]."""
+    lib = _lib.load()
+    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
+    if bias is not None:
+        _req(bias, "bias")
+    k = x.shape[-1] if k is None else int(k)
+    if x.shape[-1] != k or w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
+        raise SparsebitB200Error(f"int8_linear: x has {x.shape[-1]} features, w_q is {tuple(w_q.shape)} (need [N, {int8_padded_k(k)}])")
+    n = w_q.shape[0]
+    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"int8_linear: w_rowsum / w_scale / w_zero / bias need {n} elements")
+    m = x.numel() // k
+    out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
+    ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
+    key = (x.device, torch.cuda.current_stream(x.device).cuda_stream)
+    ws = _int8_ws.get(key)
+    if ws is None or ws.numel() < ws_bytes:
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        _int8_ws[key] = ws
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_linear(x.data_ptr(), x_scale.data_ptr(), x_zero_point.data_ptr(), int(qmin), int(qmax),
+                                    w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
+                                    bias.data_ptr() if bias is not None else None, out.data_ptr(), m, k, n, ws.data_ptr(),
+                                    ws_bytes, _stream(x)))
+    return out
+
+
 def gptq_matmul_dgrad(grad_out, qweight, grad_in, scales, zeros, bits, group_size=0, impl=None):
     """In-place ``grad_in += grad_out @ dequant(qweight).T``: the input gradient of ``gptq_matmul`` for 2 / 3 / 4-bit
     weights (sb200_gptq_matmul_dgrad).  ``grad_out`` [..., N], ``grad_in`` [..., K] fp32.  ``impl``: per-call kernel
