@@ -338,10 +338,8 @@ int sb200_gptq4_matmul(const float* x, const int32_t* qweight, float* out, const
                        int group_size, void* workspace, size_t workspace_bytes, void* stream);
 /* Per-call options instead of process-global switches.  impl: 0 = auto (M >= 32 -> 2, else 1),
  * 1 = small-M path (warp-level HMMA streaming kernel when N % 4 == 0, scalar kernel otherwise), 4 = scalar kernel,
- * 2 = wgmma with exact int4 operands and a per-128-K-group fp32 rescale of the register accumulator,
- * 3 = wgmma with the scaled weights as two fp16 planes in the register operand and whole-K accumulation, restarted
- * into a second fp32 register accumulator every chunk_k K (multiple of 64; 0 = default 512) to bound the tensor
- * core's truncating accumulation. */
+ * 2 = wgmma with exact int4 operands and a per-128-K-group fp32 rescale of the register accumulator.  Any other value
+ * (3 included) is SB200_E_INVALID.  chunk_k is reserved and must be zero, like reserved[]. */
 /* flags: SB200_GPTQ4_STATIC_WEIGHTS -- the caller guarantees that qweight / scales / zeros are constants of the model,
  * i.e. NOT written by the kernel immediately in front of this call on the stream.  The decode kernel (M <= 32) is
  * launched programmatically dependent (it may begin while its predecessor drains); with this flag it requests the
@@ -349,7 +347,7 @@ int sb200_gptq4_matmul(const float* x, const int32_t* qweight, float* out, const
 #define SB200_GPTQ4_STATIC_WEIGHTS 1
 typedef struct sb200_gptq4_options {
   int impl;
-  int chunk_k;
+  int chunk_k; /* reserved, must be zero */
   int flags;
   int reserved[5]; /* must be zero */
 } sb200_gptq4_options;
@@ -377,8 +375,8 @@ int sb200_gptq4_matmul_batch_ex(const sb200_gptq4_problem* problems, int count, 
 /* fp16 activations in, fp16 result out, WITHOUT the per-call casts of QuantLinear.forward (utils/quant.py:262-278 casts
  * x / scales / zeros / bias to fp32, materialises y = bias, and casts the result back):
  *   out_f16[m, n] = fp16( bias[n] + sum_k (scales * q - zeros) * x_f16[m, k] )          (overwrites out_f16)
- * bias may be NULL; scales / zeros are the fp32 [N, G] tables.  Prefill-sized M runs the weight-plane
- * wgmma kernel (impl 3) directly on the fp16 activations (their hi plane, no lo pass) and writes fp16 from the epilogue;
+ * bias may be NULL; scales / zeros are the fp32 [N, G] tables.  Prefill-sized M (>= 768) runs the per-group
+ * wgmma kernel (impl 2) directly on the fp16 activations (their hi plane, no lo pass) and writes fp16 from the epilogue;
  * smaller M is staged through fp32 inside the library (cast, bias, kernel, cast) -- or runs as ONE launch through
  * sb200_gptq4_linear_f16_ex below.  Same accuracy as the fp32 entry point before the final rounding to fp16.  workspace: sb200_gptq4_linear_f16_workspace_bytes(...) bytes. */
 size_t sb200_gptq4_linear_f16_workspace_bytes(int64_t m, int64_t k, int64_t n, int group_size);
@@ -453,7 +451,7 @@ int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_
                       size_t workspace_bytes, void* stream);
 
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
- * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 / 3 = the two wgmma kernels, 4 = scalar kernel. */
+ * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);
 
 /* Tuning knob of the wgmma kernels: nanoseconds their TMA producer sleeps between polls of a stage's mbarrier while it

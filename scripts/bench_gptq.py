@@ -20,7 +20,6 @@ from sparsebit_b200 import _lib, ops
 dev = torch.device("cuda:0")
 SHAPES = [("qkvo", 4096, 4096, 4), ("gate_up", 4096, 11008, 2), ("down", 11008, 4096, 1)]  # name, K, N, count per layer
 LAYERS = 32
-TS_CHUNKS = [int(c) for c in os.environ.get("SB200_TS_CHUNKS", "512").split(",")]
 # the packed weights / scales / zeros of a loaded model are constants: the decode kernel may request them while the
 # previous linear is still draining (SB200_GPTQ4_STATIC_WEIGHTS, include/sparsebit_b200.h)
 STATIC = os.environ.get("SB200_STATIC_WEIGHTS", "1") == "1"
@@ -93,12 +92,10 @@ def run(ms, with_reference=True, quiet=False):
                 # the reference's model path: fp16 activations cast to fp32 (utils/quant.py:262-277, SURVEY 8d)
                 x = x.half().float()
             y = torch.zeros(m, n, device=dev)
-            impls = [("ours_auto", 0, 0)] + ([("ours_simt", 1, 0)] if m <= 64 else []) + [("ours_wgmma_group", 2, 0)]
-            if m >= 32:  # the weight-plane kernel, accumulator restarted every chunk_k K
-                impls += [(f"ours_wgmma_ts_c{c}", 3, c) for c in TS_CHUNKS]
-            for label, impl, chunk in impls:
+            impls = [("ours_auto", 0)] + ([("ours_simt", 1)] if m <= 64 else []) + [("ours_wgmma_group", 2)]
+            for label, impl in impls:
                 try:
-                    t = timeit(lambda i: ops.gptq4_matmul(x, *ws[i % copies][:1], y, *ws[i % copies][1:], 128, impl=impl, chunk_k=chunk, static_weights=STATIC),
+                    t = timeit(lambda i: ops.gptq4_matmul(x, *ws[i % copies][:1], y, *ws[i % copies][1:], 128, impl=impl, static_weights=STATIC),
                                20 if m > 64 else 200, copies)
                 except RuntimeError as e:
                     emit({"shape": name, "M": m, "impl": label, "error": str(e)[:100]})

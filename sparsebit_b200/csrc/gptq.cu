@@ -12,15 +12,11 @@ int gptq4_simt(const float* x, const int32_t* qweight, float* out, const float* 
                long long M, long long K, long long N, long long KW, int group_size, cudaStream_t st);
 int gptq4_decode(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
                  long long K, long long N, long long KW, int group_size, int flags, cudaStream_t st);
-bool gptq4_tc_supported(const float* x, const int32_t* qweight, const float* out, long long M, long long K, long long N,
+bool gptq4_tc_supported(const void* x, const int32_t* qweight, const float* out, long long M, long long K, long long N,
                         long long KW, int group_size);
 size_t gptq4_tc_workspace(long long M, long long K, long long N, int group_size);
 int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
              long long K, long long N, long long KW, int group_size, void* workspace, size_t workspace_bytes,
-             cudaStream_t st);
-size_t gptq4_ts_workspace(long long M, long long K, long long N, int group_size);
-int gptq4_ts(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
-             long long K, long long N, long long KW, int group_size, int chunk_kb, void* workspace, size_t workspace_bytes,
              cudaStream_t st, const __half* x_h = nullptr, __half* out_h = nullptr, const float* bias = nullptr);
 size_t gptq4_decode_f16_partial_bytes(long long M, long long K, long long N);
 int gptq4_decode_f16(const __half* x_h, const int32_t* qweight, __half* out_h, const float* bias, const float* scales,
@@ -63,7 +59,7 @@ using namespace sb200;
 extern "C" {
 
 int sb200_gptq4_set_impl(int impl) {
-  SB_REQUIRE(impl >= 0 && impl <= 4, "sb200_gptq4_set_impl: impl must be 0 .. 4 (got %d)", impl);
+  SB_REQUIRE(impl >= 0 && impl <= 4 && impl != 3, "sb200_gptq4_set_impl: impl must be 0, 1, 2 or 4 (got %d)", impl);
   g_gptq_impl = impl;
   return SB200_OK;
 }
@@ -83,12 +79,11 @@ int sb200_gptq4_set_decode(int mode) {
 size_t sb200_gptq4_workspace_bytes(int64_t m, int64_t k, int64_t n, int group_size) {
   if (m <= 0 || k <= 0 || n <= 0) return 0;
   if (group_size <= 0) group_size = (int)k;
-  const size_t a = gptq4_tc_workspace(m, k, n, group_size), b = gptq4_ts_workspace(m, k, n, group_size);
-  return a > b ? a : b;
+  return gptq4_tc_workspace(m, k, n, group_size);
 }
 
 static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
-                          int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size, int impl, int chunk_k,
+                          int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size, int impl,
                           void* workspace, size_t workspace_bytes, void* stream, int flags = 0) {
   SB_REQUIRE(x && qweight && out && scales && zeros, "sb200_gptq4_matmul: null pointer argument");
   SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_gptq4_matmul: empty operand (M=%lld K=%lld N=%lld)", (long long)m,
@@ -97,8 +92,7 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
   SB_REQUIRE(qweight_rows >= (k + 7) / 8,
              "sb200_gptq4_matmul: qweight has %lld rows, need ceil(K/8) = %lld", (long long)qweight_rows,
              (long long)((k + 7) / 8));
-  SB_REQUIRE(impl >= 0 && impl <= 4, "sb200_gptq4_matmul: impl must be 0 (auto), 1 (small-M), 2 or 3 (tensor core), 4 (scalar) (got %d)", impl);
-  SB_REQUIRE(chunk_k >= 0 && chunk_k % 64 == 0, "sb200_gptq4_matmul: chunk_k must be a multiple of 64 (got %d)", chunk_k);
+  SB_REQUIRE(impl >= 0 && impl <= 4 && impl != 3, "sb200_gptq4_matmul: impl must be 0 (auto), 1 (small-M), 2 (tensor core), 4 (scalar) (got %d)", impl);
   if (group_size != 0) {
     // cuda_kernel_4bit.cu:60
     SB_REQUIRE(group_size > 0 && group_size % 128 == 0,
@@ -108,27 +102,18 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
   }
   cudaStream_t st = (cudaStream_t)stream;
   // 1 = small-M path: warp-level HMMA streaming kernel (gptq_decode.cu) when N % 4 == 0, else the scalar kernel;
-  // 4 = scalar SIMT kernel (gptq_simt.cu, any shape);  2 = wgmma, exact int4 operands + per-128-K-group fp32 rescale (gptq_tc.cu);
-  // 3 = wgmma, scaled fp16 weight planes as the register operand, whole-K accumulation (gptq_ts.cu).
+  // 4 = scalar SIMT kernel (gptq_simt.cu, any shape);  2 = wgmma, exact int4 operands + per-128-K-group fp32 rescale (gptq_tc.cu).
   int use = 1;
   if (impl != 1 && impl != 4) {
-    const bool shape_ok = gptq4_tc_supported(x, qweight, out, m, k, n, qweight_rows, group_size) && workspace;
-    const bool ok2 = shape_ok && workspace_bytes >= gptq4_tc_workspace(m, k, n, group_size);
-    const bool ok3 = shape_ok && workspace_bytes >= gptq4_ts_workspace(m, k, n, group_size);
-    if (impl == 2 || impl == 3) {
-      if (!(impl == 2 ? ok2 : ok3)) {
-        set_error("sb200_gptq4_matmul: tensor-core path forced but shape/workspace unsupported (M=%lld K=%lld N=%lld gs=%d ws=%zu)",
-                  (long long)m, (long long)k, (long long)n, group_size, workspace_bytes);
-        return SB200_E_UNSUPPORTED;
-      }
-      use = impl;
-    } else if (ok2 && m >= 32) {  // on the H100 the per-group kernel is faster than impl 3 at every M (DESIGN.md section 7)
-      use = 2;
+    const bool ok2 = gptq4_tc_supported(x, qweight, out, m, k, n, qweight_rows, group_size) && workspace &&
+                     workspace_bytes >= gptq4_tc_workspace(m, k, n, group_size);
+    if (impl == 2 && !ok2) {
+      set_error("sb200_gptq4_matmul: tensor-core path forced but shape/workspace unsupported (M=%lld K=%lld N=%lld gs=%d ws=%zu)",
+                (long long)m, (long long)k, (long long)n, group_size, workspace_bytes);
+      return SB200_E_UNSUPPORTED;
     }
+    if (ok2 && (impl == 2 || m >= 32)) use = 2;
   }
-  if (use == 3)
-    return gptq4_ts(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, chunk_k / 64, workspace,
-                    workspace_bytes, st);
   if (use == 2)
     return gptq4_tc(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, workspace, workspace_bytes, st);
   if (impl != 4 && gptq4_decode_supported(qweight, n))
@@ -139,19 +124,20 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
 int sb200_gptq4_matmul(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                        int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size, void* workspace,
                        size_t workspace_bytes, void* stream) {
-  return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, g_gptq_impl, 0, workspace,
+  return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, g_gptq_impl, workspace,
                         workspace_bytes, stream);
 }
 
 int sb200_gptq4_matmul_ex(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                           int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size,
                           const sb200_gptq4_options* options, void* workspace, size_t workspace_bytes, void* stream) {
-  const int impl = options ? options->impl : 0, chunk_k = options ? options->chunk_k : 0, flags = options ? options->flags : 0;
+  const int impl = options ? options->impl : 0, flags = options ? options->flags : 0;
   if (options) {
     SB_REQUIRE((flags & ~SB200_GPTQ4_STATIC_WEIGHTS) == 0, "sb200_gptq4_matmul_ex: unknown flags 0x%x", flags);
+    SB_REQUIRE(options->chunk_k == 0, "sb200_gptq4_matmul_ex: chunk_k is reserved and must be zero (got %d)", options->chunk_k);
     for (int i = 0; i < 5; ++i) SB_REQUIRE(options->reserved[i] == 0, "sb200_gptq4_matmul_ex: reserved option fields must be zero");
   }
-  return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, impl, chunk_k, workspace,
+  return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, impl, workspace,
                         workspace_bytes, stream, flags);
 }
 
@@ -193,10 +179,8 @@ int sb200_gptq4_linear_f16_ex(const void* x_f16, const int32_t* qweight, void* o
   cudaStream_t st = (cudaStream_t)stream;
   const __half* xh = reinterpret_cast<const __half*>(x_f16);
   __half* yh = reinterpret_cast<__half*>(out_f16);
-  const bool ts_ok = m >= 768 && (k % 8 == 0) && (n % 4 == 0) && aligned16(x_f16) && aligned16(qweight) &&
-                     gptq4_ts_workspace(m, k, n, group_size) > 0;
-  if (ts_ok)  // fp16 in, fp16 out, no fp32 round trip of x or y
-    return gptq4_ts(nullptr, qweight, nullptr, scales, zeros, m, k, n, qweight_rows, group_size, 0, workspace, workspace_bytes, st, xh, yh, bias);
+  if (m >= 768 && gptq4_tc_supported(x_f16, qweight, nullptr, m, k, n, qweight_rows, group_size))  // fp16 in, fp16 out, no fp32 round trip of x or y
+    return gptq4_tc(nullptr, qweight, nullptr, scales, zeros, m, k, n, qweight_rows, group_size, workspace, workspace_bytes, st, xh, yh, bias);
   if (state && m <= kF16SingleLaunchMaxM && gptq4_decode_supported(qweight, n) && n <= (int64_t)(kF16StateBytes / sizeof(int)) * 128) {
     // decode-sized M with a caller-provided (zero-initialised, self-resetting) arrival-counter state: ONE launch -- fp16
     // activations are read by the kernel's staging, the last K-slice CTA of every feature block writes bias + sum as fp16
@@ -215,7 +199,7 @@ int sb200_gptq4_linear_f16_ex(const void* x_f16, const int32_t* qweight, void* o
   bias_rows_kernel<<<ew_grid(m * n), 256, 0, st>>>(bias, y32, m, n);
   SB_LAUNCHED();
   // the kernel immediately in front is bias_rows_kernel (writes y32 only): the weight tables cannot be its output
-  const int rc = gptq4_dispatch(x32, qweight, y32, scales, zeros, m, k, n, qweight_rows, group_size_arg, 0, 0, rest, rest_bytes, stream,
+  const int rc = gptq4_dispatch(x32, qweight, y32, scales, zeros, m, k, n, qweight_rows, group_size_arg, 0, rest, rest_bytes, stream,
                                 SB200_GPTQ4_STATIC_WEIGHTS);
   if (rc) return rc;
   f32_to_f16_kernel<<<ew_grid(m * n), 256, 0, st>>>(y32, yh, m * n);

@@ -24,7 +24,8 @@
 //     [2^14, 2^15).  An element w of the group keeps its 22 bits while |w| >= 2^-17 max_group |w|; below that its w_lo
 //     is an fp16 subnormal and its absolute error stays under 2^-40 max_group |w|;
 //   * three m64n128k16 passes per 16 n (w_hi g_hi, w_lo g_hi, w_hi g_lo -- the last only when some g_lo != 0), into a
-//     register accumulator restarted every 512 n and added into a second one with round-to-nearest (gptq_ts.cu);
+//     register accumulator restarted every 512 n and added into a second one with round-to-nearest: the tensor core
+//     truncates instead of rounding to nearest when it accumulates, so one chain over all of N could lose ~1e-5;
 //   * epilogue grad_in[m, k] = fmaf(2^e[m], 2^-c[g] * acc, grad_in[m, k]).
 // Limits: N % 8 == 0 (16-byte rows of g' and the 8-wide permutation), K % 4 == 0 (16-byte rows of qT), grad_out 16-byte
 // aligned, group_size a multiple of 128 or one group.  Everything else runs the SIMT kernel.

@@ -19,6 +19,9 @@
 // acc += scale * partial (- zero * xsum) in fp32 registers -- the per-group rescale costs one FMA per accumulator,
 // since the accumulator never leaves the registers.
 // A prologue kernel splits x into (hi, lo), computes the per-(row, 128-K) sums and the row scales.
+//
+// fp16 activations (sb200_gptq4_linear_f16): the activations are the hi plane as they are, the lo pass never runs, and
+// the epilogue writes out_h = fp16(bias + x @ W) instead of accumulating into the fp32 `out`.
 #include "tc_common.cuh"
 
 namespace sb200 {
@@ -90,6 +93,33 @@ __global__ void __launch_bounds__(256) gptq_split_kernel(const float* __restrict
   if (__any_sync(0xffffffffu, any_lo) && lane == 0) atomicOr(need_lo, 1);
 }
 
+// fp16 activations: the hi plane IS the input (no row scaling needed: |x| <= 65504 and |q - zero| <= 1039 keep every
+// product inside fp32), copied with every 8 K permuted to (0, 4, 1, 5, 2, 6, 3, 7) to match the nibble pairs one LOP3
+// extracts; xsum[m, g] = sum over the 128-K block (only read when some zero point has a fractional part).
+__global__ void __launch_bounds__(256) gptq_permute_f16_kernel(const __half* __restrict__ x, __half* __restrict__ a_hi,
+                                                               float* __restrict__ xsum, float* __restrict__ rowscale, int K,
+                                                               int G) {
+  const int m = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const __half* xr = x + (size_t)m * K;
+  if (tid == 0) rowscale[m] = 1.f;
+  const int nchunk = K >> 3;
+  for (int c0 = 0; c0 < nchunk; c0 += 256) {
+    const int c = c0 + tid;
+    float s = 0.f;
+    if (c < nchunk) {
+      const uint4 raw = *reinterpret_cast<const uint4*>(xr + c * 8);
+      const __half* h = reinterpret_cast<const __half*>(&raw);
+      const __half p[8] = {h[0], h[4], h[1], h[5], h[2], h[6], h[3], h[7]};
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += __half2float(h[j]);
+      *reinterpret_cast<uint4*>(a_hi + (size_t)m * K + c * 8) = *reinterpret_cast<const uint4*>(p);
+    }
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((lane & 15) == 0 && (c >> 4) < G) xsum[(size_t)m * G + (c >> 4)] = s;
+  }
+}
+
 // ---------------------------------------------------------------------------------- zero-point probe
 // GPTQ checkpoints store zeros = zero * scale with an INTEGER zero (utils/quant.py:188, find_params
 // :83-89).  When that holds for every (n, g), (q - zero) is an exact fp16 integer that can go into the
@@ -108,12 +138,15 @@ __global__ void gptq_zero_probe_kernel(const float* __restrict__ scales, const f
 }
 
 // ---------------------------------------------------------------------------------- main kernel
+// F16_OUT: out_h[m, n] = fp16(bias[n] + rowscale[m] * acc), overwritten and never read, bias may be NULL; otherwise
+// out[m, n] += rowscale[m] * acc (the reference's accumulate-in-place contract) and out_h / bias are unused.
+template <bool F16_OUT>
 __global__ void __launch_bounds__(kWgThreads, 1)
 gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                 const __grid_constant__ CUtensorMap map_q, float* __restrict__ out, const float* __restrict__ scales,
                 const float* __restrict__ zeros, const float* __restrict__ xsum, const float* __restrict__ rowscale,
                 const __half* __restrict__ zint, const int* __restrict__ int_zero_flag, int M, int K, int N, int Gq,
-                int G128, int group_size, int backoff_ns) {
+                int G128, int group_size, int backoff_ns, __half* __restrict__ out_h, const float* __restrict__ bias) {
   extern __shared__ unsigned char smem_raw[];
   // stage buffers first (1024-byte aligned for SWIZZLE_128B), bookkeeping after them
   unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -206,14 +239,25 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
       }
     }
   }
-  // out[m, n] += rowscale[m] * acc   (out is pre-initialised with the bias by the caller)
+  if constexpr (F16_OUT) {
+    const float bna = (bias && live_a) ? __ldg(bias + na) : 0.f;
+    const float bnb = (bias && live_b) ? __ldg(bias + nb) : 0.f;
 #pragma unroll
-  for (int j = 0; j < 64; ++j) {
-    const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
-    const int n = (j & 2) ? nb : na;
-    if (m < M && n < N) {
-      float* o = out + (size_t)m * N + n;
-      *o = fmaf(__ldg(rowscale + m), acc[j], *o);
+    for (int j = 0; j < 64; ++j) {
+      const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
+      const int n = (j & 2) ? nb : na;
+      if (m < M && n < N) out_h[(size_t)m * N + n] = __float2half_rn(fmaf(__ldg(rowscale + m), acc[j], (j & 2) ? bnb : bna));
+    }
+  } else {
+    // out[m, n] += rowscale[m] * acc   (out is pre-initialised with the bias by the caller)
+#pragma unroll
+    for (int j = 0; j < 64; ++j) {
+      const int m = m0 + 8 * (j >> 2) + 2 * q + (j & 1);
+      const int n = (j & 2) ? nb : na;
+      if (m < M && n < N) {
+        float* o = out + (size_t)m * N + n;
+        *o = fmaf(__ldg(rowscale + m), acc[j], *o);
+      }
     }
   }
 }
@@ -246,7 +290,7 @@ static int g_tc_backoff_ns = 0;
 void gptq4_tc_set_backoff(int ns) { g_tc_backoff_ns = ns; }
 int gptq4_tc_backoff() { return g_tc_backoff_ns; }
 
-bool gptq4_tc_supported(const float* x, const int32_t* qweight, const float* out, long long M, long long K, long long N,
+bool gptq4_tc_supported(const void* x, const int32_t* qweight, const float* out, long long M, long long K, long long N,
                         long long KW, int group_size) {
   (void)out;
   (void)KW;
@@ -263,9 +307,10 @@ size_t gptq4_tc_workspace(long long M, long long K, long long N, int group_size)
   return tc_layout(M, K, N, (K + group_size - 1) / group_size).total + 1024;
 }
 
+// x_h != nullptr: fp16 activations in, fp16 `out_h = bias + x @ W` out (sb200_gptq4_linear_f16); else the fp32 contract.
 int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
              long long K, long long N, long long KW, int group_size, void* workspace, size_t workspace_bytes,
-             cudaStream_t st) {
+             cudaStream_t st, const __half* x_h, __half* out_h, const float* bias) {
   const int Gq = (int)((K + group_size - 1) / group_size);
   const TcWorkspace w = tc_layout(M, K, N, Gq);
   unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
@@ -285,7 +330,10 @@ int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* sc
   SB_CUDA(cudaMemsetAsync(flag + 1, 0, sizeof(int), st));     // [1] need_lo: set by the split kernel
   gptq_zero_probe_kernel<<<(unsigned)(((long long)N * Gq + 255) / 256), 256, 0, st>>>(scales, zeros, (long long)N * Gq, zint, flag);
   SB_LAUNCHED();
-  gptq_split_kernel<<<(unsigned)M, 256, 0, st>>>(x, a_hi, a_lo, xsum, rowscale, flag + 1, (int)K, G128);
+  if (x_h)  // need_lo stays 0: the lo plane is never loaded
+    gptq_permute_f16_kernel<<<(unsigned)M, 256, 0, st>>>(x_h, a_hi, xsum, rowscale, (int)K, G128);
+  else
+    gptq_split_kernel<<<(unsigned)M, 256, 0, st>>>(x, a_hi, a_lo, xsum, rowscale, flag + 1, (int)K, G128);
   SB_LAUNCHED();
 
   CUtensorMap map_hi, map_lo, map_q;
@@ -294,13 +342,13 @@ int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* sc
     return SB200_E_CUDA;
   }
   const size_t smem = (size_t)kTcStages * kWgStageBytes + sizeof(TcSmem) + 1024;
-  static std::atomic<int> attr_done[64];
-  SB_CUDA(ensure_dyn_smem(gptq4_tc_kernel, (int)smem, attr_done));
+  auto* const kernel = x_h ? gptq4_tc_kernel<true> : gptq4_tc_kernel<false>;
+  static std::atomic<int> attr_done[2][64];
+  SB_CUDA(ensure_dyn_smem(kernel, (int)smem, attr_done[x_h ? 1 : 0]));
   // one CTA per tile, token tile fastest: CTAs running side by side share the packed weight tile through L2
   const long long tiles = ((M + kWgTok - 1) / kWgTok) * ((N + kWgFeat - 1) / kWgFeat);
-  gptq4_tc_kernel<<<(unsigned)tiles, kWgThreads, smem, st>>>(map_hi, map_lo, map_q, out, scales, zeros, xsum, rowscale,
-                                                            zint, flag, (int)M, (int)K, (int)N, Gq, G128, group_size,
-                                                            g_tc_backoff_ns);
+  kernel<<<(unsigned)tiles, kWgThreads, smem, st>>>(map_hi, map_lo, map_q, out, scales, zeros, xsum, rowscale, zint, flag,
+                                                   (int)M, (int)K, (int)N, Gq, G128, group_size, g_tc_backoff_ns, out_h, bias);
   SB_LAUNCHED();
   return SB200_OK;
 }

@@ -1,7 +1,8 @@
-// tc_common.cuh -- pieces shared by the wgmma GPTQ kernels (gptq_tc.cu, gptq_ts.cu): mbarrier / TMA / wgmma PTX
-// wrappers, setmaxnreg, the in-register int4 -> fp16 fragment unpack, the TMA producer role, cuTensorMapEncodeTiled.
+// tc_common.cuh -- pieces shared by the wgmma kernels (gptq_tc.cu, gptq_dgrad.cu, int8_linear.cu): mbarrier / TMA /
+// wgmma PTX wrappers, setmaxnreg, the in-register int4 -> fp16 fragment unpack, the TMA producer role,
+// cuTensorMapEncodeTiled.
 //
-// Both kernels compute the transposed product D[n, m] = sum_k W[n, k] * x'[m, k] with one warpgroup-wide
+// The GPTQ kernels compute the transposed product D[n, m] = sum_k W[n, k] * x'[m, k] with one warpgroup-wide
 // wgmma.m64n128k16 per 16 K: the weights are the A operand, unpacked by every consumer thread straight into its own
 // register fragment (no shared-memory round trip for the fp16 weights), the activations x' (fp16 planes, every 8 K
 // permuted as 0,4,1,5,2,6,3,7) are the B operand, TMA-loaded as 128-token x 64-K SWIZZLE_128B tiles.

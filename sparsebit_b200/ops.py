@@ -524,7 +524,8 @@ GPTQ4_STATIC_WEIGHTS = 1  # include/sparsebit_b200.h SB200_GPTQ4_STATIC_WEIGHTS
 
 def gptq4_matmul(x, qweight, out, scales, zeros, group_size=0, impl=None, chunk_k=0, static_weights=False):
     """In-place ``out += x @ dequant(qweight)`` (vecquant4matmul contract, cuda_kernel.cpp:10-23).
-    ``impl`` / ``chunk_k``: per-call kernel selection (sb200_gptq4_matmul_ex); None = the library default.
+    ``impl``: per-call kernel selection (sb200_gptq4_matmul_ex); None = the library default.
+    ``chunk_k``: the reserved ``sb200_gptq4_options.chunk_k``; only 0 is valid, anything else raises.
     ``static_weights``: qweight / scales / zeros are constants of the model (not written by the kernel just in front on
     the stream), so the decode kernel may fetch them while its predecessor is still draining."""
     lib = _lib.load()

@@ -33,6 +33,7 @@ def test_version_and_variant_validation():
     assert lib.sb200_set_variant(7) != 0
     assert b"variant" in lib.sb200_last_error()
     assert lib.sb200_gptq4_set_impl(5) != 0
+    assert lib.sb200_gptq4_set_impl(3) != 0 and b"impl" in lib.sb200_last_error()
     assert lib.sb200_gptq4_set_impl(0) == 0
 
 
@@ -53,6 +54,11 @@ def test_argument_errors_surface_as_runtime_error():
     assert st == -1 and b"divisible by 128" in lib.sb200_last_error()
     st = lib.sb200_gptq4_matmul(p, p, p, p, p, 1, 256, 8, 3, 128, None, 0, None)  # too few packed rows
     assert st == -1
+    # per-call options: impl is 0, 1, 2 or 4, chunk_k is reserved (sb200_gptq4_options = 8 ints)
+    for impl, chunk_k, what in ((3, 0, b"impl"), (0, 512, b"chunk_k"), (2, 64, b"chunk_k")):
+        opts = (ctypes.c_int * 8)(impl, chunk_k)
+        st = lib.sb200_gptq4_matmul_ex(p, p, p, p, p, 1, 256, 8, 32, 128, opts, p, 1 << 20, None)
+        assert st == -1 and what in lib.sb200_last_error()
     assert lib.sb200_observe_hist(p, 8, p, 0, p, None) == -1
     assert lib.sb200_select_hist(p, 1, 8, 3, p, p, 0, 0, None) == -1
 

@@ -67,11 +67,12 @@ def test_vs_fp64_oracle(bshape, k, n, gs, impl):
 
 
 # per-group wgmma path forced (sb200_gptq4_set_impl(2)): ragged M / N tiles, odd number of 64-K stages,
-# group sizes 128 / 256 / 384, a single row, outlier activations (per-row power-of-two scaling).
+# group sizes 128 / 256 / 384 and one group, a single row, several 128-token tiles with ragged last tiles,
+# outlier activations (per-row power-of-two scaling).
 TC_CASES = [
     ((1,), 128, 128, 128), ((128,), 256, 128, 128), ((130,), 512, 264, 128), ((29,), 8192, 1024, 128),
     ((4,), 6144, 768, 384), ((300,), 1024, 512, 256), ((2, 130), 512, 260, 128), ((257,), 192 * 2, 132, 128),
-    ((256,), 4096, 4096, 128), ((64,), 11008, 512, 128),
+    ((256,), 4096, 4096, 128), ((64,), 11008, 512, 128), ((513,), 384, 392, -1), ((700,), 2048, 136, 128),
 ]
 
 
@@ -103,11 +104,11 @@ def test_tcgen05_path_vs_fp64_oracle(bshape, k, n, gs):
             np.testing.assert_array_less(np.abs(yf[r] - ef[r]), 1e-5 + 1e-5 * mag)
 
 
-def _run_impl(x, qw, bias, scales, zeros, gs, impl, chunk_k=0):
+def _run_impl(x, qw, bias, scales, zeros, gs, impl):
     from sparsebit_b200 import ops
 
     y = t(np.broadcast_to(bias, x.shape[:-1] + (qw.shape[1],)).copy())
-    ops.gptq4_matmul(t(x), t(qw), y, t(scales), t(zeros), 0 if gs == -1 else gs, impl=impl, chunk_k=chunk_k)
+    ops.gptq4_matmul(t(x), t(qw), y, t(scales), t(zeros), 0 if gs == -1 else gs, impl=impl)
     return y.cpu().numpy()
 
 
@@ -152,66 +153,6 @@ def test_decode_hmma_path_vs_fp64_oracle(m, k, n, gs, fp16_acts, mode, decode_mo
         np.testing.assert_array_less(np.abs(y[0] - exp[0]), 1e-5 + 1e-5 * max(1.0, np.abs(exp[0]).max()))
 
 
-# weight-plane wgmma kernel (impl 3, gptq_ts.cu): ragged token / feature tiles, odd numbers of 64-K stages,
-# several chunks, group sizes 128 / 256 / 384, a single row, several 128-token tiles and ragged last tiles
-TS_CASES = [
-    ((1,), 128, 128, 128), ((128,), 256, 128, 128), ((130,), 512, 264, 128), ((29,), 8192, 1024, 128),
-    ((4,), 6144, 768, 384), ((300,), 1024, 512, 256), ((2, 130), 512, 260, 128), ((257,), 192 * 2, 132, 128),
-    ((256,), 4096, 4096, 128), ((64,), 11008, 512, 128), ((513,), 384, 392, -1), ((700,), 2048, 136, 128),
-]
-
-
-@pytest.mark.parametrize("bshape,k,n,gs", TS_CASES)
-def test_tcgen05_ts_path_vs_fp64_oracle(bshape, k, n, gs):
-    rng = np.random.default_rng(11 * k + n + len(bshape))
-    x, qw, bias, scales, zeros = _make_case(rng, bshape, k, n, gs)
-    y = _run_impl(x, qw, bias, scales, zeros, gs, impl=3)
-    exp = ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, x.shape[:-1] + (n,)), scales, zeros, 0 if gs == -1 else gs)
-    np.testing.assert_allclose(y, exp, **TOL)  # the reference's elementwise form (test_cuda_kernel.py:47)
-
-
-def test_tcgen05_ts_outlier_rows_and_fp16_exact_activations():
-    rng = np.random.default_rng(3)
-    m, k, n = 300, 1024, 520
-    x, qw, bias, scales, zeros = _make_case(rng, (m,), k, n, 128)
-    x[0, :5] = [3e4, -7e4, 1e-6, 0.0, 123.0]  # fp16-overflowing magnitudes: per-row power-of-two scaling
-    x[2] *= 1e-4
-    y = _run_impl(x, qw, bias, scales, zeros, 128, impl=3)
-    exp = ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, (m, n)), scales, zeros, 128)
-    plain = [r for r in range(m) if r != 0]
-    np.testing.assert_allclose(y[plain], exp[plain], **TOL)
-    np.testing.assert_array_less(np.abs(y[0] - exp[0]), 1e-5 + 1e-5 * np.abs(exp[0]).max())
-    # fp16 activations cast to fp32 (the model path): the x_lo pass is skipped, rows are bit-identical to the
-    # three-pass result on the same data
-    xh = x.astype(np.float16).astype(np.float32)
-    xh[0, :2] = 1.0
-    y1 = _run_impl(xh, qw, bias, scales, zeros, 128, impl=3)
-    x2 = xh.copy()
-    x2[0, 0] += 1e-5
-    y2 = _run_impl(x2, qw, bias, scales, zeros, 128, impl=3)
-    np.testing.assert_allclose(y1, ogptq.dequant_matmul(xh, qw, np.broadcast_to(bias, (m, n)), scales, zeros, 128), **TOL)
-    np.testing.assert_allclose(y2[1:], y1[1:], rtol=0, atol=0)
-
-
-def test_tcgen05_ts_general_zero_points_and_chunking():
-    rng = np.random.default_rng(5)
-    x, qw, bias, scales, zeros = _make_case(rng, (200,), 1024, 384, 128)
-    exp_int = ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, (200, 384)), scales, zeros, 128)
-    for chunk in (64, 256, 512, 4096):  # accumulator drained every 1 / 4 / 8 stages, or once
-        np.testing.assert_allclose(_run_impl(x, qw, bias, scales, zeros, 128, impl=3, chunk_k=chunk), exp_int, **TOL)
-    # zeros that are NOT an integer multiple of scales: the prepare kernel clears the flag, the epilogue subtracts
-    # zeros * (row sums of x)
-    zeros2 = (zeros + 0.37 * scales * rng.uniform(0.5, 1.5, zeros.shape)).astype(np.float32)
-    zeros2[3, 2] = 0.0
-    y = _run_impl(x, qw, bias, scales, zeros2, 128, impl=3)
-    np.testing.assert_allclose(y, ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, (200, 384)), scales, zeros2, 128), **TOL)
-    # integer zero points far outside [0, 15] (the contract allows any fp32 zeros)
-    zeros3 = (scales * np.rint(rng.uniform(-900, 900, zeros.shape))).astype(np.float32)
-    y = _run_impl(x, qw, bias, scales, zeros3, 128, impl=3)
-    exp3 = ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, (200, 384)), scales, zeros3, 128)
-    np.testing.assert_allclose(y, exp3, rtol=1e-5, atol=1e-5 * max(1.0, np.abs(exp3).max()))
-
-
 @pytest.mark.parametrize("m,k,n", [(256, 1024, 512), (77, 512, 132)])
 def test_tcgen05_fp16_representable_activations_single_pass(m, k, n):
     """fp16 activations cast to fp32 (the reference's model path): lo == 0 everywhere, the kernel skips the
@@ -235,38 +176,52 @@ def test_tcgen05_fp16_representable_activations_single_pass(m, k, n):
 
 def test_tcgen05_general_zero_points_fall_back_to_affine_epilogue():
     """zeros that are NOT an integer multiple of scales (the contract allows any fp32 value): the
-    device-side probe must clear the integer-zero flag and the (scale, zeros) epilogue must be used."""
+    device-side probe must clear the integer-zero flag and the (scale, zeros) epilogue must be used.
+    Integer zero points far outside [0, 15] stay on the integer-zero path with |q - zero| up to ~900."""
     rng = np.random.default_rng(5)
-    x, qw, bias, scales, zeros = _make_case(rng, (200,), 1024, 384, 128)
-    zeros = (zeros + 0.37 * scales * rng.uniform(0.5, 1.5, zeros.shape)).astype(np.float32)
+    x, qw, bias, scales, zeros_int = _make_case(rng, (200,), 1024, 384, 128)
+    zeros = (zeros_int + 0.37 * scales * rng.uniform(0.5, 1.5, zeros_int.shape)).astype(np.float32)
     zeros[3, 2] = 0.0
+    zeros3 = (scales * np.rint(rng.uniform(-900, 900, zeros_int.shape))).astype(np.float32)
     lib = _lib.load()
     lib.sb200_gptq4_set_impl(2)
     try:
         y = _run(x, qw, bias, scales, zeros, 128)
+        y3 = _run(x, qw, bias, scales, zeros3, 128)
     finally:
         lib.sb200_gptq4_set_impl(0)
     exp = ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, (200, 384)), scales, zeros, 128)
     np.testing.assert_allclose(y, exp, **TOL)
+    exp3 = ogptq.dequant_matmul(x, qw, np.broadcast_to(bias, (200, 384)), scales, zeros3, 128)
+    np.testing.assert_allclose(y3, exp3, rtol=1e-5, atol=1e-5 * max(1.0, np.abs(exp3).max()))
 
 
 @pytest.mark.parametrize("m,k,n,gs", [(5, 1024, 512, 128), (300, 1024, 520, 128), (1024, 2048, 1028, 256), (777, 512, 260, -1)])
 def test_linear_f16_entry_point(m, k, n, gs):
     """sb200_gptq4_linear_f16: fp16 activations in, fp16 ``bias + x @ W`` out without eager casts -- equals the fp32
-    entry point's result rounded to fp16 (up to one fp16 ulp where the fp32 results differ in the last bits)."""
+    entry point's result rounded to fp16 (up to one fp16 ulp where the fp32 results differ in the last bits).  From
+    M = 768 the per-group wgmma kernel reads the fp16 activations directly; there it also takes fractional zero points
+    (the (scale, zeros) epilogue on the fp16 row sums) and integer zero points far outside [0, 15]."""
     from sparsebit_b200 import ops
 
     rng = np.random.default_rng(m + k)
     x, qw, bias, scales, zeros = _make_case(rng, (m,), k, n, gs)
     xh = x.astype(np.float16)
     g = 0 if gs == -1 else gs
-    y16 = ops.gptq4_linear_f16(t(xh), t(qw), t(scales), t(zeros), t(bias), g).cpu().numpy()
-    assert y16.dtype == np.float16 and y16.shape == (m, n)
-    exp = ogptq.dequant_matmul(xh.astype(np.float32), qw, np.broadcast_to(bias, (m, n)), scales, zeros, g)
-    ulp = np.abs(exp).astype(np.float16).astype(np.float32) * 2.0**-10 + 2.0**-24
-    assert np.all(np.abs(y16.astype(np.float64) - exp) <= 0.51 * ulp + 1e-5 * (1 + np.abs(exp)))
-    y_nobias = ops.gptq4_linear_f16(t(xh), t(qw), t(scales), t(zeros), None, g).cpu().numpy().astype(np.float32)
-    np.testing.assert_allclose(y_nobias, exp - bias, rtol=2e-3, atol=2e-3)
+    zero_tables = [(zeros, False)]
+    if m >= 768:
+        zero_tables += [((zeros + 0.37 * scales).astype(np.float32), False),
+                        # the fp32 sums carry zero * sum(x): their error scales with the largest output (as in the fp32 test)
+                        ((scales * np.rint(rng.uniform(-900, 900, zeros.shape))).astype(np.float32), True)]
+    for zr, by_max in zero_tables:
+        y16 = ops.gptq4_linear_f16(t(xh), t(qw), t(scales), t(zr), t(bias), g).cpu().numpy()
+        assert y16.dtype == np.float16 and y16.shape == (m, n)
+        exp = ogptq.dequant_matmul(xh.astype(np.float32), qw, np.broadcast_to(bias, (m, n)), scales, zr, g)
+        ulp = np.abs(exp).astype(np.float16).astype(np.float32) * 2.0**-10 + 2.0**-24
+        mag = np.abs(exp).max() if by_max else np.abs(exp)
+        assert np.all(np.abs(y16.astype(np.float64) - exp) <= 0.51 * ulp + 1e-5 * (1 + mag))
+        y_nobias = ops.gptq4_linear_f16(t(xh), t(qw), t(scales), t(zr), None, g).cpu().numpy().astype(np.float32)
+        np.testing.assert_allclose(y_nobias, exp - bias, rtol=2e-3, atol=2e-3)
 
 
 @pytest.mark.parametrize("m,k,n,gs", [(1, 4096, 4096, 128), (1, 1000, 132, -1), (9, 1024, 520, 128), (17, 2048, 1028, 256), (32, 1536, 384, 384)])
@@ -383,8 +338,7 @@ def test_linearity_and_accumulate_contract_at_llama_shape():
     rows = [0, 255, 256, 777, 2047]
     exp = ogptq.dequant_matmul(x[rows], qw, np.broadcast_to(bias, (len(rows), n)), scales, zeros, 128)
     np.testing.assert_allclose(y1[rows], exp, **TOL)
-    for impl in (2, 3):  # both wgmma kernels at the full shape
-        np.testing.assert_allclose(_run_impl(x, qw, bias, scales, zeros, 128, impl=impl)[rows], exp, **TOL)
+    np.testing.assert_allclose(_run_impl(x, qw, bias, scales, zeros, 128, impl=2)[rows], exp, **TOL)  # wgmma forced
 
 
 def test_argument_checks():
@@ -398,6 +352,10 @@ def test_argument_checks():
         cuda_kernel.vecquant4matmul(x[0, :], qw, y[0], s, s)
     with pytest.raises(RuntimeError, match="out_channel"):
         cuda_kernel.vecquant4matmul(x, qw, torch.zeros(4, 9, device=dev()), s, s)
+    from sparsebit_b200 import ops
+
+    with pytest.raises(RuntimeError, match="chunk_k"):  # reserved option field
+        ops.gptq4_matmul(x, qw, y, s, s, 128, chunk_k=512)
 
 
 def test_layer_streaming_equals_resident_execution():
