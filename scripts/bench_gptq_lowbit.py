@@ -1,6 +1,7 @@
-"""GPTQ 3-bit / 2-bit g128 decode (M = 1, 16) on the LLaMA-7B linear shapes: this repo's SIMT kernels vs the
-reference's own CUDA kernels (oracle/_ref/gptq_ref.so).  One JSON line per (bits, shape, M, impl) and a
-per-token summary.  Same timing method as bench_gptq.py (CUDA graphs over rotating weight copies > L2)."""
+"""GPTQ 4 / 3 / 2-bit g128 decode (M = 1, 16) on the LLaMA-7B linear shapes: this repo's SIMT kernel (gptq_simt.cu;
+4-bit forced through impl 4) vs the reference's own CUDA kernels (oracle/_ref/gptq_ref.so).  One JSON line per
+(bits, shape, M, impl) and a per-token summary.  Same timing method as bench_gptq.py (CUDA graphs over rotating weight
+copies > L2)."""
 import json
 import os
 import sys
@@ -19,7 +20,7 @@ def main():
     ref = load_ref()
     ms = [int(a) for a in sys.argv[1:]] or [1, 16]
     totals = {}
-    for bits in (3, 2):
+    for bits in (4, 3, 2):
         for m in ms:
             for name, k, n, cnt in SHAPES:
                 rows = pack_rows(k, bits)
@@ -34,9 +35,12 @@ def main():
                     ws.append((qw, sc.contiguous(), zr.contiguous()))
                 x = torch.randn(m, k, device=dev).half().float()
                 y = torch.zeros(m, n, device=dev)
-                impls = [("ours", lambda i: ops.gptq_matmul(x, ws[i % copies][0], y, ws[i % copies][1], ws[i % copies][2], bits, 128))]
+                if bits == 4:
+                    impls = [("ours", lambda i: ops.gptq4_matmul(x, ws[i % copies][0], y, ws[i % copies][1], ws[i % copies][2], 128, impl=4))]
+                else:
+                    impls = [("ours", lambda i: ops.gptq_matmul(x, ws[i % copies][0], y, ws[i % copies][1], ws[i % copies][2], bits, 128))]
                 if ref is not None:
-                    fn = ref.vecgroupquant3matmul if bits == 3 else ref.vecgroupquant2matmul
+                    fn = {4: ref.vecgroupquant4matmul, 3: ref.vecgroupquant3matmul, 2: ref.vecgroupquant2matmul}[bits]
                     impls.append(("reference_cuda", lambda i, fn=fn: fn(x, ws[i % copies][0], y, ws[i % copies][1], ws[i % copies][2], 128)))
                 for label, call in impls:
                     t = timeit(call, 200, copies)

@@ -1,41 +1,15 @@
-// gptq.cu -- C-ABI entry points of the GPTQ int4 dequant-matmul and the SIMT / tensor-core dispatch.
+// gptq.cu -- C-ABI entry points of the GPTQ 2 / 3 / 4-bit dequant-matmul and its input gradient: the argument
+// checks and the SIMT / decode / tensor-core dispatch.
 //
 // Boundary replaced: cuda_kernel.vecquant4matmul / vecgroupquant4matmul
 // (large_language_models/llama/quantization/cuda/cuda_kernel.cpp:10-23,70,73) and their argument
 // checks (cuda_kernel_4bit.cu:44-60).
-#include <cuda_fp16.h>
+#include <stdio.h>
 
-#include "common.cuh"
+#include "gptq_launch.cuh"
+#include "gptq_unpack.cuh"
 
 namespace sb200 {
-int gptq4_simt(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
-               long long M, long long K, long long N, long long KW, int group_size, cudaStream_t st);
-int gptq4_decode(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
-                 long long K, long long N, long long KW, int group_size, int flags, cudaStream_t st);
-bool gptq4_tc_supported(const void* x, const int32_t* qweight, const float* out, long long M, long long K, long long N,
-                        long long KW, int group_size);
-size_t gptq4_tc_workspace(long long M, long long K, long long N, int group_size);
-int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
-             long long K, long long N, long long KW, int group_size, void* workspace, size_t workspace_bytes,
-             cudaStream_t st, const __half* x_h = nullptr, __half* out_h = nullptr, const float* bias = nullptr);
-size_t gptq4_decode_f16_partial_bytes(long long M, long long K, long long N);
-int gptq4_decode_f16(const __half* x_h, const int32_t* qweight, __half* out_h, const float* bias, const float* scales,
-                     const float* zeros, long long M, long long K, long long N, long long KW, int group_size, float* partial,
-                     int* counters, int flags, cudaStream_t st);
-bool gptq4_decode_supported(const int32_t* qweight, long long N);
-void gptq4_tc_set_backoff(int ns);
-void gptq4_decode_set_mode(int mode);
-int gptq_lowbit(int bits, const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
-                long long M, long long K, long long N, long long KW, int group_size, cudaStream_t st);
-size_t gptq_dgrad_simt_workspace(long long M, long long K, long long N, int group_size);
-size_t gptq_dgrad_tc_workspace(long long M, long long K, long long N, int group_size);
-bool gptq_dgrad_tc_supported(const float* grad_out, long long K, long long N, int group_size);
-int gptq_dgrad_simt(int bits, const float* go, const int32_t* qweight, float* grad_in, const float* scales, const float* zeros,
-                    long long M, long long K, long long N, long long KW, int group_size, void* workspace,
-                    size_t workspace_bytes, cudaStream_t st);
-int gptq4_dgrad_tc(const float* go, const int32_t* qweight, float* grad_in, const float* scales, const float* zeros,
-                   long long M, long long K, long long N, long long KW, int group_size, void* workspace, size_t workspace_bytes,
-                   cudaStream_t st);
 static int g_gptq_impl = 0;
 
 // fp16 <-> fp32 staging for the paths of sb200_gptq4_linear_f16 that run the fp32 kernels (small M)
@@ -51,6 +25,27 @@ __global__ void __launch_bounds__(256) f32_to_f16_kernel(const float* __restrict
 static inline unsigned ew_grid(long long n) {
   long long b = (n + 255) / 256, cap = (long long)sm_count() * 16;
   return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
+}
+
+// The operand rules of every GPTQ entry point, checked before any CUDA call (cuda_kernel_{2,3,4}bit.cu argument
+// checks): 2, 3 or 4 bits, non-null operands, 1 <= M, K, N < 2^31, at least the packed rows QuantLinear allocates for K,
+// and a group size that is a multiple of 128 (2-bit: 64).  `fn` names the caller in the messages.  *group_size == 0
+// means one group and is replaced by K.
+static int check_gptq_args(const char* fn, int bits, const void* x, const int32_t* qweight, const void* out,
+                           const float* scales, const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows,
+                           int* group_size) {
+  SB_REQUIRE(bits == 2 || bits == 3 || bits == 4, "%s: only support 2/3/4 bit now (got %d)", fn, bits);
+  SB_REQUIRE(x && qweight && out && scales && zeros, "%s: null pointer argument", fn);
+  SB_REQUIRE(m > 0 && k > 0 && n > 0, "%s: empty operand (M=%lld K=%lld N=%lld)", fn, (long long)m, (long long)k, (long long)n);
+  SB_REQUIRE(m < (1LL << 31) && k < (1LL << 31) && n < (1LL << 31), "%s: dimension too large", fn);
+  const long long need = gptq_packed_rows(bits, k);
+  SB_REQUIRE(qweight_rows >= need, "%s: qweight has %lld rows, %d-bit K=%lld needs %lld", fn, (long long)qweight_rows, bits,
+             (long long)k, need);
+  const int min_group = bits == 2 ? 64 : 128;  // cuda_kernel_2bit.cu:58, cuda_kernel_3bit.cu:60, cuda_kernel_4bit.cu:60
+  SB_REQUIRE(*group_size >= 0 && *group_size % min_group == 0,
+             "only group_size divisible by %d is supported in %d-bit quantization (got %d)", min_group, bits, *group_size);
+  if (*group_size == 0) *group_size = (int)k;
+  return SB200_OK;
 }
 }  // namespace sb200
 
@@ -82,24 +77,10 @@ size_t sb200_gptq4_workspace_bytes(int64_t m, int64_t k, int64_t n, int group_si
   return gptq4_tc_workspace(m, k, n, group_size);
 }
 
+// Arguments as check_gptq_args left them, impl in {0, 1, 2, 4}.
 static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                           int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size, int impl,
                           void* workspace, size_t workspace_bytes, void* stream, int flags = 0) {
-  SB_REQUIRE(x && qweight && out && scales && zeros, "sb200_gptq4_matmul: null pointer argument");
-  SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_gptq4_matmul: empty operand (M=%lld K=%lld N=%lld)", (long long)m,
-             (long long)k, (long long)n);
-  SB_REQUIRE(m < (1LL << 31) && k < (1LL << 31) && n < (1LL << 31), "sb200_gptq4_matmul: dimension too large");
-  SB_REQUIRE(qweight_rows >= (k + 7) / 8,
-             "sb200_gptq4_matmul: qweight has %lld rows, need ceil(K/8) = %lld", (long long)qweight_rows,
-             (long long)((k + 7) / 8));
-  SB_REQUIRE(impl >= 0 && impl <= 4 && impl != 3, "sb200_gptq4_matmul: impl must be 0 (auto), 1 (small-M), 2 (tensor core), 4 (scalar) (got %d)", impl);
-  if (group_size != 0) {
-    // cuda_kernel_4bit.cu:60
-    SB_REQUIRE(group_size > 0 && group_size % 128 == 0,
-               "only group_size divisible by 128 is supported in 4-bit quantization (got %d)", group_size);
-  } else {
-    group_size = (int)k;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   // 1 = small-M path: warp-level HMMA streaming kernel (gptq_decode.cu) when N % 4 == 0, else the scalar kernel;
   // 4 = scalar SIMT kernel (gptq_simt.cu, any shape);  2 = wgmma, exact int4 operands + per-128-K-group fp32 rescale (gptq_tc.cu).
@@ -118,12 +99,14 @@ static int gptq4_dispatch(const float* x, const int32_t* qweight, float* out, co
     return gptq4_tc(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, workspace, workspace_bytes, st);
   if (impl != 4 && gptq4_decode_supported(qweight, n))
     return gptq4_decode(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, flags, st);
-  return gptq4_simt(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, st);
+  return gptq_simt(4, x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, st);
 }
 
 int sb200_gptq4_matmul(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                        int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size, void* workspace,
                        size_t workspace_bytes, void* stream) {
+  if (const int rc = check_gptq_args("sb200_gptq4_matmul", 4, x, qweight, out, scales, zeros, m, k, n, qweight_rows, &group_size))
+    return rc;
   return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, g_gptq_impl, workspace,
                         workspace_bytes, stream);
 }
@@ -133,12 +116,36 @@ int sb200_gptq4_matmul_ex(const float* x, const int32_t* qweight, float* out, co
                           const sb200_gptq4_options* options, void* workspace, size_t workspace_bytes, void* stream) {
   const int impl = options ? options->impl : 0, flags = options ? options->flags : 0;
   if (options) {
+    SB_REQUIRE(impl >= 0 && impl <= 4 && impl != 3, "sb200_gptq4_matmul_ex: impl must be 0 (auto), 1 (small-M), 2 (tensor core), 4 (scalar) (got %d)", impl);
     SB_REQUIRE((flags & ~SB200_GPTQ4_STATIC_WEIGHTS) == 0, "sb200_gptq4_matmul_ex: unknown flags 0x%x", flags);
     SB_REQUIRE(options->chunk_k == 0, "sb200_gptq4_matmul_ex: chunk_k is reserved and must be zero (got %d)", options->chunk_k);
     for (int i = 0; i < 5; ++i) SB_REQUIRE(options->reserved[i] == 0, "sb200_gptq4_matmul_ex: reserved option fields must be zero");
   }
+  if (const int rc = check_gptq_args("sb200_gptq4_matmul_ex", 4, x, qweight, out, scales, zeros, m, k, n, qweight_rows, &group_size))
+    return rc;
   return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, impl, workspace,
                         workspace_bytes, stream, flags);
+}
+
+int sb200_gptq4_matmul_batch(const sb200_gptq4_problem* problems, int count, int64_t m, void* stream) {
+  return sb200_gptq4_matmul_batch_ex(problems, count, m, 0, stream);
+}
+
+int sb200_gptq4_matmul_batch_ex(const sb200_gptq4_problem* problems, int count, int64_t m, int flags, void* stream) {
+  SB_REQUIRE((flags & ~SB200_GPTQ4_STATIC_WEIGHTS) == 0, "sb200_gptq4_matmul_batch_ex: unknown flags 0x%x", flags);
+  SB_REQUIRE(problems && count >= 1 && count <= kDecMaxProblems, "sb200_gptq4_matmul_batch: 1 .. %d problems (got %d)", kDecMaxProblems, count);
+  SB_REQUIRE(m >= 1 && m <= 32, "sb200_gptq4_matmul_batch: decode-sized M only (1 .. 32, got %lld)", (long long)m);
+  sb200_gptq4_problem p[kDecMaxProblems];
+  for (int i = 0; i < count; ++i) {
+    p[i] = problems[i];
+    char fn[64];
+    snprintf(fn, sizeof fn, "sb200_gptq4_matmul_batch: problem %d", i);
+    if (const int rc = check_gptq_args(fn, 4, p[i].x, p[i].qweight, p[i].out, p[i].scales, p[i].zeros, m, p[i].k, p[i].n,
+                                       p[i].qweight_rows, &p[i].group_size))
+      return rc;
+    SB_REQUIRE(gptq4_decode_supported(p[i].qweight, p[i].n), "%s needs N %% 4 == 0 and a 16-byte aligned qweight", fn);
+  }
+  return gptq4_decode_batch(p, count, m, flags, (cudaStream_t)stream);
 }
 
 constexpr int64_t kF16SingleLaunchMaxM = 32;
@@ -164,17 +171,10 @@ int sb200_gptq4_linear_f16(const void* x_f16, const int32_t* qweight, void* out_
 int sb200_gptq4_linear_f16_ex(const void* x_f16, const int32_t* qweight, void* out_f16, const float* bias, const float* scales,
                               const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int group_size,
                               void* state, int flags, void* workspace, size_t workspace_bytes, void* stream) {
-  SB_REQUIRE(x_f16 && qweight && out_f16 && scales && zeros, "sb200_gptq4_linear_f16: null pointer argument");
+  if (const int rc = check_gptq_args("sb200_gptq4_linear_f16", 4, x_f16, qweight, out_f16, scales, zeros, m, k, n, qweight_rows,
+                                     &group_size))
+    return rc;
   SB_REQUIRE((flags & ~SB200_GPTQ4_STATIC_WEIGHTS) == 0, "sb200_gptq4_linear_f16_ex: unknown flags 0x%x", flags);
-  const int group_size_arg = group_size;  // 0 = one group: handed on unchanged (K itself need not be a multiple of 128)
-  SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_gptq4_linear_f16: empty operand (M=%lld K=%lld N=%lld)", (long long)m, (long long)k, (long long)n);
-  SB_REQUIRE(m < (1LL << 31) && k < (1LL << 31) && n < (1LL << 31), "sb200_gptq4_linear_f16: dimension too large");
-  SB_REQUIRE(qweight_rows >= (k + 7) / 8, "sb200_gptq4_linear_f16: qweight has %lld rows, need ceil(K/8) = %lld", (long long)qweight_rows, (long long)((k + 7) / 8));
-  if (group_size != 0) {
-    SB_REQUIRE(group_size > 0 && group_size % 128 == 0, "only group_size divisible by 128 is supported in 4-bit quantization (got %d)", group_size);
-  } else {
-    group_size = (int)k;
-  }
   SB_REQUIRE(workspace && workspace_bytes >= sb200_gptq4_linear_f16_workspace_bytes(m, k, n, group_size), "sb200_gptq4_linear_f16: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   const __half* xh = reinterpret_cast<const __half*>(x_f16);
@@ -199,7 +199,7 @@ int sb200_gptq4_linear_f16_ex(const void* x_f16, const int32_t* qweight, void* o
   bias_rows_kernel<<<ew_grid(m * n), 256, 0, st>>>(bias, y32, m, n);
   SB_LAUNCHED();
   // the kernel immediately in front is bias_rows_kernel (writes y32 only): the weight tables cannot be its output
-  const int rc = gptq4_dispatch(x32, qweight, y32, scales, zeros, m, k, n, qweight_rows, group_size_arg, 0, rest, rest_bytes, stream,
+  const int rc = gptq4_dispatch(x32, qweight, y32, scales, zeros, m, k, n, qweight_rows, group_size, 0, rest, rest_bytes, stream,
                                 SB200_GPTQ4_STATIC_WEIGHTS);
   if (rc) return rc;
   f32_to_f16_kernel<<<ew_grid(m * n), 256, 0, st>>>(y32, yh, m * n);
@@ -210,26 +210,12 @@ int sb200_gptq4_linear_f16_ex(const void* x_f16, const int32_t* qweight, void* o
 int sb200_gptq_matmul(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
                       int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int bits, int group_size, void* workspace,
                       size_t workspace_bytes, void* stream) {
-  SB_REQUIRE(bits == 2 || bits == 3 || bits == 4, "sb200_gptq_matmul: only support 2/3/4 bit now (got %d)", bits);
+  if (const int rc = check_gptq_args("sb200_gptq_matmul", bits, x, qweight, out, scales, zeros, m, k, n, qweight_rows, &group_size))
+    return rc;
   if (bits == 4)
-    return sb200_gptq4_matmul(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, workspace,
-                              workspace_bytes, stream);
-  SB_REQUIRE(x && qweight && out && scales && zeros, "sb200_gptq_matmul: null pointer argument");
-  SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_gptq_matmul: empty operand (M=%lld K=%lld N=%lld)", (long long)m,
-             (long long)k, (long long)n);
-  SB_REQUIRE(m < (1LL << 31) && k < (1LL << 31) && n < (1LL << 31), "sb200_gptq_matmul: dimension too large");
-  // rows QuantLinear allocates (utils/quant.py:172-184): ceil(K*bit / (32*p)) * p, p = 3 for 3-bit
-  const int64_t need = bits == 2 ? (k + 15) / 16 : ((k * 3 + 95) / 96) * 3;
-  SB_REQUIRE(qweight_rows >= need, "sb200_gptq_matmul: qweight has %lld rows, %d-bit K=%lld needs %lld",
-             (long long)qweight_rows, bits, (long long)k, (long long)need);
-  const int min_group = bits == 2 ? 64 : 128;  // cuda_kernel_2bit.cu:58, cuda_kernel_3bit.cu:60
-  if (group_size != 0) {
-    SB_REQUIRE(group_size > 0 && group_size % min_group == 0,
-               "only group_size divisible by %d is supported in %d-bit quantization (got %d)", min_group, bits, group_size);
-  } else {
-    group_size = (int)k;
-  }
-  return gptq_lowbit(bits, x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, (cudaStream_t)stream);
+    return gptq4_dispatch(x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, g_gptq_impl, workspace,
+                          workspace_bytes, stream);
+  return gptq_simt(bits, x, qweight, out, scales, zeros, m, k, n, qweight_rows, group_size, (cudaStream_t)stream);
 }
 
 // Auto dispatch of the input gradient: the tensor-core kernel from this many rows of grad_out on (4-bit shapes it takes).
@@ -249,22 +235,10 @@ size_t sb200_gptq_dgrad_workspace_bytes(int64_t m, int64_t k, int64_t n, int bit
 int sb200_gptq_matmul_dgrad(const float* grad_out, const int32_t* qweight, float* grad_in, const float* scales,
                             const float* zeros, int64_t m, int64_t k, int64_t n, int64_t qweight_rows, int bits,
                             int group_size, int impl, void* workspace, size_t workspace_bytes, void* stream) {
-  SB_REQUIRE(bits == 2 || bits == 3 || bits == 4, "sb200_gptq_matmul_dgrad: only support 2/3/4 bit now (got %d)", bits);
-  SB_REQUIRE(grad_out && qweight && grad_in && scales && zeros, "sb200_gptq_matmul_dgrad: null pointer argument");
-  SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_gptq_matmul_dgrad: empty operand (M=%lld K=%lld N=%lld)", (long long)m,
-             (long long)k, (long long)n);
-  SB_REQUIRE(m < (1LL << 31) && k < (1LL << 31) && n < (1LL << 31), "sb200_gptq_matmul_dgrad: dimension too large");
-  const int64_t need = bits == 4 ? (k + 7) / 8 : (bits == 2 ? (k + 15) / 16 : ((k * 3 + 95) / 96) * 3);
-  SB_REQUIRE(qweight_rows >= need, "sb200_gptq_matmul_dgrad: qweight has %lld rows, %d-bit K=%lld needs %lld",
-             (long long)qweight_rows, bits, (long long)k, (long long)need);
+  if (const int rc = check_gptq_args("sb200_gptq_matmul_dgrad", bits, grad_out, qweight, grad_in, scales, zeros, m, k, n,
+                                     qweight_rows, &group_size))
+    return rc;
   SB_REQUIRE(impl >= 0 && impl <= 2, "sb200_gptq_matmul_dgrad: impl must be 0 (auto), 1 (SIMT) or 2 (tensor core) (got %d)", impl);
-  const int min_group = bits == 2 ? 64 : 128;
-  if (group_size != 0) {
-    SB_REQUIRE(group_size > 0 && group_size % min_group == 0,
-               "only group_size divisible by %d is supported in %d-bit quantization (got %d)", min_group, bits, group_size);
-  } else {
-    group_size = (int)k;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   const bool tc_ok = bits == 4 && gptq_dgrad_tc_supported(grad_out, k, n, group_size) && workspace &&
                      workspace_bytes >= gptq_dgrad_tc_workspace(m, k, n, group_size);

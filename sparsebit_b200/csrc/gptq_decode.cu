@@ -23,9 +23,7 @@
 // nibbles (2i + 1, 2i + 5) -- exactly the pairs one LOP3 extracts ((w >> 8i) & 0x000F000F, & 0x00F000F0).  The
 // activations are stored in shared memory with every 8 K permuted to (0, 4, 1, 5, 2, 6, 3, 7), so one 16-byte load
 // returns the B registers of both MMAs.
-#include <cuda_fp16.h>
-
-#include "common.cuh"
+#include "gptq_launch.cuh"
 
 namespace sb200 {
 
@@ -78,7 +76,6 @@ struct DecProblem {
   float* partial;
   int* counters;
 };
-constexpr int kDecMaxProblems = 4;
 struct DecBatch {
   DecProblem p[kDecMaxProblems];
   int count;
@@ -442,8 +439,8 @@ static int dec_launch(const DecBatch& batch, dim3 grid, size_t smem, int M, int 
   return SB200_OK;
 }
 
-// `count` problems sharing M in one launch (count == 1: the plain entry point)
-int gptq4_decode_batch(const DecProblem* probs, int count, long long M, int flags, cudaStream_t st) {
+// `count` problems sharing M in one launch
+static int dec_run(const DecProblem* probs, int count, long long M, int flags, cudaStream_t st) {
   DecBatch batch;
   batch.count = count;
   int colblocks = 0, nblk_max = 0;
@@ -482,26 +479,28 @@ int gptq4_decode_batch(const DecProblem* probs, int count, long long M, int flag
 #undef SB_GO
 }
 
+// One problem of a launch.  fp32 form: x / out; fp16 form: x_h / out_h / bias with its `partial` slots and `counters`.
+static DecProblem dec_problem(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros,
+                              long long K, long long N, long long KW, int group_size, const __half* x_h = nullptr,
+                              __half* out_h = nullptr, const float* bias = nullptr, float* partial = nullptr,
+                              int* counters = nullptr) {
+  return DecProblem{x, reinterpret_cast<const uint32_t*>(qweight), out, scales, zeros, (int)K, (int)N, (int)KW,
+                    (int)((K + group_size - 1) / group_size), group_size, 0, x_h, out_h, bias, partial, counters};
+}
+
 int gptq4_decode(const float* x, const int32_t* qweight, float* out, const float* scales, const float* zeros, long long M,
                  long long K, long long N, long long KW, int group_size, int flags, cudaStream_t st) {
-  DecProblem p;
-  p.x = x;
-  p.qw = reinterpret_cast<const uint32_t*>(qweight);
-  p.out = out;
-  p.scales = scales;
-  p.zeros = zeros;
-  p.K = (int)K;
-  p.N = (int)N;
-  p.KW = (int)KW;
-  p.G = (int)((K + group_size - 1) / group_size);
-  p.group_size = group_size;
-  p.colblock_begin = 0;
-  p.x_h = nullptr;
-  p.out_h = nullptr;
-  p.bias = nullptr;
-  p.partial = nullptr;
-  p.counters = nullptr;
-  return gptq4_decode_batch(&p, 1, M, flags, st);
+  const DecProblem p = dec_problem(x, qweight, out, scales, zeros, K, N, KW, group_size);
+  return dec_run(&p, 1, M, flags, st);
+}
+
+int gptq4_decode_batch(const sb200_gptq4_problem* problems, int count, long long M, int flags, cudaStream_t st) {
+  DecProblem p[kDecMaxProblems];
+  for (int i = 0; i < count; ++i) {
+    const sb200_gptq4_problem& q = problems[i];
+    p[i] = dec_problem(q.x, q.qweight, q.out, q.scales, q.zeros, q.k, q.n, q.qweight_rows, q.group_size);
+  }
+  return dec_run(p, count, M, flags, st);
 }
 
 // fp16 in / fp16 out in one launch; `partial` holds ceil(K / 128) * M * N floats, `counters` ceil(N / 128) zeroed ints
@@ -511,64 +510,9 @@ size_t gptq4_decode_f16_partial_bytes(long long M, long long K, long long N) {
 int gptq4_decode_f16(const __half* x_h, const int32_t* qweight, __half* out_h, const float* bias, const float* scales,
                      const float* zeros, long long M, long long K, long long N, long long KW, int group_size, float* partial,
                      int* counters, int flags, cudaStream_t st) {
-  DecProblem p;
-  p.x = nullptr;
-  p.qw = reinterpret_cast<const uint32_t*>(qweight);
-  p.out = nullptr;
-  p.scales = scales;
-  p.zeros = zeros;
-  p.K = (int)K;
-  p.N = (int)N;
-  p.KW = (int)KW;
-  p.G = (int)((K + group_size - 1) / group_size);
-  p.group_size = group_size;
-  p.colblock_begin = 0;
-  p.x_h = x_h;
-  p.out_h = out_h;
-  p.bias = bias;
-  p.partial = partial;
-  p.counters = counters;
-  return gptq4_decode_batch(&p, 1, M, flags, st);
+  const DecProblem p = dec_problem(nullptr, qweight, nullptr, scales, zeros, K, N, KW, group_size, x_h, out_h, bias, partial,
+                                   counters);
+  return dec_run(&p, 1, M, flags, st);
 }
 
 }  // namespace sb200
-
-using namespace sb200;
-
-extern "C" int sb200_gptq4_matmul_batch_ex(const sb200_gptq4_problem* problems, int count, int64_t m, int flags, void* stream);
-extern "C" int sb200_gptq4_matmul_batch(const sb200_gptq4_problem* problems, int count, int64_t m, void* stream) {
-  return sb200_gptq4_matmul_batch_ex(problems, count, m, 0, stream);
-}
-extern "C" int sb200_gptq4_matmul_batch_ex(const sb200_gptq4_problem* problems, int count, int64_t m, int flags, void* stream) {
-  SB_REQUIRE((flags & ~SB200_GPTQ4_STATIC_WEIGHTS) == 0, "sb200_gptq4_matmul_batch_ex: unknown flags 0x%x", flags);
-  SB_REQUIRE(problems && count >= 1 && count <= kDecMaxProblems, "sb200_gptq4_matmul_batch: 1 .. %d problems (got %d)", kDecMaxProblems, count);
-  SB_REQUIRE(m >= 1 && m <= 32, "sb200_gptq4_matmul_batch: decode-sized M only (1 .. 32, got %lld)", (long long)m);
-  DecProblem p[kDecMaxProblems];
-  for (int i = 0; i < count; ++i) {
-    const sb200_gptq4_problem& q = problems[i];
-    SB_REQUIRE(q.x && q.qweight && q.out && q.scales && q.zeros, "sb200_gptq4_matmul_batch: null pointer in problem %d", i);
-    SB_REQUIRE(q.k > 0 && q.n > 0 && q.k < (1LL << 31) && q.n < (1LL << 31), "sb200_gptq4_matmul_batch: bad shape in problem %d", i);
-    SB_REQUIRE(q.qweight_rows >= (q.k + 7) / 8, "sb200_gptq4_matmul_batch: qweight of problem %d has too few rows", i);
-    SB_REQUIRE(q.group_size == 0 || (q.group_size > 0 && q.group_size % 128 == 0),
-               "only group_size divisible by 128 is supported in 4-bit quantization (got %d)", q.group_size);
-    SB_REQUIRE(gptq4_decode_supported(q.qweight, q.n), "sb200_gptq4_matmul_batch: problem %d needs N %% 4 == 0 and a 16-byte aligned qweight", i);
-    const int gs = q.group_size ? q.group_size : (int)q.k;
-    p[i].x = q.x;
-    p[i].qw = reinterpret_cast<const uint32_t*>(q.qweight);
-    p[i].out = q.out;
-    p[i].scales = q.scales;
-    p[i].zeros = q.zeros;
-    p[i].K = (int)q.k;
-    p[i].N = (int)q.n;
-    p[i].KW = (int)q.qweight_rows;
-    p[i].G = (int)((q.k + gs - 1) / gs);
-    p[i].group_size = gs;
-    p[i].colblock_begin = 0;
-    p[i].x_h = nullptr;
-    p[i].out_h = nullptr;
-    p[i].bias = nullptr;
-    p[i].partial = nullptr;
-    p[i].counters = nullptr;
-  }
-  return gptq4_decode_batch(p, count, m, flags, (cudaStream_t)stream);
-}

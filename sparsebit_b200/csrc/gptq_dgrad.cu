@@ -1,11 +1,11 @@
 // gptq_dgrad.cu -- input gradient of the GPTQ dequant-matmul (2 / 3 / 4-bit), the backward of QuantLinear:
 //   grad_in[m, k] += sum_n grad_out[m, n] * (scales[n, k/gs] * q(k, n) - zeros[n, k/gs])
 // grad_out [M, N] fp32, grad_in [M, K] fp32 (accumulated in place), qweight / scales / zeros exactly the tensors the
-// forward reads (gptq.cu, gptq_lowbit.cu).  Both kernels are deterministic: no float atomics, fixed reduction orders.
+// forward reads (gptq.cu, gptq_simt.cu).  Both kernels are deterministic: no float atomics, fixed reduction orders.
 //
 // SIMT kernel (any bit width, any shape).  A CTA owns one 32-k unit of packed rows, MT rows of grad_out and one slice
 // of N.  Each thread walks the columns n = tid, tid + 128, ... of the slice (a warp reads 128 contiguous bytes of every
-// packed row), decodes the unit and applies the per-group affine the way the forward SIMT kernels do, here with the
+// packed row), decodes the unit and applies the per-group affine the way the forward SIMT kernel does, here with the
 // scale folded into the gradient:  sum_n g (s q - z) = sum_n (g s) q - sum_n g z.  The 128 per-thread partials are
 // summed through shared memory in a fixed order; with more than one N slice every slice writes its own partial and a
 // finish kernel adds them in slice order.
@@ -29,6 +29,7 @@
 //   * epilogue grad_in[m, k] = fmaf(2^e[m], 2^-c[g] * acc, grad_in[m, k]).
 // Limits: N % 8 == 0 (16-byte rows of g' and the 8-wide permutation), K % 4 == 0 (16-byte rows of qT), grad_out 16-byte
 // aligned, group_size a multiple of 128 or one group.  Everything else runs the SIMT kernel.
+#include "gptq_launch.cuh"
 #include "gptq_unpack.cuh"
 #include "tc_common.cuh"
 
@@ -39,23 +40,6 @@ namespace {
 constexpr int kDgCols = 128;        // threads per CTA; the columns n one pass of the CTA reads
 constexpr int kDgUnitK = 32;        // k per CTA (one unit)
 constexpr long long kDgTargetCtas = 1024;  // N is split until the grid has about this many CTAs (~8 per SM)
-
-template <int BITS>
-struct DgFmt {
-  static constexpr int kWords = BITS == 3 ? 3 : (BITS == 2 ? 2 : 4);  // packed rows of one 32-k unit
-};
-
-template <int BITS>
-__device__ __forceinline__ void dg_decode(const uint32_t* w, float (&q)[32]) {
-  if constexpr (BITS == 4) {
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) q[8 * r + j] = small_to_float((w[r] >> (4 * j)) & 15u);
-  } else {
-    decode_unit<BITS>(w, q);
-  }
-}
 
 // scales / zeros [N, G] -> sz[g, n] = (s, z): the SIMT kernel reads them along n, coalesced
 __global__ void __launch_bounds__(256) dgrad_sz_kernel(const float* __restrict__ scales, const float* __restrict__ zeros,
@@ -72,7 +56,7 @@ __global__ void __launch_bounds__(kDgCols) gptq_dgrad_simt_kernel(const float* _
                                                                    float* __restrict__ grad_in, const float2* __restrict__ sz,
                                                                    float* __restrict__ partial, int M, int K, int N, int KW,
                                                                    int group_size, int slice_n) {
-  constexpr int kWords = DgFmt<BITS>::kWords;
+  constexpr int kWords = GptqFmt<BITS>::kUnitWords;
   __shared__ float red[kDgUnitK][kDgCols + 1];
   const int tid = threadIdx.x;
   const int u = blockIdx.x, m0 = blockIdx.y * MT;
@@ -102,7 +86,7 @@ __global__ void __launch_bounds__(kDgCols) gptq_dgrad_simt_kernel(const float* _
       zacc[m] = fmaf(gv, p.y, zacc[m]);
     }
     float q[32];
-    dg_decode<BITS>(w, q);
+    decode_unit<BITS>(w, q);
 #pragma unroll
     for (int m = 0; m < MT; ++m)
 #pragma unroll
@@ -389,10 +373,6 @@ bool tc_shape_ok(long long K, long long N, int group_size) {
 }
 
 }  // namespace
-
-int gptq_launch_split(const float* x, __half* a_hi, __half* a_lo, float* xsum, float* rowscale, int* need_lo, long long M,
-                      int K, int G, cudaStream_t st);  // gptq_tc.cu
-int gptq4_tc_backoff();                                // gptq_tc.cu
 
 size_t gptq_dgrad_simt_workspace(long long M, long long K, long long N, int group_size) {
   const SimtPlan p = simt_plan(M, K, N, group_size);

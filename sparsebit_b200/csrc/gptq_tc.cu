@@ -22,6 +22,7 @@
 //
 // fp16 activations (sb200_gptq4_linear_f16): the activations are the hi plane as they are, the lo pass never runs, and
 // the epilogue writes out_h = fp16(bias + x @ W) instead of accumulating into the fp32 `out`.
+#include "gptq_launch.cuh"
 #include "tc_common.cuh"
 
 namespace sb200 {

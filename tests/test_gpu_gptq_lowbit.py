@@ -1,6 +1,7 @@
 """GPU parity: GPTQ 3-bit / 2-bit dequant-matmul (SURVEY 8f #3) through the ``cuda_kernel`` mirror /
 QuantLinear vs the reference's known-answer construction (test_cuda_kernel.py, bit = 2, 3 cases:
-rtol = atol = 1e-5 against Linear(dequantised W), fp32) and the fp64 oracle."""
+rtol = atol = 1e-5 against Linear(dequantised W), fp32) and the fp64 oracle.  The fp64 oracle cases also run the
+4-bit instantiations of the same SIMT kernel (gptq_simt.cu) through ``impl=4``."""
 import numpy as np
 import pytest
 import torch
@@ -19,7 +20,9 @@ GROUPED = {2: cuda_kernel.vecgroupquant2matmul, 3: cuda_kernel.vecgroupquant3mat
 
 def _run(bit, x, qw, bias, scales, zeros, gs):
     y = t(np.broadcast_to(bias, x.shape[:-1] + (qw.shape[1],)).copy())
-    if gs == -1:
+    if bit == 4:
+        ops.gptq4_matmul(t(x), t(qw), y, t(scales), t(zeros), 0 if gs == -1 else gs, impl=4)
+    elif gs == -1:
         PLAIN[bit](t(x), t(qw), y, t(scales), t(zeros))
     else:
         GROUPED[bit](t(x), t(qw), y, t(scales), t(zeros), gs)
@@ -35,12 +38,18 @@ def test_golden_known_answers(golden):
 
 
 # test_cuda_kernel.py:50-126 shapes that fit the time budget: irregular K / N, multi-batch, 3-D inputs,
-# minimum and 3x group sizes, plus LLaMA-7B linear shapes at decode M.
+# minimum and 3x group sizes, plus LLaMA-7B linear shapes at decode M.  For every bit width they run each row tile
+# MT in {1, 2, 4, 8} (M = 1, 2, 3..4, >= 5), the multi-pass M loop (M > 8), K % block != 0, N % 128 != 0, and on a
+# 132-SM H100 K slices of one block, of an odd and an even number of blocks, and a last slice shorter than the rest
+# (e.g. 4096 x 11008: 3 blocks per slice, 2 in the last).
 CASES = [
     (2, (1,), 1024, 1024, -1), (3, (1,), 1024, 1024, -1), (2, (1,), 719, 857, -1), (3, (1,), 719, 857, -1),
     (2, (31,), 6661, 1257, -1), (3, (31,), 6661, 1257, -1), (2, (4, 8), 2661, 512, -1), (3, (32, 1), 1024, 1031, -1),
     (2, (29,), 8192, 512, 64), (3, (29,), 8192, 512, 128), (2, (4,), 6144, 768, 192), (3, (4,), 6144, 768, 384),
     (2, (1,), 4096, 11008, 64), (3, (1,), 11008, 4096, 128), (3, (2,), 4096, 4096, 128), (2, (3,), 4096, 4096, 128),
+    (2, (2,), 4096, 11008, 64),
+    (4, (1,), 4096, 11008, 128), (4, (2,), 719, 857, -1), (4, (3,), 4096, 4096, 128), (4, (31,), 6661, 1257, -1),
+    (4, (2,), 11008, 4096, 128), (4, (5, 4), 2048, 11008, 256),
 ]
 
 
