@@ -450,6 +450,46 @@ int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_
                       const float* bias, float* out, int64_t m, int64_t k, int64_t n, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* ---- (5b) Integer-grid inference of a calibrated QConv2d (int8 wgmma, sm_90a) ----------------
+ * New; the reference's QConv2d (modules/conv.py) fake-quantises x and W (QDQ x 2) and runs F.conv2d.  Lowered, the
+ * convolution is the integer linear above: M = n OH OW output pixels, K = c kh kw taps in the order (c, kh, kw) of
+ * weight.reshape(c_out, -1), N = c_out.  The weights go through sb200_int8_quantize_rows as [c_out, K] rows.
+ *
+ * Geometry (host struct, passed by pointer): x is [n, c, h, w] fp32 contiguous; every size, stride and dilation > 0,
+ * the four paddings >= 0 (asymmetric padding -- e.g. PyTorch's padding='same' for even kernels -- is allowed);
+ *   OH = (h + pad_top + pad_bottom - dilation_h (kh - 1) - 1) / stride_h + 1, OW likewise.
+ * Argument checks, all before any CUDA call: null pointers, a non-positive geometry, an empty output (OH or OW < 1)
+ * and M >= 2^31 are SB200_E_INVALID, as are the range rules of the integer linear and a w_q / q not 16-byte aligned;
+ * K >= 2^17 is SB200_E_UNSUPPORTED; a workspace that is too small is SB200_E_WORKSPACE.
+ *
+ * sb200_int8_im2col_quantize: the lowering alone.  q [M, Kp] s8 (16-byte aligned, Kp = round_up(K, 16)): element
+ * (m, k) is the stored grid value (as in sb200_int8_quantize_rows) of x[img, c, oh sh - pad_top + kh dh,
+ * ow sw - pad_left + kw dw] for m = (img OH + oh) OW + ow, k = (c kh_ + kh) kw_ + kw; a tap in the padding stores
+ * rint(zero_point) - off (the grid point of the fake-quant input's zero padding); the K padding is zero.
+ * row_sum[M] int32 = sum of the stored row; nan_flag[M] uint8 = 1 if the window holds a NaN.  scale / zero_point:
+ * device, one float each.
+ *
+ * sb200_int8_conv2d: out [n, c_out, OH, OW] fp32 NCHW (overwritten) = the fake-quant conv2d of x with per-tensor
+ * device scalars x_scale / x_zero_point and the integer range [qmin_x, qmax_x], and the weights as
+ * sb200_int8_quantize_rows stored them (w_q [c_out, Kp], w_rowsum / w_scale / w_zero [c_out], bias [c_out] or NULL);
+ * the epilogue, NaN rules and guarantees are those of sb200_int8_linear (groups = 1 only).
+ * workspace: sb200_int8_conv2d_workspace_bytes(geom) bytes (a pure function; 0 for an invalid geometry). */
+typedef struct sb200_conv2d_geom {
+  int64_t n, c, h, w;                         /* input [n, c, h, w] */
+  int64_t kh, kw;                             /* kernel */
+  int64_t stride_h, stride_w;
+  int64_t dilation_h, dilation_w;
+  int64_t pad_top, pad_bottom, pad_left, pad_right;
+} sb200_conv2d_geom;
+int sb200_int8_im2col_quantize(const float* x, const sb200_conv2d_geom* geom, const float* scale,
+                               const float* zero_point, int qmin, int qmax, int8_t* q, int32_t* row_sum,
+                               uint8_t* nan_flag, void* stream);
+size_t sb200_int8_conv2d_workspace_bytes(const sb200_conv2d_geom* geom);
+int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float* x_scale, const float* x_zero_point,
+                      int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                      const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);

@@ -23,6 +23,15 @@ c_sz = ctypes.c_size_t
 c_f = ctypes.c_float
 c_d = ctypes.c_double
 
+
+class Conv2dGeom(ctypes.Structure):
+    """``sb200_conv2d_geom``: input [n, c, h, w], kernel kh x kw, stride, dilation, paddings top / bottom / left / right."""
+    _fields_ = [(name, ctypes.c_int64) for name in ("n", "c", "h", "w", "kh", "kw", "stride_h", "stride_w", "dilation_h",
+                                                    "dilation_w", "pad_top", "pad_bottom", "pad_left", "pad_right")]
+
+
+c_geom = ctypes.POINTER(Conv2dGeom)
+
 # name -> (restype, argtypes); every symbol include/sparsebit_b200.h declares
 PROTOTYPES = {
     "sb200_last_error": (ctypes.c_char_p, []),
@@ -90,6 +99,10 @@ PROTOTYPES = {
     "sb200_int8_linear_workspace_bytes": (c_sz, [c_i64, c_i64]),
     "sb200_int8_linear": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp,
                                   c_sz, c_vp]),
+    "sb200_int8_im2col_quantize": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "sb200_int8_conv2d_workspace_bytes": (c_sz, [c_geom]),
+    "sb200_int8_conv2d": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_sz,
+                                  c_vp]),
     "sb200_gptq4_set_impl": (c_int, [c_int]),
     "sb200_gptq4_set_wait_backoff": (c_int, [c_int]),
     "sb200_gptq4_set_decode": (c_int, [c_int]),

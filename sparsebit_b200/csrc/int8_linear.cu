@@ -17,6 +17,12 @@
 // then y = fp32(fp64(I * (s_x * s_w[n]))) (+ bias[n] in fp32; s_x * s_w is exact in fp64), and NaN for flagged rows.
 // |a|, |b| <= 128, so |sum a b| <= K * 2^14 fits the s32 accumulator for K < 2^17.  No atomics, no split-K, no state
 // between calls: deterministic and safe under CUDA graph capture.
+//
+// Conv2d.  A calibrated QConv2d is the same GEMM once its input is lowered: M = N OH OW output pixels, K = C KH KW,
+// N = C_out, with the K order (c, kh, kw) of weight.reshape(C_out, -1).  The lowering kernel writes the grid value of
+// every tap of every window as one s8 row per output pixel (the same grid as the row quantizer); a padding tap is the
+// grid point of the fake-quant input's zero padding, v = 0, i.e. rint(zp) - off on the stored grid, so the epilogue's
+// correction stays exact with the real K.  The GEMM then writes NCHW: out[(img N + n) P + p], m = img P + p, P = OH OW.
 #include "tc_common.cuh"
 
 namespace sb200 {
@@ -48,6 +54,17 @@ static inline int grid_offset(int qmin) { return qmin >= 0 ? 128 : 0; }
 static inline long long padded_k(long long k) { return (k + 15) / 16 * 16; }
 
 // ---------------------------------------------------------------------------------- row quantizer
+// The stored grid value g - off of v (QP / quant_round<0>, as the QDQ kernels); NaN sets `nan` and stores 0.
+__device__ __forceinline__ int stored_grid(float v, const QP& p, int off, bool& nan) {
+  float g = __fadd_rn(quant_round<0>(v, p, 0), p.zp);
+  g = fmax_nan(fmin_nan(g, p.qmax), p.qmin);
+  if (g != g) {
+    nan = true;
+    return 0;
+  }
+  return (int)g - off;
+}
+
 // 8 warps per CTA, one row per warp; lane l handles the 16-element chunks starting at 16 l, 16 (l + 32), ...
 __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __restrict__ x, const float* __restrict__ scale,
                                                                  const float* __restrict__ zero_point, int per_row, float qmin,
@@ -82,12 +99,7 @@ __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       int e = 0;  // K padding stays zero
-      if (c + i < K) {
-        float g = __fadd_rn(quant_round<0>(v[i], p, 0), p.zp);
-        g = fmax_nan(fmin_nan(g, p.qmax), p.qmin);
-        if (g != g) nan = true;
-        else e = (int)g - off;
-      }
+      if (c + i < K) e = stored_grid(v[i], p, off, nan);
       sum += e;
       packed[i >> 2] |= ((uint32_t)e & 0xFFu) << (8 * (i & 3));
     }
@@ -99,6 +111,111 @@ __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __
   if (lane == 0) {
     row_sum[row] = sum;
     nan_flag[row] = any_nan ? 1 : 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------- conv2d lowering
+// Conv geometry on the device; every product is 64-bit (M Kp passes 2^31 at ResNet-50 stem sizes from batch ~1024).
+struct ConvDims {
+  long long H, W, HW, CHW;     // input plane, image
+  long long sh, sw, dh, dw;    // stride, dilation
+  long long pt, pl;            // top / left padding
+  long long OW, P, M;          // output width, pixels per image, output pixels
+  int KH, KW, K, Kp;           // taps, taps padded to 16
+};
+
+constexpr int kLowPix = 128;              // output pixels (rows of q) per CTA
+constexpr int kLowK = 128;                // taps per chunk: one 128-byte line of each row of q
+constexpr int kLowWords = kLowK / 4 + 1;  // words per tile row, padded: the column writes are conflict-free
+constexpr int kLowThreads = 256;
+
+// One CTA per 128 consecutive output pixels, K in chunks of 128 taps.  Thread t owns pixel t % 128 and every other
+// group of 4 taps of the chunk: a warp reads one tap of 32 consecutive pixels (consecutive ow: coalesced along the
+// row of x), packs 4 taps per word into a shared tile, and the tile leaves as whole 16-byte pieces of rows of q.
+// Row sums and NaN flags stay in registers across the chunks.
+__global__ void __launch_bounds__(kLowThreads) int8_im2col_quantize_kernel(const float* __restrict__ x, ConvDims d,
+                                                                           const float* __restrict__ scale,
+                                                                           const float* __restrict__ zero_point,
+                                                                           float qmin, float qmax, int off,
+                                                                           int8_t* __restrict__ q,
+                                                                           int* __restrict__ row_sum,
+                                                                           uint8_t* __restrict__ nan_flag) {
+  __shared__ uint32_t tile[kLowPix * kLowWords];
+  __shared__ long long tap_off[kLowK], tap_dh[kLowK], tap_dw[kLowK];  // per tap of the chunk: x offset, row, column
+  __shared__ int part_sum[kLowThreads];
+  __shared__ bool part_nan[kLowThreads];
+  const int t = threadIdx.x, px = t % kLowPix, kq0 = t / kLowPix;
+  const long long m = (long long)blockIdx.x * kLowPix + px;
+  const bool live = m < d.M;
+  long long ih0 = 0, iw0 = 0, org = 0;  // top-left tap of the window and its offset in x
+  if (live) {
+    const long long img = m / d.P, pix = m - img * d.P;
+    const long long oh = pix / d.OW, ow = pix - oh * d.OW;
+    ih0 = oh * d.sh - d.pt;
+    iw0 = ow * d.sw - d.pl;
+    org = img * d.CHW + ih0 * d.W + iw0;
+  }
+  QP p;
+  p.set(__ldg(scale), __ldg(zero_point));
+  p.qmin = qmin;
+  p.qmax = qmax;
+  const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
+  int sum = 0;
+  bool nan = false;
+  for (int k0 = 0; k0 < d.Kp; k0 += kLowK) {
+    const int kc = min(kLowK, d.Kp - k0);
+    if (t < kc) {
+      const int k = k0 + t;
+      long long o = 0, a = 0, b = 0;
+      if (k < d.K) {
+        const int c = k / (d.KH * d.KW), r = k - c * (d.KH * d.KW), kh = r / d.KW, kw = r - kh * d.KW;
+        a = kh * d.dh;
+        b = kw * d.dw;
+        o = c * d.HW + a * d.W + b;
+      }
+      tap_off[t] = o, tap_dh[t] = a, tap_dw[t] = b;
+    }
+    __syncthreads();  // the tap table is written; the previous chunk's tile has been read
+#pragma unroll 4
+    for (int qd = kq0; qd < kc / 4; qd += kLowThreads / kLowPix) {
+      uint32_t packed = 0u;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int kl = 4 * qd + i;
+        int e = 0;  // K padding stays zero
+        if (live && k0 + kl < d.K) {
+          const long long ih = ih0 + tap_dh[kl], iw = iw0 + tap_dw[kl];
+          if ((unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W)
+            e = stored_grid(__ldg(x + org + tap_off[kl]), p, off, nan);
+          else
+            e = pad;
+        }
+        sum += e;
+        packed |= ((uint32_t)e & 0xFFu) << (8 * i);
+      }
+      tile[px * kLowWords + qd] = packed;
+    }
+    __syncthreads();
+    const int pieces = kc / 16;  // 16-byte pieces per row
+    for (int idx = t; idx < kLowPix * pieces; idx += kLowThreads) {
+      const int row = idx / pieces, j = idx - row * pieces;
+      const long long mr = (long long)blockIdx.x * kLowPix + row;
+      if (mr < d.M) {
+        const uint32_t* s = tile + row * kLowWords + 4 * j;
+        *reinterpret_cast<uint4*>(q + mr * d.Kp + k0 + 16 * j) = make_uint4(s[0], s[1], s[2], s[3]);
+      }
+    }
+  }
+  part_sum[t] = sum;
+  part_nan[t] = nan;
+  __syncthreads();
+  if (t < kLowPix && live) {
+    for (int h = 1; h < kLowThreads / kLowPix; ++h) {
+      sum += part_sum[t + h * kLowPix];
+      nan = nan || part_nan[t + h * kLowPix];
+    }
+    row_sum[m] = sum;
+    nan_flag[m] = nan ? 1 : 0;
   }
 }
 
@@ -126,12 +243,14 @@ __device__ __forceinline__ void wgmma_wait_s32(int (&d)[64]) {
 }
 
 // One CTA per 128-row x 128-feature tile of y (row tile fastest: neighbouring CTAs share the weight tile in L2).
+// kNchw = false: out is row-major [M, N].  kNchw = true: out is NCHW [M / P, N, P] (conv2d, P = OH OW pixels per image).
+template <bool kNchw>
 __global__ void __launch_bounds__(kI8Threads, 1)
 int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                         float* __restrict__ out, const int* __restrict__ x_sum, const uint8_t* __restrict__ x_nan,
                         const float* __restrict__ x_scale, const float* __restrict__ x_zero, int x_off,
                         const int* __restrict__ w_sum, const float* __restrict__ w_scale, const int* __restrict__ w_zero,
-                        const float* __restrict__ bias, int M, int N, int K) {
+                        const float* __restrict__ bias, int M, int N, int K, int P) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   I8Smem* sm = reinterpret_cast<I8Smem*>(stage_base + (size_t)kI8Stages * kI8StageBytes);
@@ -187,11 +306,16 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
   const int r0 = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
   long long sa[2];
   bool rnan[2];
+  size_t obase[2];  // NCHW: out offset of (row, feature 0), img N P + p; one division per row
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int m = r0 + 8 * h;
     sa[h] = m < M ? (long long)__ldg(x_sum + m) : 0;
     rnan[h] = m < M && __ldg(x_nan + m) != 0;
+    if constexpr (kNchw) {
+      const int img = m / P;
+      obase[h] = (size_t)img * N * P + (size_t)(m - img * P);
+    }
   }
   int acc[64];
 #pragma unroll
@@ -230,7 +354,8 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
         float y = __double2float_rn((double)I * col.sxw);
         if (bias) y = __fadd_rn(y, col.bias);
         if (rnan[h]) y = __int_as_float(0x7fc00000);
-        out[(size_t)m * N + n] = y;
+        if constexpr (kNchw) out[obase[h] + (size_t)n * P] = y;  // a warp stores 8 consecutive pixels per feature
+        else out[(size_t)m * N + n] = y;
       }
     }
   }
@@ -264,6 +389,95 @@ int launch_rows(const float* x, const float* scale, const float* zero_point, int
   int8_quantize_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, scale, zero_point, per_row, (float)qmin, (float)qmax,
                                                                       grid_offset(qmin), q, row_sum, nan_flag, rows, (int)k,
                                                                       (int)padded_k(k), vec);
+  SB_LAUNCHED();
+  return SB200_OK;
+}
+
+
+// The lowered activations (q, row sums, NaN flags) in the workspace, written by `lower`, then the GEMM into `out`
+// (row-major [M, N], or NCHW with P pixels per image).  Arguments are checked by the caller.
+template <bool kNchw, typename Lower>
+int run_gemm(const char* fn, long long m, long long k, long long n, long long P, int qmin_x, const float* x_scale,
+             const float* x_zero_point, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+             const int32_t* w_zero, const float* bias, float* out, void* workspace, cudaStream_t st, Lower lower) {
+  const I8Layout w = i8_layout(m, k);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
+  int8_t* xq = reinterpret_cast<int8_t*>(ws + w.off_q);
+  int* xsum = reinterpret_cast<int*>(ws + w.off_sum);
+  uint8_t* xnan = ws + w.off_nan;
+  const long long kp = padded_k(k);
+
+  CUtensorMap map_x, map_w;
+  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, xq, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, kI8BK, kI8Rows,
+                   CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, w_q, (uint64_t)kp, (uint64_t)n, (uint64_t)kp, kI8BK, kI8Feat,
+                   CU_TENSOR_MAP_SWIZZLE_128B)) {
+    set_error("%s: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", fn, m, k, n);
+    return SB200_E_CUDA;
+  }
+  if (const int rc = lower(xq, xsum, xnan, st)) return rc;
+  const size_t smem = (size_t)kI8Stages * kI8StageBytes + sizeof(I8Smem) + 1024;
+  static std::atomic<int> attr_done[64];
+  SB_CUDA(ensure_dyn_smem(int8_linear_gemm_kernel<kNchw>, (int)smem, attr_done));
+  const long long tiles = ((m + kI8Rows - 1) / kI8Rows) * ((n + kI8Feat - 1) / kI8Feat);
+  int8_linear_gemm_kernel<kNchw><<<(unsigned)tiles, kI8Threads, smem, st>>>(
+      map_x, map_w, out, xsum, xnan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(w_rowsum),
+      w_scale, reinterpret_cast<const int*>(w_zero), bias, (int)m, (int)n, (int)k, (int)P);
+  SB_LAUNCHED();
+  return SB200_OK;
+}
+
+// Output shape of a conv geometry.  Returns 0, or which rule it breaks: 1 = a size, stride or dilation <= 0, a
+// padding < 0, or a dimension >= 2^31; 2 = an empty output; 3 = M >= 2^31.  K is saturated at 2^17.
+int conv_shape(const sb200_conv2d_geom& g, ConvDims* d) {
+  const int64_t pos[] = {g.n, g.c, g.h, g.w, g.kh, g.kw, g.stride_h, g.stride_w, g.dilation_h, g.dilation_w};
+  const int64_t pads[] = {g.pad_top, g.pad_bottom, g.pad_left, g.pad_right};
+  for (int64_t v : pos)
+    if (v <= 0 || v >= (1LL << 31)) return 1;
+  for (int64_t v : pads)
+    if (v < 0 || v >= (1LL << 31)) return 1;
+  if ((__int128)g.n * g.c * g.h * g.w >= ((__int128)1 << 62)) return 1;
+  const long long oh_num = g.h + g.pad_top + g.pad_bottom - g.dilation_h * (g.kh - 1) - 1;
+  const long long ow_num = g.w + g.pad_left + g.pad_right - g.dilation_w * (g.kw - 1) - 1;
+  if (oh_num < 0 || ow_num < 0) return 2;
+  const long long OH = oh_num / g.stride_h + 1, OW = ow_num / g.stride_w + 1;
+  if ((__int128)g.n * OH * OW >= ((__int128)1 << 31)) return 3;
+  const __int128 K = (__int128)g.c * g.kh * g.kw;
+  d->H = g.h, d->W = g.w, d->HW = g.h * g.w, d->CHW = g.c * g.h * g.w;
+  d->sh = g.stride_h, d->sw = g.stride_w, d->dh = g.dilation_h, d->dw = g.dilation_w;
+  d->pt = g.pad_top, d->pl = g.pad_left;
+  d->OW = OW, d->P = OH * OW, d->M = g.n * OH * OW;
+  d->KH = (int)g.kh, d->KW = (int)g.kw;
+  d->K = K >= kI8MaxK ? (int)kI8MaxK : (int)K;
+  d->Kp = (int)padded_k(d->K);
+  return 0;
+}
+
+// Checks of the conv entry points that come before the range check
+int check_conv(const char* fn, const sb200_conv2d_geom* g, ConvDims* d) {
+  const int rule = conv_shape(*g, d);
+  SB_REQUIRE(rule != 1, "%s: empty or non-positive geometry (n=%lld c=%lld h=%lld w=%lld kernel %lldx%lld stride %lldx%lld "
+             "dilation %lldx%lld padding %lld/%lld/%lld/%lld)", fn, (long long)g->n, (long long)g->c, (long long)g->h,
+             (long long)g->w, (long long)g->kh, (long long)g->kw, (long long)g->stride_h, (long long)g->stride_w,
+             (long long)g->dilation_h, (long long)g->dilation_w, (long long)g->pad_top, (long long)g->pad_bottom,
+             (long long)g->pad_left, (long long)g->pad_right);
+  SB_REQUIRE(rule != 2, "%s: empty output (the dilated kernel does not fit the padded input)", fn);
+  SB_REQUIRE(rule != 3, "%s: too many output pixels (M = n OH OW must be < 2^31)", fn);
+  return SB200_OK;
+}
+
+int check_conv_k(const char* fn, const ConvDims& d) {
+  if (d.K >= kI8MaxK) {
+    set_error("%s: K = c kh kw >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
+    return SB200_E_UNSUPPORTED;
+  }
+  return SB200_OK;
+}
+
+int launch_im2col(const float* x, const ConvDims& d, const float* scale, const float* zero_point, int qmin, int qmax,
+                  int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st) {
+  int8_im2col_quantize_kernel<<<(unsigned)((d.M + kLowPix - 1) / kLowPix), kLowThreads, 0, st>>>(
+      x, d, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, row_sum, nan_flag);
   SB_LAUNCHED();
   return SB200_OK;
 }
@@ -309,37 +523,60 @@ int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_
               (long long)k);
     return SB200_E_UNSUPPORTED;
   }
-  const I8Layout w = i8_layout(m, k);
-  unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
   if (workspace_bytes < sb200_int8_linear_workspace_bytes(m, k)) {  // covers any alignment of the base
     set_error("sb200_int8_linear: workspace too small (%zu bytes, need %zu)", workspace_bytes,
               sb200_int8_linear_workspace_bytes(m, k));
     return SB200_E_WORKSPACE;
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  int8_t* xq = reinterpret_cast<int8_t*>(ws + w.off_q);
-  int* xsum = reinterpret_cast<int*>(ws + w.off_sum);
-  uint8_t* xnan = ws + w.off_nan;
-  const long long kp = padded_k(k);
+  return run_gemm<false>("sb200_int8_linear", m, k, n, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero,
+                         bias, out, workspace, (cudaStream_t)stream,
+                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                           return launch_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, xq, xsum, xnan, m, k, st);
+                         });
+}
 
-  CUtensorMap map_x, map_w;
-  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, xq, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, kI8BK, kI8Rows,
-                   CU_TENSOR_MAP_SWIZZLE_128B) ||
-      !make_map_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, w_q, (uint64_t)kp, (uint64_t)n, (uint64_t)kp, kI8BK, kI8Feat,
-                   CU_TENSOR_MAP_SWIZZLE_128B)) {
-    set_error("sb200_int8_linear: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", (long long)m, (long long)k,
-              (long long)n);
-    return SB200_E_CUDA;
+size_t sb200_int8_conv2d_workspace_bytes(const sb200_conv2d_geom* geom) {
+  ConvDims d;
+  if (!geom || conv_shape(*geom, &d) != 0) return 0;
+  return sb200_int8_linear_workspace_bytes(d.M, d.K);
+}
+
+int sb200_int8_im2col_quantize(const float* x, const sb200_conv2d_geom* geom, const float* scale,
+                               const float* zero_point, int qmin, int qmax, int8_t* q, int32_t* row_sum,
+                               uint8_t* nan_flag, void* stream) {
+  const char* fn = "sb200_int8_im2col_quantize";
+  SB_REQUIRE(x && geom && scale && zero_point && q && row_sum && nan_flag, "%s: null pointer argument", fn);
+  ConvDims d;
+  if (const int rc = check_conv(fn, geom, &d)) return rc;
+  if (const int rc = check_range(fn, qmin, qmax)) return rc;
+  SB_REQUIRE(aligned16(q), "%s: q must be 16-byte aligned", fn);
+  if (const int rc = check_conv_k(fn, d)) return rc;
+  return launch_im2col(x, d, scale, zero_point, qmin, qmax, q, reinterpret_cast<int*>(row_sum), nan_flag,
+                       (cudaStream_t)stream);
+}
+
+int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float* x_scale, const float* x_zero_point,
+                      int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                      const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  const char* fn = "sb200_int8_conv2d";
+  SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out && workspace,
+             "%s: null pointer argument", fn);
+  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
+  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
+  ConvDims d;
+  if (const int rc = check_conv(fn, geom, &d)) return rc;
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
+  SB_REQUIRE(aligned16(w_q), "%s: w_q must be 16-byte aligned", fn);
+  if (const int rc = check_conv_k(fn, d)) return rc;
+  const size_t need = sb200_int8_conv2d_workspace_bytes(geom);
+  if (workspace_bytes < need) {
+    set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
+    return SB200_E_WORKSPACE;
   }
-  if (const int rc = launch_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, xq, xsum, xnan, m, k, st)) return rc;
-  const size_t smem = (size_t)kI8Stages * kI8StageBytes + sizeof(I8Smem) + 1024;
-  static std::atomic<int> attr_done[64];
-  SB_CUDA(ensure_dyn_smem(int8_linear_gemm_kernel, (int)smem, attr_done));
-  const long long tiles = ((m + kI8Rows - 1) / kI8Rows) * ((n + kI8Feat - 1) / kI8Feat);
-  int8_linear_gemm_kernel<<<(unsigned)tiles, kI8Threads, smem, st>>>(map_x, map_w, out, xsum, xnan, x_scale, x_zero_point,
-                                                                     grid_offset(qmin_x), reinterpret_cast<const int*>(w_rowsum),
-                                                                     w_scale, reinterpret_cast<const int*>(w_zero), bias,
-                                                                     (int)m, (int)n, (int)k);
-  SB_LAUNCHED();
-  return SB200_OK;
+  return run_gemm<true>(fn, d.M, d.K, c_out, d.P, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
+                        out, workspace, (cudaStream_t)stream,
+                        [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                          return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st);
+                        });
 }

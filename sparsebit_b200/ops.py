@@ -685,6 +685,16 @@ def int8_quantize_rows(x, scale, zero_point, qmin, qmax):
 _int8_ws = {}
 
 
+def _int8_workspace(device, nbytes):
+    """The integer path's workspace of (device, current stream), grown on demand and shared by its entry points."""
+    key = (device, torch.cuda.current_stream(device).cuda_stream)
+    ws = _int8_ws.get(key)
+    if ws is None or ws.numel() < nbytes:
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        _int8_ws[key] = ws
+    return ws
+
+
 def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias=None, k=None):
     """``y = s_x s_w[n] sum_k v_x v_w + bias`` on the int8 tensor cores (sb200_int8_linear): the fake-quant linear of
     per-tensor activations [qmin, qmax] with the weights stored by ``int8_quantize_rows`` (w_q int8 [N, Kp], w_rowsum
@@ -704,16 +714,95 @@ def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     m = x.numel() // k
     out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
     ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
-    key = (x.device, torch.cuda.current_stream(x.device).cuda_stream)
-    ws = _int8_ws.get(key)
-    if ws is None or ws.numel() < ws_bytes:
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        _int8_ws[key] = ws
+    ws = _int8_workspace(x.device, ws_bytes)
     with torch.cuda.device(x.device):
         check(lib.sb200_int8_linear(x.data_ptr(), x_scale.data_ptr(), x_zero_point.data_ptr(), int(qmin), int(qmax),
                                     w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                     bias.data_ptr() if bias is not None else None, out.data_ptr(), m, k, n, ws.data_ptr(),
                                     ws_bytes, _stream(x)))
+    return out
+
+
+def _pair(v):
+    return (int(v), int(v)) if isinstance(v, int) else tuple(int(e) for e in v)
+
+
+def conv2d_geometry(x_shape, kernel_size, stride=1, padding=0, dilation=1):
+    """``sb200_conv2d_geom`` of an [N, C, H, W] input.  ``padding``: an int, (pad_h, pad_w) or
+    (top, bottom, left, right)."""
+    n, c, h, w = (int(d) for d in x_shape)
+    kh, kw = _pair(kernel_size)
+    sh, sw = _pair(stride)
+    dh, dw = _pair(dilation)
+    pad = _pair(padding)
+    if len(pad) == 2:
+        pad = (pad[0], pad[0], pad[1], pad[1])
+    if len(pad) != 4:
+        raise SparsebitB200Error(f"conv2d padding must be an int, 2 or 4 ints (got {padding!r})")
+    return _lib.Conv2dGeom(n, c, h, w, kh, kw, sh, sw, dh, dw, *pad)
+
+
+def conv2d_output_hw(g):
+    """(OH, OW) of a ``Conv2dGeom`` (may be < 1 for a kernel that does not fit)."""
+    oh = (g.h + g.pad_top + g.pad_bottom - g.dilation_h * (g.kh - 1) - 1) // g.stride_h + 1
+    ow = (g.w + g.pad_left + g.pad_right - g.dilation_w * (g.kw - 1) - 1) // g.stride_w + 1
+    return oh, ow
+
+
+def int8_im2col_quantize(x, kernel_size, scale, zero_point, qmin, qmax, stride=1, padding=0, dilation=1):
+    """The lowered integer grid of a conv input (sb200_int8_im2col_quantize): ``x`` [N, C, H, W] fp32 -> ``(q, row_sum,
+    nan)`` with q int8 [M, Kp], M = N OH OW (m = (n OH + oh) OW + ow), K = C KH KW (k = (c KH + kh) KW + kw), Kp =
+    round_up(K, 16); element (m, k) is the stored grid value of the tap, padding taps store rint(zp) - offset, the K
+    padding is zero; row_sum int32 [M]; nan bool [M] (the window holds a NaN).  ``scale`` / ``zero_point``: 1 element."""
+    lib = _lib.load()
+    _req(x, "data"), _req(scale, "scale"), _req(zero_point, "zero_point")
+    if x.dim() != 4:
+        raise SparsebitB200Error("int8_im2col_quantize: data must be [N, C, H, W]")
+    if scale.numel() != 1 or zero_point.numel() != 1:
+        raise SparsebitB200Error("int8_im2col_quantize: the activation qparams are per-tensor (1 element each)")
+    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
+    oh, ow = conv2d_output_hw(g)
+    m = g.n * max(oh, 0) * max(ow, 0)
+    q = torch.empty(max(m, 1), int8_padded_k(g.c * g.kh * g.kw), dtype=torch.int8, device=x.device)
+    row_sum = torch.empty(max(m, 1), dtype=torch.int32, device=x.device)
+    nan = torch.empty(max(m, 1), dtype=torch.bool, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_im2col_quantize(x.data_ptr(), ctypes.byref(g), scale.data_ptr(), zero_point.data_ptr(),
+                                             int(qmin), int(qmax), q.data_ptr(), row_sum.data_ptr(), nan.data_ptr(),
+                                             _stream(x)))
+    return q, row_sum, nan
+
+
+def int8_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, bias=None, stride=1,
+                padding=0, dilation=1):
+    """The fake-quant conv2d (groups = 1) on the int8 tensor cores (sb200_int8_conv2d): ``x`` [N, C, H, W] fp32 is
+    lowered to its integer grid and multiplied with the weights stored by ``int8_quantize_rows`` from
+    ``weight.reshape(C_out, -1)`` (w_q int8 [C_out, Kp], w_rowsum int32, w_scale fp32, w_zero int32 [C_out]), as in
+    ``int8_linear``.  Returns fp32 [N, C_out, OH, OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left,
+    right)."""
+    lib = _lib.load()
+    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
+    if bias is not None:
+        _req(bias, "bias")
+    if x.dim() != 4:
+        raise SparsebitB200Error("int8_conv2d: data must be [N, C, H, W]")
+    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
+    k = g.c * g.kh * g.kw
+    if w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
+        raise SparsebitB200Error(f"int8_conv2d: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {int8_padded_k(k)}]")
+    n = w_q.shape[0]
+    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"int8_conv2d: w_rowsum / w_scale / w_zero / bias need {n} elements")
+    oh, ow = conv2d_output_hw(g)
+    out = torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
+    ws = _int8_workspace(x.device, max(ws_bytes, 16))
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_conv2d(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(), x_zero_point.data_ptr(), int(qmin),
+                                    int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
+                                    bias.data_ptr() if bias is not None else None, out.data_ptr(), n, ws.data_ptr(),
+                                    ws.numel(), _stream(x)))
     return out
 
 

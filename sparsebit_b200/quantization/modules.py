@@ -72,12 +72,11 @@ def _qparams(quantizer, x):
     return scale.detach().float().reshape(-1), zero_point.detach().float().reshape(-1)
 
 
-def int8_ineligibility(qlinear):
-    """Why ``QLinearInt8.from_qlinear`` cannot convert ``qlinear`` (None when it can)."""
-    if not isinstance(qlinear, QLinear):
-        return f"expected a QLinear, got {type(qlinear).__name__}"
-    n = qlinear.weight.shape[0]
-    for role, q in (("input", qlinear.input_quantizer), ("weight", qlinear.weight_quantizer)):
+def _int8_quantizer_ineligibility(mod):
+    """The quantizer rules of the integer path, shared by ``QLinear`` and ``QConv2d``: ``mod`` has an input and a
+    weight quantizer and a weight whose axis 0 is the output channels."""
+    n = mod.weight.shape[0]
+    for role, q in (("input", mod.input_quantizer), ("weight", mod.weight_quantizer)):
         if q is None:
             return f"the {role} quantizer is missing"
         if q.fake_fused:
@@ -90,12 +89,12 @@ def int8_ineligibility(qlinear):
             return f"the {role} quantizer is {q.TYPE}, whose forward is not the plain fake-quant op"
         if q.bit > 8:
             return f"the {role} quantizer has {q.bit} bits (at most 8)"
-    aq, wq = qlinear.input_quantizer, qlinear.weight_quantizer
+    aq, wq = mod.input_quantizer, mod.weight_quantizer
     if aq.is_perchannel:
         return "the input quantizer is per-channel (the integer path needs one activation scale)"
     if wq.is_perchannel and wq.qdesc.ch_axis != 0:
         return f"the weight quantizer is per-channel along axis {wq.qdesc.ch_axis} (needs the output channels, axis 0)"
-    for role, q, x in (("input", aq, None), ("weight", wq, qlinear.weight)):
+    for role, q, x in (("input", aq, None), ("weight", wq, mod.weight)):
         scale, zero_point = _qparams(q, x)
         if scale.numel() not in ((1, n) if role == "weight" else (1,)) or zero_point.numel() != scale.numel():
             return f"the {role} quantizer holds {scale.numel()} scales"
@@ -109,6 +108,27 @@ def int8_ineligibility(qlinear):
             except AssertionError as e:
                 return f"the {role} quantizer: {e}"
     return None
+
+
+def int8_ineligibility(qlinear):
+    """Why ``QLinearInt8.from_qlinear`` cannot convert ``qlinear`` (None when it can)."""
+    if not isinstance(qlinear, QLinear):
+        return f"expected a QLinear, got {type(qlinear).__name__}"
+    return _int8_quantizer_ineligibility(qlinear)
+
+
+def _int8_weight_rows(wq, weight):
+    """The weights on the stored integer grid, one row per output channel (``weight.reshape(N, -1)``):
+    ``(w_q, w_rowsum, w_scale, w_zero)`` as ``ops.int8_linear`` / ``ops.int8_conv2d`` take them.  A weight row holding a
+    NaN gets ``w_scale = NaN``, which makes its output channel NaN, as in the fake-quant op."""
+    rows = weight.detach().reshape(weight.shape[0], -1)
+    n = rows.shape[0]
+    ws, wz = _qparams(wq, weight)
+    wqmin, wqmax = wq.qdesc.qrange
+    w_q, w_sum, w_nan = ops.int8_quantize_rows(rows.float().contiguous(), ws.contiguous(), wz.contiguous(), wqmin, wqmax)
+    w_scale = torch.where(w_nan, torch.full_like(w_sum, float("nan"), dtype=torch.float32), ws.expand(n))
+    w_zero = (torch.round(wz) - ops.int8_grid_offset(wqmin)).to(torch.int32).expand(n)
+    return w_q, w_sum, w_scale, w_zero
 
 
 class QLinearInt8(nn.Module):
@@ -140,15 +160,9 @@ class QLinearInt8(nn.Module):
         n, k = weight.shape
         mod = cls(k, n, weight.device)
         with torch.no_grad():
-            ws, wz = _qparams(wq, qlinear.weight)
+            for buf, v in zip((mod.w_q, mod.w_rowsum, mod.w_scale, mod.w_zero), _int8_weight_rows(wq, qlinear.weight)):
+                buf.copy_(v)
             xs, xz = _qparams(aq, None)
-            wqmin, wqmax = wq.qdesc.qrange
-            w_q, w_sum, w_nan = ops.int8_quantize_rows(weight.float().contiguous(), ws.contiguous(), wz.contiguous(), wqmin, wqmax)
-            mod.w_q.copy_(w_q)
-            mod.w_rowsum.copy_(w_sum)
-            # a weight row holding a NaN makes its output column NaN, as in the fake-quant matmul
-            mod.w_scale.copy_(torch.where(w_nan, torch.full_like(w_sum, float("nan"), dtype=torch.float32), ws.expand(n)))
-            mod.w_zero.copy_((torch.round(wz) - ops.int8_grid_offset(wqmin)).to(torch.int32).expand(n))
             mod.scale.copy_(xs.reshape(1))
             mod.zero_point.copy_(xz.reshape(1))
             if qlinear.bias is not None:
@@ -166,6 +180,115 @@ class QLinearInt8(nn.Module):
 
     def extra_repr(self):
         return f"in_features={self.in_features}, out_features={self.out_features}, qrange=[{self.qmin}, {self.qmax}]"
+
+
+def _pair(v):
+    return (int(v), int(v)) if isinstance(v, int) else tuple(int(e) for e in v)
+
+
+def resolve_conv_padding(padding, kernel_size, dilation=1, stride=1):
+    """The (top, bottom, left, right) zero padding of a conv2d's ``padding`` argument: an int, a (pad_h, pad_w) pair,
+    ``'valid'`` or ``'same'`` (total d (k - 1) per dimension, the odd one on the bottom / right, as ``F.conv2d``).
+    Raises ``ValueError`` when it does not resolve to four non-negative ints."""
+    if isinstance(padding, str):
+        if padding == "valid":
+            return (0, 0, 0, 0)
+        if padding != "same":
+            raise ValueError(f"padding {padding!r} is neither 'valid' nor 'same'")
+        if any(s != 1 for s in _pair(stride)):
+            raise ValueError("padding 'same' needs stride 1")
+        pads = []
+        for k, d in zip(_pair(kernel_size), _pair(dilation)):
+            total = d * (k - 1)
+            pads += [total // 2, total - total // 2]
+        return tuple(pads)
+    try:
+        ph, pw = _pair(padding)
+    except (TypeError, ValueError):
+        raise ValueError(f"padding {padding!r} is not an int or a pair of ints") from None
+    if ph < 0 or pw < 0:
+        raise ValueError(f"padding {padding!r} is negative")
+    return (ph, ph, pw, pw)
+
+
+def int8_conv_ineligibility(qconv):
+    """Why ``QConv2dInt8.from_qconv2d`` cannot convert ``qconv`` (None when it can)."""
+    if not isinstance(qconv, QConv2d):
+        return f"expected a QConv2d, got {type(qconv).__name__}"
+    reason = _int8_quantizer_ineligibility(qconv)
+    if reason is not None:
+        return reason
+    kw = qconv.fwd_kwargs
+    if kw["groups"] != 1:
+        return f"the conv has groups = {kw['groups']} (the integer path runs groups = 1 only)"
+    try:
+        resolve_conv_padding(kw["padding"], qconv.weight.shape[2:], kw["dilation"], kw["stride"])
+    except ValueError as e:
+        return f"the conv's {e}"
+    return None
+
+
+class QConv2dInt8(nn.Module):
+    """Inference-only replacement of a calibrated ``QConv2d`` (groups = 1): the fake-quant conv2d computed on the
+    integer grid by ``ops.int8_conv2d`` -- the input lowered to its int8 grid in one pass, exact int8 x int8 sums on the
+    tensor cores, zero points removed in int64, then s_x s_w[n] I + bias, written NCHW.  Built by ``from_qconv2d``; the
+    weights (``weight.reshape(C_out, -1)``) are quantized once at conversion.  Takes [N, C, H, W] or unbatched
+    [C, H, W]; fp16 input is up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps
+    ``QConv2d``."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device):
+        super().__init__()
+        self.in_channels, self.out_channels = int(in_channels), int(out_channels)
+        self.kernel_size, self.stride, self.dilation = tuple(kernel_size), tuple(stride), tuple(dilation)
+        self.padding = tuple(padding)  # (top, bottom, left, right)
+        kp = ops.int8_padded_k(in_channels * self.kernel_size[0] * self.kernel_size[1])
+        self.register_buffer("w_q", torch.zeros(out_channels, kp, dtype=torch.int8, device=device))
+        self.register_buffer("w_rowsum", torch.zeros(out_channels, dtype=torch.int32, device=device))
+        self.register_buffer("w_scale", torch.zeros(out_channels, dtype=torch.float32, device=device))
+        self.register_buffer("w_zero", torch.zeros(out_channels, dtype=torch.int32, device=device))
+        self.register_buffer("scale", torch.ones(1, dtype=torch.float32, device=device))
+        self.register_buffer("zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+        self.register_buffer("bias", None)
+        self.qmin, self.qmax = -128, 127
+
+    @classmethod
+    def from_qconv2d(cls, qconv):
+        reason = int8_conv_ineligibility(qconv)
+        if reason is not None:
+            raise ValueError(f"QConv2dInt8.from_qconv2d: {reason}")
+        aq, wq = qconv.input_quantizer, qconv.weight_quantizer
+        kw = qconv.fwd_kwargs
+        weight = qconv.weight.detach()
+        c_out, c_in, kh, kwd = weight.shape
+        padding = resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
+        mod = cls(c_in, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]), weight.device)
+        with torch.no_grad():
+            for buf, v in zip((mod.w_q, mod.w_rowsum, mod.w_scale, mod.w_zero), _int8_weight_rows(wq, qconv.weight)):
+                buf.copy_(v)
+            xs, xz = _qparams(aq, None)
+            mod.scale.copy_(xs.reshape(1))
+            mod.zero_point.copy_(xz.reshape(1))
+            if qconv.bias is not None:
+                mod.bias = qconv.bias.detach().float().clone().contiguous()
+        mod.qmin, mod.qmax = aq.qdesc.qrange
+        return mod
+
+    def forward(self, x_in):
+        if torch.is_grad_enabled() and x_in.requires_grad:
+            raise RuntimeError("QConv2dInt8 is inference-only and has no backward; run it under torch.no_grad() or "
+                               "keep QConv2d for training")
+        x = x_in.float() if x_in.dtype != torch.float32 else x_in
+        unbatched = x.dim() == 3
+        if unbatched:
+            x = x.unsqueeze(0)
+        y = ops.int8_conv2d(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
+                            self.w_scale, self.w_zero, self.kernel_size, self.bias, self.stride, self.padding,
+                            self.dilation)
+        return y.squeeze(0) if unbatched else y
+
+    def extra_repr(self):
+        return (f"{self.in_channels}, {self.out_channels}, kernel_size={self.kernel_size}, stride={self.stride}, "
+                f"padding={self.padding}, dilation={self.dilation}, qrange=[{self.qmin}, {self.qmax}]")
 
 
 class QReLU(QuantOpr):
