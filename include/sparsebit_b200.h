@@ -490,6 +490,41 @@ int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float
                       const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* ---- (5c) Integer-grid inference of a calibrated activation x activation matmul (int8 wgmma, sm_90a) ----
+ * New; the reference's MatMul (modules/matmul.py) multiplies two fake-quantised activations (a QIdentity carrier in
+ * front of each input) with an fp32 torch.matmul.  With both operands per-tensor the product is
+ *   y[b, m, n] = s_a * s_b * sum_k v_a[b, m, k] * v_b[b, k, n],   v = clamp(round(x / s) + Z, qmin, qmax) - Z
+ * over `batch` independent problems: a is [batch, m, k]; b is [batch, n, k] when b_k_major = 1 (the k^T of attention:
+ * its rows go through the row quantizer as they lie) or [batch, k, n] when b_k_major = 0 (the column quantizer
+ * transposes it).  All tensors fp32 contiguous, scales / zero points device scalars, the stored grid, range rules and
+ * K < 2^17 as in (5).
+ *
+ * Argument checks, all before any CUDA call: null pointers, an empty operand, batch m or batch n >= 2^31 and the range
+ * rules of the integer linear are SB200_E_INVALID, as is a q not 16-byte aligned; K >= 2^17 is SB200_E_UNSUPPORTED; a
+ * workspace that is too small is SB200_E_WORKSPACE.
+ *
+ * sb200_int8_quantize_cols: the transposing quantizer alone.  x [batch, k, n] fp32 -> q [batch, n, Kp] s8 (16-byte
+ * aligned, Kp = round_up(K, 16), padding zero): element (b, n, k) is the stored grid value (as in
+ * sb200_int8_quantize_rows) of x[b, k, n]; col_sum[batch n] int32 = sum of the stored row of q; nan_flag[batch n] uint8
+ * = 1 if the column holds a NaN (stored as 0).  +-inf clamp to qmin / qmax.  scale / zero_point: device, one float each.
+ *
+ * sb200_int8_matmul: out [batch, m, n] fp32 (overwritten).  Epilogue: the zero points are removed exactly in int64,
+ * I = sum a b - Z_b sum_k a - Z_a sum_k b + K Z_a Z_b, then y = fp32(fp64(I) * (fp64(s_a) * fp64(s_b))).  A NaN in row
+ * m of a[b] makes row m of out[b] NaN, a NaN in column n of b[b] makes column n of out[b] NaN (as the fake-quant matmul
+ * does); no other batch entry is touched.  Exact against the fp64 product of the fake-quant operands when both scales
+ * are powers of two, within 2^-21 * (|f_a| @ |f_b|) otherwise.  Deterministic, no state between calls
+ * (graph-capturable).
+ * workspace: sb200_int8_matmul_workspace_bytes(batch, m, k, n) bytes (a pure function; 0 for arguments the matmul
+ * rejects). */
+int sb200_int8_quantize_cols(const float* x, const float* scale, const float* zero_point, int qmin, int qmax,
+                             int8_t* q, int32_t* col_sum, uint8_t* nan_flag, int64_t batch, int64_t k, int64_t n,
+                             void* stream);
+size_t sb200_int8_matmul_workspace_bytes(int64_t batch, int64_t m, int64_t k, int64_t n);
+int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float* a_scale, const float* a_zero_point,
+                      int qmin_a, int qmax_a, const float* b_scale, const float* b_zero_point, int qmin_b, int qmax_b,
+                      float* out, int64_t batch, int64_t m, int64_t k, int64_t n, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);

@@ -23,6 +23,13 @@
 // every tap of every window as one s8 row per output pixel (the same grid as the row quantizer); a padding tap is the
 // grid point of the fake-quant input's zero padding, v = 0, i.e. rint(zp) - off on the stored grid, so the epilogue's
 // correction stays exact with the real K.  The GEMM then writes NCHW: out[(img N + n) P + p], m = img P + p, P = OH OW.
+//
+// MatMul.  A calibrated activation x activation matmul a [B, M, K] @ b [B, K, N] has two per-tensor operands and no
+// bias: y = s_a s_b I.  Both are quantized on the fly into [rows, Kp] s8: a, and a b that lies K-major in memory
+// ([B, N, K], the k^T of attention), by the row quantizer; a b that lies N-major ([B, K, N]) by the column quantizer,
+// which transposes through shared memory.  The batched GEMM kernel runs the same ring and wgmma loop as the linear
+// (i8_produce / i8_consume below) over 3-D tensor maps (Kp, rows, batch), so that a tile never reaches into the next
+// batch entry, with its own epilogue: per-row sum_k a, per-column sum_k b, both NaN flags, one scale product.
 #include "tc_common.cuh"
 
 namespace sb200 {
@@ -44,10 +51,22 @@ struct I8Col {
   int zw;
   float bias;
 };
-struct I8Smem {
+struct I8Ring {
   uint64_t full[kI8Stages];
   uint64_t empty[kI8Stages];
+};
+struct I8Smem {
+  I8Ring ring;
   I8Col col[kI8Feat];
+};
+// the matmul's per-column terms: both scales and zero points are scalars
+struct I8MmCol {
+  long long cn;  // K Z_a Z_b - Z_a sum_k b
+  int nan;       // the column of b holds a NaN
+};
+struct I8MmSmem {
+  I8Ring ring;
+  I8MmCol col[kI8Feat];
 };
 
 static inline int grid_offset(int qmin) { return qmin >= 0 ? 128 : 0; }
@@ -111,6 +130,102 @@ __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __
   if (lane == 0) {
     row_sum[row] = sum;
     nan_flag[row] = any_nan ? 1 : 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------- column quantizer
+constexpr int kColN = 64;                 // columns of x (rows of q) per CTA
+constexpr int kColK = 128;                // K per chunk: one 128-byte line of each row of q
+constexpr int kColWords = kColK / 4 + 1;  // words per tile row, padded: the transposing writes are conflict-free
+constexpr int kColThreads = 256;
+
+// x [batch, K, N] -> q [batch, N, Kp]: the row quantizer's grid, transposed.  One CTA per 64 columns of one batch entry,
+// K in chunks of 128.  A thread owns 4 neighbouring columns for the whole of K and, per chunk, two groups of 4 k: it
+// reads a 4 x 4 block (vec: one 16-byte load per k, 8 lanes covering a 128-byte line of the row; otherwise guarded
+// scalar loads), packs the 4 k of each column into one word of a shared tile, and the tile leaves as whole 16-byte
+// pieces of rows of q.  Column sums and NaN flags stay in registers across the chunks.
+__global__ void __launch_bounds__(kColThreads) int8_quantize_cols_kernel(const float* __restrict__ x, const float* __restrict__ scale,
+                                                                         const float* __restrict__ zero_point, float qmin,
+                                                                         float qmax, int off, int8_t* __restrict__ q,
+                                                                         int* __restrict__ col_sum,
+                                                                         uint8_t* __restrict__ nan_flag, int tiles_n, int K,
+                                                                         int N, int Kp, int vec) {
+  __shared__ uint32_t tile[kColN * kColWords];
+  __shared__ int part_sum[kColThreads / 64][kColN];
+  __shared__ int part_nan[kColThreads / 64][kColN];
+  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  const long long b = blockIdx.x / (unsigned)tiles_n;
+  const int n0 = (int)(blockIdx.x % (unsigned)tiles_n) * kColN;
+  const int nl = 4 * (8 * (warp & 1) + (lane >> 2));  // first of the thread's 4 columns, within the tile
+  const int kslot = 4 * (warp >> 1) + (lane & 3);     // the thread's k groups of a chunk: kslot and kslot + 16
+  const int n = n0 + nl;
+  const float* xb = x + b * K * N;
+  int8_t* qb = q + b * N * Kp;
+  QP p;
+  p.set(__ldg(scale), __ldg(zero_point));
+  p.qmin = qmin;
+  p.qmax = qmax;
+  int sum[4] = {0, 0, 0, 0};
+  bool nan[4] = {false, false, false, false};
+  for (int k0 = 0; k0 < Kp; k0 += kColK) {
+    const int kc = min(kColK, Kp - k0);
+#pragma unroll
+    for (int it = 0; it < 2; ++it) {
+      const int kq = kslot + 16 * it, kk = k0 + 4 * kq;
+      if (4 * kq >= kc) continue;
+      float v[4][4];  // [k][column]
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float* xr = xb + (long long)(kk + i) * N + n;
+        if (vec && kk + i < K && n < N) {
+          const float4 f = ld_stream4(reinterpret_cast<const float4*>(xr));
+          v[i][0] = f.x, v[i][1] = f.y, v[i][2] = f.z, v[i][3] = f.w;
+        } else {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) v[i][j] = (kk + i < K && n + j < N) ? ld_stream1(xr + j) : 0.f;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        uint32_t packed = 0u;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          int e = 0;  // K padding stays zero
+          if (kk + i < K && n + j < N) e = stored_grid(v[i][j], p, off, nan[j]);
+          sum[j] += e;
+          packed |= ((uint32_t)e & 0xFFu) << (8 * i);
+        }
+        tile[(nl + j) * kColWords + kq] = packed;
+      }
+    }
+    __syncthreads();
+    const int pieces = kc / 16;  // 16-byte pieces per row
+    for (int idx = t; idx < kColN * pieces; idx += kColThreads) {
+      const int row = idx / pieces, j = idx - row * pieces;
+      if (n0 + row < N) {
+        const uint32_t* s = tile + row * kColWords + 4 * j;
+        *reinterpret_cast<uint4*>(qb + (long long)(n0 + row) * Kp + k0 + 16 * j) = make_uint4(s[0], s[1], s[2], s[3]);
+      }
+    }
+    __syncthreads();  // the tile has been read
+  }
+  // a column's k groups are spread over 4 lanes of 4 warps
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    int sj = sum[j], fj = nan[j] ? 1 : 0;
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      sj += __shfl_xor_sync(0xffffffffu, sj, o);
+      fj |= __shfl_xor_sync(0xffffffffu, fj, o);
+    }
+    if ((lane & 3) == 0) part_sum[warp >> 1][nl + j] = sj, part_nan[warp >> 1][nl + j] = fj;
+  }
+  __syncthreads();
+  if (t < kColN && n0 + t < N) {
+    int sj = 0, fj = 0;
+    for (int h = 0; h < kColThreads / 64; ++h) sj += part_sum[h][t], fj |= part_nan[h][t];
+    col_sum[b * N + n0 + t] = sj;
+    nan_flag[b * N + n0 + t] = fj ? 1 : 0;
   }
 }
 
@@ -242,6 +357,59 @@ __device__ __forceinline__ void wgmma_wait_s32(int (&d)[64]) {
   for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
+// ---- the mainloop shared by the linear / conv2d kernel and the batched matmul kernel
+// thread 0, before the CTA-wide barrier
+__device__ __forceinline__ void i8_ring_init(I8Ring* ring, const CUtensorMap* map_a, const CUtensorMap* map_b) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(map_a) : "memory");
+  asm volatile("prefetch.tensormap [%0];" ::"l"(map_b) : "memory");
+  for (int s = 0; s < kI8Stages; ++s) {
+    mbar_init(&ring->full[s], 1);
+    mbar_init(&ring->empty[s], 8);  // one arrival per consumer warp
+  }
+  mbar_fence_init();
+}
+// TMA producer (one thread): rows m0.. of map_a and n0.. of map_b, 128 K per stage.  kBatched: the maps are
+// (Kp, rows, batch) and `batch` picks the matrix.
+template <bool kBatched>
+__device__ __forceinline__ void i8_produce(unsigned char* stage_base, I8Ring* ring, const CUtensorMap* map_a,
+                                           const CUtensorMap* map_b, int m0, int n0, int batch, int num_kb) {
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % kI8Stages;
+    const uint32_t ph = (uint32_t)(kb / kI8Stages) & 1u;
+    mbar_wait_relaxed(&ring->empty[s], ph ^ 1u, 0);
+    unsigned char* st = stage_base + (size_t)s * kI8StageBytes;
+    mbar_expect_tx(&ring->full[s], (uint32_t)kI8StageBytes);
+    if constexpr (kBatched) {
+      tma_load_3d(st, map_a, kb * kI8BK, m0, batch, &ring->full[s]);
+      tma_load_3d(st + kI8TileBytes, map_b, kb * kI8BK, n0, batch, &ring->full[s]);
+    } else {
+      tma_load_2d(st, map_a, kb * kI8BK, m0, &ring->full[s]);
+      tma_load_2d(st + kI8TileBytes, map_b, kb * kI8BK, n0, &ring->full[s]);
+    }
+  }
+}
+// Consumer warpgroup wg: acc = rows 64 wg .. 64 wg + 63 of the a tile times the 128 rows of the b tile, over all of K.
+__device__ __forceinline__ void i8_consume(int (&acc)[64], uint32_t stage0, I8Ring* ring, int wg, int lane, int num_kb) {
+#pragma unroll
+  for (int j = 0; j < 64; ++j) acc[j] = 0;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % kI8Stages;
+    const uint32_t ph = (uint32_t)(kb / kI8Stages) & 1u;
+    mbar_wait_relaxed(&ring->full[s], ph, 0);
+    const uint32_t xa = stage0 + (uint32_t)s * kI8StageBytes;
+    const uint64_t da = gmma_desc_sw128(xa + (uint32_t)wg * (64 * kI8BK)), db = gmma_desc_sw128(xa + kI8TileBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) wgmma_m64n128k32_s8(acc, da + 2 * j, db + 2 * j, kb > 0 || j > 0);  // +32 B per k32
+    wgmma_commit();
+    // one group stays in flight: the stage of the previous k block is free once this wait returns
+    wgmma_wait_s32<1>(acc);
+    __syncwarp();
+    if (kb > 0 && lane == 0) mbar_arrive(&ring->empty[(kb + kI8Stages - 1) % kI8Stages]);
+  }
+  wgmma_wait_s32<0>(acc);
+}
+
 // One CTA per 128-row x 128-feature tile of y (row tile fastest: neighbouring CTAs share the weight tile in L2).
 // kNchw = false: out is row-major [M, N].  kNchw = true: out is NCHW [M / P, N, P] (conv2d, P = OH OW pixels per image).
 template <bool kNchw>
@@ -259,30 +427,12 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
   const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kI8Rows, n0 = (int)(blockIdx.x / (unsigned)tiles_m) * kI8Feat;
   const int num_kb = (K + kI8BK - 1) / kI8BK;
 
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    for (int s = 0; s < kI8Stages; ++s) {
-      mbar_init(&sm->full[s], 1);
-      mbar_init(&sm->empty[s], 8);  // one arrival per consumer warp
-    }
-    mbar_fence_init();
-  }
+  if (threadIdx.x == 0) i8_ring_init(&sm->ring, &map_x, &map_w);
   __syncthreads();
 
   if (warp < 4) {
     reg_dec<40>();
-    if (threadIdx.x == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kI8Stages;
-        const uint32_t ph = (uint32_t)(kb / kI8Stages) & 1u;
-        mbar_wait_relaxed(&sm->empty[s], ph ^ 1u, 0);
-        unsigned char* st = stage_base + (size_t)s * kI8StageBytes;
-        mbar_expect_tx(&sm->full[s], (uint32_t)kI8StageBytes);
-        tma_load_2d(st, &map_x, kb * kI8BK, m0, &sm->full[s]);
-        tma_load_2d(st + kI8TileBytes, &map_w, kb * kI8BK, n0, &sm->full[s]);
-      }
-    }
+    if (threadIdx.x == 0) i8_produce<false>(stage_base, &sm->ring, &map_x, &map_w, m0, n0, 0, num_kb);
     return;
   }
   reg_inc<232>();
@@ -318,24 +468,7 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
     }
   }
   int acc[64];
-#pragma unroll
-  for (int j = 0; j < 64; ++j) acc[j] = 0;
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % kI8Stages;
-    const uint32_t ph = (uint32_t)(kb / kI8Stages) & 1u;
-    mbar_wait_relaxed(&sm->full[s], ph, 0);
-    const uint32_t xa = stage0 + (uint32_t)s * kI8StageBytes;
-    const uint64_t da = gmma_desc_sw128(xa + (uint32_t)wg * (64 * kI8BK)), db = gmma_desc_sw128(xa + kI8TileBytes);
-    wgmma_fence();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) wgmma_m64n128k32_s8(acc, da + 2 * j, db + 2 * j, kb > 0 || j > 0);  // +32 B per k32
-    wgmma_commit();
-    // one group stays in flight: the stage of the previous k block is free once this wait returns
-    wgmma_wait_s32<1>(acc);
-    __syncwarp();
-    if (kb > 0 && lane == 0) mbar_arrive(&sm->empty[(kb + kI8Stages - 1) % kI8Stages]);
-  }
-  wgmma_wait_s32<0>(acc);
+  i8_consume(acc, stage0, &sm->ring, wg, lane, num_kb);
   asm volatile("bar.sync 1, 256;" ::: "memory");  // sm->col written by both consumer warpgroups
 
   // acc[j]: row r0 + 8 ((j >> 1) & 1), feature n0 + 8 (j >> 2) + 2 q + (j & 1)
@@ -356,6 +489,87 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
         if (rnan[h]) y = __int_as_float(0x7fc00000);
         if constexpr (kNchw) out[obase[h] + (size_t)n * P] = y;  // a warp stores 8 consecutive pixels per feature
         else out[(size_t)m * N + n] = y;
+      }
+    }
+  }
+}
+
+// One CTA per 128-row x 128-column tile of one batch entry's out [M, N] (row tile fastest, batch slowest).  The maps are
+// (Kp, rows, batch): rows past M / N of the entry are zero-filled, never the next entry's.
+__global__ void __launch_bounds__(kI8Threads, 1)
+int8_matmul_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                        float* __restrict__ out, const int* __restrict__ a_sum, const uint8_t* __restrict__ a_nan,
+                        const int* __restrict__ b_sum, const uint8_t* __restrict__ b_nan, const float* __restrict__ a_scale,
+                        const float* __restrict__ a_zero, int a_off, const float* __restrict__ b_scale,
+                        const float* __restrict__ b_zero, int b_off, int M, int N, int K, int vec2) {
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  I8MmSmem* sm = reinterpret_cast<I8MmSmem*>(stage_base + (size_t)kI8Stages * kI8StageBytes);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned tiles_m = (unsigned)(M + kI8Rows - 1) / kI8Rows, tiles_n = (unsigned)(N + kI8Feat - 1) / kI8Feat;
+  const unsigned tile_n = blockIdx.x / tiles_m;
+  const int m0 = (int)(blockIdx.x % tiles_m) * kI8Rows, n0 = (int)(tile_n % tiles_n) * kI8Feat;
+  const int batch = (int)(tile_n / tiles_n);
+  const int num_kb = (K + kI8BK - 1) / kI8BK;
+
+  if (threadIdx.x == 0) i8_ring_init(&sm->ring, &map_a, &map_b);
+  __syncthreads();
+
+  if (warp < 4) {
+    reg_dec<40>();
+    if (threadIdx.x == 0) i8_produce<true>(stage_base, &sm->ring, &map_a, &map_b, m0, n0, batch, num_kb);
+    return;
+  }
+  reg_inc<232>();
+  const int wg = (warp - 4) >> 2;
+  // the epilogue's per-column and per-row terms are fetched while the ring fills
+  const double sab = (double)__ldg(a_scale) * (double)__ldg(b_scale);
+  const long long za = (long long)rintf(__ldg(a_zero)) - a_off, zb = (long long)rintf(__ldg(b_zero)) - b_off;
+  const size_t arow = (size_t)batch * M, brow = (size_t)batch * N;
+  if (threadIdx.x - 128 < (unsigned)kI8Feat) {
+    const int i = threadIdx.x - 128, n = n0 + i;
+    I8MmCol c{0, 0};
+    if (n < N) {
+      c.cn = (long long)K * za * zb - za * (long long)__ldg(b_sum + brow + n);
+      c.nan = __ldg(b_nan + brow + n);
+    }
+    sm->col[i] = c;
+  }
+  const int q = lane & 3;
+  const int r0 = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+  long long sa[2];
+  bool rnan[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = r0 + 8 * h;
+    sa[h] = m < M ? zb * (long long)__ldg(a_sum + arow + m) : 0;
+    rnan[h] = m < M && __ldg(a_nan + arow + m) != 0;
+  }
+  int acc[64];
+  i8_consume(acc, smem_u32(stage_base), &sm->ring, wg, lane, num_kb);
+  asm volatile("bar.sync 1, 256;" ::: "memory");  // sm->col written by both consumer warpgroups
+
+  // acc[j]: row r0 + 8 ((j >> 1) & 1), column n0 + 8 (j >> 2) + 2 q + (j & 1)
+  const float qnan = __int_as_float(0x7fc00000);
+#pragma unroll
+  for (int c = 0; c < 16; ++c) {
+    const int i = 8 * c + 2 * q, n = n0 + i;
+    if (n >= N) continue;
+    const I8MmCol c0 = sm->col[i], c1 = sm->col[i + 1];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = r0 + 8 * h;
+      if (m >= M) continue;
+      float y0 = __double2float_rn((double)((long long)acc[4 * c + 2 * h] - sa[h] + c0.cn) * sab);
+      float y1 = __double2float_rn((double)((long long)acc[4 * c + 2 * h + 1] - sa[h] + c1.cn) * sab);
+      if (rnan[h] || c0.nan) y0 = qnan;
+      if (rnan[h] || c1.nan) y1 = qnan;
+      float* o = out + (arow + m) * N + n;
+      if (vec2) {  // N is even: the pair is in range and 8-byte aligned
+        *reinterpret_cast<float2*>(o) = make_float2(y0, y1);
+      } else {
+        o[0] = y0;
+        if (n + 1 < N) o[1] = y1;
       }
     }
   }
@@ -423,6 +637,20 @@ int run_gemm(const char* fn, long long m, long long k, long long n, long long P,
   int8_linear_gemm_kernel<kNchw><<<(unsigned)tiles, kI8Threads, smem, st>>>(
       map_x, map_w, out, xsum, xnan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(w_rowsum),
       w_scale, reinterpret_cast<const int*>(w_zero), bias, (int)m, (int)n, (int)k, (int)P);
+  SB_LAUNCHED();
+  return SB200_OK;
+}
+
+// Workspace of the matmul: the lowered a (batch m rows) and, 1024-aligned behind it, the lowered b (batch n rows)
+size_t matmul_b_offset(long long batch, long long m, long long k) { return align_up(i8_layout(batch * m, k).total, 1024); }
+
+int launch_cols(const float* x, const float* scale, const float* zero_point, int qmin, int qmax, int8_t* q, int* col_sum,
+                uint8_t* nan_flag, long long batch, long long k, long long n, cudaStream_t st) {
+  const int vec = (n % 4 == 0) && aligned16(x);
+  const long long tiles_n = (n + kColN - 1) / kColN;
+  int8_quantize_cols_kernel<<<(unsigned)(batch * tiles_n), kColThreads, 0, st>>>(
+      x, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, col_sum, nan_flag, (int)tiles_n, (int)k, (int)n,
+      (int)padded_k(k), vec);
   SB_LAUNCHED();
   return SB200_OK;
 }
@@ -579,4 +807,89 @@ int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float
                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
                           return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st);
                         });
+}
+
+size_t sb200_int8_matmul_workspace_bytes(int64_t batch, int64_t m, int64_t k, int64_t n) {
+  if (batch <= 0 || m <= 0 || k <= 0 || n <= 0) return 0;
+  if ((__int128)batch * m >= (1LL << 31) || (__int128)batch * n >= (1LL << 31) || k >= kI8MaxK) return 0;
+  return matmul_b_offset(batch, m, k) + i8_layout(batch * n, k).total + 1024;  // + the alignment of the base
+}
+
+int sb200_int8_quantize_cols(const float* x, const float* scale, const float* zero_point, int qmin, int qmax, int8_t* q,
+                             int32_t* col_sum, uint8_t* nan_flag, int64_t batch, int64_t k, int64_t n, void* stream) {
+  const char* fn = "sb200_int8_quantize_cols";
+  SB_REQUIRE(x && scale && zero_point && q && col_sum && nan_flag, "%s: null pointer argument", fn);
+  SB_REQUIRE(batch > 0 && k > 0 && n > 0, "%s: empty operand (batch=%lld K=%lld N=%lld)", fn, (long long)batch, (long long)k,
+             (long long)n);
+  SB_REQUIRE((__int128)batch * n < (1LL << 31), "%s: too many columns (batch N = %lld x %lld must be < 2^31)", fn,
+             (long long)batch, (long long)n);
+  if (const int rc = check_range(fn, qmin, qmax)) return rc;
+  SB_REQUIRE(aligned16(q), "%s: q must be 16-byte aligned", fn);
+  if (k >= kI8MaxK) {
+    set_error("%s: K = %lld, the integer path supports K < 2^17", fn, (long long)k);
+    return SB200_E_UNSUPPORTED;
+  }
+  return launch_cols(x, scale, zero_point, qmin, qmax, q, reinterpret_cast<int*>(col_sum), nan_flag, batch, k, n,
+                     (cudaStream_t)stream);
+}
+
+int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float* a_scale, const float* a_zero_point,
+                      int qmin_a, int qmax_a, const float* b_scale, const float* b_zero_point, int qmin_b, int qmax_b,
+                      float* out, int64_t batch, int64_t m, int64_t k, int64_t n, void* workspace, size_t workspace_bytes,
+                      void* stream) {
+  const char* fn = "sb200_int8_matmul";
+  SB_REQUIRE(a && b && a_scale && a_zero_point && b_scale && b_zero_point && out && workspace, "%s: null pointer argument",
+             fn);
+  SB_REQUIRE(batch > 0 && m > 0 && k > 0 && n > 0, "%s: empty operand (batch=%lld M=%lld K=%lld N=%lld)", fn,
+             (long long)batch, (long long)m, (long long)k, (long long)n);
+  SB_REQUIRE((__int128)batch * m < (1LL << 31) && (__int128)batch * n < (1LL << 31),
+             "%s: dimension too large (batch M and batch N must be < 2^31)", fn);
+  const __int128 tiles = (__int128)batch * ((m + kI8Rows - 1) / kI8Rows) * ((n + kI8Feat - 1) / kI8Feat);
+  SB_REQUIRE(tiles < (1LL << 31), "%s: dimension too large (%lld x %lld x %lld output tiles)", fn, (long long)batch,
+             (long long)((m + kI8Rows - 1) / kI8Rows), (long long)((n + kI8Feat - 1) / kI8Feat));
+  if (const int rc = check_range(fn, qmin_a, qmax_a)) return rc;
+  if (const int rc = check_range(fn, qmin_b, qmax_b)) return rc;
+  if (k >= kI8MaxK) {
+    set_error("%s: K = %lld, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn, (long long)k);
+    return SB200_E_UNSUPPORTED;
+  }
+  const size_t need = sb200_int8_matmul_workspace_bytes(batch, m, k, n);
+  if (workspace_bytes < need) {  // covers any alignment of the base
+    set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
+    return SB200_E_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const I8Layout la = i8_layout(batch * m, k), lb = i8_layout(batch * n, k);
+  unsigned char* wa = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
+  unsigned char* wb = wa + matmul_b_offset(batch, m, k);
+  int8_t* aq = reinterpret_cast<int8_t*>(wa + la.off_q);
+  int8_t* bq = reinterpret_cast<int8_t*>(wb + lb.off_q);
+  int* asum = reinterpret_cast<int*>(wa + la.off_sum);
+  int* bsum = reinterpret_cast<int*>(wb + lb.off_sum);
+  const long long kp = padded_k(k);
+  CUtensorMap map_a, map_b;
+  if (!make_map_3d(&map_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, aq, (uint64_t)kp, (uint64_t)m, (uint64_t)batch, (uint64_t)kp, kI8BK,
+                   kI8Rows, CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_3d(&map_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, bq, (uint64_t)kp, (uint64_t)n, (uint64_t)batch, (uint64_t)kp, kI8BK,
+                   kI8Feat, CU_TENSOR_MAP_SWIZZLE_128B)) {
+    set_error("%s: cuTensorMapEncodeTiled failed (batch=%lld M=%lld K=%lld N=%lld)", fn, (long long)batch, (long long)m,
+              (long long)k, (long long)n);
+    return SB200_E_CUDA;
+  }
+  if (const int rc = launch_rows(a, a_scale, a_zero_point, 0, qmin_a, qmax_a, aq, asum, wa + la.off_nan, batch * m, k, st))
+    return rc;
+  if (const int rc = b_k_major ? launch_rows(b, b_scale, b_zero_point, 0, qmin_b, qmax_b, bq, bsum, wb + lb.off_nan,
+                                             batch * n, k, st)
+                               : launch_cols(b, b_scale, b_zero_point, qmin_b, qmax_b, bq, bsum, wb + lb.off_nan, batch, k,
+                                             n, st))
+    return rc;
+  const size_t smem = (size_t)kI8Stages * kI8StageBytes + sizeof(I8MmSmem) + 1024;
+  static std::atomic<int> attr_done[64];
+  SB_CUDA(ensure_dyn_smem(int8_matmul_gemm_kernel, (int)smem, attr_done));
+  const int vec2 = (n % 2 == 0) && (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
+  int8_matmul_gemm_kernel<<<(unsigned)tiles, kI8Threads, smem, st>>>(
+      map_a, map_b, out, asum, wa + la.off_nan, bsum, wb + lb.off_nan, a_scale, a_zero_point, grid_offset(qmin_a), b_scale,
+      b_zero_point, grid_offset(qmin_b), (int)m, (int)n, (int)k, vec2);
+  SB_LAUNCHED();
+  return SB200_OK;
 }

@@ -37,6 +37,13 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(
+          smem_u32(dst)),
+      "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
+      : "memory");
+}
 // mbarrier wait with an optional back-off between polls (sb200_gptq4_set_wait_backoff; 0 = poll continuously)
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, int backoff_ns) {
   for (;;) {
@@ -163,6 +170,21 @@ static inline bool make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const v
   const cuuint32_t box[2] = {box_inner, box_outer};
   const cuuint32_t estr[2] = {1, 1};
   return enc(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// `batch` matrices of `rows` x `inner` elements, row_bytes apart, back to back; a box is box_inner x box_rows of one
+// matrix, so rows past the end of a matrix are zero-filled instead of read from the next one
+static inline bool make_map_3d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t rows,
+                               uint64_t batch, uint64_t row_bytes, uint32_t box_inner, uint32_t box_rows,
+                               CUtensorMapSwizzle sw) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return false;
+  const cuuint64_t dims[3] = {inner, rows, batch};
+  const cuuint64_t strides[2] = {row_bytes, rows * row_bytes};
+  const cuuint32_t box[3] = {box_inner, box_rows, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  return enc(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 

@@ -723,6 +723,67 @@ def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     return out
 
 
+def int8_quantize_cols(x, scale, zero_point, qmin, qmax):
+    """Transposed integer grid of ``x`` [..., K, N] (sb200_int8_quantize_cols): returns ``(q, col_sum, nan)`` with q int8
+    [..., N, Kp], q[..., n, k] = the ``int8_quantize_rows`` grid value of x[..., k, n], the padding to Kp =
+    round_up(K, 16) zero; col_sum int32 [..., N]; nan bool [..., N].  ``scale`` / ``zero_point``: 1 element."""
+    lib = _lib.load()
+    _req(x, "data"), _req(scale, "scale"), _req(zero_point, "zero_point")
+    if x.dim() < 2:
+        raise SparsebitB200Error("int8_quantize_cols: data must be [..., K, N]")
+    if scale.numel() != 1 or zero_point.numel() != 1:
+        raise SparsebitB200Error("int8_quantize_cols: the qparams are per-tensor (1 element each)")
+    lead, (k, n) = tuple(x.shape[:-2]), x.shape[-2:]
+    batch = x.numel() // (k * n)
+    q = torch.empty(lead + (n, int8_padded_k(k)), dtype=torch.int8, device=x.device)
+    col_sum = torch.empty(lead + (n,), dtype=torch.int32, device=x.device)
+    nan = torch.empty(lead + (n,), dtype=torch.bool, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_quantize_cols(x.data_ptr(), scale.data_ptr(), zero_point.data_ptr(), int(qmin), int(qmax),
+                                           q.data_ptr(), col_sum.data_ptr(), nan.data_ptr(), batch, k, n, _stream(x)))
+    return q, col_sum, nan
+
+
+def _is_k_major(b):
+    """``b`` [..., K, N] is the transposed view of a contiguous [..., N, K] tensor."""
+    return b.stride(-2) == 1 and b.transpose(-2, -1).is_contiguous()
+
+
+def int8_matmul(a, a_scale, a_zero_point, a_qrange, b, b_scale, b_zero_point, b_qrange):
+    """``y = s_a s_b sum_k v_a v_b`` on the int8 tensor cores (sb200_int8_matmul): the ``torch.matmul`` of two per-tensor
+    fake-quantized activations, ``a`` [..., M, K] with ``(a_scale, a_zero_point, a_qrange = (qmin, qmax))`` and ``b``
+    [..., K, N] likewise, both fp32 and quantized on the fly.  Leading dimensions broadcast as in ``torch.matmul``
+    (copied only where they really broadcast).  A ``b`` that is the transposed view of a contiguous [..., N, K] tensor
+    (``k.transpose(-2, -1)``) is read as it lies; any other non-contiguous operand is made contiguous.  Returns fp32
+    [..., M, N]."""
+    lib = _lib.load()
+    for t, name in ((a, "a"), (b, "b")):
+        if not isinstance(t, torch.Tensor) or t.dim() < 2:
+            raise SparsebitB200Error(f"int8_matmul: {name} must be a tensor with at least 2 dimensions")
+    _req(a_scale, "a_scale"), _req(a_zero_point, "a_zero_point"), _req(b_scale, "b_scale"), _req(b_zero_point, "b_zero_point")
+    if any(t.numel() != 1 for t in (a_scale, a_zero_point, b_scale, b_zero_point)):
+        raise SparsebitB200Error("int8_matmul: the qparams of both operands are per-tensor (1 element each)")
+    (m, k), (kb, n) = a.shape[-2:], b.shape[-2:]
+    if k != kb:
+        raise SparsebitB200Error(f"int8_matmul: a is {tuple(a.shape)}, b is {tuple(b.shape)} (inner dimensions differ)")
+    lead = torch.broadcast_shapes(a.shape[:-2], b.shape[:-2])
+    a = a.expand(lead + (m, k)).reshape(-1, m, k).contiguous()
+    b = b.expand(lead + (k, n)).reshape(-1, k, n)
+    k_major = _is_k_major(b)
+    b = b.transpose(-2, -1) if k_major else b.contiguous()  # [batch, N, K] as it lies, or [batch, K, N]
+    _req(a, "a"), _req(b, "b")
+    batch = a.shape[0]
+    out = torch.empty(lead + (m, n), dtype=torch.float32, device=a.device)
+    ws_bytes = int(lib.sb200_int8_matmul_workspace_bytes(batch, m, k, n))
+    ws = _int8_workspace(a.device, max(ws_bytes, 16))
+    with torch.cuda.device(a.device):
+        check(lib.sb200_int8_matmul(a.data_ptr(), b.data_ptr(), int(k_major), a_scale.data_ptr(), a_zero_point.data_ptr(),
+                                    int(a_qrange[0]), int(a_qrange[1]), b_scale.data_ptr(), b_zero_point.data_ptr(),
+                                    int(b_qrange[0]), int(b_qrange[1]), out.data_ptr(), batch, m, k, n, ws.data_ptr(),
+                                    ws.numel(), _stream(a)))
+    return out
+
+
 def _pair(v):
     return (int(v), int(v)) if isinstance(v, int) else tuple(int(e) for e in v)
 

@@ -72,41 +72,58 @@ def _qparams(quantizer, x):
     return scale.detach().float().reshape(-1), zero_point.detach().float().reshape(-1)
 
 
+def _int8_plain_qdq_reason(role, q):
+    """Why quantizer ``q`` does not run the plain <= 8-bit fake-quant op that the integer path restates (None if it does)."""
+    if q is None:
+        return f"the {role} quantizer is missing"
+    if q.fake_fused:
+        return f"the {role} quantizer is fake_fused"
+    if not q.use_quant:
+        return f"the {role} quantizer is not enabled"
+    if q.export_onnx:
+        return f"the {role} quantizer is in export_onnx mode"
+    if q.TYPE.lower() not in _PLAIN_QDQ_TYPES:
+        return f"the {role} quantizer is {q.TYPE}, whose forward is not the plain fake-quant op"
+    if q.bit > 8:
+        return f"the {role} quantizer has {q.bit} bits (at most 8)"
+    return None
+
+
+def _int8_qparams_reason(role, q, x, counts):
+    """Why the qparams of ``q`` do not fit the integer path: a scale count outside ``counts``, a zero point outside the
+    integer range, or a TensorRT backend with a non-zero zero point (None if they fit)."""
+    scale, zero_point = _qparams(q, x)
+    if scale.numel() not in counts or zero_point.numel() != scale.numel():
+        return f"the {role} quantizer holds {scale.numel()} scales"
+    qmin, qmax = q.qdesc.qrange
+    z = torch.round(zero_point)
+    if bool(((z < qmin) | (z > qmax) | torch.isnan(z)).any()):
+        return f"the {role} zero point lies outside [{qmin}, {qmax}]"
+    if q.backend == Backend.TENSORRT:
+        try:
+            check_trt_symmetric(zero_point)
+        except AssertionError as e:
+            return f"the {role} quantizer: {e}"
+    return None
+
+
 def _int8_quantizer_ineligibility(mod):
     """The quantizer rules of the integer path, shared by ``QLinear`` and ``QConv2d``: ``mod`` has an input and a
     weight quantizer and a weight whose axis 0 is the output channels."""
     n = mod.weight.shape[0]
     for role, q in (("input", mod.input_quantizer), ("weight", mod.weight_quantizer)):
-        if q is None:
-            return f"the {role} quantizer is missing"
-        if q.fake_fused:
-            return f"the {role} quantizer is fake_fused"
-        if not q.use_quant:
-            return f"the {role} quantizer is not enabled"
-        if q.export_onnx:
-            return f"the {role} quantizer is in export_onnx mode"
-        if q.TYPE.lower() not in _PLAIN_QDQ_TYPES:
-            return f"the {role} quantizer is {q.TYPE}, whose forward is not the plain fake-quant op"
-        if q.bit > 8:
-            return f"the {role} quantizer has {q.bit} bits (at most 8)"
+        reason = _int8_plain_qdq_reason(role, q)
+        if reason is not None:
+            return reason
     aq, wq = mod.input_quantizer, mod.weight_quantizer
     if aq.is_perchannel:
         return "the input quantizer is per-channel (the integer path needs one activation scale)"
     if wq.is_perchannel and wq.qdesc.ch_axis != 0:
         return f"the weight quantizer is per-channel along axis {wq.qdesc.ch_axis} (needs the output channels, axis 0)"
-    for role, q, x in (("input", aq, None), ("weight", wq, mod.weight)):
-        scale, zero_point = _qparams(q, x)
-        if scale.numel() not in ((1, n) if role == "weight" else (1,)) or zero_point.numel() != scale.numel():
-            return f"the {role} quantizer holds {scale.numel()} scales"
-        qmin, qmax = q.qdesc.qrange
-        z = torch.round(zero_point)
-        if bool(((z < qmin) | (z > qmax) | torch.isnan(z)).any()):
-            return f"the {role} zero point lies outside [{qmin}, {qmax}]"
-        if q.backend == Backend.TENSORRT:
-            try:
-                check_trt_symmetric(zero_point)
-            except AssertionError as e:
-                return f"the {role} quantizer: {e}"
+    for role, q, x, counts in (("input", aq, None, (1,)), ("weight", wq, mod.weight, (1, n))):
+        reason = _int8_qparams_reason(role, q, x, counts)
+        if reason is not None:
+            return reason
     return None
 
 
@@ -305,3 +322,83 @@ class QIdentity(QuantOpr):
 
     def forward(self, x_in):
         return self.input_quantizer(x_in)
+
+
+class QMatMul(nn.Module):
+    """The activation x activation matmul (modules/matmul.py MatMul) together with the two carriers that the reference
+    inserts in front of its inputs: ``left`` and ``right`` are ``QIdentity`` operators, each owning the input quantizer
+    of one operand.  The module itself has no quantizer attributes, so calibration sees the two carriers."""
+
+    def __init__(self, org_module=None):
+        super().__init__()
+        self.left, self.right = QIdentity(), QIdentity()
+
+    def build_quantizer(self, a_cfg, backend=Backend.VIRTUAL):
+        self.left.build_quantizer(a_cfg, backend=backend)
+        self.right.build_quantizer(a_cfg, backend=backend)
+        return self
+
+    def set_quant(self, w_quant=False, a_quant=False):
+        self.left.set_quant(w_quant, a_quant)
+        self.right.set_quant(w_quant, a_quant)
+
+    def forward(self, x_left, x_right):
+        return torch.matmul(self.left(x_left), self.right(x_right))
+
+
+def int8_matmul_ineligibility(qmatmul):
+    """Why ``QMatMulInt8.from_qmatmul`` cannot convert ``qmatmul`` (None when it can)."""
+    if not isinstance(qmatmul, QMatMul):
+        return f"expected a QMatMul, got {type(qmatmul).__name__}"
+    for role, q in (("left", qmatmul.left.input_quantizer), ("right", qmatmul.right.input_quantizer)):
+        reason = _int8_plain_qdq_reason(role, q)
+        if reason is not None:
+            return reason
+        if q.is_perchannel:
+            return f"the {role} quantizer is per-channel (the integer matmul needs one scale per operand)"
+        reason = _int8_qparams_reason(role, q, None, (1,))
+        if reason is not None:
+            return reason
+    return None
+
+
+class QMatMulInt8(nn.Module):
+    """Inference-only replacement of a calibrated ``QMatMul``: the matmul of the two fake-quant operands computed on the
+    integer grid by ``ops.int8_matmul`` -- both operands quantized on the fly, exact int8 x int8 sums on the tensor
+    cores, zero points removed in int64, then s_left s_right I.  Built by ``from_qmatmul``.  Operands have at least 2
+    dimensions and broadcast as in ``torch.matmul``; fp16 input is up-cast and the output is fp32, as in the fake-quant
+    op.  There is no backward: QAT keeps ``QMatMul``."""
+
+    def __init__(self, device):
+        super().__init__()
+        for side in ("left", "right"):
+            self.register_buffer(f"{side}_scale", torch.ones(1, dtype=torch.float32, device=device))
+            self.register_buffer(f"{side}_zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+        self.left_qrange, self.right_qrange = (-128, 127), (-128, 127)
+
+    @classmethod
+    def from_qmatmul(cls, qmatmul):
+        reason = int8_matmul_ineligibility(qmatmul)
+        if reason is not None:
+            raise ValueError(f"QMatMulInt8.from_qmatmul: {reason}")
+        lq, rq = qmatmul.left.input_quantizer, qmatmul.right.input_quantizer
+        (ls, lz), (rs, rz) = _qparams(lq, None), _qparams(rq, None)
+        mod = cls(ls.device)
+        with torch.no_grad():
+            for buf, v in ((mod.left_scale, ls), (mod.left_zero_point, lz), (mod.right_scale, rs), (mod.right_zero_point, rz)):
+                buf.copy_(v.reshape(1))
+        mod.left_qrange, mod.right_qrange = tuple(lq.qdesc.qrange), tuple(rq.qdesc.qrange)
+        return mod
+
+    def forward(self, x_left, x_right):
+        if torch.is_grad_enabled() and (x_left.requires_grad or x_right.requires_grad):
+            raise RuntimeError("QMatMulInt8 is inference-only and has no backward; run it under torch.no_grad() or "
+                               "keep QMatMul for training")
+        if x_left.dim() < 2 or x_right.dim() < 2:
+            raise ValueError(f"QMatMulInt8 takes operands with at least 2 dimensions (got {x_left.dim()}-D and "
+                             f"{x_right.dim()}-D); 1-D operands are not supported")
+        return ops.int8_matmul(x_left.float(), self.left_scale, self.left_zero_point, self.left_qrange,
+                               x_right.float(), self.right_scale, self.right_zero_point, self.right_qrange)
+
+    def extra_repr(self):
+        return f"left_qrange={list(self.left_qrange)}, right_qrange={list(self.right_qrange)}"
