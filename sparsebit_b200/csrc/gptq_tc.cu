@@ -58,9 +58,11 @@ __global__ void __launch_bounds__(256) gptq_split_kernel(const float* __restrict
   amax = red[0];
 #pragma unroll
   for (int i = 1; i < 8; ++i) amax = fmaxf(amax, red[i]);
-  // scaled row max in [2^14, 2^15): fp16 never overflows, the low part keeps as many bits as possible
+  // scaled row max in [2^14, 2^15): fp16 never overflows, the low part keeps as many bits as possible.  e >= -126 (as
+  // the decode kernel clamps its exponent) keeps 2^-e and 2^e finite normal numbers for rows with max |x| < 2^-112:
+  // below 2^-113, 2^-e would overflow to +inf and turn the whole output row into NaN (0 * inf, inf - inf)
   int e = 0;
-  if (amax > 0.f && amax < __int_as_float(0x7f800000)) e = ilogbf(amax) - 14;
+  if (amax > 0.f && amax < __int_as_float(0x7f800000)) e = max(ilogbf(amax) - 14, -126);
   const float down = ldexpf(1.f, -e);
   if (tid == 0) rowscale[m] = ldexpf(1.f, e);
   const int nchunk = K >> 3;
