@@ -511,8 +511,38 @@ def mask_apply_qdq_perchannel(w, mask, scale, zero_point, qmin, qmax, ch_axis=0,
     return out
 
 
+# ----------------------------------------------------------------------------- per-stream workspaces
+class _StreamWorkspaces:
+    """Scratch buffers of one family of entry points, one per key (device, stream[, kind]), grown on demand.
+
+    A CUDA graph captured on a stream keeps the raw address of the workspace its kernels used.  So a workspace used
+    while its stream is capturing is pinned: when a later, larger call outgrows it, it moves to ``retired`` and stays
+    allocated for the life of the process instead of going back to the caching allocator, which would hand it to the
+    next allocation on the stream for every replay to overwrite.  An unpinned workspace is replaced and freed as
+    before, so eager-only use holds one workspace per key."""
+
+    def __init__(self):
+        self.live = {}     # key -> uint8 tensor
+        self.pinned = set()  # keys whose live workspace a captured graph holds
+        self.retired = {}  # key -> [outgrown workspaces captured graphs hold]
+
+    def get(self, key, device, nbytes):
+        ws = self.live.get(key)
+        if ws is None or ws.numel() < nbytes:
+            if key in self.pinned:
+                self.retired.setdefault(key, []).append(ws)
+                self.pinned.discard(key)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+            self.live[key] = ws
+        with torch.cuda.device(device):
+            if torch.cuda.is_current_stream_capturing():
+                self.pinned.add(key)
+        return ws
+
+
 # ----------------------------------------------------------------------------- GPTQ
-_gptq_ws = {}
+_gptq_workspaces = _StreamWorkspaces()
+_gptq_ws = _gptq_workspaces.live
 
 
 class _Gptq4Options(ctypes.Structure):  # include/sparsebit_b200.h sb200_gptq4_options
@@ -543,11 +573,7 @@ def gptq4_matmul(x, qweight, out, scales, zeros, group_size=0, impl=None, chunk_
     ws_bytes = int(lib.sb200_gptq4_workspace_bytes(m, k, n, int(group_size)))
     ws = None
     if ws_bytes:
-        key = (x.device, torch.cuda.current_stream(x.device).cuda_stream)
-        ws = _gptq_ws.get(key)
-        if ws is None or ws.numel() < ws_bytes:
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-            _gptq_ws[key] = ws
+        ws = _gptq_workspaces.get((x.device, torch.cuda.current_stream(x.device).cuda_stream), x.device, ws_bytes)
     with torch.cuda.device(x.device):
         if impl is None and not chunk_k and not static_weights:
             check(lib.sb200_gptq4_matmul(x.data_ptr(), qweight.data_ptr(), out.data_ptr(), scales.data_ptr(), zeros.data_ptr(),
@@ -609,10 +635,7 @@ def gptq4_linear_f16(x, qweight, scales, zeros, bias=None, group_size=0, static_
     out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float16, device=x.device)
     ws_bytes = int(lib.sb200_gptq4_linear_f16_workspace_bytes(m, k, n, int(group_size)))
     key = (x.device, torch.cuda.current_stream(x.device).cuda_stream, "f16")
-    ws = _gptq_ws.get(key)
-    if ws is None or ws.numel() < ws_bytes:
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        _gptq_ws[key] = ws
+    ws = _gptq_workspaces.get(key, x.device, ws_bytes)
     state = None
     if single_launch and m <= 32:
         skey = key[:2]
@@ -682,17 +705,18 @@ def int8_quantize_rows(x, scale, zero_point, qmin, qmax):
     return q, row_sum, nan
 
 
-_int8_ws = {}
+_int8_workspaces = _StreamWorkspaces()
+_int8_ws = _int8_workspaces.live
 
 
 def _int8_workspace(device, nbytes):
-    """The integer path's workspace of (device, current stream), grown on demand and shared by its entry points."""
-    key = (device, torch.cuda.current_stream(device).cuda_stream)
-    ws = _int8_ws.get(key)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        _int8_ws[key] = ws
-    return ws
+    """The integer path's workspace of (device, current stream), grown on demand and shared by its entry points.
+
+    A workspace used during CUDA graph capture is pinned: a captured graph keeps writing the lowered activations to its
+    address on every replay, so when a larger eager call outgrows it (a prefill after a captured decode step) it is
+    retired, kept allocated, rather than freed to the caching allocator.  Workspaces never used under capture are
+    simply replaced (see _StreamWorkspaces)."""
+    return _int8_workspaces.get((device, torch.cuda.current_stream(device).cuda_stream), device, nbytes)
 
 
 def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias=None, k=None):
@@ -886,10 +910,7 @@ def gptq_matmul_dgrad(grad_out, qweight, grad_in, scales, zeros, bits, group_siz
         raise SparsebitB200Error("grad_in and grad_out must have the same number of rows")
     ws_bytes = int(lib.sb200_gptq_dgrad_workspace_bytes(m, k, n, int(bits), int(group_size)))
     key = (grad_out.device, torch.cuda.current_stream(grad_out.device).cuda_stream, "dgrad")
-    ws = _gptq_ws.get(key)
-    if ws is None or ws.numel() < ws_bytes:
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=grad_out.device)
-        _gptq_ws[key] = ws
+    ws = _gptq_workspaces.get(key, grad_out.device, ws_bytes)
     with torch.cuda.device(grad_out.device):
         check(lib.sb200_gptq_matmul_dgrad(grad_out.data_ptr(), qweight.data_ptr(), grad_in.data_ptr(), scales.data_ptr(),
                                           zeros.data_ptr(), m, k, n, qweight.shape[0], int(bits), int(group_size), int(impl or 0),
