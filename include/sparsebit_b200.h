@@ -525,6 +525,32 @@ int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float
                       float* out, int64_t batch, int64_t m, int64_t k, int64_t n, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* ---- (5d) Integer-grid inference of a calibrated grouped / depthwise QConv2d (direct int8 kernel, sm_90a) ----
+ * New; the reference's QConv2d with groups > 1 fake-quantises x and W and runs a grouped F.conv2d.  With C_g = c /
+ * groups input channels and C_out / groups output channels per group, g(n) = n / (c_out / groups):
+ *   y[img, n, oh, ow] = fp32(fp64(I) * (fp64(s_x) * fp64(s_w[n])))  (+ bias[n] in fp32)
+ *   I = sum over the C_g channels of group g(n) and the kh x kw taps of (v_x - Z_x)(v_w[n] - Z_w[n])
+ * computed exactly in int32 / int64 by one kernel that quantizes its input tile (stored grid as in (5), padding taps
+ * at the zero point) into shared memory; no workspace.  The epilogue is that of (5) operation for operation, so that a
+ * group's output is bit-identical to sb200_int8_conv2d run on that group's channel slice and weight rows.
+ *
+ * x [n, c, h, w] fp32 contiguous, geometry as in (5b); out [n, c_out, OH, OW] fp32 NCHW (overwritten).  The weights
+ * are sb200_int8_quantize_rows of weight.reshape(c_out, -1): w_q [c_out, round_up(K_g, 16)] s8 with K_g = C_g kh kw in
+ * the order (c, kh, kw), w_rowsum / w_scale / w_zero [c_out]; bias [c_out] or NULL.  The zero points must lie in
+ * their integer ranges.  A NaN in input channel c makes NaN every output of group g(c) whose window covers it, and no
+ * other output; a weight row holding a NaN is marked by w_scale[n] = NaN and gives a NaN channel.  +-inf clamp.
+ * Exact against the fp64 conv2d of the fake-quant operands when s_x and s_w are powers of two, within
+ * 2^-21 (conv(|f_x|, |f_w|) + |bias|) elementwise otherwise.  Deterministic, no state between calls (graph-capturable).
+ *
+ * Argument checks, all before any CUDA call: null pointers, c_out <= 0 or >= 2^31, a non-positive geometry, an empty
+ * output, n OH OW >= 2^31, groups < 2 (groups = 1 is sb200_int8_conv2d), c or c_out not divisible by groups and the
+ * range rules of the integer linear are SB200_E_INVALID; K_g >= 2^17 (|sum a b| <= K_g 2^14 must fit int32) is
+ * SB200_E_UNSUPPORTED. */
+int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                            const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                            const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
+                            void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);

@@ -30,8 +30,8 @@
 // which transposes through shared memory.  The batched GEMM kernel runs the same ring and wgmma loop as the linear
 // (i8_produce / i8_consume below) over 3-D tensor maps (Kp, rows, batch), so that a tile never reaches into the next
 // batch entry, with its own epilogue: per-row sum_k a, per-column sum_k b, both NaN flags, one scale product.
+#include "int8_grid.cuh"
 #include "tc_common.cuh"
-
 namespace sb200 {
 namespace {
 
@@ -73,16 +73,16 @@ static inline int grid_offset(int qmin) { return qmin >= 0 ? 128 : 0; }
 static inline long long padded_k(long long k) { return (k + 15) / 16 * 16; }
 
 // ---------------------------------------------------------------------------------- row quantizer
-// The stored grid value g - off of v (QP / quant_round<0>, as the QDQ kernels); NaN sets `nan` and stores 0.
-__device__ __forceinline__ int stored_grid(float v, const QP& p, int off, bool& nan) {
-  float g = __fadd_rn(quant_round<0>(v, p, 0), p.zp);
-  g = fmax_nan(fmin_nan(g, p.qmax), p.qmin);
-  if (g != g) {
-    nan = true;
-    return 0;
-  }
-  return (int)g - off;
-}
+// Every kernel of this file stores an element through stored_grid(v, p, off, nan) of int8_grid.cuh, the one
+// quantizer of the integer path, which the grouped conv kernel (int8_group_conv.cu) shares:
+//   g = clamp(quant_round<0>(v, p) + rint(zp), qmin, qmax)   (QP / quant_round<0> of common.cuh, as the QDQ kernels:
+//                                                             half-to-even, +-inf clamp to qmin / qmax)
+//   stored value = (int)g - off,   off = 128 for unsigned ranges, 0 otherwise
+// A NaN (g != g) sets the caller's `nan` and stores 0.  Because all of them go through this one function, a window
+// of the conv2d lowering below and the grouped conv kernel's shared-memory tile hold the same stored values for the
+// same input, and a grouped conv's group is bit-identical to this file's conv2d run on that group's channel slice.
+// The row quantizer below writes the stored value of every element of a row, its int32 row sum and a NaN flag; the
+// column quantizer and the conv2d lowering are the same per element.
 
 // 8 warps per CTA, one row per warp; lane l handles the 16-element chunks starting at 16 l, 16 (l + 32), ...
 __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __restrict__ x, const float* __restrict__ scale,
@@ -893,3 +893,13 @@ int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float
   SB_LAUNCHED();
   return SB200_OK;
 }
+
+// ---------------------------------------------------------------------------------- shared with int8_group_conv.cu
+namespace sb200 {
+int int8_check_conv(const char* fn, const sb200_conv2d_geom* g) {
+  ConvDims d;
+  return check_conv(fn, g, &d);
+}
+int int8_check_range(const char* fn, int qmin, int qmax) { return check_range(fn, qmin, qmax); }
+int int8_grid_offset(int qmin) { return grid_offset(qmin); }
+}  // namespace sb200

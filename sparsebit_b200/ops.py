@@ -891,6 +891,39 @@ def int8_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     return out
 
 
+def int8_group_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups, bias=None,
+                      stride=1, padding=0, dilation=1):
+    """The fake-quant grouped / depthwise conv2d (groups >= 2) on the integer grid (sb200_int8_group_conv2d): one direct
+    int8 kernel that quantizes its input tile on the fly.  ``x`` [N, C, H, W] fp32; the weights as ``int8_conv2d``
+    takes them, stored by ``int8_quantize_rows`` from ``weight.reshape(C_out, -1)`` (w_q int8 [C_out, Kp] with Kp =
+    round_up(C / groups KH KW, 16), w_rowsum int32, w_scale fp32, w_zero int32 [C_out]).  Returns fp32 [N, C_out, OH,
+    OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right).  No workspace."""
+    lib = _lib.load()
+    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
+    if bias is not None:
+        _req(bias, "bias")
+    if x.dim() != 4:
+        raise SparsebitB200Error("int8_group_conv2d: data must be [N, C, H, W]")
+    groups = int(groups)
+    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
+    if groups < 1 or g.c % groups:
+        raise SparsebitB200Error(f"int8_group_conv2d: groups = {groups} does not divide C = {g.c}")
+    k = g.c // groups * g.kh * g.kw
+    if w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
+        raise SparsebitB200Error(f"int8_group_conv2d: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {int8_padded_k(k)}]")
+    n = w_q.shape[0]
+    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"int8_group_conv2d: w_rowsum / w_scale / w_zero / bias need {n} elements")
+    oh, ow = conv2d_output_hw(g)
+    out = torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_group_conv2d(x.data_ptr(), ctypes.byref(g), groups, x_scale.data_ptr(),
+                                          x_zero_point.data_ptr(), int(qmin), int(qmax), w_q.data_ptr(),
+                                          w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
+                                          bias.data_ptr() if bias is not None else None, out.data_ptr(), n, _stream(x)))
+    return out
+
 def gptq_matmul_dgrad(grad_out, qweight, grad_in, scales, zeros, bits, group_size=0, impl=None):
     """In-place ``grad_in += grad_out @ dequant(qweight).T``: the input gradient of ``gptq_matmul`` for 2 / 3 / 4-bit
     weights (sb200_gptq_matmul_dgrad).  ``grad_out`` [..., N], ``grad_in`` [..., K] fp32.  ``impl``: per-call kernel

@@ -308,6 +308,92 @@ class QConv2dInt8(nn.Module):
                 f"padding={self.padding}, dilation={self.dilation}, qrange=[{self.qmin}, {self.qmax}]")
 
 
+INT8_MAX_KG = 1 << 17  # sb200_int8_group_conv2d: K_g = C / groups KH KW must stay below 2^17 (exact int32 sums)
+
+
+def int8_group_conv_ineligibility(qconv):
+    """Why ``QConv2dGroupInt8.from_qconv2d`` cannot convert ``qconv`` (None when it can)."""
+    if not isinstance(qconv, QConv2d):
+        return f"expected a QConv2d, got {type(qconv).__name__}"
+    reason = _int8_quantizer_ineligibility(qconv)
+    if reason is not None:
+        return reason
+    kw = qconv.fwd_kwargs
+    if kw["groups"] == 1:
+        return "groups = 1: use QConv2dInt8 / to_integer_convs"
+    c_out, c_g, kh, kwd = qconv.weight.shape
+    if c_g * kh * kwd >= INT8_MAX_KG:
+        return f"K_g = C / groups KH KW = {c_g * kh * kwd} >= 2^17 (the integer sums must stay exact in int32)"
+    try:
+        resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
+    except ValueError as e:
+        return f"the conv's {e}"
+    return None
+
+
+class QConv2dGroupInt8(QConv2dInt8):
+    """Inference-only replacement of a calibrated grouped or depthwise ``QConv2d`` (groups >= 2): the fake-quant conv2d
+    computed on the integer grid by ``ops.int8_group_conv2d`` -- one direct int8 kernel that quantizes its input tile
+    on the fly, exact integer sums per group, zero points removed in int64, then s_x s_w[n] I + bias, written NCHW.
+    Built by ``from_qconv2d``; the weights (``weight.reshape(C_out, -1)``, C / groups KH KW per row) are quantized
+    once at conversion.  Takes [N, C, H, W] or unbatched [C, H, W]; fp16 input is up-cast and the output is fp32, as in
+    the fake-quant op.  There is no backward: QAT keeps ``QConv2d``."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, groups, device):
+        nn.Module.__init__(self)
+        self.in_channels, self.out_channels, self.groups = int(in_channels), int(out_channels), int(groups)
+        self.kernel_size, self.stride, self.dilation = tuple(kernel_size), tuple(stride), tuple(dilation)
+        self.padding = tuple(padding)  # (top, bottom, left, right)
+        kp = ops.int8_padded_k(in_channels // self.groups * self.kernel_size[0] * self.kernel_size[1])
+        self.register_buffer("w_q", torch.zeros(out_channels, kp, dtype=torch.int8, device=device))
+        self.register_buffer("w_rowsum", torch.zeros(out_channels, dtype=torch.int32, device=device))
+        self.register_buffer("w_scale", torch.zeros(out_channels, dtype=torch.float32, device=device))
+        self.register_buffer("w_zero", torch.zeros(out_channels, dtype=torch.int32, device=device))
+        self.register_buffer("scale", torch.ones(1, dtype=torch.float32, device=device))
+        self.register_buffer("zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+        self.register_buffer("bias", None)
+        self.qmin, self.qmax = -128, 127
+
+    @classmethod
+    def from_qconv2d(cls, qconv):
+        reason = int8_group_conv_ineligibility(qconv)
+        if reason is not None:
+            raise ValueError(f"QConv2dGroupInt8.from_qconv2d: {reason}")
+        aq, wq = qconv.input_quantizer, qconv.weight_quantizer
+        kw = qconv.fwd_kwargs
+        weight = qconv.weight.detach()
+        c_out, c_g, kh, kwd = weight.shape
+        groups = int(kw["groups"])
+        padding = resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
+        mod = cls(c_g * groups, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]), groups,
+                  weight.device)
+        with torch.no_grad():
+            for buf, v in zip((mod.w_q, mod.w_rowsum, mod.w_scale, mod.w_zero), _int8_weight_rows(wq, qconv.weight)):
+                buf.copy_(v)
+            xs, xz = _qparams(aq, None)
+            mod.scale.copy_(xs.reshape(1))
+            mod.zero_point.copy_(xz.reshape(1))
+            if qconv.bias is not None:
+                mod.bias = qconv.bias.detach().float().clone().contiguous()
+        mod.qmin, mod.qmax = aq.qdesc.qrange
+        return mod
+
+    def forward(self, x_in):
+        if torch.is_grad_enabled() and x_in.requires_grad:
+            raise RuntimeError("QConv2dGroupInt8 is inference-only and has no backward; run it under torch.no_grad() or "
+                               "keep QConv2d for training")
+        x = x_in.float() if x_in.dtype != torch.float32 else x_in
+        unbatched = x.dim() == 3
+        if unbatched:
+            x = x.unsqueeze(0)
+        y = ops.int8_group_conv2d(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.w_q,
+                                  self.w_rowsum, self.w_scale, self.w_zero, self.kernel_size, self.groups, self.bias,
+                                  self.stride, self.padding, self.dilation)
+        return y.squeeze(0) if unbatched else y
+
+    def extra_repr(self):
+        return super().extra_repr() + f", groups={self.groups}"
+
 class QReLU(QuantOpr):
     def __init__(self, org_module=None):
         super().__init__()

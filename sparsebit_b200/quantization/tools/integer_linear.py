@@ -1,8 +1,10 @@
 """Turn a calibrated model into an integer-inference model: every eligible ``QLinear`` becomes a ``QLinearInt8``
 (``to_integer_linears``), every eligible ``QConv2d`` a ``QConv2dInt8`` (``to_integer_convs``), every eligible ``QMatMul``
-a ``QMatMulInt8`` (``to_integer_matmuls``)."""
-from ..modules import (QConv2d, QConv2dInt8, QLinear, QLinearInt8, QMatMul, QMatMulInt8, int8_conv_ineligibility,
-                       int8_ineligibility, int8_matmul_ineligibility)
+a ``QMatMulInt8`` (``to_integer_matmuls``), every eligible grouped or depthwise ``QConv2d`` a ``QConv2dGroupInt8``
+(``to_integer_group_convs``)."""
+from ..modules import (QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, QLinearInt8, QMatMul, QMatMulInt8,
+                       int8_conv_ineligibility, int8_group_conv_ineligibility, int8_ineligibility,
+                       int8_matmul_ineligibility)
 
 
 def _swap(model, kind, ineligibility, convert):
@@ -36,3 +38,10 @@ def to_integer_matmuls(model):
     """Swap, in place, every ``QMatMul`` of ``model`` that ``QMatMulInt8.from_qmatmul`` accepts; the others stay
     ``QMatMul``.  Returns the qualified names of the converted modules, in ``named_modules`` order."""
     return _swap(model, QMatMul, int8_matmul_ineligibility, QMatMulInt8.from_qmatmul)
+
+
+def to_integer_group_convs(model):
+    """Swap, in place, every grouped or depthwise ``QConv2d`` of ``model`` that ``QConv2dGroupInt8.from_qconv2d``
+    accepts; dense convs (groups = 1, see ``to_integer_convs``) and ineligible ones stay ``QConv2d``.  Returns the
+    qualified names of the converted modules, in ``named_modules`` order."""
+    return _swap(model, QConv2d, int8_group_conv_ineligibility, QConv2dGroupInt8.from_qconv2d)
