@@ -551,6 +551,38 @@ int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64
                             const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
                             void* stream);
 
+/* ---- (5e) Integer-grid inference of a calibrated attention, fused (int8 wgmma, sm_90a) ----
+ * New; the reference runs MatMul -> Softmax -> MatMul with a QIdentity carrier in front of every matmul input, so q,
+ * k, the softmax output p and v are each fake-quantised per tensor.  Per batch entry, with q [tq, d], k [tk, d] and
+ * v [tk, dv] fp32 contiguous:
+ *   s = RN32(fp64(I_qk) * (fp64(s_q) * fp64(s_k)))  (then RN32(s * scale) when has_scale)
+ *   I_qk = sum over d of (v_q - Z_q)(v_k - Z_k), exact: s is bit-identical to sb200_int8_matmul(q, k^T)
+ *   p = softmax(s) along the keys, in fp32; g_p = its stored grid (the QDQ rule with p's qparams)
+ *   out = RN32(fp64(I_pv) * (fp64(s_p) * fp64(s_v))),  I_pv = sum over the keys of (g_p - Z_p)(v_v - Z_v), exact
+ * One kernel computes the scores, the softmax, p's grid and p @ v; the [tq, tk] scores never reach memory.  Only p is
+ * inexact: |p - p64| <= 13 * 2^-24 * p64 + 2^-125, p64 the fp64 softmax of the same fp32 scores.
+ * out [batch, tq, dv] fp32 (overwritten).  p_q: NULL, or [batch, tq, round_up(tk, 16)] s8 (16-byte aligned) that
+ * receives the stored grid of p, the key padding 0.  scale: a host float, used when has_scale != 0.  Scales and zero
+ * points: device, one float each; the stored grid and range rules as in (5).
+ * NaN: a NaN in row i of q makes row i of out NaN; a NaN anywhere in k makes all of that entry's out NaN; a NaN in
+ * column n of v makes column n of that entry's out NaN; +-inf clamp.  Deterministic, no state between calls
+ * (graph-capturable).
+ *
+ * Argument checks, all before any CUDA call: null pointers, an empty dimension, batch tq or batch tk >= 2^31, the
+ * range rules of the four operands, a non-finite scale with has_scale and a p_q not 16-byte aligned are
+ * SB200_E_INVALID; d > 128, dv > 128 or tk >= 2^17 is SB200_E_UNSUPPORTED; a workspace that is too small is
+ * SB200_E_WORKSPACE.
+ * workspace: sb200_int8_attention_workspace_bytes(batch, tq, tk, d, dv) bytes, O(batch (tq + tk) d + batch dv tk)
+ * (a pure function; 0 for arguments the attention rejects). */
+size_t sb200_int8_attention_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv);
+int sb200_int8_attention(const float* q, const float* k, const float* v, const float* q_scale,
+                         const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale,
+                         const float* k_zero_point, int qmin_k, int qmax_k, const float* p_scale,
+                         const float* p_zero_point, int qmin_p, int qmax_p, const float* v_scale,
+                         const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale, float* out,
+                         int8_t* p_q, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);

@@ -1,0 +1,430 @@
+// int8_attention.cu -- integer-grid inference of a calibrated QAttention: softmax(q k^T [* scale]) v with q, k, the
+// softmax output p and v each on its own per-tensor int8 grid, in one kernel that never writes the [Tq, Tk] scores.
+//
+// Operands.  q [B, Tq, d] and k [B, Tk, d] go through int8_quantize_rows_kernel, v [B, Tk, dv] through
+// int8_quantize_cols_kernel (v^T K-major, [B, dv, Tkp]), all into the workspace with their sums and NaN flags
+// (int8_linear.cu, unchanged).  Everything after that is int8_attention_kernel.
+//
+// CTA = 128 query rows of one batch entry: warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 own 64
+// rows each.  The q tile is loaded once; k blocks (128 keys) and v^T blocks (128 keys of all dv <= 128 columns) stream
+// through a ring of kAtStages stages.  The key blocks are walked twice:
+//   pass 1  (k only)   s = the scores of the block; per row a running max m and sum l = sum exp(s - m) in fp64
+//   pass 2  (k and v)  the same scores again; p = exp(s - m) * RN32(1 / l) in fp32, quantized by the QDQ rule
+//                      (stored_grid, int8_grid.cuh) into a SWIZZLE_128B s8 tile in shared memory, which is the K-major
+//                      A operand of the p @ v wgmma accumulating into s32 over all key blocks.
+// Both passes read k from global (L2) memory; nothing of size O(Tq Tk) is written unless the caller asks for p_q.
+//
+// Scores.  I = sum (v_q - Z_q)(v_k - Z_k) exactly (wgmma s32.s8.s8, zero points in int64), s = RN32(fp64(I) *
+// (fp64(s_q) fp64(s_k))): operation for operation the epilogue of int8_matmul_gemm_kernel, so s is bit-identical to
+// sb200_int8_matmul(q, k^T).  With a scale, s = RN32(s * scale).
+// Softmax.  exp(s - m) is expf of the rounded difference corrected by its exact rounding error (exp_diff); l is
+// summed in fp64 and rescaled with the fp64 exp.  DESIGN §4 derives |p - p64| <= 13 2^-24 p64 + 2^-125, p64 the fp64
+// softmax of the same fp32 scores.
+// p @ v.  I_pv = sum_j (g_p - Z_p)(v_v - Z_v) exactly (|products| <= 2^14, Tk < 2^17), out = RN32(fp64(I_pv) *
+// (fp64(s_p) fp64(s_v))), the epilogue of int8_matmul_gemm_kernel with p as the left operand.
+// NaN.  A NaN in row i of q makes row i NaN; a NaN anywhere in k of an entry makes the entry NaN; a NaN in column n of
+// v makes column n NaN; a NaN p (only from non-finite scores) makes its row NaN.  No atomics, no state between calls.
+#include "int8_grid.cuh"
+#include "tc_common.cuh"
+
+namespace sb200 {
+namespace {
+
+constexpr int kAtRows = 128;                    // query rows per CTA (two consumer warpgroups x 64)
+constexpr int kAtKeys = 128;                    // keys per block: wgmma N of q k^T, K of p v
+constexpr int kAtStages = 4;
+constexpr int kAtThreads = 384;
+constexpr int kAtTile = 128 * 128;              // 16 KB: the q tile, a k block, a v^T block (128 rows x 128 bytes)
+constexpr int kAtStageBytes = 2 * kAtTile;      // k block | v^T block
+constexpr int kAtPBytes = 64 * 128;             // one warpgroup's p tile (64 rows x 128 keys)
+constexpr int kAtMaxDim = 128;                  // d, dv
+constexpr long long kAtMaxTk = 1LL << 17;       // exact s32 sums of p v
+constexpr size_t kAtSmem = 1024 + kAtTile + (size_t)kAtStages * kAtStageBytes + 2 * kAtPBytes + 128;
+
+struct AtParams {
+  const int* q_sum;
+  const uint8_t* q_nan;
+  const int* k_sum;
+  const uint8_t* k_nan;
+  const int* v_sum;
+  const uint8_t* v_nan;
+  const float *q_scale, *q_zero, *k_scale, *k_zero, *p_scale, *p_zero, *v_scale, *v_zero;
+  int q_off, k_off, p_off, v_off;
+  float p_qmin, p_qmax;
+  int has_scale;
+  float scale;
+  float* out;
+  int8_t* p_q;  // [B, Tq, Tkp] or null
+  int Tq, Tk, Tkp, d, dp, dv, vec2;
+};
+
+// exp(s - m) for fp32 s <= m: the difference is split exactly into hi + lo (TwoSum), expf(hi) is corrected by lo.
+// Differences below -104 underflow to 0 in fp32 anyway and return 0 (also for a masked s = -inf); NaN propagates.
+__device__ __forceinline__ float exp_diff(float s, float m) {
+  const float hi = __fsub_rn(s, m);
+  if (s == -INFINITY || hi < -104.f) return 0.f;
+  const float bb = __fsub_rn(hi, s);
+  const float lo = __fadd_rn(__fsub_rn(s, __fsub_rn(hi, bb)), __fsub_rn(-m, bb));
+  const float e = expf(hi);
+  return __fmaf_rn(e, lo, e);
+}
+
+// acc = the q tile rows of this warpgroup times the 128 keys of a k block, over nk32 steps of 32 d
+__device__ __forceinline__ void qk_mma(int (&acc)[64], uint64_t dq, uint64_t dk, int nk32) {
+  wgmma_fence();
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    if (j < nk32) wgmma_m64n128k32_s8(acc, dq + 2 * j, dk + 2 * j, j > 0);
+  wgmma_commit();
+  wgmma_wait_s32<0>(acc);
+}
+
+__device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
+// One CTA per 128 query rows of one batch entry (row tile fastest).  Maps: q (dp, Tq, B), k (dp, Tk, B), v^T
+// (Tkp, dv, B), boxes of 128 x 128 bytes: rows past Tq / Tk / dv and bytes past dp / Tkp are zero-filled.
+__global__ void __launch_bounds__(kAtThreads, 1)
+int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+                      const __grid_constant__ CUtensorMap map_v, const __grid_constant__ AtParams a) {
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* q_tile = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  unsigned char* stages = q_tile + kAtTile;
+  unsigned char* p_tiles = stages + (size_t)kAtStages * kAtStageBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(p_tiles + 2 * kAtPBytes);  // full[kAtStages] | empty[kAtStages] | q
+  uint64_t *full = bars, *empty = bars + kAtStages, *qbar = bars + 2 * kAtStages;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned tiles_q = (unsigned)(a.Tq + kAtRows - 1) / kAtRows;
+  const int m0 = (int)(blockIdx.x % tiles_q) * kAtRows, batch = (int)(blockIdx.x / tiles_q);
+  const int nkb = (a.Tk + kAtKeys - 1) / kAtKeys;
+
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
+    for (int s = 0; s < kAtStages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);  // one arrival per consumer warp
+    }
+    mbar_init(qbar, 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    reg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(qbar, (uint32_t)kAtTile);
+      tma_load_3d(q_tile, &map_q, 0, m0, batch, qbar);
+      // block i < nkb: pass 1 (k block i); i >= nkb: pass 2 (k and v^T block i - nkb)
+      for (int i = 0; i < 2 * nkb; ++i) {
+        const int s = i % kAtStages;
+        const uint32_t ph = (uint32_t)(i / kAtStages) & 1u;
+        const int kb = i < nkb ? i : i - nkb;
+        mbar_wait_relaxed(&empty[s], ph ^ 1u, 0);
+        unsigned char* st = stages + (size_t)s * kAtStageBytes;
+        mbar_expect_tx(&full[s], (uint32_t)(i < nkb ? kAtTile : kAtStageBytes));
+        tma_load_3d(st, &map_k, 0, kb * kAtKeys, batch, &full[s]);
+        if (i >= nkb) tma_load_3d(st + kAtTile, &map_v, kb * kAtKeys, 0, batch, &full[s]);
+      }
+    }
+    return;
+  }
+  reg_inc<232>();
+  const int wg = (warp - 4) >> 2, q4 = lane & 3;
+  const int rl = 16 * (warp & 3) + (lane >> 2);  // the thread's first row within the warpgroup's 64; the second is +8
+  const size_t qrow0 = (size_t)batch * a.Tq, krow0 = (size_t)batch * a.Tk, vrow0 = (size_t)batch * a.dv;
+  const double sqk = (double)__ldg(a.q_scale) * (double)__ldg(a.k_scale);
+  const long long zq = (long long)rintf(__ldg(a.q_zero)) - a.q_off, zk = (long long)rintf(__ldg(a.k_zero)) - a.k_off;
+  const long long zv = (long long)rintf(__ldg(a.v_zero)) - a.v_off;
+  QP pp;
+  pp.set(__ldg(a.p_scale), __ldg(a.p_zero));
+  pp.qmin = a.p_qmin;
+  pp.qmax = a.p_qmax;
+  const long long zp = (long long)pp.zp - a.p_off;
+  int row[2];
+  long long rterm[2];  // d Z_q Z_k - Z_k sum_k v_q of the row
+  bool bad[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    row[h] = m0 + 64 * wg + rl + 8 * h;
+    const bool live = row[h] < a.Tq;
+    rterm[h] = (long long)a.d * zq * zk - (live ? zk * (long long)__ldg(a.q_sum + qrow0 + row[h]) : 0);
+    bad[h] = live && __ldg(a.q_nan + qrow0 + row[h]) != 0;
+  }
+  const int nk32 = (a.dp + 31) / 32;
+  mbar_wait_relaxed(qbar, 0, 0);
+  const uint64_t dq = gmma_desc_sw128(smem_u32(q_tile) + (uint32_t)wg * (64 * 128));
+  const uint32_t stage0 = smem_u32(stages);
+  int acc[64];
+
+  // ---- pass 1: row max and sum.  Each thread keeps (m, l) of its 32 keys per block; the quad combines them.
+  float mx[2] = {-INFINITY, -INFINITY};
+  double l[2] = {0.0, 0.0};
+  bool knan = false;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int s = kb % kAtStages;
+    mbar_wait_relaxed(&full[s], (uint32_t)(kb / kAtStages) & 1u, 0);
+    qk_mma(acc, dq, gmma_desc_sw128(stage0 + (uint32_t)s * kAtStageBytes), nk32);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+    float bm[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 64; j += 2) {  // acc[j], acc[j + 1]: keys 8 (j >> 2) + 2 q4 + {0, 1}, row h = (j >> 1) & 1
+      const int h = (j >> 1) & 1;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int key = kb * kAtKeys + 8 * (j >> 2) + 2 * q4 + e;
+        float sc = -INFINITY;
+        if (key < a.Tk) {
+          const long long I = (long long)acc[j + e] + rterm[h] - zq * (long long)__ldg(a.k_sum + krow0 + key);
+          sc = __double2float_rn((double)I * sqk);
+          if (a.has_scale) sc = __fmul_rn(sc, a.scale);
+          if (h == 0) knan |= __ldg(a.k_nan + krow0 + key) != 0;
+        }
+        acc[j + e] = __float_as_int(sc);
+        bm[h] = fmaxf(bm[h], sc);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (bm[h] > mx[h]) {
+        l[h] *= exp((double)mx[h] - (double)bm[h]);
+        mx[h] = bm[h];
+      }
+#pragma unroll
+    for (int j = 0; j < 64; ++j) {
+      const int h = (j >> 1) & 1;
+      l[h] += (double)exp_diff(__int_as_float(acc[j]), mx[h]);
+    }
+  }
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float m = mx[h];
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    double lh = l[h] == 0.0 ? 0.0 : l[h] * exp((double)mx[h] - (double)m);
+    lh += __shfl_xor_sync(0xffffffffu, lh, 1);
+    lh += __shfl_xor_sync(0xffffffffu, lh, 2);
+    mx[h] = m;
+    inv[h] = __double2float_rn(1.0 / lh);
+  }
+  const bool kbad = __any_sync(0xffffffffu, knan);  // the quad's keys are all keys; every quad saw them
+
+  // ---- pass 2: p on its grid into shared memory, then p @ v
+  unsigned char* my_p = p_tiles + wg * kAtPBytes;
+  const uint64_t dp_desc = gmma_desc_sw128(smem_u32(my_p));
+  int o[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) o[j] = 0;
+  int psum[2] = {0, 0};
+  bool pnan[2] = {false, false};
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int i = nkb + kb, s = i % kAtStages;
+    mbar_wait_relaxed(&full[s], (uint32_t)(i / kAtStages) & 1u, 0);
+    const uint32_t st = stage0 + (uint32_t)s * kAtStageBytes;
+    qk_mma(acc, dq, gmma_desc_sw128(st), nk32);
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      const int kl = 8 * c + 2 * q4, key = kb * kAtKeys + kl;  // the pair kl, kl + 1 of the block
+      long long kz[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) kz[e] = key + e < a.Tk ? zq * (long long)__ldg(a.k_sum + krow0 + key + e) : 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t pair = 0u;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          if (key + e >= a.Tk) continue;  // masked keys store 0: with v^T zero there, they add nothing
+          const long long I = (long long)acc[4 * c + 2 * h + e] + rterm[h] - kz[e];
+          float sc = __double2float_rn((double)I * sqk);
+          if (a.has_scale) sc = __fmul_rn(sc, a.scale);
+          const float p = __fmul_rn(exp_diff(sc, mx[h]), inv[h]);
+          const int g = stored_grid(p, pp, a.p_off, pnan[h]);
+          psum[h] += g;
+          pair |= ((uint32_t)g & 0xFFu) << (8 * e);
+        }
+        const int r = rl + 8 * h;  // SWIZZLE_128B: 16-byte chunk kl / 16 of row r sits at chunk (kl / 16) ^ (r % 8)
+        *reinterpret_cast<uint16_t*>(my_p + r * 128 + ((((kl >> 4) ^ (r & 7))) << 4) + (kl & 15)) = (uint16_t)pair;
+        if (a.p_q != nullptr && row[h] < a.Tq && key < a.Tkp)
+          *reinterpret_cast<uint16_t*>(a.p_q + (qrow0 + row[h]) * (size_t)a.Tkp + key) = (uint16_t)pair;
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the p tile is visible to the wgmma
+    bar_wg(wg);
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) wgmma_m64n128k32_s8(o, dp_desc + 2 * j, gmma_desc_sw128(st + kAtTile) + 2 * j, 1);
+    wgmma_commit();
+    wgmma_wait_s32<0>(o);  // the stage and the p tile are free again
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+  }
+
+  // ---- epilogue: I_pv = sum g_p v - Z_v sum g_p - Z_p sum v + Tk Z_p Z_v, out = RN32(fp64(I_pv) s_p s_v)
+  const double spv = (double)__ldg(a.p_scale) * (double)__ldg(a.v_scale);
+  const float qnan = __int_as_float(0x7fc00000);
+  long long rp[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int ps = psum[h], pn = pnan[h] ? 1 : 0;
+    ps += __shfl_xor_sync(0xffffffffu, ps, 1);
+    pn |= __shfl_xor_sync(0xffffffffu, pn, 1);
+    ps += __shfl_xor_sync(0xffffffffu, ps, 2);
+    pn |= __shfl_xor_sync(0xffffffffu, pn, 2);
+    rp[h] = (long long)a.Tk * zp * zv - zv * (long long)ps;
+    bad[h] = bad[h] || kbad || pn != 0;
+  }
+#pragma unroll
+  for (int c = 0; c < 16; ++c) {
+    const int n = 8 * c + 2 * q4;
+    if (n >= a.dv) continue;
+    long long cn[2];
+    bool cnan[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const bool live = n + e < a.dv;
+      cn[e] = live ? zp * (long long)__ldg(a.v_sum + vrow0 + n + e) : 0;
+      cnan[e] = live && __ldg(a.v_nan + vrow0 + n + e) != 0;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (row[h] >= a.Tq) continue;
+      float y[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        y[e] = __double2float_rn((double)((long long)o[4 * c + 2 * h + e] + rp[h] - cn[e]) * spv);
+        if (bad[h] || cnan[e]) y[e] = qnan;
+      }
+      float* dst = a.out + (qrow0 + row[h]) * (size_t)a.dv + n;
+      if (a.vec2) {  // dv is even: the pair is in range and 8-byte aligned
+        *reinterpret_cast<float2*>(dst) = make_float2(y[0], y[1]);
+      } else {
+        dst[0] = y[0];
+        if (n + 1 < a.dv) dst[1] = y[1];
+      }
+    }
+  }
+}
+
+static inline long long padded16(long long k) { return (k + 15) / 16 * 16; }
+
+// Workspace: the three stored operands, each 1024-aligned and followed by its int32 sums and NaN flags
+struct AtLayout {
+  size_t q, q_sum, q_nan, k, k_sum, k_nan, v, v_sum, v_nan, total;
+};
+AtLayout at_layout(long long batch, long long tq, long long tk, long long d, long long dv) {
+  AtLayout w;
+  size_t o = 0;
+  const long long rows[3] = {batch * tq, batch * tk, batch * dv}, width[3] = {padded16(d), padded16(d), padded16(tk)};
+  size_t* q[3][3] = {{&w.q, &w.q_sum, &w.q_nan}, {&w.k, &w.k_sum, &w.k_nan}, {&w.v, &w.v_sum, &w.v_nan}};
+  for (int i = 0; i < 3; ++i) {
+    *q[i][0] = o;
+    o = align_up(o + (size_t)rows[i] * (size_t)width[i], 256);
+    *q[i][1] = o;
+    o = align_up(o + (size_t)rows[i] * 4, 256);
+    *q[i][2] = o;
+    o = align_up(o + (size_t)rows[i], 1024);
+  }
+  w.total = o;
+  return w;
+}
+
+// 0 when the dimensions are acceptable, else the SB200 code; sets the message
+int check_dims(const char* fn, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv) {
+  SB_REQUIRE(batch > 0 && tq > 0 && tk > 0 && d > 0 && dv > 0,
+             "%s: empty operand (batch=%lld Tq=%lld Tk=%lld d=%lld dv=%lld)", fn, (long long)batch, (long long)tq,
+             (long long)tk, (long long)d, (long long)dv);
+  if (d > kAtMaxDim || dv > kAtMaxDim || tk >= kAtMaxTk) {
+    set_error("%s: d = %lld, dv = %lld, Tk = %lld; the fused attention supports d <= 128, dv <= 128 and Tk < 2^17",
+              fn, (long long)d, (long long)dv, (long long)tk);
+    return SB200_E_UNSUPPORTED;
+  }
+  SB_REQUIRE((__int128)batch * tq < (1LL << 31) && (__int128)batch * tk < (1LL << 31) &&
+                 (__int128)batch * ((tq + kAtRows - 1) / kAtRows) < (1LL << 31),
+             "%s: dimension too large (batch Tq and batch Tk must be < 2^31)", fn);
+  return SB200_OK;
+}
+
+}  // namespace
+}  // namespace sb200
+
+using namespace sb200;
+
+size_t sb200_int8_attention_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv) {
+  if (batch <= 0 || tq <= 0 || tk <= 0 || d <= 0 || dv <= 0 || d > kAtMaxDim || dv > kAtMaxDim || tk >= kAtMaxTk)
+    return 0;
+  if ((__int128)batch * tq >= (1LL << 31) || (__int128)batch * tk >= (1LL << 31)) return 0;
+  return at_layout(batch, tq, tk, d, dv).total + 1024;  // + the alignment of the base
+}
+
+int sb200_int8_attention(const float* q, const float* k, const float* v, const float* q_scale,
+                         const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale,
+                         const float* k_zero_point, int qmin_k, int qmax_k, const float* p_scale,
+                         const float* p_zero_point, int qmin_p, int qmax_p, const float* v_scale,
+                         const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale, float* out,
+                         int8_t* p_q, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  const char* fn = "sb200_int8_attention";
+  SB_REQUIRE(q && k && v && q_scale && q_zero_point && k_scale && k_zero_point && p_scale && p_zero_point && v_scale &&
+                 v_zero_point && out && workspace,
+             "%s: null pointer argument", fn);
+  if (const int rc = check_dims(fn, batch, tq, tk, d, dv)) return rc;
+  const int ranges[4][2] = {{qmin_q, qmax_q}, {qmin_k, qmax_k}, {qmin_p, qmax_p}, {qmin_v, qmax_v}};
+  for (const auto& r : ranges)
+    if (const int rc = int8_check_range(fn, r[0], r[1])) return rc;
+  SB_REQUIRE(!has_scale || (scale == scale && scale - scale == 0.f), "%s: the scale %g is not finite", fn, (double)scale);
+  SB_REQUIRE(p_q == nullptr || aligned16(p_q), "%s: p_q must be 16-byte aligned", fn);
+  const size_t need = sb200_int8_attention_workspace_bytes(batch, tq, tk, d, dv);
+  if (workspace_bytes < need) {  // covers any alignment of the base
+    set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
+    return SB200_E_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const AtLayout w = at_layout(batch, tq, tk, d, dv);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
+  int8_t *qq = reinterpret_cast<int8_t*>(ws + w.q), *kq = reinterpret_cast<int8_t*>(ws + w.k);
+  int8_t* vq = reinterpret_cast<int8_t*>(ws + w.v);
+  const long long dp = padded16(d), tkp = padded16(tk);
+  CUtensorMap map_q, map_k, map_v;
+  if (!make_map_3d(&map_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, qq, (uint64_t)dp, (uint64_t)tq, (uint64_t)batch, (uint64_t)dp,
+                   128, kAtRows, CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_3d(&map_k, CU_TENSOR_MAP_DATA_TYPE_UINT8, kq, (uint64_t)dp, (uint64_t)tk, (uint64_t)batch, (uint64_t)dp,
+                   128, kAtKeys, CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_3d(&map_v, CU_TENSOR_MAP_DATA_TYPE_UINT8, vq, (uint64_t)tkp, (uint64_t)dv, (uint64_t)batch,
+                   (uint64_t)tkp, kAtKeys, 128, CU_TENSOR_MAP_SWIZZLE_128B)) {
+    set_error("%s: cuTensorMapEncodeTiled failed (batch=%lld Tq=%lld Tk=%lld d=%lld dv=%lld)", fn, (long long)batch,
+              (long long)tq, (long long)tk, (long long)d, (long long)dv);
+    return SB200_E_CUDA;
+  }
+  if (const int rc = sb200_int8_quantize_rows(q, q_scale, q_zero_point, 0, qmin_q, qmax_q, qq,
+                                              reinterpret_cast<int32_t*>(ws + w.q_sum), ws + w.q_nan, batch * tq, d,
+                                              stream))
+    return rc;
+  if (const int rc = sb200_int8_quantize_rows(k, k_scale, k_zero_point, 0, qmin_k, qmax_k, kq,
+                                              reinterpret_cast<int32_t*>(ws + w.k_sum), ws + w.k_nan, batch * tk, d,
+                                              stream))
+    return rc;
+  if (const int rc = sb200_int8_quantize_cols(v, v_scale, v_zero_point, qmin_v, qmax_v, vq,
+                                              reinterpret_cast<int32_t*>(ws + w.v_sum), ws + w.v_nan, batch, tk, dv,
+                                              stream))
+    return rc;
+  AtParams a;
+  a.q_sum = reinterpret_cast<const int*>(ws + w.q_sum), a.q_nan = ws + w.q_nan;
+  a.k_sum = reinterpret_cast<const int*>(ws + w.k_sum), a.k_nan = ws + w.k_nan;
+  a.v_sum = reinterpret_cast<const int*>(ws + w.v_sum), a.v_nan = ws + w.v_nan;
+  a.q_scale = q_scale, a.q_zero = q_zero_point, a.k_scale = k_scale, a.k_zero = k_zero_point;
+  a.p_scale = p_scale, a.p_zero = p_zero_point, a.v_scale = v_scale, a.v_zero = v_zero_point;
+  a.q_off = int8_grid_offset(qmin_q), a.k_off = int8_grid_offset(qmin_k);
+  a.p_off = int8_grid_offset(qmin_p), a.v_off = int8_grid_offset(qmin_v);
+  a.p_qmin = (float)qmin_p, a.p_qmax = (float)qmax_p;
+  a.has_scale = has_scale != 0, a.scale = has_scale ? scale : 1.f;
+  a.out = out, a.p_q = p_q;
+  a.Tq = (int)tq, a.Tk = (int)tk, a.Tkp = (int)tkp, a.d = (int)d, a.dp = (int)dp, a.dv = (int)dv;
+  a.vec2 = (dv % 2 == 0) && (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
+  static std::atomic<int> attr_done[64];
+  SB_CUDA(ensure_dyn_smem(int8_attention_kernel, (int)kAtSmem, attr_done));
+  const long long ctas = batch * ((tq + kAtRows - 1) / kAtRows);
+  int8_attention_kernel<<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a);
+  SB_LAUNCHED();
+  return SB200_OK;
+}

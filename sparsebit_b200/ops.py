@@ -808,6 +808,47 @@ def int8_matmul(a, a_scale, a_zero_point, a_qrange, b, b_scale, b_zero_point, b_
     return out
 
 
+def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=None, return_p=False):
+    """``softmax(q @ k^T [* scale]) @ v`` with q, k, the softmax output p and v each on a per-tensor int8 grid, in one
+    fused kernel (sb200_int8_attention) that never writes the [Tq, Tk] scores: the scores are bit-identical to
+    ``int8_matmul(q, k^T)``, p is the fp32 softmax quantized with ``p_qparams``, and ``p @ v`` is exact on the grid.
+    ``q`` [..., Tq, d], ``k`` [..., Tk, d], ``v`` [..., Tk, dv] fp32 with equal leading dimensions (no broadcasting);
+    non-contiguous operands are made contiguous.  Each ``*_qparams`` is ``(scale, zero_point, (qmin, qmax))`` with
+    1-element fp32 tensors.  Returns fp32 [..., Tq, dv], and with ``return_p`` also the stored int8 grid of p
+    [..., Tq, round_up(Tk, 16)]."""
+    lib = _lib.load()
+    for x, name in ((q, "q"), (k, "k"), (v, "v")):
+        if not isinstance(x, torch.Tensor) or x.dim() < 2:
+            raise SparsebitB200Error(f"int8_attention: {name} must be a tensor with at least 2 dimensions")
+    qp = []
+    for (s, z, qrange), name in ((q_qparams, "q"), (k_qparams, "k"), (p_qparams, "p"), (v_qparams, "v")):
+        _req(s, f"{name}_scale"), _req(z, f"{name}_zero_point")
+        if s.numel() != 1 or z.numel() != 1:
+            raise SparsebitB200Error("int8_attention: the qparams of every operand are per-tensor (1 element each)")
+        qp += [s.data_ptr(), z.data_ptr(), int(qrange[0]), int(qrange[1])]
+    lead = tuple(q.shape[:-2])
+    if tuple(k.shape[:-2]) != lead or tuple(v.shape[:-2]) != lead:
+        raise SparsebitB200Error(f"int8_attention: q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} need equal "
+                                 "leading dimensions (no broadcasting)")
+    (tq, d), (tk, dk), (tkv, dv) = q.shape[-2:], k.shape[-2:], v.shape[-2:]
+    if dk != d or tkv != tk:
+        raise SparsebitB200Error(f"int8_attention: q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} do not "
+                                 "chain (q and k need the same d, k and v the same Tk)")
+    q, k, v = (x.reshape(-1, *x.shape[-2:]).contiguous() for x in (q, k, v))
+    _req(q, "q"), _req(k, "k"), _req(v, "v")
+    batch = q.shape[0]
+    out = torch.empty(lead + (tq, dv), dtype=torch.float32, device=q.device)
+    p_q = torch.empty(lead + (tq, int8_padded_k(tk)), dtype=torch.int8, device=q.device) if return_p else None
+    ws_bytes = int(lib.sb200_int8_attention_workspace_bytes(batch, tq, tk, d, dv))
+    ws = _int8_workspace(q.device, max(ws_bytes, 16))
+    with torch.cuda.device(q.device):
+        check(lib.sb200_int8_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), *qp, int(scale is not None),
+                                       float(scale) if scale is not None else 1.0, out.data_ptr(),
+                                       p_q.data_ptr() if p_q is not None else None, batch, tq, tk, d, dv, ws.data_ptr(),
+                                       ws.numel(), _stream(q)))
+    return (out, p_q) if return_p else out
+
+
 def _pair(v):
     return (int(v), int(v)) if isinstance(v, int) else tuple(int(e) for e in v)
 

@@ -4,6 +4,8 @@ an operator owning an ``input_quantizer`` (and a ``weight_quantizer`` when it ha
 the ``config.A`` / ``config.W`` sub-trees, switched by ``set_quant``.  Graph conversion, fusion and the
 ~40 other operator wrappers of the reference are out of scope (SURVEY §8: control plane); any module
 exposing these attributes works with ``tools.CalibrationRunner``."""
+import math
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -488,3 +490,99 @@ class QMatMulInt8(nn.Module):
 
     def extra_repr(self):
         return f"left_qrange={list(self.left_qrange)}, right_qrange={list(self.right_qrange)}"
+
+
+class QAttention(nn.Module):
+    """Softmax attention between two ``QMatMul``: ``qk`` (carriers of q and k^T) and ``pv`` (carriers of the softmax
+    output p and of v), the reference's MatMul -> Softmax -> MatMul behind its four ``QIdentity`` carriers.
+    ``forward(q, k, v) = pv(softmax(qk(q, k^T) [* scale], -1), v)``.  Like ``QMatMul`` it is not itself a quant
+    operator, so calibration (streaming or the fx replay) sees the four carriers."""
+
+    def __init__(self, scale=None):
+        super().__init__()
+        self.scale = scale
+        self.qk, self.pv = QMatMul(), QMatMul()
+
+    def build_quantizer(self, a_cfg, p_cfg=None, backend=Backend.VIRTUAL):
+        """``a_cfg`` builds the carriers of q, k and v; ``p_cfg`` (default ``a_cfg``) that of p, ``pv.left``, so that
+        the softmax output can use an unsigned affine range."""
+        self.qk.build_quantizer(a_cfg, backend=backend)
+        self.pv.build_quantizer(a_cfg, backend=backend)
+        if p_cfg is not None:
+            self.pv.left.build_quantizer(p_cfg, backend=backend)
+        return self
+
+    def set_quant(self, w_quant=False, a_quant=False):
+        self.qk.set_quant(w_quant, a_quant)
+        self.pv.set_quant(w_quant, a_quant)
+
+    def forward(self, q, k, v):
+        s = self.qk(q, k.transpose(-2, -1))
+        if self.scale is not None:
+            s = s * self.scale
+        return self.pv(s.softmax(-1), v)
+
+    def extra_repr(self):
+        return f"scale={self.scale}"
+
+
+def int8_attention_ineligibility(qattn):
+    """Why ``QAttentionInt8.from_qattention`` cannot convert ``qattn`` (None when it can)."""
+    if not isinstance(qattn, QAttention):
+        return f"expected a QAttention, got {type(qattn).__name__}"
+    for role in ("qk", "pv"):
+        child = getattr(qattn, role)
+        if isinstance(child, QMatMulInt8):
+            return (f"the {role} matmul is already a QMatMulInt8: run to_integer_attentions before "
+                    "to_integer_matmuls")
+        reason = int8_matmul_ineligibility(child)
+        if reason is not None:
+            return f"the {role} matmul: {reason}"
+    if qattn.scale is not None and not math.isfinite(float(qattn.scale)):
+        return f"the scale {qattn.scale} is not finite"
+    return None
+
+
+class QAttentionInt8(nn.Module):
+    """Inference-only replacement of a calibrated ``QAttention``: ``ops.int8_attention``, one fused kernel on the
+    integer grid -- q and k quantized on the fly, exact int8 scores on the tensor cores (bit-identical to
+    ``QMatMulInt8``), the softmax in fp32 registers quantized with p's qparams, exact p @ v on the grid; the [Tq, Tk]
+    scores never reach memory.  Built by ``from_qattention``.  q, k, v have equal leading dimensions; fp16 input is
+    up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps ``QAttention``."""
+
+    ROLES = ("q", "k", "p", "v")
+
+    def __init__(self, device, scale=None):
+        super().__init__()
+        self.scale = scale
+        for role in self.ROLES:
+            self.register_buffer(f"{role}_scale", torch.ones(1, dtype=torch.float32, device=device))
+            self.register_buffer(f"{role}_zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+        self.qranges = {role: (-128, 127) for role in self.ROLES}
+
+    @classmethod
+    def from_qattention(cls, qattn):
+        reason = int8_attention_ineligibility(qattn)
+        if reason is not None:
+            raise ValueError(f"QAttentionInt8.from_qattention: {reason}")
+        carriers = dict(zip(cls.ROLES, (qattn.qk.left, qattn.qk.right, qattn.pv.left, qattn.pv.right)))
+        qparams = {role: _qparams(c.input_quantizer, None) for role, c in carriers.items()}
+        mod = cls(qparams["q"][0].device, None if qattn.scale is None else float(qattn.scale))
+        for role, carrier in carriers.items():
+            q = carrier.input_quantizer
+            s, z = qparams[role]
+            with torch.no_grad():
+                getattr(mod, f"{role}_scale").copy_(s.reshape(1))
+                getattr(mod, f"{role}_zero_point").copy_(z.reshape(1))
+            mod.qranges[role] = tuple(q.qdesc.qrange)
+        return mod
+
+    def forward(self, q, k, v):
+        if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+            raise RuntimeError("QAttentionInt8 is inference-only and has no backward; run it under torch.no_grad() or "
+                               "keep QAttention for training")
+        qp = [(getattr(self, f"{r}_scale"), getattr(self, f"{r}_zero_point"), self.qranges[r]) for r in self.ROLES]
+        return ops.int8_attention(q.float(), k.float(), v.float(), *qp, scale=self.scale)
+
+    def extra_repr(self):
+        return f"scale={self.scale}, " + ", ".join(f"{r}_qrange={list(self.qranges[r])}" for r in self.ROLES)

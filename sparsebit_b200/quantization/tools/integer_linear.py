@@ -1,10 +1,10 @@
 """Turn a calibrated model into an integer-inference model: every eligible ``QLinear`` becomes a ``QLinearInt8``
 (``to_integer_linears``), every eligible ``QConv2d`` a ``QConv2dInt8`` (``to_integer_convs``), every eligible ``QMatMul``
 a ``QMatMulInt8`` (``to_integer_matmuls``), every eligible grouped or depthwise ``QConv2d`` a ``QConv2dGroupInt8``
-(``to_integer_group_convs``)."""
-from ..modules import (QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, QLinearInt8, QMatMul, QMatMulInt8,
-                       int8_conv_ineligibility, int8_group_conv_ineligibility, int8_ineligibility,
-                       int8_matmul_ineligibility)
+(``to_integer_group_convs``), every eligible ``QAttention`` a ``QAttentionInt8`` (``to_integer_attentions``)."""
+from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, QLinearInt8, QMatMul,
+                       QMatMulInt8, int8_attention_ineligibility, int8_conv_ineligibility, int8_group_conv_ineligibility,
+                       int8_ineligibility, int8_matmul_ineligibility)
 
 
 def _swap(model, kind, ineligibility, convert):
@@ -45,3 +45,10 @@ def to_integer_group_convs(model):
     accepts; dense convs (groups = 1, see ``to_integer_convs``) and ineligible ones stay ``QConv2d``.  Returns the
     qualified names of the converted modules, in ``named_modules`` order."""
     return _swap(model, QConv2d, int8_group_conv_ineligibility, QConv2dGroupInt8.from_qconv2d)
+
+
+def to_integer_attentions(model):
+    """Swap, in place, every ``QAttention`` of ``model`` that ``QAttentionInt8.from_qattention`` accepts; the others
+    stay ``QAttention``.  Run it before ``to_integer_matmuls``, which would otherwise convert the two matmuls of each
+    attention separately.  Returns the qualified names of the converted modules, in ``named_modules`` order."""
+    return _swap(model, QAttention, int8_attention_ineligibility, QAttentionInt8.from_qattention)
