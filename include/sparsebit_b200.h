@@ -583,6 +583,38 @@ int sb200_int8_attention(const float* q, const float* k, const float* v, const f
                          int8_t* p_q, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* ---- (5f) The fused attention of (5e) with an additive mask and a causal mode (int8 wgmma, sm_90a) ----
+ * New; the reference's BERT (GLUE) adds a key-padding mask (1 - m) * -10000 to the scaled scores, its GPT-2 (wikitext)
+ * keeps the scores of a causal band and adds an attention mask.  Per batch entry b, after s (and its scale) of (5e):
+ *   causal: s[i, j] = -inf where j > i + (tk - tq)  (the band aligned bottom-right, as the GPT-2 example; this is not
+ *           the top-left is_causal of PyTorch's scaled_dot_product_attention when tq != tk)
+ *   mask:   s[i, j] = RN32(s[i, j] + mask[(b / mask_inner) mask_stride_outer + (b % mask_inner) mask_stride_inner
+ *                                         + i mask_stride_row + j])          (fp32, column stride 1, 64-bit offsets)
+ * then p, its grid and out as in (5e), with the same bound on p against the fp64 softmax of the masked fp32 scores.
+ * A [B, 1, 1, tk] mask over [B, H] entries is mask_inner = H, mask_stride_outer = tk, mask_stride_inner = 0,
+ * mask_stride_row = 0.  Under causal a block of 128 keys that no row of a 128-row tile sees is not read or computed;
+ * its keys have p = 0 (p_q receives their grid).  A row that sees no key (causal with tq > tk, or an all -inf mask row)
+ * is NaN.  NaN: as (5e), except that a NaN in k poisons only the rows whose band contains its key; a NaN in column n of
+ * v still makes column n NaN (0 * NaN); a NaN or +inf mask value at a key of a skipped block is not read.
+ * mask: NULL for none, then the four mask arguments are not read.  causal: 0 or 1.  mask == NULL with causal == 0
+ * computes exactly sb200_int8_attention.
+ *
+ * Argument checks, all before any CUDA call: those of (5e); causal not 0 or 1, and with a mask a negative stride,
+ * mask_inner <= 0 or not dividing batch, a mask not 4-byte aligned or a last offset >= 2^62 are SB200_E_INVALID.
+ * workspace: sb200_int8_attention_masked_workspace_bytes(batch, tq, tk, d, dv, causal) bytes: that of (5e), and with
+ * causal also batch dv ceil(tk / 128) int32 column sums of v (a pure function; 0 for arguments it rejects). */
+size_t sb200_int8_attention_masked_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv,
+                                                   int causal);
+int sb200_int8_attention_masked(const float* q, const float* k, const float* v, const float* q_scale,
+                                const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale,
+                                const float* k_zero_point, int qmin_k, int qmax_k, const float* p_scale,
+                                const float* p_zero_point, int qmin_p, int qmax_p, const float* v_scale,
+                                const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale,
+                                const float* mask, int64_t mask_stride_outer, int64_t mask_stride_inner,
+                                int64_t mask_inner, int64_t mask_stride_row, int causal, float* out, int8_t* p_q,
+                                int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);

@@ -113,6 +113,11 @@ PROTOTYPES = {
     "sb200_int8_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int,
                                      c_int, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
                                      c_i64, c_vp, c_sz, c_vp]),
+    "sb200_int8_attention_masked_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_i64, c_int]),
+    "sb200_int8_attention_masked": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp,
+                                            c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_i64, c_i64,
+                                            c_i64, c_i64, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp,
+                                            c_sz, c_vp]),
     "sb200_gptq4_set_impl": (c_int, [c_int]),
     "sb200_gptq4_set_wait_backoff": (c_int, [c_int]),
     "sb200_gptq4_set_decode": (c_int, [c_int]),

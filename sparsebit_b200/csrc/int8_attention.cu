@@ -24,6 +24,16 @@
 // (fp64(s_p) fp64(s_v))), the epilogue of int8_matmul_gemm_kernel with p as the left operand.
 // NaN.  A NaN in row i of q makes row i NaN; a NaN anywhere in k of an entry makes the entry NaN; a NaN in column n of
 // v makes column n NaN; a NaN p (only from non-finite scores) makes its row NaN.  No atomics, no state between calls.
+//
+// Masks (int8_attention_kernel<true>).  After the scale, s = -inf where key j is hidden from row i by the causal band
+// (j > i + Tk - Tq, aligned bottom-right), then s = RN32(s + mask[i, j]): the composition of QAttention, score for
+// score, in both passes.  Under causal a key block that no row of the CTA can see is neither loaded nor computed
+// (at_visible_blocks, the same count in the producer and the consumers), so a CTA visits a prefix of the key blocks.
+// Its skipped keys have p = 0, whose grid is Z_p, so their products vanish; the epilogue's sum of v covers the visited
+// prefix only (int8_attention_vprefix_kernel: per-block column sums of v^T, accumulated), and a zero point off the
+// range adds its exact (g_0 - Z_p) sum (v - Z_v) over the skipped keys.  p_q receives the grid of 0 * RN32(1 / l)
+// at skipped keys, as at a hidden key the kernel visits.  A NaN in k poisons only the rows that see its key; a row
+// without a visible key is NaN.
 #include "int8_grid.cuh"
 #include "tc_common.cuh"
 
@@ -58,6 +68,23 @@ struct AtParams {
   int Tq, Tk, Tkp, d, dp, dv, vec2;
 };
 
+// The mask of the masked instantiation, a separate kernel argument so that AtParams keeps its layout.  Entry b of the
+// batch reads mask + (b / inner) stride_outer + (b % inner) stride_inner + i stride_row + j (all 64-bit).
+struct AtMask {
+  const float* mask;  // or null
+  long long stride_outer, stride_inner, stride_row;
+  const int* v_pre;  // causal: [B, dv, nkb] running column sums of v^T over the key blocks
+  int inner, causal, batch;
+};
+
+// Key blocks a CTA of rows [m0, m0 + 128) visits: all of them, or under causal those up to the last key its last row
+// sees (0 when no row sees a key).
+__device__ __forceinline__ int at_visible_blocks(int m0, int Tq, int Tk, int nkb, int causal) {
+  if (!causal) return nkb;
+  const long long last = (long long)min(m0 + kAtRows, Tq) - 1 + Tk - Tq;  // the last key the CTA's last row sees
+  return last < 0 ? 0 : min(nkb, (int)(last / kAtKeys) + 1);
+}
+
 // exp(s - m) for fp32 s <= m: the difference is split exactly into hi + lo (TwoSum), expf(hi) is corrected by lo.
 // Differences below -104 underflow to 0 in fp32 anyway and return 0 (also for a masked s = -inf); NaN propagates.
 __device__ __forceinline__ float exp_diff(float s, float m) {
@@ -81,11 +108,14 @@ __device__ __forceinline__ void qk_mma(int (&acc)[64], uint64_t dq, uint64_t dk,
 
 __device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// One CTA per 128 query rows of one batch entry (row tile fastest).  Maps: q (dp, Tq, B), k (dp, Tk, B), v^T
-// (Tkp, dv, B), boxes of 128 x 128 bytes: rows past Tq / Tk / dv and bytes past dp / Tkp are zero-filled.
+// One CTA per 128 query rows of one batch entry (row tile fastest; under causal batch fastest, the last row tiles,
+// which visit the most key blocks, first).  Maps: q (dp, Tq, B), k (dp, Tk, B), v^T (Tkp, dv, B), boxes of 128 x 128
+// bytes: rows past Tq / Tk / dv and bytes past dp / Tkp are zero-filled.  kMasked = false ignores mk.
+template <bool kMasked>
 __global__ void __launch_bounds__(kAtThreads, 1)
 int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                      const __grid_constant__ CUtensorMap map_v, const __grid_constant__ AtParams a) {
+                      const __grid_constant__ CUtensorMap map_v, const __grid_constant__ AtParams a,
+                      const __grid_constant__ AtMask mk) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* q_tile = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* stages = q_tile + kAtTile;
@@ -94,8 +124,15 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   uint64_t *full = bars, *empty = bars + kAtStages, *qbar = bars + 2 * kAtStages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned tiles_q = (unsigned)(a.Tq + kAtRows - 1) / kAtRows;
-  const int m0 = (int)(blockIdx.x % tiles_q) * kAtRows, batch = (int)(blockIdx.x / tiles_q);
+  int m0 = (int)(blockIdx.x % tiles_q) * kAtRows, batch = (int)(blockIdx.x / tiles_q);
   const int nkb = (a.Tk + kAtKeys - 1) / kAtKeys;
+  int nvb = nkb;  // the key blocks this CTA visits
+  if constexpr (kMasked) {
+    if (mk.causal) {
+      m0 = (int)(tiles_q - 1 - blockIdx.x / (unsigned)mk.batch) * kAtRows, batch = (int)(blockIdx.x % (unsigned)mk.batch);
+      nvb = at_visible_blocks(m0, a.Tq, a.Tk, nkb, 1);
+    }
+  }
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
@@ -114,16 +151,16 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     if (threadIdx.x == 0) {
       mbar_expect_tx(qbar, (uint32_t)kAtTile);
       tma_load_3d(q_tile, &map_q, 0, m0, batch, qbar);
-      // block i < nkb: pass 1 (k block i); i >= nkb: pass 2 (k and v^T block i - nkb)
-      for (int i = 0; i < 2 * nkb; ++i) {
+      // block i < nvb: pass 1 (k block i); i >= nvb: pass 2 (k and v^T block i - nvb)
+      for (int i = 0; i < 2 * nvb; ++i) {
         const int s = i % kAtStages;
         const uint32_t ph = (uint32_t)(i / kAtStages) & 1u;
-        const int kb = i < nkb ? i : i - nkb;
+        const int kb = i < nvb ? i : i - nvb;
         mbar_wait_relaxed(&empty[s], ph ^ 1u, 0);
         unsigned char* st = stages + (size_t)s * kAtStageBytes;
-        mbar_expect_tx(&full[s], (uint32_t)(i < nkb ? kAtTile : kAtStageBytes));
+        mbar_expect_tx(&full[s], (uint32_t)(i < nvb ? kAtTile : kAtStageBytes));
         tma_load_3d(st, &map_k, 0, kb * kAtKeys, batch, &full[s]);
-        if (i >= nkb) tma_load_3d(st + kAtTile, &map_v, kb * kAtKeys, 0, batch, &full[s]);
+        if (i >= nvb) tma_load_3d(st + kAtTile, &map_v, kb * kAtKeys, 0, batch, &full[s]);
       }
     }
     return;
@@ -150,6 +187,16 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     rterm[h] = (long long)a.d * zq * zk - (live ? zk * (long long)__ldg(a.q_sum + qrow0 + row[h]) : 0);
     bad[h] = live && __ldg(a.q_nan + qrow0 + row[h]) != 0;
   }
+  const float* mrow[2] = {nullptr, nullptr};  // the mask row of each of the thread's rows (none past Tq)
+  long long vis[2] = {0, 0};                  // causal: the last key each row sees
+  if constexpr (kMasked) {
+    const long long base = (long long)(batch / mk.inner) * mk.stride_outer + (long long)(batch % mk.inner) * mk.stride_inner;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (mk.mask != nullptr && row[h] < a.Tq) mrow[h] = mk.mask + base + (long long)row[h] * mk.stride_row;
+      vis[h] = mk.causal ? (long long)row[h] + a.Tk - a.Tq : (long long)a.Tk;
+    }
+  }
   const int nk32 = (a.dp + 31) / 32;
   mbar_wait_relaxed(qbar, 0, 0);
   const uint64_t dq = gmma_desc_sw128(smem_u32(q_tile) + (uint32_t)wg * (64 * 128));
@@ -159,8 +206,8 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   // ---- pass 1: row max and sum.  Each thread keeps (m, l) of its 32 keys per block; the quad combines them.
   float mx[2] = {-INFINITY, -INFINITY};
   double l[2] = {0.0, 0.0};
-  bool knan = false;
-  for (int kb = 0; kb < nkb; ++kb) {
+  bool knan = false, knr[2] = {false, false};  // knr: the masked kernel's per-row NaN key
+  for (int kb = 0; kb < nvb; ++kb) {
     const int s = kb % kAtStages;
     mbar_wait_relaxed(&full[s], (uint32_t)(kb / kAtStages) & 1u, 0);
     qk_mma(acc, dq, gmma_desc_sw128(stage0 + (uint32_t)s * kAtStageBytes), nk32);
@@ -178,7 +225,14 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
           const long long I = (long long)acc[j + e] + rterm[h] - zq * (long long)__ldg(a.k_sum + krow0 + key);
           sc = __double2float_rn((double)I * sqk);
           if (a.has_scale) sc = __fmul_rn(sc, a.scale);
-          if (h == 0) knan |= __ldg(a.k_nan + krow0 + key) != 0;
+          if constexpr (kMasked) {
+            const bool seen = key <= vis[h];
+            if (!seen) sc = -INFINITY;
+            if (mrow[h] != nullptr) sc = __fadd_rn(sc, __ldg(mrow[h] + key));
+            knr[h] |= seen && __ldg(a.k_nan + krow0 + key) != 0;
+          } else {
+            if (h == 0) knan |= __ldg(a.k_nan + krow0 + key) != 0;
+          }
         }
         acc[j + e] = __float_as_int(sc);
         bm[h] = fmaxf(bm[h], sc);
@@ -209,6 +263,13 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     inv[h] = __double2float_rn(1.0 / lh);
   }
   const bool kbad = __any_sync(0xffffffffu, knan);  // the quad's keys are all keys; every quad saw them
+  if constexpr (kMasked) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // the quad's keys are all keys of the row
+      knr[h] = __shfl_xor_sync(0xffffffffu, (int)knr[h], 1) | knr[h];
+      knr[h] = __shfl_xor_sync(0xffffffffu, (int)knr[h], 2) | knr[h];
+    }
+  }
 
   // ---- pass 2: p on its grid into shared memory, then p @ v
   unsigned char* my_p = p_tiles + wg * kAtPBytes;
@@ -218,8 +279,8 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   for (int j = 0; j < 64; ++j) o[j] = 0;
   int psum[2] = {0, 0};
   bool pnan[2] = {false, false};
-  for (int kb = 0; kb < nkb; ++kb) {
-    const int i = nkb + kb, s = i % kAtStages;
+  for (int kb = 0; kb < nvb; ++kb) {
+    const int i = nvb + kb, s = i % kAtStages;
     mbar_wait_relaxed(&full[s], (uint32_t)(i / kAtStages) & 1u, 0);
     const uint32_t st = stage0 + (uint32_t)s * kAtStageBytes;
     qk_mma(acc, dq, gmma_desc_sw128(st), nk32);
@@ -238,6 +299,10 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
           const long long I = (long long)acc[4 * c + 2 * h + e] + rterm[h] - kz[e];
           float sc = __double2float_rn((double)I * sqk);
           if (a.has_scale) sc = __fmul_rn(sc, a.scale);
+          if constexpr (kMasked) {
+            if (key + e > vis[h]) sc = -INFINITY;
+            if (mrow[h] != nullptr) sc = __fadd_rn(sc, __ldg(mrow[h] + key + e));
+          }
           const float p = __fmul_rn(exp_diff(sc, mx[h]), inv[h]);
           const int g = stored_grid(p, pp, a.p_off, pnan[h]);
           psum[h] += g;
@@ -259,10 +324,31 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
+  if constexpr (kMasked) {  // the skipped keys' p is 0 (NaN in a row without a visible key): its grid into p_q
+    if (a.p_q != nullptr) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (row[h] >= a.Tq) continue;
+        bool unused = false;
+        const uint32_t g0 = (uint32_t)stored_grid(__fmul_rn(0.f, inv[h]), pp, a.p_off, unused) & 0xFFu;
+        int8_t* dst = a.p_q + (qrow0 + row[h]) * (size_t)a.Tkp;
+        for (int key = nvb * kAtKeys + 2 * q4; key < a.Tkp; key += 8)
+          *reinterpret_cast<uint16_t*>(dst + key) = (uint16_t)((key < a.Tk ? g0 : 0u) | (key + 1 < a.Tk ? g0 << 8 : 0u));
+      }
+    }
+  }
 
   // ---- epilogue: I_pv = sum g_p v - Z_v sum g_p - Z_p sum v + Tk Z_p Z_v, out = RN32(fp64(I_pv) s_p s_v)
   const double spv = (double)__ldg(a.p_scale) * (double)__ldg(a.v_scale);
   const float qnan = __int_as_float(0x7fc00000);
+  // the masked kernel over a visited prefix of nvis keys: - Z_p sum v over the prefix, and (g_0 - Z_p) (v - Z_v) for
+  // each skipped key, g_0 the grid of p = 0 (the products of the skipped keys vanish when Z_p lies in the range)
+  const int nvis = kMasked ? min(nvb * kAtKeys, a.Tk) : a.Tk;
+  long long d0 = 0;
+  if constexpr (kMasked) {
+    bool unused = false;
+    d0 = (long long)stored_grid(0.f, pp, a.p_off, unused) - zp;
+  }
   long long rp[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -271,8 +357,12 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     pn |= __shfl_xor_sync(0xffffffffu, pn, 1);
     ps += __shfl_xor_sync(0xffffffffu, ps, 2);
     pn |= __shfl_xor_sync(0xffffffffu, pn, 2);
-    rp[h] = (long long)a.Tk * zp * zv - zv * (long long)ps;
+    rp[h] = (long long)nvis * zp * zv - zv * (long long)ps;
     bad[h] = bad[h] || kbad || pn != 0;
+    if constexpr (kMasked) {
+      rp[h] -= d0 * (long long)(a.Tk - nvis) * zv;
+      bad[h] = bad[h] || knr[h] || mx[h] == -INFINITY;  // a NaN key the row sees; no visible key
+    }
   }
 #pragma unroll
   for (int c = 0; c < 16; ++c) {
@@ -284,6 +374,13 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     for (int e = 0; e < 2; ++e) {
       const bool live = n + e < a.dv;
       cn[e] = live ? zp * (long long)__ldg(a.v_sum + vrow0 + n + e) : 0;
+      if constexpr (kMasked) {
+        if (live && nvis < a.Tk) {  // causal: the column's sum over the visited prefix
+          const long long all = __ldg(a.v_sum + vrow0 + n + e);
+          const long long pre = nvb > 0 ? __ldg(mk.v_pre + (vrow0 + n + e) * (size_t)nkb + nvb - 1) : 0;
+          cn[e] = zp * pre - d0 * (all - pre);
+        }
+      }
       cnan[e] = live && __ldg(a.v_nan + vrow0 + n + e) != 0;
     }
 #pragma unroll
@@ -303,6 +400,26 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         if (n + 1 < a.dv) dst[1] = y[1];
       }
     }
+  }
+}
+
+// Causal: pre[r, kb] = the sum of the stored v^T row r (one column of v) over key blocks 0 .. kb (|sum| < 2^24).
+// One warp per row, each lane 4 of a block's 128 bytes; Tkp is a multiple of 16, so a lane's 4 bytes are all in range
+// or all past it.
+__global__ void __launch_bounds__(256) int8_attention_vprefix_kernel(const int8_t* __restrict__ vq, int* __restrict__ pre,
+                                                                     long long rows, int tkp, int nkb) {
+  const long long r = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const int8_t* src = vq + r * tkp;
+  int run = 0;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int c = kb * kAtKeys + 4 * lane;
+    int x = c < tkp ? __dp4a(*reinterpret_cast<const int*>(src + c), 0x01010101, 0) : 0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    run += x;
+    if (lane == 0) pre[r * nkb + kb] = run;
   }
 }
 
@@ -345,26 +462,27 @@ int check_dims(const char* fn, int64_t batch, int64_t tq, int64_t tk, int64_t d,
   return SB200_OK;
 }
 
-}  // namespace
-}  // namespace sb200
+// Causal: the running column sums of v^T (int8_attention_vprefix_kernel) after the operands, [batch dv, nkb] int32
+size_t at_vpre_bytes(long long batch, long long tk, long long dv) {
+  return align_up((size_t)(batch * dv) * (size_t)((tk + kAtKeys - 1) / kAtKeys) * 4, 1024);
+}
 
-using namespace sb200;
-
-size_t sb200_int8_attention_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv) {
+size_t at_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, int causal) {
   if (batch <= 0 || tq <= 0 || tk <= 0 || d <= 0 || dv <= 0 || d > kAtMaxDim || dv > kAtMaxDim || tk >= kAtMaxTk)
     return 0;
   if ((__int128)batch * tq >= (1LL << 31) || (__int128)batch * tk >= (1LL << 31)) return 0;
-  return at_layout(batch, tq, tk, d, dv).total + 1024;  // + the alignment of the base
+  return at_layout(batch, tq, tk, d, dv).total + (causal ? at_vpre_bytes(batch, tk, dv) : 0) +
+         1024;  // + the alignment of the base
 }
 
-int sb200_int8_attention(const float* q, const float* k, const float* v, const float* q_scale,
-                         const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale,
-                         const float* k_zero_point, int qmin_k, int qmax_k, const float* p_scale,
-                         const float* p_zero_point, int qmin_p, int qmax_p, const float* v_scale,
-                         const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale, float* out,
-                         int8_t* p_q, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
-                         size_t workspace_bytes, void* stream) {
-  const char* fn = "sb200_int8_attention";
+// The shared host code of both entry points; mask == null and causal == 0 runs int8_attention_kernel<false>.
+int attention_run(const char* fn, const float* q, const float* k, const float* v, const float* q_scale,
+                  const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale, const float* k_zero_point,
+                  int qmin_k, int qmax_k, const float* p_scale, const float* p_zero_point, int qmin_p, int qmax_p,
+                  const float* v_scale, const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale,
+                  const float* mask, int64_t mask_stride_outer, int64_t mask_stride_inner, int64_t mask_inner,
+                  int64_t mask_stride_row, int causal, float* out, int8_t* p_q, int64_t batch, int64_t tq, int64_t tk,
+                  int64_t d, int64_t dv, void* workspace, size_t workspace_bytes, void* stream) {
   SB_REQUIRE(q && k && v && q_scale && q_zero_point && k_scale && k_zero_point && p_scale && p_zero_point && v_scale &&
                  v_zero_point && out && workspace,
              "%s: null pointer argument", fn);
@@ -374,7 +492,19 @@ int sb200_int8_attention(const float* q, const float* k, const float* v, const f
     if (const int rc = int8_check_range(fn, r[0], r[1])) return rc;
   SB_REQUIRE(!has_scale || (scale == scale && scale - scale == 0.f), "%s: the scale %g is not finite", fn, (double)scale);
   SB_REQUIRE(p_q == nullptr || aligned16(p_q), "%s: p_q must be 16-byte aligned", fn);
-  const size_t need = sb200_int8_attention_workspace_bytes(batch, tq, tk, d, dv);
+  SB_REQUIRE(causal == 0 || causal == 1, "%s: causal must be 0 or 1, got %d", fn, causal);
+  if (mask != nullptr) {
+    SB_REQUIRE(mask_stride_outer >= 0 && mask_stride_inner >= 0 && mask_stride_row >= 0,
+               "%s: negative mask stride (outer %lld, inner %lld, row %lld)", fn, (long long)mask_stride_outer,
+               (long long)mask_stride_inner, (long long)mask_stride_row);
+    SB_REQUIRE(mask_inner > 0 && batch % mask_inner == 0, "%s: mask_inner = %lld must be positive and divide batch = %lld",
+               fn, (long long)mask_inner, (long long)batch);
+    SB_REQUIRE((reinterpret_cast<uintptr_t>(mask) & 3u) == 0, "%s: the mask must be 4-byte aligned", fn);
+    const __int128 last = (__int128)(batch / mask_inner - 1) * mask_stride_outer +
+                          (__int128)(mask_inner - 1) * mask_stride_inner + (__int128)(tq - 1) * mask_stride_row + tk - 1;
+    SB_REQUIRE(last < ((__int128)1 << 62), "%s: the mask's offsets exceed 2^62 elements", fn);
+  }
+  const size_t need = at_workspace_bytes(batch, tq, tk, d, dv, causal);
   if (workspace_bytes < need) {  // covers any alignment of the base
     set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
     return SB200_E_WORKSPACE;
@@ -408,6 +538,16 @@ int sb200_int8_attention(const float* q, const float* k, const float* v, const f
                                               reinterpret_cast<int32_t*>(ws + w.v_sum), ws + w.v_nan, batch, tk, dv,
                                               stream))
     return rc;
+  AtMask mk = {mask, mask_stride_outer, mask_stride_inner, mask_stride_row, nullptr, (int)(mask ? mask_inner : 1), causal,
+               (int)batch};
+  if (causal) {
+    int* pre = reinterpret_cast<int*>(ws + w.total);
+    const long long rows = batch * dv;
+    int8_attention_vprefix_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(vq, pre, rows, (int)tkp,
+                                                                              (int)((tk + kAtKeys - 1) / kAtKeys));
+    SB_LAUNCHED();
+    mk.v_pre = pre;
+  }
   AtParams a;
   a.q_sum = reinterpret_cast<const int*>(ws + w.q_sum), a.q_nan = ws + w.q_nan;
   a.k_sum = reinterpret_cast<const int*>(ws + w.k_sum), a.k_nan = ws + w.k_nan;
@@ -421,10 +561,58 @@ int sb200_int8_attention(const float* q, const float* k, const float* v, const f
   a.out = out, a.p_q = p_q;
   a.Tq = (int)tq, a.Tk = (int)tk, a.Tkp = (int)tkp, a.d = (int)d, a.dp = (int)dp, a.dv = (int)dv;
   a.vec2 = (dv % 2 == 0) && (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
-  static std::atomic<int> attr_done[64];
-  SB_CUDA(ensure_dyn_smem(int8_attention_kernel, (int)kAtSmem, attr_done));
   const long long ctas = batch * ((tq + kAtRows - 1) / kAtRows);
-  int8_attention_kernel<<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a);
+  if (mask == nullptr && !causal) {
+    static std::atomic<int> attr_done[64];
+    SB_CUDA(ensure_dyn_smem(int8_attention_kernel<false>, (int)kAtSmem, attr_done));
+    int8_attention_kernel<false><<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a, mk);
+  } else {
+    static std::atomic<int> attr_done[64];
+    SB_CUDA(ensure_dyn_smem(int8_attention_kernel<true>, (int)kAtSmem, attr_done));
+    int8_attention_kernel<true><<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a, mk);
+  }
   SB_LAUNCHED();
   return SB200_OK;
+}
+
+}  // namespace
+}  // namespace sb200
+
+using namespace sb200;
+
+size_t sb200_int8_attention_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv) {
+  return at_workspace_bytes(batch, tq, tk, d, dv, 0);
+}
+
+size_t sb200_int8_attention_masked_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv,
+                                                   int causal) {
+  return causal == 0 || causal == 1 ? at_workspace_bytes(batch, tq, tk, d, dv, causal) : 0;
+}
+
+int sb200_int8_attention(const float* q, const float* k, const float* v, const float* q_scale,
+                         const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale,
+                         const float* k_zero_point, int qmin_k, int qmax_k, const float* p_scale,
+                         const float* p_zero_point, int qmin_p, int qmax_p, const float* v_scale,
+                         const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale, float* out,
+                         int8_t* p_q, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  return attention_run("sb200_int8_attention", q, k, v, q_scale, q_zero_point, qmin_q, qmax_q, k_scale, k_zero_point,
+                       qmin_k, qmax_k, p_scale, p_zero_point, qmin_p, qmax_p, v_scale, v_zero_point, qmin_v, qmax_v,
+                       has_scale, scale, nullptr, 0, 0, 1, 0, 0, out, p_q, batch, tq, tk, d, dv, workspace,
+                       workspace_bytes, stream);
+}
+
+int sb200_int8_attention_masked(const float* q, const float* k, const float* v, const float* q_scale,
+                                const float* q_zero_point, int qmin_q, int qmax_q, const float* k_scale,
+                                const float* k_zero_point, int qmin_k, int qmax_k, const float* p_scale,
+                                const float* p_zero_point, int qmin_p, int qmax_p, const float* v_scale,
+                                const float* v_zero_point, int qmin_v, int qmax_v, int has_scale, float scale,
+                                const float* mask, int64_t mask_stride_outer, int64_t mask_stride_inner,
+                                int64_t mask_inner, int64_t mask_stride_row, int causal, float* out, int8_t* p_q,
+                                int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  return attention_run("sb200_int8_attention_masked", q, k, v, q_scale, q_zero_point, qmin_q, qmax_q, k_scale,
+                       k_zero_point, qmin_k, qmax_k, p_scale, p_zero_point, qmin_p, qmax_p, v_scale, v_zero_point,
+                       qmin_v, qmax_v, has_scale, scale, mask, mask_stride_outer, mask_stride_inner, mask_inner,
+                       mask_stride_row, causal, out, p_q, batch, tq, tk, d, dv, workspace, workspace_bytes, stream);
 }

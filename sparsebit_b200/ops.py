@@ -808,13 +808,66 @@ def int8_matmul(a, a_scale, a_zero_point, a_qrange, b, b_scale, b_zero_point, b_
     return out
 
 
-def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=None, return_p=False):
-    """``softmax(q @ k^T [* scale]) @ v`` with q, k, the softmax output p and v each on a per-tensor int8 grid, in one
-    fused kernel (sb200_int8_attention) that never writes the [Tq, Tk] scores: the scores are bit-identical to
-    ``int8_matmul(q, k^T)``, p is the fp32 softmax quantized with ``p_qparams``, and ``p @ v`` is exact on the grid.
+def attention_mask_check(attn_mask):
+    """``attn_mask`` as the fp32 additive mask the attention adds to its scores: float32 as is, float16 / bfloat16
+    up-cast (exact); a bool or any other mask raises ``TypeError``, since a bool mask has two conventions (True = keep in
+    ``scaled_dot_product_attention``, True = hide elsewhere) and the reference's models use additive masks."""
+    if not isinstance(attn_mask, torch.Tensor):
+        raise TypeError(f"attn_mask must be a tensor, got {type(attn_mask).__name__}")
+    if attn_mask.dtype == torch.bool:
+        raise TypeError("attn_mask is a bool mask; pass an additive float mask instead: 0 where a key is seen, -inf (or a "
+                        "large negative value such as -10000) where it is not, e.g. (1 - keep.float()) * -10000")
+    if attn_mask.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+        raise TypeError(f"attn_mask must be an additive float32, float16 or bfloat16 mask, got {attn_mask.dtype}")
+    return attn_mask.float()
+
+
+def attention_mask_strides(shape, strides, lead, tq, tk):
+    """How sb200_int8_attention_masked addresses a mask of ``shape`` and ``strides`` (in elements) broadcast to
+    ``lead + (tq, tk)``, the batch entries flattened: ``(stride_outer, stride_inner, inner, stride_row)`` with entry b at
+    ``(b // inner) stride_outer + (b % inner) stride_inner``, or None when the broadcast view cannot be addressed so (a
+    key stride other than 1, or batch dimensions that do not fold into two).  Raises ``ValueError`` when ``shape`` does
+    not broadcast to ``lead + (tq, tk)``."""
+    full = tuple(int(n) for n in lead) + (int(tq), int(tk))
+    shape, strides = tuple(int(n) for n in shape), tuple(int(s) for s in strides)
+    if len(shape) > len(full):
+        raise ValueError(f"a mask of shape {shape} does not broadcast to {full}")
+    pad = len(full) - len(shape)
+    shape, strides = (1,) * pad + shape, (0,) * pad + strides
+    es = []
+    for n, m, st in zip(full, shape, strides):
+        if m != n and m != 1:
+            raise ValueError(f"a mask of shape {shape[pad:]} does not broadcast to {full}")
+        es.append(st if m == n and n > 1 else 0)
+    if tk > 1 and es[-1] != 1:
+        return None
+    dims = []  # the batch dimensions of size > 1, adjacent ones folded where their strides allow
+    for n, st in zip(full[:-2], es[:-2]):
+        if n == 1:
+            continue
+        if dims and dims[-1][1] == st * n:
+            dims[-1] = (dims[-1][0] * n, st)
+        else:
+            dims.append((n, st))
+    if len(dims) > 2:
+        return None
+    if len(dims) < 2:
+        return (dims[0][1] if dims else 0, 0, 1, es[-2])
+    return (dims[0][1], dims[1][1], dims[1][0], es[-2])
+
+
+def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=None, return_p=False, attn_mask=None,
+                   causal=False):
+    """``softmax(q @ k^T [* scale] [masked]) @ v`` with q, k, the softmax output p and v each on a per-tensor int8 grid,
+    in one fused kernel (sb200_int8_attention, or sb200_int8_attention_masked with a mask or ``causal``) that never
+    writes the [Tq, Tk] scores: the scores are bit-identical to ``int8_matmul(q, k^T)``, p is the fp32 softmax
+    quantized with ``p_qparams``, and ``p @ v`` is exact on the grid.
     ``q`` [..., Tq, d], ``k`` [..., Tk, d], ``v`` [..., Tk, dv] fp32 with equal leading dimensions (no broadcasting);
     non-contiguous operands are made contiguous.  Each ``*_qparams`` is ``(scale, zero_point, (qmin, qmax))`` with
-    1-element fp32 tensors.  Returns fp32 [..., Tq, dv], and with ``return_p`` also the stored int8 grid of p
+    1-element fp32 tensors.  ``causal`` hides key j from row i when j > i + (Tk - Tq) (bottom-right, as
+    ``QAttention``); ``attn_mask`` is an additive float mask broadcastable to [..., Tq, Tk], added after the scale and
+    the causal band, read in place as a strided view when its broadcast can be addressed so (``attention_mask_strides``)
+    and copied otherwise.  Returns fp32 [..., Tq, dv], and with ``return_p`` also the stored int8 grid of p
     [..., Tq, round_up(Tk, 16)]."""
     lib = _lib.load()
     for x, name in ((q, "q"), (k, "k"), (v, "v")):
@@ -834,18 +887,41 @@ def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=No
     if dk != d or tkv != tk:
         raise SparsebitB200Error(f"int8_attention: q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} do not "
                                  "chain (q and k need the same d, k and v the same Tk)")
+    if causal not in (False, True):
+        raise SparsebitB200Error(f"int8_attention: causal must be a bool, got {causal!r}")
+    mask = None
+    if attn_mask is not None:
+        mask = attention_mask_check(attn_mask)
+        if mask.device != q.device:
+            raise SparsebitB200Error(f"int8_attention: attn_mask is on {mask.device}, q on {q.device}")
+        try:
+            plan = attention_mask_strides(mask.shape, mask.stride(), lead, tq, tk)
+        except ValueError as e:
+            raise SparsebitB200Error(f"int8_attention: attn_mask: {e}") from None
+        if plan is None:  # materialise the batch dimensions and the keys, keep a broadcast row
+            shape = (1,) * (len(lead) + 2 - mask.dim()) + tuple(mask.shape)
+            mask = mask.reshape(shape).expand(lead + (shape[-2], tk)).contiguous()
+            plan = attention_mask_strides(mask.shape, mask.stride(), lead, tq, tk)
     q, k, v = (x.reshape(-1, *x.shape[-2:]).contiguous() for x in (q, k, v))
     _req(q, "q"), _req(k, "k"), _req(v, "v")
     batch = q.shape[0]
     out = torch.empty(lead + (tq, dv), dtype=torch.float32, device=q.device)
     p_q = torch.empty(lead + (tq, int8_padded_k(tk)), dtype=torch.int8, device=q.device) if return_p else None
-    ws_bytes = int(lib.sb200_int8_attention_workspace_bytes(batch, tq, tk, d, dv))
-    ws = _int8_workspace(q.device, max(ws_bytes, 16))
-    with torch.cuda.device(q.device):
-        check(lib.sb200_int8_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), *qp, int(scale is not None),
-                                       float(scale) if scale is not None else 1.0, out.data_ptr(),
-                                       p_q.data_ptr() if p_q is not None else None, batch, tq, tk, d, dv, ws.data_ptr(),
-                                       ws.numel(), _stream(q)))
+    tail = [out.data_ptr(), p_q.data_ptr() if p_q is not None else None, batch, tq, tk, d, dv]
+    scl = [int(scale is not None), float(scale) if scale is not None else 1.0]
+    if mask is None and not causal:
+        ws_bytes = int(lib.sb200_int8_attention_workspace_bytes(batch, tq, tk, d, dv))
+        ws = _int8_workspace(q.device, max(ws_bytes, 16))
+        with torch.cuda.device(q.device):
+            check(lib.sb200_int8_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), *qp, *scl, *tail, ws.data_ptr(),
+                                           ws.numel(), _stream(q)))
+    else:
+        mk = [mask.data_ptr(), *plan[:3], plan[3]] if mask is not None else [None, 0, 0, 1, 0]
+        ws_bytes = int(lib.sb200_int8_attention_masked_workspace_bytes(batch, tq, tk, d, dv, int(causal)))
+        ws = _int8_workspace(q.device, max(ws_bytes, 16))
+        with torch.cuda.device(q.device):
+            check(lib.sb200_int8_attention_masked(q.data_ptr(), k.data_ptr(), v.data_ptr(), *qp, *scl, *mk, int(causal),
+                                                  *tail, ws.data_ptr(), ws.numel(), _stream(q)))
     return (out, p_q) if return_p else out
 
 

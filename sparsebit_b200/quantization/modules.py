@@ -7,6 +7,7 @@ exposing these attributes works with ``tools.CalibrationRunner``."""
 import math
 
 import torch
+import torch.fx
 import torch.nn as nn
 import torch.nn.functional as F
 
@@ -492,11 +493,37 @@ class QMatMulInt8(nn.Module):
         return f"left_qrange={list(self.left_qrange)}, right_qrange={list(self.right_qrange)}"
 
 
+def masked_scores(s, attn_mask=None, causal=False):
+    """The scores of ``QAttention`` after its mask: with ``causal`` the keys j > i + (Tk - Tq) of row i become -inf (the
+    band aligned bottom-right), then ``attn_mask`` is added in fp32.  A leaf of ``torch.fx`` traces (``fx.wrap``)."""
+    if causal:
+        tq, tk = s.shape[-2], s.shape[-1]
+        i = torch.arange(tq, device=s.device)[:, None]
+        j = torch.arange(tk, device=s.device)[None, :]
+        s = s.masked_fill(j > i + (tk - tq), float("-inf"))
+    if attn_mask is not None:
+        s = s + ops.attention_mask_check(attn_mask)
+    return s
+
+
+torch.fx.wrap("masked_scores")
+
+
 class QAttention(nn.Module):
     """Softmax attention between two ``QMatMul``: ``qk`` (carriers of q and k^T) and ``pv`` (carriers of the softmax
     output p and of v), the reference's MatMul -> Softmax -> MatMul behind its four ``QIdentity`` carriers.
-    ``forward(q, k, v) = pv(softmax(qk(q, k^T) [* scale], -1), v)``.  Like ``QMatMul`` it is not itself a quant
-    operator, so calibration (streaming or the fx replay) sees the four carriers."""
+    ``forward(q, k, v, attn_mask=None, causal=False)`` is, in this order::
+
+        s = qk(q, k^T); s = s * scale (when scale is not None)
+        causal:    s = where(j <= i + (Tk - Tq), s, -inf)   for query row i and key j
+        attn_mask: s = s + attn_mask                         (additive float, broadcastable to [..., Tq, Tk])
+        out = pv(softmax(s, -1), v)
+
+    The causal band is aligned bottom-right, as in the reference's GPT-2 example: with Tq < Tk the last query row sees
+    every key.  This is not the top-left ``is_causal`` of ``torch.nn.functional.scaled_dot_product_attention`` when
+    Tq != Tk.  A query row that sees no key (causal with Tq > Tk, or an all -inf mask row) is NaN, as ``softmax`` gives.
+    float16 / bfloat16 masks are up-cast (exact); a bool mask raises ``TypeError``.  Like ``QMatMul`` it is not itself a
+    quant operator, so calibration (streaming or the fx replay) sees the four carriers, p after the mask."""
 
     def __init__(self, scale=None):
         super().__init__()
@@ -516,10 +543,12 @@ class QAttention(nn.Module):
         self.qk.set_quant(w_quant, a_quant)
         self.pv.set_quant(w_quant, a_quant)
 
-    def forward(self, q, k, v):
+    def forward(self, q, k, v, attn_mask=None, causal=False):
         s = self.qk(q, k.transpose(-2, -1))
         if self.scale is not None:
             s = s * self.scale
+        if attn_mask is not None or causal:
+            s = masked_scores(s, attn_mask, causal)
         return self.pv(s.softmax(-1), v)
 
     def extra_repr(self):
@@ -548,7 +577,9 @@ class QAttentionInt8(nn.Module):
     integer grid -- q and k quantized on the fly, exact int8 scores on the tensor cores (bit-identical to
     ``QMatMulInt8``), the softmax in fp32 registers quantized with p's qparams, exact p @ v on the grid; the [Tq, Tk]
     scores never reach memory.  Built by ``from_qattention``.  q, k, v have equal leading dimensions; fp16 input is
-    up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps ``QAttention``."""
+    up-cast and the output is fp32, as in the fake-quant op.  ``attn_mask`` and ``causal`` are those of
+    ``QAttention.forward``, computed in the kernel (``ops.int8_attention``).  There is no backward: QAT keeps
+    ``QAttention``."""
 
     ROLES = ("q", "k", "p", "v")
 
@@ -577,12 +608,13 @@ class QAttentionInt8(nn.Module):
             mod.qranges[role] = tuple(q.qdesc.qrange)
         return mod
 
-    def forward(self, q, k, v):
+    def forward(self, q, k, v, attn_mask=None, causal=False):
         if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
             raise RuntimeError("QAttentionInt8 is inference-only and has no backward; run it under torch.no_grad() or "
                                "keep QAttention for training")
         qp = [(getattr(self, f"{r}_scale"), getattr(self, f"{r}_zero_point"), self.qranges[r]) for r in self.ROLES]
-        return ops.int8_attention(q.float(), k.float(), v.float(), *qp, scale=self.scale)
+        return ops.int8_attention(q.float(), k.float(), v.float(), *qp, scale=self.scale, attn_mask=attn_mask,
+                                  causal=causal)
 
     def extra_repr(self):
         return f"scale={self.scale}, " + ", ".join(f"{r}_qrange={list(self.qranges[r])}" for r in self.ROLES)
