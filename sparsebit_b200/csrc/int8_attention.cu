@@ -423,8 +423,6 @@ __global__ void __launch_bounds__(256) int8_attention_vprefix_kernel(const int8_
   }
 }
 
-static inline long long padded16(long long k) { return (k + 15) / 16 * 16; }
-
 // Workspace: the three stored operands, each 1024-aligned and followed by its int32 sums and NaN flags
 struct AtLayout {
   size_t q, q_sum, q_nan, k, k_sum, k_nan, v, v_sum, v_nan, total;
@@ -432,7 +430,7 @@ struct AtLayout {
 AtLayout at_layout(long long batch, long long tq, long long tk, long long d, long long dv) {
   AtLayout w;
   size_t o = 0;
-  const long long rows[3] = {batch * tq, batch * tk, batch * dv}, width[3] = {padded16(d), padded16(d), padded16(tk)};
+  const long long rows[3] = {batch * tq, batch * tk, batch * dv}, width[3] = {padded_k(d), padded_k(d), padded_k(tk)};
   size_t* q[3][3] = {{&w.q, &w.q_sum, &w.q_nan}, {&w.k, &w.k_sum, &w.k_nan}, {&w.v, &w.v_sum, &w.v_nan}};
   for (int i = 0; i < 3; ++i) {
     *q[i][0] = o;
@@ -489,7 +487,7 @@ int attention_run(const char* fn, const float* q, const float* k, const float* v
   if (const int rc = check_dims(fn, batch, tq, tk, d, dv)) return rc;
   const int ranges[4][2] = {{qmin_q, qmax_q}, {qmin_k, qmax_k}, {qmin_p, qmax_p}, {qmin_v, qmax_v}};
   for (const auto& r : ranges)
-    if (const int rc = int8_check_range(fn, r[0], r[1])) return rc;
+    if (const int rc = check_range(fn, r[0], r[1])) return rc;
   SB_REQUIRE(!has_scale || (scale == scale && scale - scale == 0.f), "%s: the scale %g is not finite", fn, (double)scale);
   SB_REQUIRE(p_q == nullptr || aligned16(p_q), "%s: p_q must be 16-byte aligned", fn);
   SB_REQUIRE(causal == 0 || causal == 1, "%s: causal must be 0 or 1, got %d", fn, causal);
@@ -504,17 +502,13 @@ int attention_run(const char* fn, const float* q, const float* k, const float* v
                           (__int128)(mask_inner - 1) * mask_stride_inner + (__int128)(tq - 1) * mask_stride_row + tk - 1;
     SB_REQUIRE(last < ((__int128)1 << 62), "%s: the mask's offsets exceed 2^62 elements", fn);
   }
-  const size_t need = at_workspace_bytes(batch, tq, tk, d, dv, causal);
-  if (workspace_bytes < need) {  // covers any alignment of the base
-    set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
-    return SB200_E_WORKSPACE;
-  }
+  if (const int rc = check_workspace(fn, workspace_bytes, at_workspace_bytes(batch, tq, tk, d, dv, causal))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const AtLayout w = at_layout(batch, tq, tk, d, dv);
   unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
   int8_t *qq = reinterpret_cast<int8_t*>(ws + w.q), *kq = reinterpret_cast<int8_t*>(ws + w.k);
   int8_t* vq = reinterpret_cast<int8_t*>(ws + w.v);
-  const long long dp = padded16(d), tkp = padded16(tk);
+  const long long dp = padded_k(d), tkp = padded_k(tk);
   CUtensorMap map_q, map_k, map_v;
   if (!make_map_3d(&map_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, qq, (uint64_t)dp, (uint64_t)tq, (uint64_t)batch, (uint64_t)dp,
                    128, kAtRows, CU_TENSOR_MAP_SWIZZLE_128B) ||
@@ -554,8 +548,8 @@ int attention_run(const char* fn, const float* q, const float* k, const float* v
   a.v_sum = reinterpret_cast<const int*>(ws + w.v_sum), a.v_nan = ws + w.v_nan;
   a.q_scale = q_scale, a.q_zero = q_zero_point, a.k_scale = k_scale, a.k_zero = k_zero_point;
   a.p_scale = p_scale, a.p_zero = p_zero_point, a.v_scale = v_scale, a.v_zero = v_zero_point;
-  a.q_off = int8_grid_offset(qmin_q), a.k_off = int8_grid_offset(qmin_k);
-  a.p_off = int8_grid_offset(qmin_p), a.v_off = int8_grid_offset(qmin_v);
+  a.q_off = grid_offset(qmin_q), a.k_off = grid_offset(qmin_k);
+  a.p_off = grid_offset(qmin_p), a.v_off = grid_offset(qmin_v);
   a.p_qmin = (float)qmin_p, a.p_qmax = (float)qmax_p;
   a.has_scale = has_scale != 0, a.scale = has_scale ? scale : 1.f;
   a.out = out, a.p_q = p_q;

@@ -409,11 +409,12 @@ int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64
   SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
   SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
   SB_REQUIRE(groups >= 2, "%s: groups = %lld; a conv with groups = 1 runs on sb200_int8_conv2d", fn, (long long)groups);
-  if (const int rc = int8_check_conv(fn, geom)) return rc;
+  long long oh, ow;
+  if (const int rc = int8_check_conv(fn, geom, &oh, &ow)) return rc;
   const sb200_conv2d_geom& g = *geom;
   SB_REQUIRE(g.c % groups == 0 && c_out % groups == 0, "%s: groups = %lld does not divide c = %lld and c_out = %lld", fn,
              (long long)groups, (long long)g.c, (long long)c_out);
-  if (const int rc = int8_check_range(fn, qmin_x, qmax_x)) return rc;
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
   const long long kg = (g.c / groups) * g.kh * g.kw;  // c, kh, kw < 2^31 each: c / groups * kh stays far below 2^63 / kw
   if ((__int128)(g.c / groups) * g.kh * g.kw >= kGcMaxKg) {
     set_error("%s: K_g = c / groups kh kw = %lld x %lld x %lld >= 2^17, the integer path supports K_g < 2^17 (|sum| <= "
@@ -421,16 +422,14 @@ int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64
     return SB200_E_UNSUPPORTED;
   }
   GcDims d{};
-  d.N = g.n, d.C = g.c, d.H = g.h, d.W = g.w, d.Cout = c_out;
-  d.OH = (g.h + g.pad_top + g.pad_bottom - g.dilation_h * (g.kh - 1) - 1) / g.stride_h + 1;
-  d.OW = (g.w + g.pad_left + g.pad_right - g.dilation_w * (g.kw - 1) - 1) / g.stride_w + 1;
+  d.N = g.n, d.C = g.c, d.H = g.h, d.W = g.w, d.Cout = c_out, d.OH = oh, d.OW = ow;
   d.Cg = (int)(g.c / groups), d.Mg = (int)(c_out / groups);
   d.KH = (int)g.kh, d.KW = (int)g.kw, d.sh = (int)g.stride_h, d.sw = (int)g.stride_w;
   d.dh = (int)g.dilation_h, d.dw = (int)g.dilation_w, d.pt = (int)g.pad_top, d.pl = (int)g.pad_left;
-  d.Kg = (int)kg, d.Kp = (int)(kg + 15) / 16 * 16;
+  d.Kg = (int)kg, d.Kp = (int)padded_k(kg);
   const int mode = gc_plan(&d, x);
   cudaStream_t st = (cudaStream_t)stream;
-  const int off = int8_grid_offset(qmin_x);
+  const int off = grid_offset(qmin_x);
   if (mode == kDirect) {
     const long long total = d.N * d.Cout * d.OH * d.OW;
     const unsigned grid = (unsigned)min(cdiv(total, kGcThreads), kGcMaxGrid);

@@ -69,9 +69,6 @@ struct I8MmSmem {
   I8MmCol col[kI8Feat];
 };
 
-static inline int grid_offset(int qmin) { return qmin >= 0 ? 128 : 0; }
-static inline long long padded_k(long long k) { return (k + 15) / 16 * 16; }
-
 // ---------------------------------------------------------------------------------- row quantizer
 // Every kernel of this file stores an element through stored_grid(v, p, off, nan) of int8_grid.cuh, the one
 // quantizer of the integer path, which the grouped conv kernel (int8_group_conv.cu) shares:
@@ -587,14 +584,11 @@ I8Layout i8_layout(long long M, long long K) {
   return w;
 }
 
-// the integer range [qmin, qmax] must fit s8 after the offset
-int check_range(const char* fn, int qmin, int qmax) {
-  SB_REQUIRE(qmin <= qmax, "%s: qmin %d > qmax %d", fn, qmin, qmax);
-  SB_REQUIRE((long long)qmax - qmin <= 255, "%s: integer range [%d, %d] is wider than 8 bits", fn, qmin, qmax);
-  const int off = grid_offset(qmin);
-  SB_REQUIRE(qmin - off >= -128 && qmax - off <= 127,
-             "%s: integer range [%d, %d] is neither signed 8-bit [-128, 127] nor unsigned 8-bit [0, 255]", fn, qmin, qmax);
-  return SB200_OK;
+// |a|, |b| <= 128: the s32 accumulator holds |sum a b| <= K * 2^14 for K < 2^17
+int check_k(const char* fn, long long k) {
+  if (k < kI8MaxK) return SB200_OK;
+  set_error("%s: K >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
+  return SB200_E_UNSUPPORTED;
 }
 
 int launch_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax, int8_t* q,
@@ -694,14 +688,6 @@ int check_conv(const char* fn, const sb200_conv2d_geom* g, ConvDims* d) {
   return SB200_OK;
 }
 
-int check_conv_k(const char* fn, const ConvDims& d) {
-  if (d.K >= kI8MaxK) {
-    set_error("%s: K = c kh kw >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
-    return SB200_E_UNSUPPORTED;
-  }
-  return SB200_OK;
-}
-
 int launch_im2col(const float* x, const ConvDims& d, const float* scale, const float* zero_point, int qmin, int qmax,
                   int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st) {
   int8_im2col_quantize_kernel<<<(unsigned)((d.M + kLowPix - 1) / kLowPix), kLowThreads, 0, st>>>(
@@ -727,10 +713,7 @@ int sb200_int8_quantize_rows(const float* x, const float* scale, const float* ze
   SB_REQUIRE(rows < (1LL << 31), "sb200_int8_quantize_rows: too many rows (%lld)", (long long)rows);
   if (const int rc = check_range("sb200_int8_quantize_rows", qmin, qmax)) return rc;
   SB_REQUIRE(aligned16(q), "sb200_int8_quantize_rows: q must be 16-byte aligned");
-  if (k >= kI8MaxK) {
-    set_error("sb200_int8_quantize_rows: K = %lld, the integer path supports K < 2^17", (long long)k);
-    return SB200_E_UNSUPPORTED;
-  }
+  if (const int rc = check_k("sb200_int8_quantize_rows", k)) return rc;
   return launch_rows(x, scale, zero_point, per_row != 0, qmin, qmax, q, reinterpret_cast<int*>(row_sum), nan_flag, rows, k,
                      (cudaStream_t)stream);
 }
@@ -746,16 +729,9 @@ int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_
   SB_REQUIRE(m < (1LL << 31) && n < (1LL << 31), "sb200_int8_linear: dimension too large");
   if (const int rc = check_range("sb200_int8_linear", qmin_x, qmax_x)) return rc;
   SB_REQUIRE(aligned16(w_q), "sb200_int8_linear: w_q must be 16-byte aligned");
-  if (k >= kI8MaxK) {
-    set_error("sb200_int8_linear: K = %lld, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)",
-              (long long)k);
-    return SB200_E_UNSUPPORTED;
-  }
-  if (workspace_bytes < sb200_int8_linear_workspace_bytes(m, k)) {  // covers any alignment of the base
-    set_error("sb200_int8_linear: workspace too small (%zu bytes, need %zu)", workspace_bytes,
-              sb200_int8_linear_workspace_bytes(m, k));
-    return SB200_E_WORKSPACE;
-  }
+  if (const int rc = check_k("sb200_int8_linear", k)) return rc;
+  if (const int rc = check_workspace("sb200_int8_linear", workspace_bytes, sb200_int8_linear_workspace_bytes(m, k)))
+    return rc;
   return run_gemm<false>("sb200_int8_linear", m, k, n, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero,
                          bias, out, workspace, (cudaStream_t)stream,
                          [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
@@ -778,7 +754,7 @@ int sb200_int8_im2col_quantize(const float* x, const sb200_conv2d_geom* geom, co
   if (const int rc = check_conv(fn, geom, &d)) return rc;
   if (const int rc = check_range(fn, qmin, qmax)) return rc;
   SB_REQUIRE(aligned16(q), "%s: q must be 16-byte aligned", fn);
-  if (const int rc = check_conv_k(fn, d)) return rc;
+  if (const int rc = check_k(fn, d.K)) return rc;
   return launch_im2col(x, d, scale, zero_point, qmin, qmax, q, reinterpret_cast<int*>(row_sum), nan_flag,
                        (cudaStream_t)stream);
 }
@@ -796,12 +772,8 @@ int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float
   if (const int rc = check_conv(fn, geom, &d)) return rc;
   if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
   SB_REQUIRE(aligned16(w_q), "%s: w_q must be 16-byte aligned", fn);
-  if (const int rc = check_conv_k(fn, d)) return rc;
-  const size_t need = sb200_int8_conv2d_workspace_bytes(geom);
-  if (workspace_bytes < need) {
-    set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
-    return SB200_E_WORKSPACE;
-  }
+  if (const int rc = check_k(fn, d.K)) return rc;
+  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
   return run_gemm<true>(fn, d.M, d.K, c_out, d.P, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
                         out, workspace, (cudaStream_t)stream,
                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
@@ -825,10 +797,7 @@ int sb200_int8_quantize_cols(const float* x, const float* scale, const float* ze
              (long long)batch, (long long)n);
   if (const int rc = check_range(fn, qmin, qmax)) return rc;
   SB_REQUIRE(aligned16(q), "%s: q must be 16-byte aligned", fn);
-  if (k >= kI8MaxK) {
-    set_error("%s: K = %lld, the integer path supports K < 2^17", fn, (long long)k);
-    return SB200_E_UNSUPPORTED;
-  }
+  if (const int rc = check_k(fn, k)) return rc;
   return launch_cols(x, scale, zero_point, qmin, qmax, q, reinterpret_cast<int*>(col_sum), nan_flag, batch, k, n,
                      (cudaStream_t)stream);
 }
@@ -849,15 +818,8 @@ int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float
              (long long)((m + kI8Rows - 1) / kI8Rows), (long long)((n + kI8Feat - 1) / kI8Feat));
   if (const int rc = check_range(fn, qmin_a, qmax_a)) return rc;
   if (const int rc = check_range(fn, qmin_b, qmax_b)) return rc;
-  if (k >= kI8MaxK) {
-    set_error("%s: K = %lld, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn, (long long)k);
-    return SB200_E_UNSUPPORTED;
-  }
-  const size_t need = sb200_int8_matmul_workspace_bytes(batch, m, k, n);
-  if (workspace_bytes < need) {  // covers any alignment of the base
-    set_error("%s: workspace too small (%zu bytes, need %zu)", fn, workspace_bytes, need);
-    return SB200_E_WORKSPACE;
-  }
+  if (const int rc = check_k(fn, k)) return rc;
+  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_matmul_workspace_bytes(batch, m, k, n))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const I8Layout la = i8_layout(batch * m, k), lb = i8_layout(batch * n, k);
   unsigned char* wa = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
@@ -896,10 +858,10 @@ int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float
 
 // ---------------------------------------------------------------------------------- shared with int8_group_conv.cu
 namespace sb200 {
-int int8_check_conv(const char* fn, const sb200_conv2d_geom* g) {
+int int8_check_conv(const char* fn, const sb200_conv2d_geom* g, long long* oh, long long* ow) {
   ConvDims d;
-  return check_conv(fn, g, &d);
+  if (const int rc = check_conv(fn, g, &d)) return rc;
+  *oh = d.P / d.OW, *ow = d.OW;
+  return SB200_OK;
 }
-int int8_check_range(const char* fn, int qmin, int qmax) { return check_range(fn, qmin, qmax); }
-int int8_grid_offset(int qmin) { return grid_offset(qmin); }
 }  // namespace sb200

@@ -683,6 +683,28 @@ def int8_padded_k(k):
     return (int(k) + 15) // 16 * 16
 
 
+def _check_per_tensor(fn, *qparams):
+    """The activation operands of the integer path are per-tensor: one scale and one zero point each."""
+    if any(t.numel() != 1 for t in qparams):
+        raise SparsebitB200Error(f"{fn}: the qparams are per-tensor (1 element each)")
+
+
+def _req_int8_operands(x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias):
+    """The dtypes of a per-tensor fp32 activation and of the weight operand ``int8_quantize_rows`` stores."""
+    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
+    if bias is not None:
+        _req(bias, "bias")
+
+
+def _int8_weight_rows(fn, w_q, w_rowsum, w_scale, w_zero, bias):
+    """N, the rows of the stored weight operand (w_q [N, Kp]), which each per-row term must match."""
+    n = w_q.shape[0]
+    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"{fn}: w_rowsum / w_scale / w_zero / bias need {n} elements")
+    return n
+
+
 def int8_quantize_rows(x, scale, zero_point, qmin, qmax):
     """Integer grid of every row of ``x`` [rows, K] (sb200_int8_quantize_rows): returns ``(q, row_sum, nan)`` with
     q int8 [rows, Kp] = clamp(round(x / s) + rint(zp), qmin, qmax) - int8_grid_offset(qmin), the padding to
@@ -725,16 +747,11 @@ def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     int32 [N], w_scale fp32 [N], w_zero int32 [N] = rint(zero point) - int8_grid_offset).  ``x`` [..., K] fp32; returns
     fp32 [..., N].  ``k`` defaults to x.shape[-1]."""
     lib = _lib.load()
-    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
-    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
-    if bias is not None:
-        _req(bias, "bias")
+    _req_int8_operands(x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias)
     k = x.shape[-1] if k is None else int(k)
     if x.shape[-1] != k or w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
         raise SparsebitB200Error(f"int8_linear: x has {x.shape[-1]} features, w_q is {tuple(w_q.shape)} (need [N, {int8_padded_k(k)}])")
-    n = w_q.shape[0]
-    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
-        raise SparsebitB200Error(f"int8_linear: w_rowsum / w_scale / w_zero / bias need {n} elements")
+    n = _int8_weight_rows("int8_linear", w_q, w_rowsum, w_scale, w_zero, bias)
     m = x.numel() // k
     out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
     ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
@@ -755,8 +772,7 @@ def int8_quantize_cols(x, scale, zero_point, qmin, qmax):
     _req(x, "data"), _req(scale, "scale"), _req(zero_point, "zero_point")
     if x.dim() < 2:
         raise SparsebitB200Error("int8_quantize_cols: data must be [..., K, N]")
-    if scale.numel() != 1 or zero_point.numel() != 1:
-        raise SparsebitB200Error("int8_quantize_cols: the qparams are per-tensor (1 element each)")
+    _check_per_tensor("int8_quantize_cols", scale, zero_point)
     lead, (k, n) = tuple(x.shape[:-2]), x.shape[-2:]
     batch = x.numel() // (k * n)
     q = torch.empty(lead + (n, int8_padded_k(k)), dtype=torch.int8, device=x.device)
@@ -785,8 +801,7 @@ def int8_matmul(a, a_scale, a_zero_point, a_qrange, b, b_scale, b_zero_point, b_
         if not isinstance(t, torch.Tensor) or t.dim() < 2:
             raise SparsebitB200Error(f"int8_matmul: {name} must be a tensor with at least 2 dimensions")
     _req(a_scale, "a_scale"), _req(a_zero_point, "a_zero_point"), _req(b_scale, "b_scale"), _req(b_zero_point, "b_zero_point")
-    if any(t.numel() != 1 for t in (a_scale, a_zero_point, b_scale, b_zero_point)):
-        raise SparsebitB200Error("int8_matmul: the qparams of both operands are per-tensor (1 element each)")
+    _check_per_tensor("int8_matmul", a_scale, a_zero_point, b_scale, b_zero_point)
     (m, k), (kb, n) = a.shape[-2:], b.shape[-2:]
     if k != kb:
         raise SparsebitB200Error(f"int8_matmul: a is {tuple(a.shape)}, b is {tuple(b.shape)} (inner dimensions differ)")
@@ -876,8 +891,7 @@ def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=No
     qp = []
     for (s, z, qrange), name in ((q_qparams, "q"), (k_qparams, "k"), (p_qparams, "p"), (v_qparams, "v")):
         _req(s, f"{name}_scale"), _req(z, f"{name}_zero_point")
-        if s.numel() != 1 or z.numel() != 1:
-            raise SparsebitB200Error("int8_attention: the qparams of every operand are per-tensor (1 element each)")
+        _check_per_tensor("int8_attention", s, z)
         qp += [s.data_ptr(), z.data_ptr(), int(qrange[0]), int(qrange[1])]
     lead = tuple(q.shape[:-2])
     if tuple(k.shape[:-2]) != lead or tuple(v.shape[:-2]) != lead:
@@ -951,6 +965,25 @@ def conv2d_output_hw(g):
     return oh, ow
 
 
+def _int8_conv_prelude(fn, x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups, bias, stride,
+                       padding, dilation):
+    """The argument checks of ``int8_conv2d`` (groups = 1) and ``int8_group_conv2d``: returns the ``Conv2dGeom``, C_out
+    and the fp32 [N, C_out, OH, OW] output (one pixel when the kernel does not fit, which the C entry points reject)."""
+    _req_int8_operands(x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias)
+    if x.dim() != 4:
+        raise SparsebitB200Error(f"{fn}: data must be [N, C, H, W]")
+    groups = int(groups)
+    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
+    if groups < 1 or g.c % groups:
+        raise SparsebitB200Error(f"{fn}: groups = {groups} does not divide C = {g.c}")
+    kp = int8_padded_k(g.c // groups * g.kh * g.kw)
+    if w_q.dim() != 2 or w_q.shape[1] != kp:
+        raise SparsebitB200Error(f"{fn}: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {kp}]")
+    n = _int8_weight_rows(fn, w_q, w_rowsum, w_scale, w_zero, bias)
+    oh, ow = conv2d_output_hw(g)
+    return g, n, torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+
+
 def int8_im2col_quantize(x, kernel_size, scale, zero_point, qmin, qmax, stride=1, padding=0, dilation=1):
     """The lowered integer grid of a conv input (sb200_int8_im2col_quantize): ``x`` [N, C, H, W] fp32 -> ``(q, row_sum,
     nan)`` with q int8 [M, Kp], M = N OH OW (m = (n OH + oh) OW + ow), K = C KH KW (k = (c KH + kh) KW + kw), Kp =
@@ -960,8 +993,7 @@ def int8_im2col_quantize(x, kernel_size, scale, zero_point, qmin, qmax, stride=1
     _req(x, "data"), _req(scale, "scale"), _req(zero_point, "zero_point")
     if x.dim() != 4:
         raise SparsebitB200Error("int8_im2col_quantize: data must be [N, C, H, W]")
-    if scale.numel() != 1 or zero_point.numel() != 1:
-        raise SparsebitB200Error("int8_im2col_quantize: the activation qparams are per-tensor (1 element each)")
+    _check_per_tensor("int8_im2col_quantize", scale, zero_point)
     g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
     oh, ow = conv2d_output_hw(g)
     m = g.n * max(oh, 0) * max(ow, 0)
@@ -983,21 +1015,8 @@ def int8_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     ``int8_linear``.  Returns fp32 [N, C_out, OH, OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left,
     right)."""
     lib = _lib.load()
-    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
-    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
-    if bias is not None:
-        _req(bias, "bias")
-    if x.dim() != 4:
-        raise SparsebitB200Error("int8_conv2d: data must be [N, C, H, W]")
-    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
-    k = g.c * g.kh * g.kw
-    if w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
-        raise SparsebitB200Error(f"int8_conv2d: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {int8_padded_k(k)}]")
-    n = w_q.shape[0]
-    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
-        raise SparsebitB200Error(f"int8_conv2d: w_rowsum / w_scale / w_zero / bias need {n} elements")
-    oh, ow = conv2d_output_hw(g)
-    out = torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    g, n, out = _int8_conv_prelude("int8_conv2d", x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, kernel_size, 1,
+                                   bias, stride, padding, dilation)
     ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     ws = _int8_workspace(x.device, max(ws_bytes, 16))
     with torch.cuda.device(x.device):
@@ -1016,26 +1035,10 @@ def int8_group_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_sca
     round_up(C / groups KH KW, 16), w_rowsum int32, w_scale fp32, w_zero int32 [C_out]).  Returns fp32 [N, C_out, OH,
     OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right).  No workspace."""
     lib = _lib.load()
-    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
-    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
-    if bias is not None:
-        _req(bias, "bias")
-    if x.dim() != 4:
-        raise SparsebitB200Error("int8_group_conv2d: data must be [N, C, H, W]")
-    groups = int(groups)
-    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
-    if groups < 1 or g.c % groups:
-        raise SparsebitB200Error(f"int8_group_conv2d: groups = {groups} does not divide C = {g.c}")
-    k = g.c // groups * g.kh * g.kw
-    if w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
-        raise SparsebitB200Error(f"int8_group_conv2d: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {int8_padded_k(k)}]")
-    n = w_q.shape[0]
-    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
-        raise SparsebitB200Error(f"int8_group_conv2d: w_rowsum / w_scale / w_zero / bias need {n} elements")
-    oh, ow = conv2d_output_hw(g)
-    out = torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    g, n, out = _int8_conv_prelude("int8_group_conv2d", x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero,
+                                   kernel_size, groups, bias, stride, padding, dilation)
     with torch.cuda.device(x.device):
-        check(lib.sb200_int8_group_conv2d(x.data_ptr(), ctypes.byref(g), groups, x_scale.data_ptr(),
+        check(lib.sb200_int8_group_conv2d(x.data_ptr(), ctypes.byref(g), int(groups), x_scale.data_ptr(),
                                           x_zero_point.data_ptr(), int(qmin), int(qmax), w_q.data_ptr(),
                                           w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                           bias.data_ptr() if bias is not None else None, out.data_ptr(), n, _stream(x)))

@@ -12,6 +12,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
+from ..ops import _pair
 from .common import Backend
 from .quantizers import build_quantizer
 from .quantizers.quant_tensor import check_trt_symmetric
@@ -151,17 +152,21 @@ def _int8_weight_rows(wq, weight):
     return w_q, w_sum, w_scale, w_zero
 
 
-class QLinearInt8(nn.Module):
-    """Inference-only replacement of a calibrated ``QLinear``: the fake-quant linear computed on the integer grid by
-    ``ops.int8_linear`` (exact int8 x int8 sums on the tensor cores, zero points removed in int64, then
-    s_x s_w[n] I + bias).  Built by ``from_qlinear``; the weights are quantized once at conversion.  fp16 input is
-    up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps ``QLinear``."""
+def _check_inference_only(mod, training_cls, *inputs):
+    """The integer-grid modules have no backward: an input that needs a gradient is an error, not a silent detach."""
+    if torch.is_grad_enabled() and any(x.requires_grad for x in inputs):
+        raise RuntimeError(f"{type(mod).__name__} is inference-only and has no backward; run it under torch.no_grad() or "
+                           f"keep {training_cls} for training")
 
-    def __init__(self, in_features, out_features, device):
+
+class _Int8WeightModule(nn.Module):
+    """The stored weight operand of ``QLinearInt8`` / ``QConv2dInt8``: ``w_q`` int8 [N, Kp] and ``w_rowsum`` /
+    ``w_scale`` / ``w_zero`` [N] as ``_int8_weight_rows`` stores them, the per-tensor activation ``scale`` /
+    ``zero_point`` and integer range ``qmin`` / ``qmax``, and ``bias`` (fp32 or None)."""
+
+    def __init__(self, out_features, k, device):
         super().__init__()
-        self.in_features, self.out_features = int(in_features), int(out_features)
-        kp = ops.int8_padded_k(in_features)
-        self.register_buffer("w_q", torch.zeros(out_features, kp, dtype=torch.int8, device=device))
+        self.register_buffer("w_q", torch.zeros(out_features, ops.int8_padded_k(k), dtype=torch.int8, device=device))
         self.register_buffer("w_rowsum", torch.zeros(out_features, dtype=torch.int32, device=device))
         self.register_buffer("w_scale", torch.zeros(out_features, dtype=torch.float32, device=device))
         self.register_buffer("w_zero", torch.zeros(out_features, dtype=torch.int32, device=device))
@@ -171,39 +176,50 @@ class QLinearInt8(nn.Module):
         self.qmin, self.qmax = -128, 127
 
     @classmethod
-    def from_qlinear(cls, qlinear):
-        reason = int8_ineligibility(qlinear)
+    def _check_eligible(cls, reason, method):
         if reason is not None:
-            raise ValueError(f"QLinearInt8.from_qlinear: {reason}")
-        aq, wq = qlinear.input_quantizer, qlinear.weight_quantizer
-        weight = qlinear.weight.detach()
-        n, k = weight.shape
-        mod = cls(k, n, weight.device)
+            raise ValueError(f"{cls.__name__}.{method}: {reason}")
+
+    def _load(self, qmod):
+        """Fills the buffers from the calibrated ``qmod`` (a ``QLinear`` or ``QConv2d``); returns ``self``."""
+        aq = qmod.input_quantizer
         with torch.no_grad():
-            for buf, v in zip((mod.w_q, mod.w_rowsum, mod.w_scale, mod.w_zero), _int8_weight_rows(wq, qlinear.weight)):
+            for buf, v in zip((self.w_q, self.w_rowsum, self.w_scale, self.w_zero),
+                              _int8_weight_rows(qmod.weight_quantizer, qmod.weight)):
                 buf.copy_(v)
             xs, xz = _qparams(aq, None)
-            mod.scale.copy_(xs.reshape(1))
-            mod.zero_point.copy_(xz.reshape(1))
-            if qlinear.bias is not None:
-                mod.bias = qlinear.bias.detach().float().clone().contiguous()
-        mod.qmin, mod.qmax = aq.qdesc.qrange
-        return mod
+            self.scale.copy_(xs.reshape(1))
+            self.zero_point.copy_(xz.reshape(1))
+            if qmod.bias is not None:
+                self.bias = qmod.bias.detach().float().clone().contiguous()
+        self.qmin, self.qmax = aq.qdesc.qrange
+        return self
+
+
+class QLinearInt8(_Int8WeightModule):
+    """Inference-only replacement of a calibrated ``QLinear``: the fake-quant linear computed on the integer grid by
+    ``ops.int8_linear`` (exact int8 x int8 sums on the tensor cores, zero points removed in int64, then
+    s_x s_w[n] I + bias).  Built by ``from_qlinear``; the weights are quantized once at conversion.  fp16 input is
+    up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps ``QLinear``."""
+
+    def __init__(self, in_features, out_features, device):
+        super().__init__(out_features, in_features, device)
+        self.in_features, self.out_features = int(in_features), int(out_features)
+
+    @classmethod
+    def from_qlinear(cls, qlinear):
+        cls._check_eligible(int8_ineligibility(qlinear), "from_qlinear")
+        n, k = qlinear.weight.shape
+        return cls(k, n, qlinear.weight.device)._load(qlinear)
 
     def forward(self, x_in):
-        if torch.is_grad_enabled() and x_in.requires_grad:
-            raise RuntimeError("QLinearInt8 is inference-only and has no backward; run it under torch.no_grad() or "
-                               "keep QLinear for training")
+        _check_inference_only(self, "QLinear", x_in)
         x = x_in.float() if x_in.dtype != torch.float32 else x_in
         return ops.int8_linear(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
                                self.w_scale, self.w_zero, self.bias, k=self.in_features)
 
     def extra_repr(self):
         return f"in_features={self.in_features}, out_features={self.out_features}, qrange=[{self.qmin}, {self.qmax}]"
-
-
-def _pair(v):
-    return (int(v), int(v)) if isinstance(v, int) else tuple(int(e) for e in v)
 
 
 def resolve_conv_padding(padding, kernel_size, dilation=1, stride=1):
@@ -231,24 +247,36 @@ def resolve_conv_padding(padding, kernel_size, dilation=1, stride=1):
     return (ph, ph, pw, pw)
 
 
-def int8_conv_ineligibility(qconv):
-    """Why ``QConv2dInt8.from_qconv2d`` cannot convert ``qconv`` (None when it can)."""
+def _int8_conv_ineligibility(qconv, groups_rule):
+    """The conversion rules of a ``QConv2d`` in the order they are reported: the quantizer rules, then
+    ``groups_rule(groups, K_g)`` (a reason or None; K_g = C / groups KH KW), then the padding."""
     if not isinstance(qconv, QConv2d):
         return f"expected a QConv2d, got {type(qconv).__name__}"
     reason = _int8_quantizer_ineligibility(qconv)
     if reason is not None:
         return reason
     kw = qconv.fwd_kwargs
-    if kw["groups"] != 1:
-        return f"the conv has groups = {kw['groups']} (the integer path runs groups = 1 only)"
+    c_out, c_g, kh, kwd = qconv.weight.shape
+    reason = groups_rule(kw["groups"], c_g * kh * kwd)
+    if reason is not None:
+        return reason
     try:
-        resolve_conv_padding(kw["padding"], qconv.weight.shape[2:], kw["dilation"], kw["stride"])
+        resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
     except ValueError as e:
         return f"the conv's {e}"
     return None
 
 
-class QConv2dInt8(nn.Module):
+def _dense_conv_rule(groups, k_g):
+    return None if groups == 1 else f"the conv has groups = {groups} (the integer path runs groups = 1 only)"
+
+
+def int8_conv_ineligibility(qconv):
+    """Why ``QConv2dInt8.from_qconv2d`` cannot convert ``qconv`` (None when it can)."""
+    return _int8_conv_ineligibility(qconv, _dense_conv_rule)
+
+
+class QConv2dInt8(_Int8WeightModule):
     """Inference-only replacement of a calibrated ``QConv2d`` (groups = 1): the fake-quant conv2d computed on the
     integer grid by ``ops.int8_conv2d`` -- the input lowered to its int8 grid in one pass, exact int8 x int8 sums on the
     tensor cores, zero points removed in int64, then s_x s_w[n] I + bias, written NCHW.  Built by ``from_qconv2d``; the
@@ -256,54 +284,36 @@ class QConv2dInt8(nn.Module):
     [C, H, W]; fp16 input is up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps
     ``QConv2d``."""
 
-    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device):
-        super().__init__()
-        self.in_channels, self.out_channels = int(in_channels), int(out_channels)
+    _ineligibility = staticmethod(int8_conv_ineligibility)
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device, groups=1):
+        super().__init__(out_channels, in_channels // int(groups) * kernel_size[0] * kernel_size[1], device)
+        self.in_channels, self.out_channels, self.groups = int(in_channels), int(out_channels), int(groups)
         self.kernel_size, self.stride, self.dilation = tuple(kernel_size), tuple(stride), tuple(dilation)
         self.padding = tuple(padding)  # (top, bottom, left, right)
-        kp = ops.int8_padded_k(in_channels * self.kernel_size[0] * self.kernel_size[1])
-        self.register_buffer("w_q", torch.zeros(out_channels, kp, dtype=torch.int8, device=device))
-        self.register_buffer("w_rowsum", torch.zeros(out_channels, dtype=torch.int32, device=device))
-        self.register_buffer("w_scale", torch.zeros(out_channels, dtype=torch.float32, device=device))
-        self.register_buffer("w_zero", torch.zeros(out_channels, dtype=torch.int32, device=device))
-        self.register_buffer("scale", torch.ones(1, dtype=torch.float32, device=device))
-        self.register_buffer("zero_point", torch.zeros(1, dtype=torch.float32, device=device))
-        self.register_buffer("bias", None)
-        self.qmin, self.qmax = -128, 127
 
     @classmethod
     def from_qconv2d(cls, qconv):
-        reason = int8_conv_ineligibility(qconv)
-        if reason is not None:
-            raise ValueError(f"QConv2dInt8.from_qconv2d: {reason}")
-        aq, wq = qconv.input_quantizer, qconv.weight_quantizer
+        cls._check_eligible(cls._ineligibility(qconv), "from_qconv2d")
         kw = qconv.fwd_kwargs
-        weight = qconv.weight.detach()
-        c_out, c_in, kh, kwd = weight.shape
+        c_out, c_g, kh, kwd = qconv.weight.shape
+        groups = int(kw["groups"])
         padding = resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
-        mod = cls(c_in, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]), weight.device)
-        with torch.no_grad():
-            for buf, v in zip((mod.w_q, mod.w_rowsum, mod.w_scale, mod.w_zero), _int8_weight_rows(wq, qconv.weight)):
-                buf.copy_(v)
-            xs, xz = _qparams(aq, None)
-            mod.scale.copy_(xs.reshape(1))
-            mod.zero_point.copy_(xz.reshape(1))
-            if qconv.bias is not None:
-                mod.bias = qconv.bias.detach().float().clone().contiguous()
-        mod.qmin, mod.qmax = aq.qdesc.qrange
-        return mod
+        return cls(c_g * groups, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]),
+                   device=qconv.weight.device, groups=groups)._load(qconv)
+
+    def _conv(self, x):
+        return ops.int8_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
+                               self.w_scale, self.w_zero, self.kernel_size, self.bias, self.stride, self.padding,
+                               self.dilation)
 
     def forward(self, x_in):
-        if torch.is_grad_enabled() and x_in.requires_grad:
-            raise RuntimeError("QConv2dInt8 is inference-only and has no backward; run it under torch.no_grad() or "
-                               "keep QConv2d for training")
+        _check_inference_only(self, "QConv2d", x_in)
         x = x_in.float() if x_in.dtype != torch.float32 else x_in
         unbatched = x.dim() == 3
         if unbatched:
             x = x.unsqueeze(0)
-        y = ops.int8_conv2d(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
-                            self.w_scale, self.w_zero, self.kernel_size, self.bias, self.stride, self.padding,
-                            self.dilation)
+        y = self._conv(x.contiguous())
         return y.squeeze(0) if unbatched else y
 
     def extra_repr(self):
@@ -314,24 +324,17 @@ class QConv2dInt8(nn.Module):
 INT8_MAX_KG = 1 << 17  # sb200_int8_group_conv2d: K_g = C / groups KH KW must stay below 2^17 (exact int32 sums)
 
 
+def _group_conv_rule(groups, k_g):
+    if groups == 1:
+        return "groups = 1: use QConv2dInt8 / to_integer_convs"
+    if k_g >= INT8_MAX_KG:
+        return f"K_g = C / groups KH KW = {k_g} >= 2^17 (the integer sums must stay exact in int32)"
+    return None
+
+
 def int8_group_conv_ineligibility(qconv):
     """Why ``QConv2dGroupInt8.from_qconv2d`` cannot convert ``qconv`` (None when it can)."""
-    if not isinstance(qconv, QConv2d):
-        return f"expected a QConv2d, got {type(qconv).__name__}"
-    reason = _int8_quantizer_ineligibility(qconv)
-    if reason is not None:
-        return reason
-    kw = qconv.fwd_kwargs
-    if kw["groups"] == 1:
-        return "groups = 1: use QConv2dInt8 / to_integer_convs"
-    c_out, c_g, kh, kwd = qconv.weight.shape
-    if c_g * kh * kwd >= INT8_MAX_KG:
-        return f"K_g = C / groups KH KW = {c_g * kh * kwd} >= 2^17 (the integer sums must stay exact in int32)"
-    try:
-        resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
-    except ValueError as e:
-        return f"the conv's {e}"
-    return None
+    return _int8_conv_ineligibility(qconv, _group_conv_rule)
 
 
 class QConv2dGroupInt8(QConv2dInt8):
@@ -342,60 +345,19 @@ class QConv2dGroupInt8(QConv2dInt8):
     once at conversion.  Takes [N, C, H, W] or unbatched [C, H, W]; fp16 input is up-cast and the output is fp32, as in
     the fake-quant op.  There is no backward: QAT keeps ``QConv2d``."""
 
+    _ineligibility = staticmethod(int8_group_conv_ineligibility)
+
     def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, groups, device):
-        nn.Module.__init__(self)
-        self.in_channels, self.out_channels, self.groups = int(in_channels), int(out_channels), int(groups)
-        self.kernel_size, self.stride, self.dilation = tuple(kernel_size), tuple(stride), tuple(dilation)
-        self.padding = tuple(padding)  # (top, bottom, left, right)
-        kp = ops.int8_padded_k(in_channels // self.groups * self.kernel_size[0] * self.kernel_size[1])
-        self.register_buffer("w_q", torch.zeros(out_channels, kp, dtype=torch.int8, device=device))
-        self.register_buffer("w_rowsum", torch.zeros(out_channels, dtype=torch.int32, device=device))
-        self.register_buffer("w_scale", torch.zeros(out_channels, dtype=torch.float32, device=device))
-        self.register_buffer("w_zero", torch.zeros(out_channels, dtype=torch.int32, device=device))
-        self.register_buffer("scale", torch.ones(1, dtype=torch.float32, device=device))
-        self.register_buffer("zero_point", torch.zeros(1, dtype=torch.float32, device=device))
-        self.register_buffer("bias", None)
-        self.qmin, self.qmax = -128, 127
+        super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, device, groups)
 
-    @classmethod
-    def from_qconv2d(cls, qconv):
-        reason = int8_group_conv_ineligibility(qconv)
-        if reason is not None:
-            raise ValueError(f"QConv2dGroupInt8.from_qconv2d: {reason}")
-        aq, wq = qconv.input_quantizer, qconv.weight_quantizer
-        kw = qconv.fwd_kwargs
-        weight = qconv.weight.detach()
-        c_out, c_g, kh, kwd = weight.shape
-        groups = int(kw["groups"])
-        padding = resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
-        mod = cls(c_g * groups, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]), groups,
-                  weight.device)
-        with torch.no_grad():
-            for buf, v in zip((mod.w_q, mod.w_rowsum, mod.w_scale, mod.w_zero), _int8_weight_rows(wq, qconv.weight)):
-                buf.copy_(v)
-            xs, xz = _qparams(aq, None)
-            mod.scale.copy_(xs.reshape(1))
-            mod.zero_point.copy_(xz.reshape(1))
-            if qconv.bias is not None:
-                mod.bias = qconv.bias.detach().float().clone().contiguous()
-        mod.qmin, mod.qmax = aq.qdesc.qrange
-        return mod
-
-    def forward(self, x_in):
-        if torch.is_grad_enabled() and x_in.requires_grad:
-            raise RuntimeError("QConv2dGroupInt8 is inference-only and has no backward; run it under torch.no_grad() or "
-                               "keep QConv2d for training")
-        x = x_in.float() if x_in.dtype != torch.float32 else x_in
-        unbatched = x.dim() == 3
-        if unbatched:
-            x = x.unsqueeze(0)
-        y = ops.int8_group_conv2d(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.w_q,
-                                  self.w_rowsum, self.w_scale, self.w_zero, self.kernel_size, self.groups, self.bias,
-                                  self.stride, self.padding, self.dilation)
-        return y.squeeze(0) if unbatched else y
+    def _conv(self, x):
+        return ops.int8_group_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
+                                     self.w_scale, self.w_zero, self.kernel_size, self.groups, self.bias, self.stride,
+                                     self.padding, self.dilation)
 
     def extra_repr(self):
         return super().extra_repr() + f", groups={self.groups}"
+
 
 class QReLU(QuantOpr):
     def __init__(self, org_module=None):
@@ -451,6 +413,25 @@ def int8_matmul_ineligibility(qmatmul):
     return None
 
 
+def _register_operand_qparams(mod, roles, device):
+    """One per-tensor ``{role}_scale`` / ``{role}_zero_point`` buffer pair per operand role of ``mod``."""
+    for role in roles:
+        mod.register_buffer(f"{role}_scale", torch.ones(1, dtype=torch.float32, device=device))
+        mod.register_buffer(f"{role}_zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+
+
+def _from_operand_quantizers(cls, quantizers, *args):
+    """``cls(device, *args)`` with the buffers of ``_register_operand_qparams`` holding the qparams of ``quantizers``
+    ({role: per-tensor quantizer}), and the integer ranges {role: (qmin, qmax)}."""
+    qparams = {role: _qparams(q, None) for role, q in quantizers.items()}
+    mod = cls(next(iter(qparams.values()))[0].device, *args)
+    with torch.no_grad():
+        for role, (s, z) in qparams.items():
+            getattr(mod, f"{role}_scale").copy_(s.reshape(1))
+            getattr(mod, f"{role}_zero_point").copy_(z.reshape(1))
+    return mod, {role: tuple(q.qdesc.qrange) for role, q in quantizers.items()}
+
+
 class QMatMulInt8(nn.Module):
     """Inference-only replacement of a calibrated ``QMatMul``: the matmul of the two fake-quant operands computed on the
     integer grid by ``ops.int8_matmul`` -- both operands quantized on the fly, exact int8 x int8 sums on the tensor
@@ -460,9 +441,7 @@ class QMatMulInt8(nn.Module):
 
     def __init__(self, device):
         super().__init__()
-        for side in ("left", "right"):
-            self.register_buffer(f"{side}_scale", torch.ones(1, dtype=torch.float32, device=device))
-            self.register_buffer(f"{side}_zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+        _register_operand_qparams(self, ("left", "right"), device)
         self.left_qrange, self.right_qrange = (-128, 127), (-128, 127)
 
     @classmethod
@@ -470,19 +449,13 @@ class QMatMulInt8(nn.Module):
         reason = int8_matmul_ineligibility(qmatmul)
         if reason is not None:
             raise ValueError(f"QMatMulInt8.from_qmatmul: {reason}")
-        lq, rq = qmatmul.left.input_quantizer, qmatmul.right.input_quantizer
-        (ls, lz), (rs, rz) = _qparams(lq, None), _qparams(rq, None)
-        mod = cls(ls.device)
-        with torch.no_grad():
-            for buf, v in ((mod.left_scale, ls), (mod.left_zero_point, lz), (mod.right_scale, rs), (mod.right_zero_point, rz)):
-                buf.copy_(v.reshape(1))
-        mod.left_qrange, mod.right_qrange = tuple(lq.qdesc.qrange), tuple(rq.qdesc.qrange)
+        mod, qranges = _from_operand_quantizers(cls, {"left": qmatmul.left.input_quantizer,
+                                                      "right": qmatmul.right.input_quantizer})
+        mod.left_qrange, mod.right_qrange = qranges["left"], qranges["right"]
         return mod
 
     def forward(self, x_left, x_right):
-        if torch.is_grad_enabled() and (x_left.requires_grad or x_right.requires_grad):
-            raise RuntimeError("QMatMulInt8 is inference-only and has no backward; run it under torch.no_grad() or "
-                               "keep QMatMul for training")
+        _check_inference_only(self, "QMatMul", x_left, x_right)
         if x_left.dim() < 2 or x_right.dim() < 2:
             raise ValueError(f"QMatMulInt8 takes operands with at least 2 dimensions (got {x_left.dim()}-D and "
                              f"{x_right.dim()}-D); 1-D operands are not supported")
@@ -586,9 +559,7 @@ class QAttentionInt8(nn.Module):
     def __init__(self, device, scale=None):
         super().__init__()
         self.scale = scale
-        for role in self.ROLES:
-            self.register_buffer(f"{role}_scale", torch.ones(1, dtype=torch.float32, device=device))
-            self.register_buffer(f"{role}_zero_point", torch.zeros(1, dtype=torch.float32, device=device))
+        _register_operand_qparams(self, self.ROLES, device)
         self.qranges = {role: (-128, 127) for role in self.ROLES}
 
     @classmethod
@@ -596,22 +567,14 @@ class QAttentionInt8(nn.Module):
         reason = int8_attention_ineligibility(qattn)
         if reason is not None:
             raise ValueError(f"QAttentionInt8.from_qattention: {reason}")
-        carriers = dict(zip(cls.ROLES, (qattn.qk.left, qattn.qk.right, qattn.pv.left, qattn.pv.right)))
-        qparams = {role: _qparams(c.input_quantizer, None) for role, c in carriers.items()}
-        mod = cls(qparams["q"][0].device, None if qattn.scale is None else float(qattn.scale))
-        for role, carrier in carriers.items():
-            q = carrier.input_quantizer
-            s, z = qparams[role]
-            with torch.no_grad():
-                getattr(mod, f"{role}_scale").copy_(s.reshape(1))
-                getattr(mod, f"{role}_zero_point").copy_(z.reshape(1))
-            mod.qranges[role] = tuple(q.qdesc.qrange)
+        carriers = (qattn.qk.left, qattn.qk.right, qattn.pv.left, qattn.pv.right)
+        mod, qranges = _from_operand_quantizers(cls, {r: c.input_quantizer for r, c in zip(cls.ROLES, carriers)},
+                                                None if qattn.scale is None else float(qattn.scale))
+        mod.qranges.update(qranges)
         return mod
 
     def forward(self, q, k, v, attn_mask=None, causal=False):
-        if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
-            raise RuntimeError("QAttentionInt8 is inference-only and has no backward; run it under torch.no_grad() or "
-                               "keep QAttention for training")
+        _check_inference_only(self, "QAttention", q, k, v)
         qp = [(getattr(self, f"{r}_scale"), getattr(self, f"{r}_zero_point"), self.qranges[r]) for r in self.ROLES]
         return ops.int8_attention(q.float(), k.float(), v.float(), *qp, scale=self.scale, attn_mask=attn_mask,
                                   causal=causal)

@@ -279,3 +279,18 @@ def test_to_integer_convs_skips_ineligible_layers():
     model = nn.Sequential(_qconv(w_type="dorefa"), nn.ReLU(), _qconv(groups=2), _qconv(a_bit=9))
     assert to_integer_convs(model) == []
     assert all(isinstance(model[i], QConv2d) for i in (0, 2, 3))
+
+
+def test_qconv2d_int8_module_contract():
+    mod = QConv2dInt8(3, 5, (3, 2), (1, 2), (1, 0, 1, 1), (2, 1), torch.device("cpu"))
+    buffers = {name: (b.dtype, tuple(b.shape)) for name, b in mod.named_buffers()}
+    assert buffers == {"w_q": (torch.int8, (5, 32)), "w_rowsum": (torch.int32, (5,)), "w_scale": (torch.float32, (5,)),
+                       "w_zero": (torch.int32, (5,)), "scale": (torch.float32, (1,)), "zero_point": (torch.float32, (1,))}
+    assert set(mod.state_dict()) == set(buffers) and "bias" in mod._buffers and mod.bias is None
+    assert (mod.in_channels, mod.out_channels, mod.qmin, mod.qmax) == (3, 5, -128, 127)
+    assert (mod.kernel_size, mod.stride, mod.padding, mod.dilation) == ((3, 2), (1, 2), (1, 0, 1, 1), (2, 1))
+    assert repr(mod) == ("QConv2dInt8(3, 5, kernel_size=(3, 2), stride=(1, 2), padding=(1, 0, 1, 1), dilation=(2, 1), "
+                         "qrange=[-128, 127])")
+    for x in (torch.zeros(1, 3, 6, 6, requires_grad=True), torch.zeros(3, 6, 6, requires_grad=True)):
+        with pytest.raises(RuntimeError, match=r"^QConv2dInt8 is inference-only and has no backward; .* keep QConv2d for"):
+            mod(x)

@@ -15,6 +15,7 @@ from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.common import Backend
 from sparsebit_b200.quantization.modules import (QConv2d, QConv2dGroupInt8, QLinear, int8_conv_ineligibility,
                                                  int8_group_conv_ineligibility)
+from sparsebit_b200.quantization.modules import QConv2dInt8
 from sparsebit_b200.quantization.tools import to_integer_convs, to_integer_group_convs
 from test_gpu_int8_group_branches import BIG, CASES, case_branches
 
@@ -199,3 +200,19 @@ def test_each_branch_case_reaches_its_branch():
         assert branch in case_branches(CASES[name]), (name, branch, case_branches(CASES[name]))
     assert "grid.loop" in case_branches(BIG)
     assert case_branches(CASES["grp_shrunk"]) >= {"path.grouped"}
+
+
+def test_qconv2d_group_int8_module_contract():
+    mod = QConv2dGroupInt8(8, 16, (3, 3), (2, 1), (1, 1, 0, 2), (1, 2), 4, torch.device("cpu"))
+    assert isinstance(mod, QConv2dInt8)
+    buffers = {name: (b.dtype, tuple(b.shape)) for name, b in mod.named_buffers()}
+    assert buffers == {"w_q": (torch.int8, (16, 32)), "w_rowsum": (torch.int32, (16,)), "w_scale": (torch.float32, (16,)),
+                       "w_zero": (torch.int32, (16,)), "scale": (torch.float32, (1,)), "zero_point": (torch.float32, (1,))}
+    assert set(mod.state_dict()) == set(buffers) and "bias" in mod._buffers and mod.bias is None
+    assert (mod.in_channels, mod.out_channels, mod.groups, mod.qmin, mod.qmax) == (8, 16, 4, -128, 127)
+    assert (mod.kernel_size, mod.stride, mod.padding, mod.dilation) == ((3, 3), (2, 1), (1, 1, 0, 2), (1, 2))
+    assert repr(mod) == ("QConv2dGroupInt8(8, 16, kernel_size=(3, 3), stride=(2, 1), padding=(1, 1, 0, 2), dilation=(1, 2), "
+                         "qrange=[-128, 127], groups=4)")
+    for x in (torch.zeros(1, 8, 6, 6, requires_grad=True), torch.zeros(8, 6, 6, requires_grad=True)):
+        with pytest.raises(RuntimeError, match=r"^QConv2dGroupInt8 is inference-only and has no backward; .* keep QConv2d "):
+            mod(x)

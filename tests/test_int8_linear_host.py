@@ -205,3 +205,15 @@ def test_to_integer_linears_skips_ineligible_layers():
     model = nn.Sequential(_qlinear(w_type="dorefa"), nn.ReLU(), _qlinear(a_bit=9))
     assert to_integer_linears(model) == []
     assert all(isinstance(model[i], QLinear) for i in (0, 2))
+
+
+def test_qlinear_int8_module_contract():
+    mod = QLinearInt8(20, 6, torch.device("cpu"))
+    buffers = {name: (b.dtype, tuple(b.shape)) for name, b in mod.named_buffers()}
+    assert buffers == {"w_q": (torch.int8, (6, 32)), "w_rowsum": (torch.int32, (6,)), "w_scale": (torch.float32, (6,)),
+                       "w_zero": (torch.int32, (6,)), "scale": (torch.float32, (1,)), "zero_point": (torch.float32, (1,))}
+    assert set(mod.state_dict()) == set(buffers) and "bias" in mod._buffers and mod.bias is None
+    assert (mod.in_features, mod.out_features, mod.qmin, mod.qmax) == (20, 6, -128, 127)
+    assert repr(mod) == "QLinearInt8(in_features=20, out_features=6, qrange=[-128, 127])"
+    with pytest.raises(RuntimeError, match=r"^QLinearInt8 is inference-only and has no backward; .* keep QLinear for"):
+        mod(torch.zeros(2, 20, requires_grad=True))
