@@ -11,28 +11,18 @@ TFLOP/s data-sheet dense FP16 rate of the H100 SXM.  The card name and power lim
 Usage: python scripts/bench_gptq_dgrad.py [M ...]   (default 32 256 2048 4096)"""
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 
+from bench_util import card, timeit
 from sparsebit_b200 import ops
 
 SHAPES = [("qkvo", 4096, 4096), ("gate_up", 4096, 11008), ("down", 11008, 4096)]  # (name, K = in, N = out)
 GS = 128
 PEAK_F16 = 989e12
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = (s.strip() for s in out.split(","))
-    except (OSError, IndexError, ValueError, subprocess.SubprocessError):
-        name, power, clock = torch.cuda.get_device_name(), "unknown", "unknown"
-    return {"card": name, "power_limit": power, "max_sm_clock": clock}
 
 
 def dequant(qw, sc, zr, k, dtype):
@@ -42,24 +32,6 @@ def dequant(qw, sc, zr, k, dtype):
     q = ((qw.unsqueeze(1) >> shifts) & 15).reshape(-1, qw.shape[1])[:k].to(ct)
     gi = torch.arange(k, device=qw.device) // GS
     return (q * sc.t().to(ct)[gi] - zr.t().to(ct)[gi]).to(dtype)
-
-
-def timeit(fn, warmup=3, budget_s=0.3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    b.synchronize()
-    iters = max(3, min(100, int(budget_s / max(a.elapsed_time(b) * 1e-3, 1e-6))))
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) * 1e-3 / iters
 
 
 def main():
@@ -86,7 +58,7 @@ def main():
                 "deq_f16_hgemm": lambda: gi.add_(torch.matmul(go.half(), dequant(qw, sc, zr, k, torch.float16).t()).float()),
             }
             for label, fn in paths.items():
-                t = timeit(fn)
+                t = timeit(fn, max_iters=100) * 1e-6  # seconds
                 gi.zero_()
                 fn()
                 err = (gi[:256].double() - exp).abs().max().item()

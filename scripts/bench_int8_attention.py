@@ -28,7 +28,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "scripts"))
 import torch
 
-from bench_int8_matmul import MODELS, SIGNED, UNSIGNED, Operand, card, kernel_times, set_tf32, timeit
+from bench_int8_matmul import MODELS, SIGNED, UNSIGNED, Operand
+from bench_util import card, kernel_times, set_tf32, timeit
 from sparsebit_b200 import ops
 
 FIT = "does not fit"
@@ -81,12 +82,12 @@ def bench(family, bsz, heads, tokens, dim, info):
     for _ in range(3):
         for name, fn, tf32 in live:
             set_tf32(tf32)
-            runs[name].append(timeit(fn))
+            runs[name].append(timeit(fn, warmup=2, budget_s=0.2))
     set_tf32(False)
     for name, v_ in runs.items():
         rec[name + "_us"] = statistics.median(v_)
         rec[name + "_us_range"] = [min(v_), max(v_)]
-    kt = kernel_times(fused, ["int8_attention_kernel", "int8_quantize_rows_kernel", "int8_quantize_cols_kernel"])
+    kt = kernel_times(fused, ["int8_attention_kernel", "int8_quantize_rows_kernel", "int8_quantize_cols_kernel"], reps=5)
     rec["fused_kernel_us"] = kt.get("int8_attention_kernel")
     rec["rows_us"] = kt.get("int8_quantize_rows_kernel")
     rec["cols_us"] = kt.get("int8_quantize_cols_kernel")

@@ -27,7 +27,8 @@ sys.path.insert(0, os.path.join(ROOT, "scripts"))
 import torch
 
 from bench_int8_attention import p_operand
-from bench_int8_matmul import SIGNED, UNSIGNED, Operand, card, kernel_times, set_tf32, timeit
+from bench_int8_matmul import SIGNED, UNSIGNED, Operand
+from bench_util import card, kernel_times, set_tf32, timeit
 from sparsebit_b200 import ops
 
 
@@ -80,13 +81,13 @@ def bench(family, bsz, heads, tokens, dim, causal, padded, info):
     runs = {name: [] for name, _ in paths}
     for _ in range(3):
         for name, fn in paths:
-            runs[name].append(timeit(fn))
+            runs[name].append(timeit(fn, warmup=2, budget_s=0.2))
     for name, v_ in runs.items():
         rec[name + "_us"] = statistics.median(v_)
         rec[name + "_us_range"] = [min(v_), max(v_)]
-    rec["fused_kernel_us"] = kernel_times(fused, ["int8_attention_kernel<true>"]).get("int8_attention_kernel<true>")
+    rec["fused_kernel_us"] = kernel_times(fused, ["int8_attention_kernel<true>"], reps=5).get("int8_attention_kernel<true>")
     if causal:
-        kt = kernel_times(lambda: fused(None, False), ["int8_attention_kernel<false>"])
+        kt = kernel_times(lambda: fused(None, False), ["int8_attention_kernel<false>"], reps=5)
         rec["fused_unmasked_kernel_us"] = kt.get("int8_attention_kernel<false>")
         rec["causal_vs_unmasked"] = rec["fused_us"] / rec["fused_unmasked_us"]
     for name in ("fq_f32", "unfused"):

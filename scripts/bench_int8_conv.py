@@ -25,7 +25,8 @@ sys.path.insert(0, os.path.join(ROOT, "scripts"))
 import torch
 import torch.nn.functional as F
 
-from bench_int8_linear import PEAK_INT8, card, kernel_times, set_tf32, timeit
+from bench_int8_linear import PEAK_INT8
+from bench_util import card, kernel_times, set_tf32, timeit
 from sparsebit_b200 import fake_quant, ops
 
 

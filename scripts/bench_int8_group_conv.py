@@ -28,7 +28,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from bench_int8_linear import card, set_tf32, timeit
+from bench_util import card, set_tf32, timeit
 from sparsebit_b200 import fake_quant, ops
 
 HBM_PEAK = 3.35e12

@@ -15,7 +15,6 @@ events over repeated calls after warm-up.  The card name and power limit are rea
 Usage: python scripts/bench_int8_linear.py [--quick]"""
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,59 +22,13 @@ sys.path.insert(0, ROOT)
 import torch
 import torch.nn.functional as F
 
+from bench_util import card, kernel_times, set_tf32, timeit
 from sparsebit_b200 import fake_quant, ops
 
 DEIT = [("qkv", 768, 2304), ("proj", 768, 768), ("fc1", 768, 3072), ("fc2", 3072, 768)]  # (name, K, N)
 LLAMA = [("q", 4096, 4096), ("k", 4096, 4096), ("v", 4096, 4096), ("o", 4096, 4096), ("gate", 4096, 11008),
          ("up", 4096, 11008), ("down", 11008, 4096)]
 PEAK_INT8 = 1979e12
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = (s.strip() for s in out.split(","))
-    except (OSError, IndexError, ValueError, subprocess.SubprocessError):
-        name, power, clock = torch.cuda.get_device_name(), "unknown", "unknown"
-    return {"card": name, "power_limit": power, "max_sm_clock": clock}
-
-
-def timeit(fn, warmup=3, budget_s=0.3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    b.synchronize()
-    iters = max(3, min(200, int(budget_s / max(a.elapsed_time(b) * 1e-3, 1e-6))))
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) * 1e3 / iters
-
-
-def kernel_times(fn, names, reps=10):
-    """Mean device time (us) per call of each kernel whose name contains one of ``names`` (torch.profiler)."""
-    fn()
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA], acc_events=True) as prof:
-        for _ in range(reps):
-            fn()
-        torch.cuda.synchronize()
-    out = {}
-    for e in prof.key_averages():
-        for n in names:
-            if n in e.key:
-                tot = getattr(e, "self_device_time_total", None)
-                if tot is None:
-                    tot = e.self_cuda_time_total
-                out[n] = out.get(n, 0.0) + tot / reps
-    return out
 
 
 class Layer:
@@ -105,11 +58,6 @@ class Layer:
         fx = fake_quant.quant_pertensor_forward(x, self.xs, self.xz, -128, 127, 0).double()
         fw = fake_quant.quant_perchannel_forward(self.w, self.ws, self.wz, -128, 127, 0, 0).double()
         return fx @ fw.t() + self.bias.double()
-
-
-def set_tf32(on):
-    torch.backends.cuda.matmul.allow_tf32 = on
-    torch.backends.cudnn.allow_tf32 = on
 
 
 def bench_shape(family, name, k, n, m, info):

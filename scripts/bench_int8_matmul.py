@@ -21,69 +21,18 @@ are read in the same run.  Usage: python scripts/bench_int8_matmul.py [--quick]"
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 
+from bench_util import card, kernel_times, set_tf32, timeit
 from sparsebit_b200 import fake_quant, ops
 
 PEAK_INT8 = 1979e12
 MODELS = [("deit_tiny", 3), ("deit_small", 6), ("deit_base", 12)]
 SIGNED, UNSIGNED = (-128, 127), (0, 255)
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = (s.strip() for s in out.split(","))
-    except (OSError, IndexError, ValueError, subprocess.SubprocessError):
-        name, power, clock = torch.cuda.get_device_name(), "unknown", "unknown"
-    return {"card": name, "power_limit": power, "max_sm_clock": clock}
-
-
-def timeit(fn, warmup=2, budget_s=0.2):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    b.synchronize()
-    iters = max(3, min(200, int(budget_s / max(a.elapsed_time(b) * 1e-3, 1e-6))))
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) * 1e3 / iters
-
-
-def kernel_times(fn, names, reps=5):
-    """Mean device time (us) per call of ``fn`` spent in each kernel whose name contains one of ``names``."""
-    fn()
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA], acc_events=True) as prof:
-        for _ in range(reps):
-            fn()
-        torch.cuda.synchronize()
-    out = {}
-    for e in prof.key_averages():
-        for n in names:
-            if n in e.key:
-                tot = getattr(e, "self_device_time_total", None)
-                if tot is None:
-                    tot = e.self_cuda_time_total
-                out[n] = out.get(n, 0.0) + tot / reps
-    return out
-
-
-def set_tf32(on):
-    torch.backends.cuda.matmul.allow_tf32 = on
 
 
 class Operand:
@@ -130,12 +79,12 @@ def bench_shape(family, product, a, b, info):
     for _ in range(3):  # the three paths alternated
         for name, fn, tf32 in (("fq_f32_us", fq, False), ("fq_tf32_us", fq, True), ("int8_us", int8, False)):
             set_tf32(tf32)
-            runs[name].append(timeit(fn))
+            runs[name].append(timeit(fn, warmup=2, budget_s=0.2))
     set_tf32(False)
     for name, v in runs.items():
         rec[name] = statistics.median(v)
         rec[name + "_range"] = [min(v), max(v)]
-    kt = kernel_times(int8, ["int8_matmul_gemm_kernel", "int8_quantize_rows_kernel", "int8_quantize_cols_kernel"])
+    kt = kernel_times(int8, ["int8_matmul_gemm_kernel", "int8_quantize_rows_kernel", "int8_quantize_cols_kernel"], reps=5)
     rec["gemm_us"] = kt.get("int8_matmul_gemm_kernel")
     rec["rows_us"] = kt.get("int8_quantize_rows_kernel")
     rec["cols_us"] = kt.get("int8_quantize_cols_kernel")

@@ -1,5 +1,9 @@
+import zlib
+
 import numpy as np
 import torch
+
+from sparsebit_b200 import _lib
 
 
 def dev():
@@ -18,3 +22,31 @@ def bits_equal(a, b):
 
 def t(x, device=None):
     return torch.from_numpy(np.ascontiguousarray(x)).to(device or dev())
+
+
+def on_device(a, offset=0, *, unit="elem"):
+    """A device copy of ``a`` that starts ``offset`` elements (``unit="byte"``: bytes) into a fresh zeroed allocation,
+    which the caching allocator aligns to at least 16 bytes, with at least 16 bytes of slack behind it."""
+    assert unit in ("elem", "byte"), unit
+    a = np.array(a, order="C")
+    byte_off = offset * a.itemsize if unit == "elem" else offset
+    raw = torch.zeros(byte_off + a.nbytes + 16, dtype=torch.uint8, device=dev())
+    view = raw[byte_off:byte_off + a.nbytes].view(torch.from_numpy(a.reshape(-1)[:0]).dtype).view(a.shape)
+    view.copy_(torch.from_numpy(a))
+    return view
+
+
+def stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def real_sm():
+    return int(_lib.load().sb200_sm_count())
+
+
+def seed(name):
+    return zlib.crc32(name.encode())
+
+
+def seed_of(name, *extra):
+    return zlib.crc32(repr((name,) + extra).encode())

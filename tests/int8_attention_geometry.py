@@ -6,6 +6,7 @@ changes, this file has to follow.  Line numbers are of csrc/int8_attention.cu.
 
 There is one kernel and one way through it: K and v^T are streamed through the ring in both passes (no resident
 variant was built), so the branches are the tails, the block counts and the options."""
+from int8_geometry import cdiv
 
 ROWS = 128          # :33 kAtRows, query rows per CTA
 KEYS = 128          # :34 kAtKeys, keys per block
@@ -17,10 +18,6 @@ ALL = ("q_tail", "q_full_tile", "q_many_tiles", "key_tail", "key_full_block", "o
        "ring_wraps", "k16_pad", "d_steps_lt4", "d_steps_4", "dv_tail", "dv_full", "dv_odd_scalar", "dv_even_vec2",
        "p_q_on", "p_q_off", "scale_on", "scale_off", "max_rescaled", "exp_underflow",
        "nan_q", "nan_k", "nan_v")
-
-
-def cdiv(a, b):
-    return (a + b - 1) // b
 
 
 def plan(batch, tq, tk, d, dv):

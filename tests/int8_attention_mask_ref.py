@@ -12,6 +12,7 @@ reaches (the unmasked kernel's list stays in tests/int8_attention_geometry.py)."
 import numpy as np
 
 import int8_attention_ref as ref
+from int8_geometry import cdiv
 from int8_matmul_ref import BOUND, stored_grid
 from oracle import qdq as oqdq
 
@@ -21,10 +22,6 @@ ROWS = KEYS = 128
 ALL = ("masked", "mask_row_broadcast", "mask_full", "mask_two_level_batch", "causal_diagonal_block",
        "causal_skipped_blocks", "causal_no_skip", "rows_without_keys", "cta_without_keys", "p_q_fill", "nan_k_hidden",
        "nan_v_hidden")
-
-
-def cdiv(a, b):
-    return (a + b - 1) // b
 
 
 def visible(tq, tk, causal):

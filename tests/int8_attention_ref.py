@@ -7,7 +7,9 @@ are (scale, zero_point, qmin, qmax).  The kernel computes, per batch entry,
     g   = the stored grid of p (QDQ rule)
     out = RN32(fp64(I_pv) * (fp64(s_p) fp64(s_v))),  I_pv = sum_j (g - Z_p)(v_v - Z_v)  -- exact given g
 The accuracy contract of p (DESIGN §4): |p - p64| <= EPS p64 + ALPHA, p64 the fp64 softmax of the same fp32 scores.
-A grid value is admissible when it is the grid of some fp32 t within those bounds of p64."""
+A grid value is admissible when it is the grid of some fp32 t within those bounds of p64.
+
+The branch suites (test_gpu_int8_attention*_branches.py) share their inputs and output sentinels from here."""
 import numpy as np
 
 from int8_matmul_ref import BOUND, grid_offset, stored_grid
@@ -16,6 +18,27 @@ from oracle import qdq as oqdq
 F32, F64 = np.float32, np.float64
 EPS = 13 * 2.0 ** -24
 ALPHA = 2.0 ** -125
+SENTINEL = 1234.5   # out is pre-filled with this, TAIL elements past its end included
+PSENT = 0x5A        # ... and p_q with this byte
+TAIL = 64
+
+
+def case_qkv(name, lead, tq, tk, d, dv):
+    """(rng, q, k, v) of a branch case: standard normal q [*lead, Tq, d], k [*lead, Tk, d], v [*lead, Tk, dv], drawn in
+    that order from a generator seeded by the case name, which the case goes on drawing from."""
+    rng = np.random.default_rng(sum(map(ord, name)))
+    q = rng.standard_normal(lead + (tq, d)).astype(F32)
+    k = rng.standard_normal(lead + (tk, d)).astype(F32)
+    v = rng.standard_normal(lead + (tk, dv)).astype(F32)
+    return rng, q, k, v
+
+
+def case_operands(q, k, v):
+    """Operand tuples with scales from the largest magnitude, NaNs aside: q and k signed 8-bit at zero point 0, v
+    unsigned 8-bit at zero point 7."""
+    return ((q, F32(np.nanmax(np.abs(q)) / 127), F32(0), -128, 127),
+            (k, F32(np.nanmax(np.abs(k)) / 127), F32(0), -128, 127),
+            (v, F32(np.nanmax(np.abs(v)) / 255), F32(7), 0, 255))
 
 
 def padded(k):

@@ -4,6 +4,8 @@ byte offset of x from a 16-byte aligned allocation, ``branches`` names the kerne
 cases of tests/test_gpu_int8_group_branches.py can be tied to the branch each exists for and a CPU test can check that
 together they reach every branch.  When the .cu file changes, this file has to follow.  Line numbers are of
 csrc/int8_group_conv.cu."""
+from int8_conv_ref import _pads, _pair
+from int8_geometry import cdiv
 
 THREADS = 256           # :33 kGcThreads
 SMEM_MAX = 48 * 1024    # :34 kGcSmemMax
@@ -12,19 +14,6 @@ MAX_TW = 128            # :36 kGcMaxTW
 MAX_MB = 64             # :37 kGcMaxMB
 MAX_GRID = 1 << 16      # :38 kGcMaxGrid
 MAX_KG = 1 << 17        # :39 kGcMaxKg
-
-
-def cdiv(a, b):
-    return (a + b - 1) // b
-
-
-def _pads(padding):
-    p = (padding, padding) if isinstance(padding, int) else tuple(padding)
-    return (p[0], p[0], p[1], p[1]) if len(p) == 2 else tuple(p)
-
-
-def _pair(v):
-    return (v, v) if isinstance(v, int) else tuple(v)
 
 
 def smem_bytes(mode, cb, ob, c4, tih, tiw, kh, kw):

@@ -7,14 +7,10 @@ and the accuracy bound the integer path is held to,
 Operands are (x, scale, zero_point, qmin, qmax) tuples; ``a`` is [..., M, K], ``b`` is [..., K, N]."""
 import numpy as np
 
+from int8_linear_ref import BOUND, grid_offset
 from oracle import qdq as oqdq
 
-BOUND = 2.0 ** -21
 F32 = np.float32
-
-
-def grid_offset(qmin):
-    return 128 if qmin >= 0 else 0
 
 
 def stored_grid(x, s, z, qmin, qmax):

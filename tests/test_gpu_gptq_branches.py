@@ -107,15 +107,14 @@ the single-launch fp16 path.
 """
 import ctypes
 import re
-import zlib
-from dataclasses import dataclass, field
 
 import numpy as np
 import pytest
 import torch
 
 import gptq_geometry as geo
-from gpu_util import dev
+from branch_cases import C, assert_table_covers, check_reach, params
+from gpu_util import dev, on_device, real_sm, seed, stream
 from oracle import gptq as ogptq
 from sparsebit_b200 import _lib, ops
 
@@ -126,52 +125,36 @@ DEFAULT_MODE = geo.DEC_DEFAULT_MODE
 
 
 # -------------------------------------------------------------------------------------------------- cases
-@dataclass(frozen=True)
-class Case:
-    name: str
-    op: str  # fwd | batch | f16 | dgrad
-    spec: dict = field(hash=False)
-    targets: frozenset = frozenset()
-    claims: frozenset = frozenset()
-
-    def get(self, key, default=None):
-        return self.spec.get(key, default)
-
-    def kw(self, k=None):
-        return geo.packed_rows(self.get("bits", 4), self.get("k") if k is None else k) + self.get("kw_extra", 0)
-
-    def gs(self):
-        return self.get("gs") or self.get("k")
-
-    def branches(self, sm):
-        s = self.spec
-        if self.op == "fwd":
-            bits, m, k, n = s.get("bits", 4), s["m"], s["k"], s["n"]
-            if bits != 4:
-                return {f"dispatch.bits{bits}"} | geo.simt_branches(bits, m, k, n, self.kw(), sm)
-            kernel, b = geo.dispatch(m, k, n, self.gs(), s["impl"], s.get("x_off", 0), s.get("qw_off", 0), s.get("ws", "ok"))
-            b.add("dispatch.via." + s.get("via", "global"))
-            if kernel == "tc":
-                b |= geo.tc_branches(m, k, n, self.kw(), self.gs())
-            elif kernel == "decode":
-                b |= geo.dec_branches([(k, n, self.kw())], m, s.get("mode", DEFAULT_MODE), sm)
-            elif kernel == "simt":
-                b |= geo.simt_branches(4, m, k, n, self.kw(), sm)
-            return b
-        if self.op == "batch":
-            probs = [(k, n, geo.packed_rows(4, k)) for k, n in s["problems"]]
-            return geo.dec_branches(probs, s["m"], s.get("mode", DEFAULT_MODE), sm)
-        if self.op == "f16":
-            return geo.f16_branches(s["m"], s["k"], s["n"], self.kw(), self.gs(), s["state"], s["bias"], sm)
-        return geo.dgrad_branches(s.get("bits", 4), s["m"], s["k"], s["n"], self.kw(), self.gs(), s["impl"])
+# op: fwd | batch | f16 | dgrad
+def _kw(case):
+    return geo.packed_rows(case.get("bits", 4), case.get("k")) + case.get("kw_extra", 0)
 
 
-def fs(*a):
-    return frozenset(a)
+def _gs(case):
+    return case.get("gs") or case.get("k")
 
 
-def C(name, op, targets, claims=(), **spec):
-    return Case(name, op, spec, fs(*targets) | fs(*claims), fs(*claims))
+def branches(case, sm):
+    s = case.spec
+    if case.op == "fwd":
+        bits, m, k, n = s.get("bits", 4), s["m"], s["k"], s["n"]
+        if bits != 4:
+            return {f"dispatch.bits{bits}"} | geo.simt_branches(bits, m, k, n, _kw(case), sm)
+        kernel, b = geo.dispatch(m, k, n, _gs(case), s["impl"], s.get("x_off", 0), s.get("qw_off", 0), s.get("ws", "ok"))
+        b.add("dispatch.via." + s.get("via", "global"))
+        if kernel == "tc":
+            b |= geo.tc_branches(m, k, n, _kw(case), _gs(case))
+        elif kernel == "decode":
+            b |= geo.dec_branches([(k, n, _kw(case))], m, s.get("mode", DEFAULT_MODE), sm)
+        elif kernel == "simt":
+            b |= geo.simt_branches(4, m, k, n, _kw(case), sm)
+        return b
+    if case.op == "batch":
+        probs = [(k, n, geo.packed_rows(4, k)) for k, n in s["problems"]]
+        return geo.dec_branches(probs, s["m"], s.get("mode", DEFAULT_MODE), sm)
+    if case.op == "f16":
+        return geo.f16_branches(s["m"], s["k"], s["n"], _kw(case), _gs(case), s["state"], s["bias"], sm)
+    return geo.dgrad_branches(s.get("bits", 4), s["m"], s["k"], s["n"], _kw(case), _gs(case), s["impl"])
 
 
 SPLIT_DATA = ("split.zero_row", "split.nonfinite_row", "split.tiny_row", "split.subnormal_row")
@@ -296,35 +279,15 @@ REQUIRED = {
 }
 
 
-def doc_alias(b):
-    """The docstring names the SIMT ids of the three bit widths through simt<b>."""
-    return b if b == "simt3.straddle" else re.sub(r"^simt[234]\.", "simt<b>.", b)
-
-
-def check_reach(case, sm):
-    reached = case.branches(sm) | case.claims
-    assert case.targets <= reached, f"{case.name} at {sm} SMs reaches {sorted(reached)}, not {sorted(case.targets - reached)}"
-    return case.targets
-
-
-def _params(cases):
-    return [pytest.param(c, id=c.name) for c in cases]
+def doc_alias(x):
+    """The docstring names the SIMT cases and ids of the three bit widths through simt<b>."""
+    return x if x == "simt3.straddle" else re.sub(r"^simt[234]([._])", r"simt<b>\1", x)
 
 
 # -------------------------------------------------------------------------------------------------- CPU tests
 def test_case_table_covers_every_branch():
-    covered = set()
-    for case in ALL_CASES:
-        covered |= check_reach(case, geo.SM_COUNT_H100)
-    missing = REQUIRED - covered
-    assert not missing, f"no case reaches {sorted(missing)}"
-    unknown = covered - REQUIRED
-    assert not unknown, f"targets outside REQUIRED: {sorted(unknown)}"
-    assert len({c.name for c in ALL_CASES}) == len(ALL_CASES)
-    for case in ALL_CASES:  # the docstring table names every case ...
-        assert re.sub(r"^simt[234]_", "simt<b>_", case.name) in __doc__, case.name
-    for b in REQUIRED:  # ... and every branch
-        assert doc_alias(b) in __doc__, b
+    assert_table_covers(ALL_CASES, REQUIRED, lambda c: check_reach(c, branches(c, geo.SM_COUNT_H100)), __doc__,
+                        doc_alias=doc_alias, reject_unknown=True)
 
 
 def test_geometry_matches_documented_launches():
@@ -398,27 +361,6 @@ def test_pack_and_truth_match_hand_packed_words():
 
 
 # -------------------------------------------------------------------------------------------------- helpers
-def _seed(name):
-    return zlib.crc32(name.encode())
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def real_sm():
-    return int(_lib.load().sb200_sm_count())
-
-
-def on_device(a, offset=0):
-    """A device copy of `a` starting `offset` elements into a fresh (16-byte aligned) allocation."""
-    a = np.ascontiguousarray(a)
-    buf = torch.empty(a.size + offset + 4, dtype=torch.from_numpy(a.reshape(-1)[:0]).dtype, device=dev())
-    view = buf[offset:offset + a.size]
-    view.copy_(torch.from_numpy(a.reshape(-1)))
-    return view.view(a.shape)
-
-
 def filled_bytes(nbytes):
     return torch.full((max(int(nbytes), 16),), WS_FILL, dtype=torch.uint8, device=dev())
 
@@ -610,13 +552,13 @@ def _fwd_call(case, x_d, qw_d, out, sc_d, zr_d, ws, ws_bytes, gptq_globals):
     wsp = ws.data_ptr() if ws is not None else None
     if bits != 4:
         gptq_globals(impl=2, mode=mode)  # the 2 / 3-bit entry point ignores the process-wide 4-bit selection
-        return lib.sb200_gptq_matmul(*args, bits, gs, wsp, ws_bytes, _stream())
+        return lib.sb200_gptq_matmul(*args, bits, gs, wsp, ws_bytes, stream())
     if case.get("via", "global") == "ex":
         gptq_globals(impl=4 if impl != 4 else 1, mode=mode)  # a decoy: the per-call option must win
         opts = ops._Gptq4Options(impl, 0, 0)
-        return lib.sb200_gptq4_matmul_ex(*args, gs, ctypes.byref(opts), wsp, ws_bytes, _stream())
+        return lib.sb200_gptq4_matmul_ex(*args, gs, ctypes.byref(opts), wsp, ws_bytes, stream())
     gptq_globals(impl=impl, mode=mode)
-    return lib.sb200_gptq4_matmul(*args, gs, wsp, ws_bytes, _stream())
+    return lib.sb200_gptq4_matmul(*args, gs, wsp, ws_bytes, stream())
 
 
 def _check_data_claims(case, x, scales, zeros):
@@ -638,12 +580,12 @@ def _check_data_claims(case, x, scales, zeros):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(FWD_CASES + [c for c in TINY_CASES if c.op == "fwd"]))
+@pytest.mark.parametrize("case", params(FWD_CASES + [c for c in TINY_CASES if c.op == "fwd"]))
 def test_forward_branch_vs_fp64(case, gptq_globals):
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, branches(case, real_sm()))
+    rng = np.random.default_rng(seed(case.name))
     bits, m, k, n = case.get("bits", 4), case.get("m"), case.get("k"), case.get("n")
-    gs = case.gs()
+    gs = _gs(case)
     qw, scales, zeros = make_weights(rng, bits, k, n, gs, case.get("kw_extra", 0), case.get("zeros", "int"))
     x, outliers = activations(rng, case, m, k)
     _check_data_claims(case, x, scales, zeros)
@@ -700,7 +642,7 @@ def test_decode_tiny_rows_lose_only_flushed_subnormals(gptq_globals):
     subnormal rounding) of the fp64 truth, except outputs that are exactly zero where the truth is below 2^-126 (plus
     that bound): nothing but the flush is lost.  The flush does occur at these magnitudes."""
     gptq_globals()
-    rng = np.random.default_rng(_seed("decode_tiny_rows_lose_only_flushed_subnormals"))
+    rng = np.random.default_rng(seed("decode_tiny_rows_lose_only_flushed_subnormals"))
     qw, scales, zeros = make_weights(rng, 4, 128, 512, 128)
     qw_d, sc_d, zr_d = on_device(qw), on_device(scales), on_device(zeros)
     r = tiny_rows(rng, 128)[0]
@@ -721,11 +663,11 @@ def test_decode_tiny_rows_lose_only_flushed_subnormals(gptq_globals):
 
 # -------------------------------------------------------------------------------------------------- batch
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(BATCH_CASES))
+@pytest.mark.parametrize("case", params(BATCH_CASES))
 def test_batch_branch_vs_fp64(case, gptq_globals):
-    check_reach(case, real_sm())
+    check_reach(case, branches(case, real_sm()))
     gptq_globals(mode=case.get("mode", DEFAULT_MODE))
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     m = case.get("m")
     probs, keep = [], []
     for k, n in case.get("problems"):
@@ -739,7 +681,7 @@ def test_batch_branch_vs_fp64(case, gptq_globals):
         keep.append((t, prefill, k))
     arr = (ops._Gptq4Problem * len(probs))(*probs)
     before = _lib.launch_count()
-    assert _lib.load().sb200_gptq4_matmul_batch(arr, len(probs), m, _stream()) == 0
+    assert _lib.load().sb200_gptq4_matmul_batch(arr, len(probs), m, stream()) == 0
     assert _lib.launch_count() - before == 1
     for (x_d, qw_d, out, sc_d, zr_d), prefill, k in keep:
         exp, _ = truth(x_d, qw_d, sc_d, zr_d, k, 128, 4, prefill)
@@ -755,12 +697,12 @@ def _ulp16(v):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(F16_CASES))
+@pytest.mark.parametrize("case", params(F16_CASES))
 def test_linear_f16_branch_vs_fp64(case, gptq_globals):
-    check_reach(case, real_sm())
+    check_reach(case, branches(case, real_sm()))
     gptq_globals()
-    rng = np.random.default_rng(_seed(case.name))
-    m, k, n, gs = case.get("m"), case.get("k"), case.get("n"), case.gs()
+    rng = np.random.default_rng(seed(case.name))
+    m, k, n, gs = case.get("m"), case.get("k"), case.get("n"), _gs(case)
     qw, scales, zeros = make_weights(rng, 4, k, n, gs)
     xh = rng.standard_normal((m, k)).astype(F16)
     bias = rng.standard_normal(n).astype(F32) if case.get("bias") else None
@@ -776,7 +718,7 @@ def test_linear_f16_branch_vs_fp64(case, gptq_globals):
         before = _lib.launch_count()
         rc = lib.sb200_gptq4_linear_f16_ex(x_d.data_ptr(), qw_d.data_ptr(), out.data_ptr(), b_d.data_ptr() if b_d is not None else None,
                                            sc_d.data_ptr(), zr_d.data_ptr(), m, k, n, qw.shape[0], case.get("gs"),
-                                           state.data_ptr() if state is not None else None, 0, ws.data_ptr(), ws.numel(), _stream())
+                                           state.data_ptr() if state is not None else None, 0, ws.data_ptr(), ws.numel(), stream())
         assert rc == 0, lib.sb200_last_error()
         if "f16.single" in case.targets:
             assert _lib.launch_count() - before == 1
@@ -797,11 +739,11 @@ def test_linear_f16_branch_vs_fp64(case, gptq_globals):
 
 # -------------------------------------------------------------------------------------------------- input gradient
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(DGRAD_CASES + [c for c in TINY_CASES if c.op == "dgrad"]))
+@pytest.mark.parametrize("case", params(DGRAD_CASES + [c for c in TINY_CASES if c.op == "dgrad"]))
 def test_dgrad_branch_vs_fp64(case):
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
-    bits, m, k, n, gs = case.get("bits", 4), case.get("m"), case.get("k"), case.get("n"), case.gs()
+    check_reach(case, branches(case, real_sm()))
+    rng = np.random.default_rng(seed(case.name))
+    bits, m, k, n, gs = case.get("bits", 4), case.get("m"), case.get("k"), case.get("n"), _gs(case)
     qw, scales, zeros = make_weights(rng, bits, k, n, gs, 0, case.get("zeros", "int"))
     go, _ = activations(rng, case, m, n)
     _check_data_claims(case, go, scales, zeros)
@@ -818,7 +760,7 @@ def test_dgrad_branch_vs_fp64(case):
         before = _lib.launch_count()
         rc = lib.sb200_gptq_matmul_dgrad(go_d.data_ptr(), qw_d.data_ptr(), gi.data_ptr(), sc_d.data_ptr(), zr_d.data_ptr(), m, k,
                                          n, qw.shape[0], bits, case.get("gs"), case.get("impl"), ws.data_ptr(), ws.numel(),
-                                         _stream())
+                                         stream())
         if "dg.impl2.error" in case.targets:
             assert rc == E_UNSUPPORTED and b"unsupported" in lib.sb200_last_error()
             assert _lib.launch_count() == before and torch.equal(gi, prefill)

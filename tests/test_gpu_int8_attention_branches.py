@@ -10,12 +10,10 @@ import torch
 import int8_attention_geometry as geo
 import int8_attention_ref as ref
 from gpu_util import dev, t
+from int8_attention_ref import PSENT, SENTINEL, TAIL
 from sparsebit_b200 import _lib, ops
 
 F32 = np.float32
-SENTINEL = 1234.5
-PSENT = 0x5A
-TAIL = 64
 
 # name -> (batch, tq, tk, d, dv, p_q, scale, p_signed, ramp, spread, nan)
 CASES = {
@@ -37,17 +35,12 @@ def case_branches(c):
 
 def _inputs(name):
     batch, tq, tk, d, dv, p_q, scale, p_signed, ramp, spread, nan = CASES[name]
-    rng = np.random.default_rng(sum(map(ord, name)))
-    q = rng.standard_normal((batch, tq, d)).astype(F32)
-    k = rng.standard_normal((batch, tk, d)).astype(F32)
-    v = rng.standard_normal((batch, tk, dv)).astype(F32)
+    _, q, k, v = ref.case_qkv(name, (batch,), tq, tk, d, dv)
     if ramp:  # later keys score higher: the running max of a row grows block by block
         k = (k * 0.2 + np.linspace(0, 3, tk, dtype=F32)[None, :, None] * np.sign(q.mean(1, keepdims=True))).astype(F32)
     if spread:
         q *= 3
-    sq = F32(np.abs(q).max() / 127)
-    sk = F32(np.abs(k).max() / 127)
-    ops_ = [(q, sq, F32(0), -128, 127), (k, sk, F32(0), -128, 127), (v, F32(np.abs(v).max() / 255), F32(7), 0, 255)]
+    ops_ = ref.case_operands(q, k, v)
     p = (F32(1 / 127), F32(0), -128, 127) if p_signed else (F32(1 / 255), F32(0), 0, 255)
     for o in nan:
         x = ops_["qkv".index(o)][0]

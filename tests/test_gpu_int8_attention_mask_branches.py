@@ -11,12 +11,10 @@ import torch
 import int8_attention_mask_ref as mref
 import int8_attention_ref as ref
 from gpu_util import dev, t
+from int8_attention_ref import PSENT, SENTINEL, TAIL
 from sparsebit_b200 import _lib, ops
 
 F32 = np.float32
-SENTINEL = 1234.5
-PSENT = 0x5A
-TAIL = 64
 
 # name -> (heads, entries per head group, tq, tk, d, dv, mask_kind, causal, p_q, nan); batch = entries * heads
 CASES = {
@@ -37,11 +35,8 @@ def case_branches(c):
 
 def _inputs(name):
     heads, entries, tq, tk, d, dv, mask_kind, causal, p_q, nan = CASES[name]
-    rng = np.random.default_rng(sum(map(ord, name)))
     lead = (entries, heads)
-    q = rng.standard_normal(lead + (tq, d)).astype(F32)
-    k = rng.standard_normal(lead + (tk, d)).astype(F32)
-    v = rng.standard_normal(lead + (tk, dv)).astype(F32)
+    rng, q, k, v = ref.case_qkv(name, lead, tq, tk, d, dv)
     mask = None
     if mask_kind is not None and mask_kind.startswith("row"):  # key padding per entry, broadcast over heads and rows
         mask = np.zeros((entries, 1, 1, tk), F32)
@@ -54,11 +49,8 @@ def _inputs(name):
         k[-1, -1, 200, 3] = np.nan
     if "v_hidden" in nan:
         v[-1, -1, 220, 5] = np.nan
-    qo = (q, F32(np.abs(q).max() / 127), F32(0), -128, 127)
-    ko = (k, F32(np.nanmax(np.abs(k)) / 127), F32(0), -128, 127)
-    vo = (v, F32(np.nanmax(np.abs(v)) / 255), F32(7), 0, 255)
     p = (F32(1 / 255), F32(0), 0, 255)
-    return lead, (qo, ko, vo), p, 0.125, mask, causal, p_q
+    return lead, ref.case_operands(q, k, v), p, 0.125, mask, causal, p_q
 
 
 def check_p(g, s, bad, p, tq, tk, causal, label):

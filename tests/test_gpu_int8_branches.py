@@ -47,8 +47,6 @@ test_graph_keeps_its_workspace_when_a_later_call_grows_it: a graph captured at a
 was captured with; an eager call that outgrows that workspace must not hand its memory to later allocations.
 """
 import ctypes
-import zlib
-from dataclasses import dataclass, field
 from fractions import Fraction
 
 import numpy as np
@@ -56,7 +54,8 @@ import pytest
 import torch
 
 import int8_geometry as geo
-from gpu_util import dev
+from branch_cases import C, assert_table_covers, check_reach, params
+from gpu_util import dev, on_device, seed, stream
 from int8_conv_ref import integer_terms as conv_integer_terms
 from int8_conv_ref import lowered, to_nchw
 from int8_conv_ref import truth as conv_truth
@@ -77,27 +76,20 @@ RANGES = {"s8": (-128, 127), "u8": (0, 255), "s4": (-8, 7), "u4": (0, 15), "s2":
 
 
 # -------------------------------------------------------------------------------------------------- cases
-@dataclass(frozen=True)
-class Case:
-    name: str
-    op: str  # rows | cols | im2col | linear | conv | matmul
-    spec: dict = field(hash=False)
-    targets: frozenset = frozenset()
-    claims: frozenset = frozenset()
-
-    def get(self, key, default=None):
-        return self.spec.get(key, default)
-
-    def branches(self):
-        return geo.branches(self.op, **{k: v for k, v in self.spec.items() if k in _GEOMETRY_KEYS})
-
-
+# op: rows | cols | im2col | linear | conv | matmul; the spec's offsets (x_off, a_off, b_off, out_off) are in bytes
 _GEOMETRY_KEYS = {"rows", "k", "x_off", "per_row", "batch", "n", "c", "h", "w", "kh", "kw", "stride", "pad", "dilation",
                   "m", "bias", "c_out", "b_k_major", "a_off", "b_off", "out_off"}
 
 
-def C(name, op, targets, claims=(), **spec):
-    return Case(name, op, spec, frozenset(targets) | frozenset(claims), frozenset(claims))
+def branches(case):
+    return geo.branches(case.op, **{k: v for k, v in case.spec.items() if k in _GEOMETRY_KEYS})
+
+
+def _covers(case):
+    """Everything the case reaches, not only its targets: REQUIRED must name every id the geometry produces."""
+    reached = branches(case) | case.claims
+    check_reach(case, reached)
+    return reached
 
 
 CASES = [
@@ -156,28 +148,9 @@ CASES = [
 ]
 
 
-def check_reach(case):
-    reached = case.branches() | case.claims
-    assert case.targets <= reached, f"{case.name} reaches {sorted(reached)}, not {sorted(case.targets - reached)}"
-    return reached
-
-
-def _params(cases):
-    return [pytest.param(c, id=c.name) for c in cases]
-
-
 # -------------------------------------------------------------------------------------------------- CPU tests
 def test_case_table_covers_every_branch():
-    covered = set()
-    for case in CASES:
-        covered |= check_reach(case)
-    missing = geo.REQUIRED - covered
-    assert not missing, f"no case reaches {sorted(missing)}"
-    unknown = covered - geo.REQUIRED
-    assert not unknown, f"branches outside REQUIRED: {sorted(unknown)}"
-    assert len({c.name for c in CASES}) == len(CASES)
-    for case in CASES:
-        assert case.name in __doc__, case.name
+    assert_table_covers(CASES, geo.REQUIRED, _covers, __doc__, reject_unknown=True, doc_branches=False)
 
 
 def test_geometry_matches_hand_worked_launches():
@@ -259,10 +232,6 @@ def test_references_reproduce_hand_worked_outputs():
 
 
 # -------------------------------------------------------------------------------------------------- data
-def _seed(name):
-    return zlib.crc32(name.encode())
-
-
 def _zp(qr, at):
     qmin, qmax = RANGES[qr]
     return F32({"min": qmin, "max": qmax, "mid": (qmin + qmax) // 2 + 0.5 * (qmax - qmin > 8)}[at])
@@ -294,15 +263,6 @@ def weights(rng, n, k, wr):
     return w.astype(F32), ws, wz
 
 
-def on_device(a, byte_off=0):
-    """A device copy of ``a`` starting ``byte_off`` bytes into a fresh allocation."""
-    a = np.array(a, order="C")
-    raw = torch.zeros(byte_off + a.nbytes + 16, dtype=torch.uint8, device=dev())
-    view = raw[byte_off:byte_off + a.nbytes].view(torch.from_numpy(a.reshape(-1)[:0]).dtype).view(a.shape)
-    view.copy_(torch.from_numpy(a))
-    return view
-
-
 def scalar(v):
     return torch.tensor([float(v)], dtype=torch.float32, device=dev())
 
@@ -324,15 +284,12 @@ class Guarded:
         return bool((self.raw[:self.off] == self.fill).all() and (self.raw[self.off + self.n:] == self.fill).all())
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 def _check(rc):
     assert rc == 0, _lib.load().sb200_last_error()
 
 
-def bits_equal(a, b):
+def bytes_equal(a, b):
+    """The same shape and the same bytes: unlike gpu_util.bits_equal, +0 and -0 differ and so do NaN payloads."""
     a, b = np.asarray(a), np.asarray(b)
     return a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
 
@@ -341,7 +298,7 @@ def same_floats(a, b):
     """Bit for bit, any NaN equal to any NaN."""
     a, b = np.asarray(a, F32), np.asarray(b, F32)
     na, nb = np.isnan(a), np.isnan(b)
-    return a.shape == b.shape and np.array_equal(na, nb) and bits_equal(a[~na], b[~nb])
+    return a.shape == b.shape and np.array_equal(na, nb) and bytes_equal(a[~na], b[~nb])
 
 
 def within_truth(y, t, bound):
@@ -372,7 +329,7 @@ def _run_quantizer(call, outs):
         assert all(b.intact() for b in bufs), "a quantizer wrote past its output"
         runs.append([b.view(dt, sh).cpu().numpy() for b, (_, dt, sh) in zip(bufs, outs)])
     for r in runs[1:]:
-        assert all(bits_equal(u, v) for u, v in zip(runs[0], r))
+        assert all(bytes_equal(u, v) for u, v in zip(runs[0], r))
     return runs[0]
 
 
@@ -380,10 +337,10 @@ QUANT_CASES = [c for c in CASES if c.op in ("rows", "cols", "im2col")]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(QUANT_CASES))
+@pytest.mark.parametrize("case", params(QUANT_CASES))
 def test_quantizer_branch_is_the_oracle_grid(case, no_tf32):
-    check_reach(case)
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, branches(case))
+    rng = np.random.default_rng(seed(case.name))
     qr, lib = case.get("xr"), _lib.load()
     qmin, qmax = RANGES[qr]
     s, z = F32(0.0371), _zp(qr, case.get("zp"))
@@ -398,11 +355,11 @@ def test_quantizer_branch_is_the_oracle_grid(case, no_tf32):
         sv, zv = np.broadcast_to(s, (rows,)) if case.get("per_row") else np.array([s], F32), \
             np.broadcast_to(z, (rows,)) if case.get("per_row") else np.array([z], F32)
         x = activations(rng, (rows, k), float(np.max(s)), float(np.min(z)), qr, (1, k // 2))
-        x_d, s_d, z_d = on_device(x, x_off), on_device(sv), on_device(zv)
+        x_d, s_d, z_d = on_device(x, x_off, unit="byte"), on_device(sv), on_device(zv)
         q, rsum, nan = _run_quantizer(
             lambda pq, ps, pn: lib.sb200_int8_quantize_rows(x_d.data_ptr(), s_d.data_ptr(), z_d.data_ptr(),
                                                             int(bool(case.get("per_row"))), qmin, qmax, pq, ps, pn, rows, k,
-                                                            _stream()),
+                                                            stream()),
             [(rows * kp, torch.int8, (rows, kp)), (rows * 4, torch.int32, (rows,)), (rows, torch.uint8, (rows,))])
         g = oqdq.quantize_int(x, sv if case.get("per_row") else s, zv if case.get("per_row") else z, qmin, qmax)
         en = np.isnan(g)
@@ -415,10 +372,10 @@ def test_quantizer_branch_is_the_oracle_grid(case, no_tf32):
         batch, k, n = case.get("batch"), case.get("k"), case.get("n")
         kp = geo.padded_k(k)
         x = activations(rng, (batch, k, n), s, z, qr, (0, k // 3, n - 1))
-        x_d, s_d, z_d = on_device(x, x_off), scalar(s), scalar(z)
+        x_d, s_d, z_d = on_device(x, x_off, unit="byte"), scalar(s), scalar(z)
         q, rsum, nan = _run_quantizer(
             lambda pq, ps, pn: lib.sb200_int8_quantize_cols(x_d.data_ptr(), s_d.data_ptr(), z_d.data_ptr(), qmin, qmax, pq,
-                                                            ps, pn, batch, k, n, _stream()),
+                                                            ps, pn, batch, k, n, stream()),
             [(batch * n * kp, torch.int8, (batch, n, kp)), (batch * n * 4, torch.int32, (batch, n)),
              (batch * n, torch.uint8, (batch, n))])
         eq, esum, enan = quantize_cols(x, s, z, qmin, qmax)
@@ -433,7 +390,7 @@ def test_quantizer_branch_is_the_oracle_grid(case, no_tf32):
         g = ops.conv2d_geometry(x.shape, (kh, kw), stride, pad, dil)
         q, rsum, nan = _run_quantizer(
             lambda pq, ps, pn: lib.sb200_int8_im2col_quantize(x_d.data_ptr(), ctypes.byref(g), s_d.data_ptr(),
-                                                              z_d.data_ptr(), qmin, qmax, pq, ps, pn, _stream()),
+                                                              z_d.data_ptr(), qmin, qmax, pq, ps, pn, stream()),
             [(m * kp, torch.int8, (m, kp)), (m * 4, torch.int32, (m,)), (m, torch.uint8, (m,))])
         eq, esum, enan = lowered(x, (kh, kw), s, z, qmin, qmax, stride, pad, dil)
         wrapped = ops.int8_im2col_quantize(x_d, (kh, kw), s_d, z_d, qmin, qmax, stride, pad, dil)
@@ -444,7 +401,7 @@ def test_quantizer_branch_is_the_oracle_grid(case, no_tf32):
     assert np.array_equal(nan.astype(bool), enan) and enan.any() and not enan.all()
     assert nan.max() <= 1
     wq, wsum, wnan = (t.cpu().numpy() for t in wrapped)
-    assert bits_equal(wq, q) and bits_equal(wsum, rsum) and np.array_equal(wnan, nan.astype(bool))
+    assert bytes_equal(wq, q) and bytes_equal(wsum, rsum) and np.array_equal(wnan, nan.astype(bool))
 
 
 # -------------------------------------------------------------------------------------------------- GEMMs
@@ -462,7 +419,7 @@ def _run_gemm(call, out_bytes, ws_bytes, out_off=0, offsets=WS_OFFSETS):
         runs.append(out.view(torch.float32, (out_bytes // 4,)).cpu().numpy())
         del out, ws
     for r in runs[1:]:
-        assert bits_equal(runs[0], r), "the calls differ"
+        assert bytes_equal(runs[0], r), "the calls differ"
     return runs[0]
 
 
@@ -481,13 +438,13 @@ def _linear_case(case, rng, lib):
     x = activations(rng, (m, k), s, z, xr, (m // 2, k - 1))
     w, ws, wz = weights(rng, n, k, wr)
     bias = rng.standard_normal(n).astype(F32) if case.get("bias", True) else None
-    x_d, s_d, z_d = on_device(x, x_off), scalar(s), scalar(z)
+    x_d, s_d, z_d = on_device(x, x_off, unit="byte"), scalar(s), scalar(z)
     w_q, w_sum, ws_d, wz_d = _w_device(w, ws, wz, wr)
     b_d = on_device(bias) if bias is not None else None
     need = int(lib.sb200_int8_linear_workspace_bytes(m, k))
     y = _run_gemm(lambda po, pw, nb: lib.sb200_int8_linear(
         x_d.data_ptr(), s_d.data_ptr(), z_d.data_ptr(), qmin, qmax, w_q.data_ptr(), w_sum.data_ptr(), ws_d.data_ptr(),
-        wz_d.data_ptr(), b_d.data_ptr() if b_d is not None else None, po, m, k, n, pw, nb, _stream()), m * n * 4, need)
+        wz_d.data_ptr(), b_d.data_ptr() if b_d is not None else None, po, m, k, n, pw, nb, stream()), m * n * 4, need)
     y = y.reshape(m, n)
     wrapped = ops.int8_linear(x_d, s_d, z_d, qmin, qmax, w_q, w_sum, ws_d, wz_d, b_d).cpu().numpy()
     nan_rows = np.isnan(oqdq.quantize_int(x, s, z, qmin, qmax)).any(1)
@@ -523,7 +480,7 @@ def _conv_case(case, rng, lib, images=None):
     out_n = n * c_out * p["p"]
     y = _run_gemm(lambda po, pw, nb: lib.sb200_int8_conv2d(
         x_d.data_ptr(), ctypes.byref(g), s_d.data_ptr(), z_d.data_ptr(), qmin, qmax, w_q.data_ptr(), w_sum.data_ptr(),
-        ws_d.data_ptr(), wz_d.data_ptr(), b_d.data_ptr() if b_d is not None else None, po, c_out, pw, nb, _stream()),
+        ws_d.data_ptr(), wz_d.data_ptr(), b_d.data_ptr() if b_d is not None else None, po, c_out, pw, nb, stream()),
         out_n * 4, need, offsets=WS_OFFSETS if images is None else (0, 16))
     y = y.reshape(n, c_out, p["oh"], p["ow"])
     wrapped = ops.int8_conv2d(x_d, s_d, z_d, qmin, qmax, w_q, w_sum, ws_d, wz_d, (kh, kw), b_d, stride, pad, dil)
@@ -549,15 +506,15 @@ def _matmul_case(case, rng, lib):
     sa, za, sb, zb = F32(0.0371), _zp(ar, case.get("zp")), F32(0.0213), _zp(br, case.get("bzp"))
     xa = activations(rng, (batch, m, k), sa, za, ar, (batch - 1, m // 2, k // 3))
     xb = activations(rng, (batch, k, n), sb, zb, br, (0, k // 2, n - 2))
-    a_d = on_device(xa, case.get("a_off", 0))
+    a_d = on_device(xa, case.get("a_off", 0), unit="byte")
     b_host = np.ascontiguousarray(np.swapaxes(xb, -1, -2)) if kmaj else xb
-    b_d = on_device(b_host, case.get("b_off", 0))
+    b_d = on_device(b_host, case.get("b_off", 0), unit="byte")
     pa = (scalar(sa), scalar(za), *RANGES[ar])
     pb = (scalar(sb), scalar(zb), *RANGES[br])
     need = int(lib.sb200_int8_matmul_workspace_bytes(batch, m, k, n))
     y = _run_gemm(lambda po, pw, nb: lib.sb200_int8_matmul(
         a_d.data_ptr(), b_d.data_ptr(), int(kmaj), pa[0].data_ptr(), pa[1].data_ptr(), pa[2], pa[3], pb[0].data_ptr(),
-        pb[1].data_ptr(), pb[2], pb[3], po, batch, m, k, n, pw, nb, _stream()), batch * m * n * 4, need, out_off)
+        pb[1].data_ptr(), pb[2], pb[3], po, batch, m, k, n, pw, nb, stream()), batch * m * n * 4, need, out_off)
     y = y.reshape(batch, m, n)
     bt = b_d.transpose(-2, -1) if kmaj else b_d
     wrapped = ops.int8_matmul(a_d, pa[0], pa[1], pa[2:], bt, pb[0], pb[1], pb[2:]).cpu().numpy()
@@ -572,10 +529,10 @@ GEMM_CASES = [c for c in CASES if c.op in ("linear", "conv", "matmul") and c.nam
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(GEMM_CASES))
+@pytest.mark.parametrize("case", params(GEMM_CASES))
 def test_gemm_branch_is_the_integer_form(case, no_tf32):
-    check_reach(case)
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, branches(case))
+    rng = np.random.default_rng(seed(case.name))
     lib = _lib.load()
     if case.op == "linear":
         y, wrapped, exact, t, bound, nan_rows = _linear_case(case, rng, lib)
@@ -599,7 +556,7 @@ def test_conv_gemm_far_end_of_a_workspace_past_2_31(no_tf32):
     """M Kp >= 2^31 through the GEMM as well as the lowering: 700 x 1 x 224^2, 7x7, padding 3, C_out = 8.  The first and
     the last image are the oracle's; both equal the integer form bit for bit."""
     case = next(c for c in CASES if c.name == "conv_far_end")
-    check_reach(case)
+    check_reach(case, branches(case))
     p = geo.low_plan(700, 1, 224, 224, 7, 7, 1, 3, 1)
     need = p["m"] * p["kp"] + 5 * p["m"] + 700 * 224 * 224 * 4 + 2 * p["m"] * 8 * 4 + (1 << 30)
     free = torch.cuda.mem_get_info()[0]
@@ -609,7 +566,7 @@ def test_conv_gemm_far_end_of_a_workspace_past_2_31(no_tf32):
     side.wait_stream(torch.cuda.current_stream())
     try:
         with torch.cuda.stream(side):  # the ops wrapper's 2.3 GB workspace is this stream's, dropped below
-            y, wrapped, exact, t, bound, _ = _conv_case(case, np.random.default_rng(_seed(case.name)), _lib.load(), images=True)
+            y, wrapped, exact, t, bound, _ = _conv_case(case, np.random.default_rng(seed(case.name)), _lib.load(), images=True)
         torch.cuda.synchronize()
         assert same_floats(wrapped, y) and same_floats(y, exact)
         assert np.isnan(y[1]).any() and not np.isnan(y[0]).any()
@@ -667,7 +624,7 @@ def test_graph_keeps_its_workspace_when_a_later_call_grows_it(which):
     """Capture at a small M on a side stream, run a larger call eagerly on that stream (it outgrows the workspace), then
     allocate a dozen tensors of the old workspace's size there and replay: the tensors keep their pattern and the replay
     still gives the eager result."""
-    rng = np.random.default_rng(_seed(which))
+    rng = np.random.default_rng(seed(which))
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(side):

@@ -8,8 +8,7 @@ import pytest
 import torch
 
 import int8_group_geometry as geo
-from gpu_util import dev, t
-from int8_conv_ref import grid_offset
+from gpu_util import dev, on_device, t
 from int8_group_conv_ref import group_integer_form
 from sparsebit_b200 import _lib, ops
 
@@ -64,10 +63,8 @@ def test_branch_case(name):
     plan = geo.plan(n, c, h, w, c_out, groups, kernel, stride, padding, dilation, x_off)
     assert exp.shape[2:] == (plan["oh"], plan["ow"])
     # x at a byte offset x_off from a 16-byte aligned buffer
-    buf = torch.zeros(x.size + 4, device=dev())
-    assert buf.data_ptr() % 16 == 0
-    xv = buf[x_off // 4:x_off // 4 + x.size]
-    xv.copy_(t(x).reshape(-1))
+    xv = on_device(x, x_off, unit="byte")
+    assert (xv.data_ptr() - x_off) % 16 == 0
     out = torch.full(exp.shape, SENTINEL, device=dev())
     w_q, w_sum, w_nan = ops.int8_quantize_rows(t(wt.reshape(c_out, -1)), t(ws), t(np.zeros(c_out, F32)), -128, 127)
     w_zero = torch.zeros(c_out, dtype=torch.int32, device=dev())

@@ -115,16 +115,17 @@ oracle.observers.percentile(per_channel=True) for the alphas where the reference
 (test_percentile_ranks_stay_in_range); a rank set directly to >= n reads out NaN (test_select_rank_beyond_population).
 """
 import ctypes
-import zlib
 from dataclasses import dataclass
 
 import numpy as np
 import pytest
 import torch
 
+import branch_cases
 import observe_geometry as geo
 import qdq_geometry as qgeo
-from gpu_util import bits_equal, dev
+from branch_cases import assert_table_covers, check_reach, fs, params
+from gpu_util import bits_equal, dev, on_device, real_sm, seed_of, stream
 from oracle import observers as oobs
 from oracle import qdq as oqdq
 from sparsebit_b200 import _lib, ops
@@ -146,27 +147,6 @@ def dec(k):
     return np.where(k & U32(0x80000000), k & U32(0x7FFFFFFF), ~k).astype(U32).view(F32)
 
 
-def _seed(name, *extra):
-    return zlib.crc32(repr((name,) + extra).encode())
-
-
-def on_device(a, offset=0):
-    """A contiguous device copy of `a` that starts `offset` elements into a fresh (16-byte aligned) allocation."""
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    buf = torch.empty(t.numel() + offset, dtype=t.dtype, device=dev())
-    view = buf[offset:].view(a.shape)
-    view.copy_(t)
-    return view
-
-
-def real_sm():
-    return int(_lib.load().sb200_sm_count())
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 def subnormals(rng, n):
     bits = rng.integers(1, 1 << 23, n, dtype=np.int64).astype(U32)
     bits |= (rng.random(n) < 0.5).astype(U32) << U32(31)
@@ -179,26 +159,22 @@ def signed_zeros(rng, n):
 
 # -------------------------------------------------------------------------------------------------- cases
 @dataclass(frozen=True)
-class Case:
-    name: str
-    op: str  # mm | mmt | hist | mse | sel | pct | cs | mom
-    shape: tuple
-    targets: frozenset
+class Case(branch_cases.Case):
+    """op: mm | mmt | hist | mse | sel | pct | cs | mom; spec: the input shape."""
     x_off: int = 0
     arg: tuple = ()
-    claims: frozenset = frozenset()  # (data) ids, checked on the data by the GPU run
 
     def branches(self, sm):
-        n = int(np.prod(self.shape))
+        n = int(np.prod(self.spec))
         if self.op == "mm":
-            outer, c, inner = qgeo.channel_geometry(self.shape, self.arg[0])
+            outer, c, inner = qgeo.channel_geometry(self.spec, self.arg[0])
             return geo.minmax_branches(outer, c, inner, sm, self.x_off)
         if self.op == "mmt":
             return geo.minmax_tensor_branches(n, sm, self.x_off)
         if self.op == "hist":
             bins, lo, hi = self.arg
             return geo.hist_branches(n, sm, self.x_off) | {f"hist.bins{bins}"} | ({"hist.empty_range"} if lo == hi else set())
-        rows, row_len = self.shape
+        rows, row_len = self.spec
         if self.op == "mse":
             return geo.mse_branches(rows, row_len, self.arg[0], sm, self.x_off)
         if self.op == "sel":
@@ -210,10 +186,6 @@ class Case:
         if self.op == "cs":
             return geo.count_sign_branches(rows, row_len, sm)
         return geo.moments_branches(rows, row_len, self.arg[0], sm)
-
-
-def fs(*a):
-    return frozenset(a)
 
 
 MM_CASES = [
@@ -310,27 +282,10 @@ REQUIRED = {
 }
 
 
-def check_reach(case, sm):
-    reached = case.branches(sm) | case.claims
-    assert case.targets <= reached, f"{case.name} at {sm} SMs reaches {sorted(reached)}, not {sorted(case.targets - reached)}"
-    return case.targets
-
-
-def _params(cases):
-    return [pytest.param(c, id=c.name) for c in cases]
-
-
 # -------------------------------------------------------------------------------------------------- CPU tests
 def test_case_table_covers_every_branch():
-    covered = set()
-    for case in ALL_CASES:
-        covered |= check_reach(case, geo.SM_COUNT_H100)
-    missing = REQUIRED - covered
-    assert not missing, f"no case reaches {sorted(missing)}"
-    for case in ALL_CASES:  # the docstring table names every case
-        assert case.name in __doc__, case.name
-    for b in REQUIRED:  # ... and every branch
-        assert b in __doc__, b
+    assert_table_covers(ALL_CASES, REQUIRED, lambda c: check_reach(c, c.branches(geo.SM_COUNT_H100)), __doc__,
+                        reject_unknown=True)
 
 
 def test_geometry_matches_documented_launches():
@@ -432,7 +387,7 @@ def _specials(x3, rng):
 
 
 def _mm_data(case, rng, sm, update):
-    n = int(np.prod(case.shape))
+    n = int(np.prod(case.spec))
     if case.op == "mmt":
         x = rng.standard_normal(n).astype(F32)
         x[n // 2] = subnormals(rng, 1)[0]
@@ -444,7 +399,7 @@ def _mm_data(case, rng, sm, update):
         else:
             x[n - 1] = np.nan
         return x
-    outer, c, inner = qgeo.channel_geometry(case.shape, case.arg[0])
+    outer, c, inner = qgeo.channel_geometry(case.spec, case.arg[0])
     x3 = rng.standard_normal((outer, c, inner)).astype(F32)
     if inner == 1:
         vec = c % 4 == 0 and case.x_off % 4 == 0
@@ -453,8 +408,8 @@ def _mm_data(case, rng, sm, update):
         _plant_rows(x3, rng)
     _specials(x3, rng)
     # view [outer, C, inner] back in the case's shape with the channel on its axis
-    ch_axis = case.arg[0] % len(case.shape)
-    pre, post = case.shape[:ch_axis], case.shape[ch_axis + 1:]
+    ch_axis = case.arg[0] % len(case.spec)
+    pre, post = case.spec[:ch_axis], case.spec[ch_axis + 1:]
     return x3.reshape(pre + (c,) + post)
 
 
@@ -473,13 +428,13 @@ def _mm_expected(x, ch_axis):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(MM_CASES))
+@pytest.mark.parametrize("case", params(MM_CASES))
 def test_minmax_branch_vs_total_order(case):
     sm = real_sm()
-    check_reach(case, sm)
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, case.branches(sm))
+    rng = np.random.default_rng(seed_of(case.name))
     ch_axis = case.arg[0] if case.op == "mm" else None
-    c = 1 if ch_axis is None else case.shape[ch_axis]
+    c = 1 if ch_axis is None else case.spec[ch_axis]
     st = ops.minmax_new(c, dev())
     exp = np.full(2 * c, 0, U32)
     exp[0::2] = NAN_KEY
@@ -518,12 +473,12 @@ def _hist_data(n, bins, lo, hi, rng):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(HIST_CASES))
+@pytest.mark.parametrize("case", params(HIST_CASES))
 def test_hist_branch_vs_histc(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     bins, lo, hi = case.arg
-    n = case.shape[0]
-    rng = np.random.default_rng(_seed(case.name))
+    n = case.spec[0]
+    rng = np.random.default_rng(seed_of(case.name))
     rg = on_device(np.float32([lo, hi]))
     counts = torch.zeros(bins, dtype=torch.int64, device=dev())
     exp = np.zeros(bins, np.int64)
@@ -566,7 +521,7 @@ def _mse_reference(x2d, cs, cz, qmin, qmax):
 
 
 def _mse_data(case, rng):
-    rows, row_len = case.shape
+    rows, row_len = case.spec
     ncand, qmin, qmax = case.arg
     scale = rng.uniform(0.5, 3.0, rows).astype(F32)
     x = (rng.standard_normal((rows, row_len)) * scale[:, None]).astype(F32)
@@ -578,11 +533,11 @@ def _mse_data(case, rng):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(MSE_CASES))
+@pytest.mark.parametrize("case", params(MSE_CASES))
 def test_mse_sweep_branch_vs_oracle(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     ncand, qmin, qmax = case.arg
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed_of(case.name))
     x, cs, cz = _mse_data(case, rng)
     exp, tol = _mse_reference(x, cs, cz, qmin, qmax)
     assert np.all(tol <= 1e-5 * exp), "the derived bound must be no looser than rtol = 1e-5"
@@ -617,7 +572,7 @@ def test_mse_workspace_contract(rows, row_len, ncand):
 
     def call(nbytes):
         return lib.sb200_observe_mse_sweep(x.data_ptr(), rows, row_len, cs.data_ptr(), cz.data_ptr(), ncand, -8, 7,
-                                           sse.data_ptr(), ws.data_ptr(), ctypes.c_size_t(nbytes), _stream())
+                                           sse.data_ptr(), ws.data_ptr(), ctypes.c_size_t(nbytes), stream())
 
     assert call(need) == 0
     torch.cuda.synchronize()
@@ -638,7 +593,7 @@ def key_value_bits(k):
 
 
 def _sel_data(case, rng):
-    rows, n = case.shape
+    rows, n = case.spec
     x = (rng.standard_normal((rows, n)) * rng.uniform(0.01, 100, (rows, 1))).astype(F32)
     ranks = rng.integers(0, n, (rows, 2))
     ranks[0] = [0, n - 1]
@@ -684,10 +639,10 @@ def _run_select(x, ranks, case):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(SEL_CASES))
+@pytest.mark.parametrize("case", params(SEL_CASES))
 def test_select_branch_vs_sort(case):
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, case.branches(real_sm()))
+    rng = np.random.default_rng(seed_of(case.name))
     x, ranks = _sel_data(case, rng)
     ntpr, key_mode = case.arg
     keys = np.sort(sel_keys(x, key_mode), axis=1)
@@ -714,12 +669,12 @@ def _pct_rows(rng):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(PCT_CASES))
+@pytest.mark.parametrize("case", params(PCT_CASES))
 def test_percentile_path_vs_oracle(case):
     """hist_pass(0, with_counts) -> percentile_ranks -> scans, as the percentile observer runs it on one batch."""
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
-    rows, n = case.shape
+    check_reach(case, case.branches(real_sm()))
+    rng = np.random.default_rng(seed_of(case.name))
+    rows, n = case.spec
     x = _pct_rows(rng) if case.name == "pct_rows" else (rng.standard_normal((rows, n)) * (1 + np.arange(rows)[:, None])).astype(F32)
     xd = on_device(x, case.x_off)
     neg, pos = (x < 0).sum(axis=1), (x >= 0).sum(axis=1)
@@ -780,30 +735,30 @@ def _count_sign_data(rows, n, rng):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(CS_CASES))
+@pytest.mark.parametrize("case", params(CS_CASES))
 def test_count_sign_branch_vs_numpy(case):
     """sb200_count_sign: #(x < 0) and #(x >= 0) per row (-0 counts as >= 0, NaN as neither), accumulated."""
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
-    rows, n = case.shape
+    check_reach(case, case.branches(real_sm()))
+    rng = np.random.default_rng(seed_of(case.name))
+    rows, n = case.spec
     x = _count_sign_data(rows, n, rng)
     exp = np.stack([(x < 0).sum(axis=1), (x >= 0).sum(axis=1)], axis=1).reshape(-1)
     lib = _lib.load()
     xd = on_device(x)
     counts = torch.zeros(rows * 2, dtype=torch.int64, device=dev())
-    assert lib.sb200_count_sign(xd.data_ptr(), rows, n, counts.data_ptr(), _stream()) == 0
+    assert lib.sb200_count_sign(xd.data_ptr(), rows, n, counts.data_ptr(), stream()) == 0
     assert np.array_equal(counts.cpu().numpy(), exp)
-    assert lib.sb200_count_sign(xd.data_ptr(), rows, n, counts.data_ptr(), _stream()) == 0
+    assert lib.sb200_count_sign(xd.data_ptr(), rows, n, counts.data_ptr(), stream()) == 0
     assert np.array_equal(counts.cpu().numpy(), 2 * exp)
 
 
 # -------------------------------------------------------------------------------------------------- moments
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(MOM_CASES))
+@pytest.mark.parametrize("case", params(MOM_CASES))
 def test_moments_branch_vs_fp64(case):
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
-    rows, n = case.shape
+    check_reach(case, case.branches(real_sm()))
+    rng = np.random.default_rng(seed_of(case.name))
+    rows, n = case.spec
     x = (rng.standard_normal((rows, n)) * 3 + 0.5).astype(F32)
     centre = rng.standard_normal(rows) if case.arg[0] else None
     ct = torch.from_numpy(centre).to(dev()) if centre is not None else None

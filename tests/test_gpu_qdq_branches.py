@@ -61,7 +61,6 @@ The two-row loop's drain (bwd.cu:262-266) cannot run: the four-row loop leaves k
 two-row loop runs at most once after it (test_bwd_cols_two_row_drain_is_unreachable).
 """
 import ctypes
-import zlib
 from dataclasses import dataclass
 
 import numpy as np
@@ -69,7 +68,8 @@ import pytest
 import torch
 
 import qdq_geometry as geo
-from gpu_util import bits_equal, dev
+from branch_cases import assert_table_covers, fs
+from gpu_util import bits_equal, dev, on_device, real_sm, seed_of
 from oracle import qdq as oqdq
 from oracle import sparse as osparse
 from sparsebit_b200 import _lib, ops
@@ -135,26 +135,9 @@ def make_x(shape, ch_axis, s, z, rng, data, qmin=-128, qmax=127):
     return x.reshape(shape)
 
 
-def _seed(name, *extra):
-    return zlib.crc32(repr((name,) + extra).encode())
-
-
-def on_device(a, offset=0, dtype=None):
-    """Copy a numpy array to the GPU as a contiguous view that starts `offset` elements into a fresh allocation."""
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    buf = torch.empty(t.numel() + offset, dtype=dtype or t.dtype, device=dev())
-    view = buf[offset:].view(a.shape)
-    view.copy_(t.to(view.dtype))
-    return view
-
-
 def empty_at(shape, offset):
     n = int(np.prod(shape))
     return torch.empty(n + offset, dtype=torch.float32, device=dev())[offset:].view(shape)
-
-
-def real_sm():
-    return int(_lib.load().sb200_sm_count())
 
 
 # -------------------------------------------------------------------------------------------------- case tables
@@ -193,10 +176,6 @@ class BwdCase:
 
     def branches(self, sm):
         return geo.bwd_branches(self.shape, self.ch_axis, sm, self.x_off, self.gy_off)
-
-
-def fs(*a):
-    return frozenset(a)
 
 
 FWD_CASES = [
@@ -278,15 +257,9 @@ def case_coverage(case, sm):
 
 # -------------------------------------------------------------------------------------------------- CPU: coverage
 def test_case_table_covers_every_branch():
-    covered = set()
-    for case in FWD_CASES + BWD_CASES:
-        covered |= case_coverage(case, geo.SM_COUNT_H100)
-    missing = REQUIRED - covered
-    assert not missing, f"no case reaches {sorted(missing)}"
-    for b in _FWD_CORE + _BWD_CORE:  # the docstring table names every branch and every case
-        assert b in __doc__, b
-    for case in FWD_CASES + BWD_CASES:
-        assert case.name in __doc__, case.name
+    # the docstring table names every case and every branch; R-1@ and <data>@ ids through the branch they qualify
+    assert_table_covers(FWD_CASES + BWD_CASES, REQUIRED, lambda c: case_coverage(c, geo.SM_COUNT_H100), __doc__,
+                        doc_alias=lambda b: b.split("@")[-1])
 
 
 def test_bwd_cols_two_row_drain_is_unreachable():
@@ -318,7 +291,7 @@ def _fwd_params():
 
 def _run_fwd(case, rounding, qmin=-128, qmax=127):
     assert case.targets <= case.branches(real_sm()), (case.name, sorted(case.branches(real_sm())))
-    rng = np.random.default_rng(_seed(case.name, rounding, qmin, qmax))
+    rng = np.random.default_rng(seed_of(case.name, rounding, qmin, qmax))
     if case.op == "pertensor":
         s = np.float32([0.0173])
         z = np.float32([2.5])
@@ -406,7 +379,7 @@ def _close(got, exp, l1):
 def test_backward_branch_vs_oracle(case, rounding):
     assert case.targets <= case.branches(real_sm()), (case.name, sorted(case.branches(real_sm())))
     qmin, qmax = -16, 15
-    rng = np.random.default_rng(_seed(case.name, rounding))
+    rng = np.random.default_rng(seed_of(case.name, rounding))
     c = 1 if case.ch_axis is None else case.shape[case.ch_axis]
     s = rng.uniform(0.01, 0.05, c).astype(F32)
     z = np.rint(rng.uniform(-3, 3, c)).astype(F32)

@@ -30,7 +30,7 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import bits_equal, dev
+from gpu_util import bits_equal, dev, on_device
 from oracle import qdq as oqdq
 from sparsebit_b200 import _lib, ops
 
@@ -106,13 +106,6 @@ def make_x(n, s, z, rng, data, qmin, qmax):
     elif data == "nan_last":
         x[-1] = np.nan
     return x
-
-
-def on_device(a, offset=0):
-    buf = torch.empty(a.size + offset, dtype=torch.float32, device=dev())
-    view = buf[offset:]
-    view.copy_(torch.from_numpy(a))
-    return view
 
 
 def empty_at(n, offset):

@@ -111,15 +111,16 @@ mask_apply_qdq_perchannel entry points, and test_multi_plan_count_limits checks 
 refuses 4097.
 """
 import ctypes
-import zlib
 from dataclasses import dataclass
 
 import numpy as np
 import pytest
 import torch
 
+import branch_cases
 import weight_geometry as geo
-from gpu_util import bits_equal, dev
+from branch_cases import assert_table_covers, check_reach, fs, params
+from gpu_util import bits_equal, dev, on_device, real_sm, seed, stream
 from oracle import observers as oobs
 from oracle import qdq as oqdq
 from oracle import sparse as osp
@@ -135,27 +136,6 @@ STRETCH, GAMMA = F32(1.1 - (-0.1)), F32(-0.1)  # adaround.cu:22-23
 
 
 # -------------------------------------------------------------------------------------------------- helpers
-def _seed(name):
-    return zlib.crc32(name.encode())
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def real_sm():
-    return int(_lib.load().sb200_sm_count())
-
-
-def on_device(a, offset=0):
-    """A device copy of `a` starting `offset` elements into a fresh (16-byte aligned) allocation."""
-    a = np.ascontiguousarray(a)
-    buf = torch.empty(a.size + offset + 4, dtype=torch.from_numpy(a[:0]).dtype, device=dev())
-    view = buf[offset:offset + a.size]
-    view.copy_(torch.from_numpy(a.reshape(-1)))
-    return view
-
-
 def sentinel(n, offset=0, dtype=torch.float32):
     """`n` elements `offset` into a fresh allocation, filled (with the slack around them) with the sentinel."""
     buf = torch.empty(n + offset + 4, dtype=dtype, device=dev())
@@ -208,12 +188,8 @@ def ulp_steps(r, k):
 
 # -------------------------------------------------------------------------------------------------- cases
 @dataclass(frozen=True)
-class Case:
-    name: str
-    op: str  # multi | rows | clamp | ada | dorefa | absmax | gt | mulf | qp
-    spec: tuple
-    targets: frozenset
-    claims: frozenset = frozenset()  # (data) ids: planted by the case's data
+class Case(branch_cases.Case):
+    """op: multi | rows | clamp | ada | dorefa | absmax | gt | mulf | qp; spec: a tuple, laid out per op below."""
 
     def branches(self, sm):
         s = self.spec
@@ -234,10 +210,6 @@ class Case:
             n, w_off, m_off, o_off = s
             return geo.mask_apply_f32_branches(n, dict(w=w_off, m=m_off, out=o_off), sm)
         return geo.qparams_branches([(c, sym) for c, sym, _, _ in s])
-
-
-def fs(*a):
-    return frozenset(a)
 
 
 MULTI_CAP_SKIP2 = (  # (outer, C, inner, x_off, out_off, mask_off or None, qmin, qmax)
@@ -355,27 +327,10 @@ DOC_ALIASES = {  # ids the docstring names through the row "<family>.<op>.vec, .
 }
 
 
-def check_reach(case, sm):
-    reached = case.branches(sm) | case.claims
-    assert case.targets <= reached, f"{case.name} at {sm} SMs reaches {sorted(reached)}, not {sorted(case.targets - reached)}"
-    return case.targets
-
-
-def _params(cases):
-    return [pytest.param(c, id=c.name) for c in cases]
-
-
 # -------------------------------------------------------------------------------------------------- CPU tests
 def test_case_table_covers_every_branch():
-    covered = set()
-    for case in ALL_CASES:
-        covered |= check_reach(case, geo.SM_COUNT_H100)
-    missing = REQUIRED - covered
-    assert not missing, f"no case reaches {sorted(missing)}"
-    for case in ALL_CASES:  # the docstring table names every case
-        assert case.name in __doc__, case.name
-    for b in REQUIRED:  # ... and every branch
-        assert DOC_ALIASES.get(b, b) in __doc__, b
+    assert_table_covers(ALL_CASES, REQUIRED, lambda c: check_reach(c, c.branches(geo.SM_COUNT_H100)), __doc__,
+                        doc_alias=lambda b: DOC_ALIASES.get(b, b))
 
 
 def test_geometry_matches_documented_launches():
@@ -482,7 +437,7 @@ def _multi_plan(descs):
     arr = (ops._QdqTensorDesc * len(descs))(*descs)
     table = torch.empty(max(int(lib.sb200_qdq_multi_table_bytes(len(descs))), 64), dtype=torch.uint8, device=dev())
     rows = ctypes.c_int64(0)
-    rc = lib.sb200_qdq_multi_plan(arr, len(descs), table.data_ptr(), table.numel(), ctypes.byref(rows), _stream())
+    rc = lib.sb200_qdq_multi_plan(arr, len(descs), table.data_ptr(), table.numel(), ctypes.byref(rows), stream())
     return rc, table, rows.value
 
 
@@ -496,15 +451,15 @@ def _multi_expected(data, spec):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(MULTI_CASES))
+@pytest.mark.parametrize("case", params(MULTI_CASES))
 def test_multi_branch_vs_oracle(case):
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, case.branches(real_sm()))
+    rng = np.random.default_rng(seed(case.name))
     data, descs, keep, os_ = _multi_setup(case.spec, rng)
     rc, table, rows = _multi_plan(descs)
     assert rc == 0 and rows == sum(o * c for o, c, *_ in case.spec)
     lib = _lib.load()
-    assert lib.sb200_qdq_multi_run(table.data_ptr(), len(descs), rows, _stream()) == 0
+    assert lib.sb200_qdq_multi_run(table.data_ptr(), len(descs), rows, stream()) == 0
     got = host(keep[1])
     for k, (e, t) in enumerate(zip(_multi_expected(data, case.spec), case.spec)):
         g = got[os_[k]:os_[k] + e.size].reshape(e.shape)
@@ -520,11 +475,11 @@ def test_multi_equals_per_tensor_calls():
     mask_apply_qdq_perchannel call per tensor computes."""
     spec = MULTI_CAP_SKIP2
     assert "multi.stride.skip2" in geo.multi_branches([t[:6] for t in spec], real_sm())
-    rng = np.random.default_rng(_seed("multi_equals_per_tensor_calls"))
+    rng = np.random.default_rng(seed("multi_equals_per_tensor_calls"))
     data, descs, keep, os_ = _multi_setup(spec, rng)
     rc, table, rows = _multi_plan(descs)
     assert rc == 0
-    assert _lib.load().sb200_qdq_multi_run(table.data_ptr(), len(descs), rows, _stream()) == 0
+    assert _lib.load().sb200_qdq_multi_run(table.data_ptr(), len(descs), rows, stream()) == 0
     got = host(keep[1])
     for k, ((x, s, zp, mask), t) in enumerate(zip(data, spec)):
         xd, sd, zd = on_device(x).view(x.shape), on_device(s), on_device(zp)
@@ -553,11 +508,11 @@ def test_multi_plan_count_limits():
 
 # -------------------------------------------------------------------------------------------------- structured mask
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(ROWS_CASES))
+@pytest.mark.parametrize("case", params(ROWS_CASES))
 def test_mask_rows_gt_branch_vs_numpy(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     rows, inner, off = case.spec
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     th = F32(0.0)
     score = rng.standard_normal(rows).astype(F32)
     score[::7] = th  # score == thresh: pruned (strict >)
@@ -565,7 +520,7 @@ def test_mask_rows_gt_branch_vs_numpy(case):
     mask = sentinel(rows * inner, off)
     lib = _lib.load()
     assert lib.sb200_mask_rows_gt(on_device(score).data_ptr(), on_device(np.array([th], F32)).data_ptr(), mask.data_ptr(),
-                                  rows, inner, _stream()) == 0
+                                  rows, inner, stream()) == 0
     want = np.repeat((score > th).astype(F32), inner)
     assert bits_equal(host(mask), want)
 
@@ -603,15 +558,15 @@ def _clamp_run(x_d, gy_d, gx, g_hi, g_lo, n, ws):
     lo, hi = on_device(np.array([LO], F32)), on_device(np.array([HI], F32))
     return lib.sb200_clamp_bwd(x_d.data_ptr(), gy_d.data_ptr(), lo.data_ptr(), hi.data_ptr(), gx.data_ptr(),
                                g_hi.data_ptr() if g_hi is not None else None, g_lo.data_ptr() if g_lo is not None else None,
-                               n, ws.data_ptr(), ws.numel(), _stream())
+                               n, ws.data_ptr(), ws.numel(), stream())
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(CLAMP_CASES))
+@pytest.mark.parametrize("case", params(CLAMP_CASES))
 def test_clamp_bwd_branch_vs_oracle(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     n, x_off, gy_off, gx_off, null_hi, null_lo = case.spec
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     x, gy = _clamp_data(rng, n, positive=case.name == "clamp_flush")
     x_d, gy_d = on_device(x, x_off), on_device(gy, gy_off)
     lib = _lib.load()
@@ -654,12 +609,12 @@ def test_clamp_workspace_contract():
     before = _lib.launch_count()
     lo, hi = on_device(np.array([LO], F32)), on_device(np.array([HI], F32))
     rc = lib.sb200_clamp_bwd(x.data_ptr(), x.data_ptr(), lo.data_ptr(), hi.data_ptr(), gx.data_ptr(), g_hi.data_ptr(),
-                             g_lo.data_ptr(), n, ws.data_ptr(), need - 1, _stream())
+                             g_lo.data_ptr(), n, ws.data_ptr(), need - 1, stream())
     assert rc == E_WORKSPACE and b"workspace too small" in lib.sb200_last_error()
     assert _lib.launch_count() == before
     assert (host(gx).view(U32) == SENTINEL.view(U32)).all()
     assert lib.sb200_clamp_bwd(x.data_ptr(), x.data_ptr(), lo.data_ptr(), hi.data_ptr(), gx.data_ptr(), g_hi.data_ptr(),
-                               g_lo.data_ptr(), n, ws.data_ptr(), need, _stream()) == 0
+                               g_lo.data_ptr(), n, ws.data_ptr(), need, stream()) == 0
     assert _lib.launch_count() == before + 2
     assert bits_equal(host(gx), np.ones(n, F32)) and host(g_hi)[0] == 0 and host(g_lo)[0] == 0
 
@@ -726,13 +681,13 @@ def _ada_data(rng, outer, c, inner, qmin, qmax):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(ADA_CASES))
+@pytest.mark.parametrize("case", params(ADA_CASES))
 def test_adaround_branch_vs_oracle(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     op, outer, c, inner, offs = case.spec
     offs = dict(offs)
     qmin, qmax = -8, 7
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     x, v, gy, s, zp = _ada_data(rng, outer, c, inner, qmin, qmax)
     n = x.size
     xd, vd, gyd = on_device(x, offs.get("x", 0)), on_device(v, offs.get("v", 0)), on_device(gy, offs.get("gy", 0))
@@ -741,12 +696,12 @@ def test_adaround_branch_vs_oracle(case):
     lib = _lib.load()
     if op in ("hard", "soft"):
         rc = lib.sb200_adaround_fwd(xd.data_ptr(), vd.data_ptr(), sd.data_ptr(), zd.data_ptr(), out.data_ptr(), outer, c, inner,
-                                    qmin, qmax, int(op == "soft"), _stream())
+                                    qmin, qmax, int(op == "soft"), stream())
     elif op == "bwd":
         rc = lib.sb200_adaround_bwd(xd.data_ptr(), vd.data_ptr(), sd.data_ptr(), zd.data_ptr(), gyd.data_ptr(), out.data_ptr(),
-                                    outer, c, inner, qmin, qmax, _stream())
+                                    outer, c, inner, qmin, qmax, stream())
     else:
-        rc = lib.sb200_adaround_init(xd.data_ptr(), sd.data_ptr(), out.data_ptr(), outer, c, inner, _stream())
+        rc = lib.sb200_adaround_init(xd.data_ptr(), sd.data_ptr(), out.data_ptr(), outer, c, inner, stream())
     assert rc == 0
     got = host(out).reshape(x.shape)
     s3, z3 = s[None, :, None], zp[None, :, None]
@@ -786,7 +741,7 @@ def _dorefa_x(rng, n):
 def _fwd(lib, xd, md, sd, zd, out, outer, c, inner, qmin, qmax, quantize):
     return lib.sb200_dorefa_fwd(xd.data_ptr(), md.data_ptr(), sd.data_ptr() if sd is not None else None,
                                 zd.data_ptr() if zd is not None else None, out.data_ptr(), outer, c, inner, qmin, qmax,
-                                quantize, _stream())
+                                quantize, stream())
 
 
 def _kernel_tanh(x):
@@ -807,13 +762,13 @@ def _kernel_tanh(x):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(DOREFA_CASES))
+@pytest.mark.parametrize("case", params(DOREFA_CASES))
 def test_dorefa_branch_vs_kernel_tanh(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     op, outer, c, inner, offs = case.spec
     offs = dict(offs)
     qmin, qmax = -8, 7
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     n = outer * c * inner
     x = _dorefa_x(rng, n)
     t = _kernel_tanh(x)
@@ -827,7 +782,7 @@ def test_dorefa_branch_vs_kernel_tanh(case):
     out = sentinel(n, offs.get("out", 0))
     if op == "bwd":
         rc = lib.sb200_dorefa_bwd(xd.data_ptr(), md.data_ptr(), sd.data_ptr(), zd.data_ptr(), gyd.data_ptr(), out.data_ptr(),
-                                  outer, c, inner, qmin, qmax, _stream())
+                                  outer, c, inner, qmin, qmax, stream())
     else:
         rc = _fwd(lib, xd, md, sd, zd, out, outer, c, inner, qmin, qmax, int(op == "qdq"))
     assert rc == 0
@@ -845,11 +800,11 @@ def test_dorefa_branch_vs_kernel_tanh(case):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(ABSMAX_CASES))
+@pytest.mark.parametrize("case", params(ABSMAX_CASES))
 def test_dorefa_absmax_branch_vs_kernel_tanh(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     n, x_off = case.spec
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     x = rng.uniform(-0.5, 0.5, n).astype(F32)
     x[-3:] = [0.1, 0.2, F32(-0.9)]  # the largest |tanh| in the scalar tail
     x[n // 3] = F32(0.85)  # ... and the runner-up in the vector body
@@ -857,18 +812,18 @@ def test_dorefa_absmax_branch_vs_kernel_tanh(case):
         x[n // 2] = np.nan
     t = _kernel_tanh(x)
     m = torch.zeros(1, dtype=torch.float32, device=dev())  # the caller's initial state (ops.dorefa_absmax)
-    assert _lib.load().sb200_dorefa_absmax(on_device(x, x_off).data_ptr(), n, m.data_ptr(), _stream()) == 0
+    assert _lib.load().sb200_dorefa_absmax(on_device(x, x_off).data_ptr(), n, m.data_ptr(), stream()) == 0
     want = F32(np.nan) if np.isnan(t).any() else np.abs(t).max()
     assert bits_equal(host(m), np.array([want], F32)), (host(m)[0], want)
 
 
 # -------------------------------------------------------------------------------------------------- qdq.cu mask helpers
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(GT_CASES))
+@pytest.mark.parametrize("case", params(GT_CASES))
 def test_mask_gt_branch_vs_numpy(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     n, w_off, m_off = case.spec
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     th = F32(0.5)
     w = rng.uniform(-1, 1, n).astype(F32)
     plant(rng, w, [0.5, -0.5, np.nextafter(th, F32(1)), np.nextafter(th, F32(0))] + NONFINITE + list(subnormals(rng, 4)),
@@ -876,23 +831,23 @@ def test_mask_gt_branch_vs_numpy(case):
     w[-3:] = [-0.5, 0.75, 0.5]
     mask = sentinel(n, m_off, torch.uint8)
     assert _lib.load().sb200_mask_gt(on_device(w, w_off).data_ptr(), on_device(np.array([th], F32)).data_ptr(),
-                                     mask.data_ptr(), n, _stream()) == 0
+                                     mask.data_ptr(), n, stream()) == 0
     assert np.array_equal(host(mask), (np.abs(w) > th).astype(np.uint8))
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(MULF_CASES))
+@pytest.mark.parametrize("case", params(MULF_CASES))
 def test_mask_apply_f32_branch_vs_oracle(case):
-    check_reach(case, real_sm())
+    check_reach(case, case.branches(real_sm()))
     n, w_off, m_off, o_off = case.spec
-    rng = np.random.default_rng(_seed(case.name))
+    rng = np.random.default_rng(seed(case.name))
     w = rng.standard_normal(n).astype(F32)
     plant(rng, w, NONFINITE + list(subnormals(rng, 4)), frac=0.01)
     m = (rng.random(n) < 0.6).astype(F32)
     m[np.flatnonzero(np.isinf(w))[::2]] = 0.0  # inf * 0 = NaN
     out = sentinel(n, o_off)
     assert _lib.load().sb200_mask_apply_f32(on_device(w, w_off).data_ptr(), on_device(m, m_off).data_ptr(), out.data_ptr(),
-                                            n, _stream()) == 0
+                                            n, stream()) == 0
     with np.errstate(invalid="ignore"):
         want = osp.mask_apply(w, m)
     assert bits_equal(host(out), want)
@@ -939,10 +894,10 @@ def _qp_state(rng, c, qmin, qmax):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", _params(QP_CASES))
+@pytest.mark.parametrize("case", params(QP_CASES))
 def test_minmax_qparams_branch_vs_oracle(case):
-    check_reach(case, real_sm())
-    rng = np.random.default_rng(_seed(case.name))
+    check_reach(case, case.branches(real_sm()))
+    rng = np.random.default_rng(seed(case.name))
     lib = _lib.load()
     states, outs, descs = [], [], []
     for c, sym, qmin, qmax in case.spec:
@@ -954,7 +909,7 @@ def test_minmax_qparams_branch_vs_oracle(case):
         descs.append(ops._QparamsDesc(st.data_ptr(), *[t.data_ptr() for t in o], c, qmin, qmax, int(sym)))
     arr = (ops._QparamsDesc * len(descs))(*descs)
     table = torch.empty(64 * len(descs), dtype=torch.uint8, device=dev())
-    assert lib.sb200_minmax_qparams_multi(arr, len(descs), table.data_ptr(), table.numel(), _stream()) == 0
+    assert lib.sb200_minmax_qparams_multi(arr, len(descs), table.data_ptr(), table.numel(), stream()) == 0
     for (c, sym, qmin, qmax), (keys, _), o in zip(case.spec, states, outs):
         mn, mx = dec(keys[0::2]), dec(keys[1::2])
         with np.errstate(all="ignore"):
