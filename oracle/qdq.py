@@ -73,6 +73,12 @@ def ste_backward(x, scale, zero_point, grad_y, qmin, qmax, ch_axis=0, rounding=0
     (fake_quant_tensor.cu:264), i.e. vq == qmax counts as clipped for the zero-point gradient only (SURVEY Q4).
     Pinned to MySTE.backward outputs (tests/golden/bwd.npz) and, on the GPU box, to the reference's own
     kernels (tests/test_gpu_reference_ext.py).  Returns gx (fp32), gs, gzp (fp64, shape [C] or [1])."""
+    gx, gs_e, gz_e = _ste_terms(x, scale, zero_point, grad_y, qmin, qmax, ch_axis, rounding, gzp_open_top)
+    return gx, _per_channel_sum(gs_e, scale, ch_axis), _per_channel_sum(gz_e, scale, ch_axis)
+
+
+def _ste_terms(x, scale, zero_point, grad_y, qmin, qmax, ch_axis=0, rounding=0, gzp_open_top=False):
+    """ste_backward before the reduction: gx (fp32) and the elementwise scale / zero-point terms (fp64)."""
     x = np.asarray(x, dtype=F32)
     gy = np.asarray(grad_y, dtype=F32)
     s = _bcast(scale, x, ch_axis)
@@ -88,11 +94,14 @@ def ste_backward(x, scale, zero_point, grad_y, qmin, qmax, ch_axis=0, rounding=0
     gs_e = term.astype(np.float64) * gy.astype(np.float64)
     inside_z = inside & (vq < F32(qmax)) if gzp_open_top else inside
     gz_e = np.where(inside_z, 0.0, (-s).astype(np.float64) * gy.astype(np.float64))
-    nch = np.asarray(scale).size
-    if nch == 1:
-        return gx, np.array([gs_e.sum()]), np.array([gz_e.sum()])
-    axes = tuple(a for a in range(x.ndim) if a != ch_axis)
-    return gx, gs_e.sum(axis=axes), gz_e.sum(axis=axes)
+    return gx, gs_e, gz_e
+
+
+def _per_channel_sum(e, scale, ch_axis):
+    """fp64 sum of elementwise terms per qparam: shape [1] per tensor, [C] along ``ch_axis`` per channel."""
+    if np.asarray(scale).size == 1:
+        return np.array([e.sum()])
+    return e.sum(axis=tuple(a for a in range(e.ndim) if a != ch_axis))
 
 
 # --------------------------------------------------------------------------------------------
@@ -136,6 +145,71 @@ def dorefa_grad_x(x, scale, zero_point, grad_y, qmin, qmax, ch_axis=0):
     gx_ste, _, _ = ste_backward(xn, scale, zero_point, grad_y, qmin, qmax, ch_axis)
     with np.errstate(all="ignore"):
         return ((gx_ste / m).astype(F32) * (F32(1) - (t * t).astype(F32)).astype(F32)).astype(F32)
+
+
+# --------------------------------------------------------------------------------------------
+# QAT train-mode chains: what autograd derives for x and the learnable qparams of each quantizer when the loss is
+# sum(y * grad_y).  Every function returns (y, gx, grads) with grads = {name: (gradient, l1)}: the fp64 gradient shaped
+# like the parameter (flattened) and the L1 norm of the terms summed into it, which bounds any summation order's error.
+def grad_scale_ratio(shape, qmax, ch_axis=None):
+    """lsq.py:68-76: GradScale ratio 1 / sqrt(n * qmax); n = numel per tensor, numel / C per channel."""
+    n = float(np.prod(shape))
+    if ch_axis is not None:
+        n /= shape[ch_axis]
+    return 1.0 / np.sqrt(n * qmax)
+
+
+def lsq_grads(x, scale, zero_point, grad_y, qmin, qmax, ch_axis=None, learn_zero_point=False):
+    """LSQ (lsq.py:53-76) and LSQ+ (lsq_plus.py:57-82): s = |scale|, zp = clamp(zero_point, qmin, qmax), both through
+    GradScale, then the STE.  d|s|/ds = sign(s); the clamp passes the zero point's gradient on the closed interval
+    (ATen).  ``ch_axis`` None: per tensor.  ``learn_zero_point``: LSQ+ per tensor, whose zero point is a Parameter."""
+    x = np.asarray(x, F32)
+    scale = np.asarray(scale, F32).reshape(-1)
+    zero_point = np.asarray(zero_point, F32).reshape(-1)
+    s, zp = np.abs(scale), np.clip(zero_point, F32(qmin), F32(qmax))
+    ax = 0 if ch_axis is None else ch_axis
+    y = qdq(x, s, zp, qmin, qmax, ax)
+    gx, gs_e, gz_e = _ste_terms(x, s, zp, grad_y, qmin, qmax, ax)
+    ratio = grad_scale_ratio(x.shape, qmax, ch_axis)
+    grads = {"scale": (_per_channel_sum(gs_e, s, ax) * ratio * np.sign(scale),
+                       _per_channel_sum(np.abs(gs_e), s, ax) * ratio)}
+    if learn_zero_point:
+        live = (zero_point >= qmin) & (zero_point <= qmax)
+        grads["zero_point"] = (_per_channel_sum(gz_e, s, ax) * ratio * live, _per_channel_sum(np.abs(gz_e), s, ax) * ratio)
+    return y, gx, grads
+
+
+def pact_grads(x, alpha, grad_y, qmin, qmax):
+    """PACT (pact.py:33-46): xc = clamp(x, lower, alpha) -> STE, with the grid of calc_qparams_with_minmax(lower,
+    alpha.detach()) (observers/base.py:63-79).  Signed ranges (lower = -alpha, SURVEY Q19), m(v) the STE mask:
+        gx      = gy [-alpha <= x <= alpha] m(xc)
+        d alpha = sum_{x > alpha} gy m(alpha) - sum_{x < -alpha} gy m(-alpha) + GS / (qmax - qmin)
+    where GS is the STE scale gradient over xc, reaching alpha through -alpha, the 1/2 of the maximum tie and
+    2 / (qmax - qmin).  Unsigned ranges (lower = 0, scale from alpha.detach()): d alpha is the first sum alone."""
+    from .observers import calc_qparams_with_minmax
+
+    x = np.asarray(x, F32)
+    alpha = F32(np.asarray(alpha, F32).reshape(-1)[0])
+    signed = qmin < 0
+    lower = -alpha if signed else F32(0)
+    scale, zp = calc_qparams_with_minmax(lower, alpha, qmin, qmax, signed)
+    xc = np.clip(x, lower, alpha)
+    y = qdq(xc, scale, zp, qmin, qmax)
+    gx_ste, gs_e, _ = _ste_terms(xc, scale, zp, grad_y, qmin, qmax)
+    gx, g_hi, g_lo = clamp_backward(x, gx_ste, lower, alpha)
+    g = g_hi - g_lo if signed else g_hi
+    edge = (x > alpha) | (x < lower) if signed else x > alpha
+    l1 = np.abs(gx_ste.astype(np.float64))[edge].sum()
+    if signed:
+        span = float(qmax - qmin)
+        g, l1 = g + gs_e.sum() / span, l1 + np.abs(gs_e).sum() / span
+    return y, gx, {"alpha": (np.array([g]), np.array([l1]))}
+
+
+def dorefa_grads(x, scale, zero_point, grad_y, qmin, qmax, ch_axis=0):
+    """DoReFa (dorefa.py:15-20): scale / zero_point are buffers, so only x has a gradient."""
+    return dorefa_forward(x, scale, zero_point, qmin, qmax, ch_axis), \
+        dorefa_grad_x(x, scale, zero_point, grad_y, qmin, qmax, ch_axis), {}
 
 
 # --------------------------------------------------------------------------------------------

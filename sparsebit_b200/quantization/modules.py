@@ -103,6 +103,9 @@ def _int8_qparams_reason(role, q, x, counts):
     z = torch.round(zero_point)
     if bool(((z < qmin) | (z > qmax) | torch.isnan(z)).any()):
         return f"the {role} zero point lies outside [{qmin}, {qmax}]"
+    if q.TYPE == "PACT" and qmin < 0 and bool(torch.round(q.alpha.detach().reshape(-1) / scale) <= qmax):
+        # SURVEY Q19: -alpha then rounds to qmin + 1, so the clamp narrows the grid below the QDQ kernels' [qmin, qmax]
+        return f"the {role} quantizer is PACT with alpha on the grid, whose clamp narrows it to [{qmin + 1}, {qmax}]"
     if q.backend == Backend.TENSORRT:
         try:
             check_trt_symmetric(zero_point)

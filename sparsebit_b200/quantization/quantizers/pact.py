@@ -1,11 +1,19 @@
 """``TYPE = "pact"`` (sparsebit/quantization/quantizers/pact.py:13-46): activations are clamped to a
 learnable [-alpha, alpha] (or [0, alpha]) before the fake-quant op whose qparams follow alpha.
 
-The reference runs ``torch.clamp`` as a separate 8 B/elem pass in front of the fake-quant op.  The clamp does not change
-the forward value -- the QDQ grid derived from [lower, alpha] (``calc_qparams_with_minmax(lower, alpha)``) clamps to the
-very same end points -- it only matters for the gradients (``alpha`` learns from the clipped region).  Here the forward
-is the native QDQ alone and the backward is ``sb200_clamp_bwd`` (gx = gy inside [lower, alpha]; d/d alpha = sum of gy
-above alpha minus, for the symmetric range, the sum below -alpha): same values as autograd through clamp -> STE."""
+The reference runs ``torch.clamp`` in front of the fake-quant op and lets autograd chain the two.  What that chain
+computes depends on the range:
+
+* Unsigned ([0, alpha], the grid's ``scale`` built from ``alpha.detach()``): every clamped value quantises inside
+  [qmin, qmax], so the clamp changes neither the forward value nor the straight-through mask.  The forward is the
+  native QDQ alone and the backward is ``sb200_clamp_bwd`` (gx = gy inside [0, alpha]; d/d alpha = sum of gy above
+  alpha).
+* Signed ([-alpha, alpha], SURVEY Q19): ``alpha / scale`` is ``(qmax - qmin) / 2``, a half-integer, so ``+alpha``
+  rounds to ``qmax + 1`` for most alphas and the straight-through mask drops every element clamped to it; for the
+  others ``-alpha`` rounds to ``qmin + 1`` and the clamp narrows the forward grid.  ``scale`` also depends on alpha
+  through the non-detached ``lower = -alpha``.  The forward therefore fake-quantises the clamped tensor, and the
+  backward runs the STE backward kernel on it, then ``sb200_clamp_bwd`` on that gradient; the scale gradient returns to
+  alpha through the port's own ``calc_qparams_with_minmax`` graph (``-alpha``, the ``maximum`` tie, ``/ span``)."""
 import torch
 import torch.nn as nn
 
@@ -16,26 +24,43 @@ from . import register_quantizer
 from .quant_tensor import STE, fake_quant_factory
 
 
+def _f32c(t):
+    t = t.detach()
+    return (t if t.dtype == torch.float32 else t.float()).contiguous()
+
+
 class PactSTE(torch.autograd.Function):
-    """clamp(x, lower, alpha) -> fake-quant, fused: forward = fake-quant only, backward = the clamp's gradients (the
-    STE mask is all ones on the clamped tensor: every clamped value quantises inside [qmin, qmax])."""
+    """clamp(x, lower, alpha) -> fake-quant as one op with the reference chain's gradients for x, alpha, lower and
+    scale.  On unsigned ranges the clamp is folded into the fake-quant grid and the backward is the clamp's alone (see
+    the module docstring)."""
 
     @staticmethod
-    def forward(ctx, x, alpha, lower, lower_follows_alpha, scale, zero_point, qdesc, backend):
-        ctx.save_for_backward(x, alpha, lower)
-        ctx.lower_follows_alpha = lower_follows_alpha
-        return fake_quant_factory[backend](x, scale, zero_point, qdesc)
+    def forward(ctx, x, alpha, lower, signed, scale, zero_point, qdesc, backend):
+        ctx.signed, ctx.qdesc = signed, qdesc
+        if not signed:
+            ctx.save_for_backward(x, alpha, lower)
+            return fake_quant_factory[backend](x, scale, zero_point, qdesc)
+        xc = torch.clamp(_f32c(x), _f32c(lower).reshape(1), _f32c(alpha).reshape(1))
+        ctx.save_for_backward(x, alpha, lower, xc, scale, zero_point)
+        return fake_quant_factory[backend](xc, scale, zero_point, qdesc)
 
     @staticmethod
     def backward(ctx, gout):
-        x, alpha, lower = ctx.saved_tensors
+        x, alpha, lower = ctx.saved_tensors[:3]
         if not x.is_cuda:
             raise NotImplementedError("We recommended that use cuda to speedup when training")  # like STE, quant_tensor.py:113-116
-        xf = x.float().contiguous() if x.dtype != torch.float32 else x.contiguous()
-        gx, g_hi, g_lo = ops.clamp_backward(xf, gout.float().contiguous(), lower.detach().float().reshape(1).contiguous(),
-                                            alpha.detach().float().reshape(1).contiguous())
-        g_alpha = (g_hi - g_lo) if ctx.lower_follows_alpha else g_hi
-        return gx, g_alpha.reshape(alpha.shape), None, None, None, None, None, None
+        lo, hi = _f32c(lower).reshape(1), _f32c(alpha).reshape(1)
+        gy = _f32c(gout)
+        gs = None
+        if ctx.signed:
+            xc, scale, zero_point = ctx.saved_tensors[3:]
+            qmin, qmax = ctx.qdesc.qrange
+            gy, gs, _ = ops.qdq_backward(xc, _f32c(scale).reshape(1), _f32c(zero_point).reshape(1), gy, qmin, qmax,
+                                         need_gs=ctx.needs_input_grad[4], need_gzp=False)
+            gs = gs.reshape(scale.shape) if ctx.needs_input_grad[4] else None
+        gx, g_hi, g_lo = ops.clamp_backward(_f32c(x), gy, lo, hi)
+        g_lo = g_lo.reshape(lower.shape) if ctx.needs_input_grad[2] else None
+        return gx, g_hi.reshape(alpha.shape), g_lo, None, gs, None, None, None
 
 
 @register_quantizer

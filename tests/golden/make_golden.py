@@ -539,9 +539,145 @@ def gen_sparse_structured():
     save("sparse_structured", **out)
 
 
+def _plant_grid_edges(x, s, zp, qmin, qmax, ch_axis=None):
+    """Write rounding ties (k + 0.5)·s and values landing exactly on qmin / qmax (and half a step beyond them) at the head
+    of every quantisation row of ``x`` (the whole tensor per tensor, each channel along ``ch_axis`` per channel)."""
+    xn = x.numpy()
+    rows = xn.reshape(1, -1) if ch_axis is None else np.moveaxis(xn, ch_axis, 0)
+    s, zp = np.asarray(s, np.float32).reshape(-1), np.rint(np.asarray(zp, np.float32).reshape(-1))
+    for c in range(rows.shape[0]):
+        sc, z = s[min(c, s.size - 1)], zp[min(c, zp.size - 1)]
+        units = [0.5, 1.5, -2.5, qmax - z - 0.5, qmin - z + 0.5, qmax - z, qmin - z, qmax - z + 0.5, qmin - z - 0.5]
+        for i, u in enumerate(units):
+            rows[c].flat[i] = np.float32(u) * sc
+
+
+def gen_qat():
+    """Train-mode gradients of the learnable quantizers (uniform, LSQ, LSQ+, PACT, DoReFa): calibrate, set the
+    parameters, enable_quant, forward, ``(y * gy).sum().backward()``.  The production ``STE.backward`` is CUDA-only
+    (quant_tensor.py:113-116), so ``STE`` is rebound in each quantizer module to a Function whose forward is the
+    reference ``STE.forward`` (CPU fake-quant branch) and whose backward is the reference ``MySTE.backward``
+    (quant_tensor.py:46-71), reduced to the parameter shapes.  Its ctx stand-in carries ``zero_point.round()`` as a
+    tensor that still requires grad when the zero point does: ``MySTE.forward`` rounds under no-grad, which would drop
+    the LSQ+ zero-point gradient.  MySTE differs from the per-channel CUDA kernel only in the zero-point rule (SURVEY
+    Q4), which no case reaches: no per-channel zero point is learnable."""
+    from sparsebit.quantization.quantizers import dorefa, lsq, lsq_plus, pact, uniform
+    from sparsebit.quantization.quantizers import quant_tensor as qt
+
+    class RefSTE(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, x, scale, zero_point, qdesc, backend):
+            return qt.STE.forward(ctx, x, scale, zero_point, qdesc, backend)
+
+        @staticmethod
+        def backward(ctx, gout):
+            x, scale, zero_point = ctx.saved_tensors
+            need_s, need_z = ctx.needs_input_grad[1:3]
+
+            class Ctx:
+                saved_tensors = (x, scale.detach().requires_grad_(need_s), zero_point.detach().round().requires_grad_(need_z))
+                qdesc = ctx.qdesc
+
+            gx, gs, gz, _, _ = qt.MySTE.backward(Ctx, gout)
+            return (gx, gs.sum_to_size(scale.shape) if need_s else None, gz.sum_to_size(zero_point.shape) if need_z else None,
+                    None, None)
+
+    for mod in (uniform, lsq, lsq_plus, pact, dorefa):
+        mod.STE = RefSTE
+
+    # the signed 8-bit PACT alpha whose bound alpha / scale lands just below 127.5 (rounds to qmax, not qmax + 1)
+    al = np.linspace(1.0, 2.0, 4001, dtype=np.float32)
+    sc = (al * np.float32(2)) / np.float32(255)
+    alpha_qmax = float(al[np.rint(al / sc) == 127][0])
+
+    g = torch.Generator().manual_seed(515)
+    out, cases = {}, []
+    specs = [
+        # name, qtype, scheme, bit, target, layout, shape, x multiplier, parameter setup
+        ("uni_pt_s8", "uniform", "per-tensor-symmetric", 8, "feature", "NCHW", (2, 3, 5, 5), 1.5, None),
+        ("uni_pt_a8_nlc", "uniform", "per-tensor-affine", 8, "feature", "NLC", (2, 6, 12), 1.5, None),
+        ("uni_pc_w4", "uniform", "per-channel-symmetric", 4, "weight", None, (6, 4, 3, 3), 0.3, None),
+        ("lsq_pt_s4", "lsq", "per-tensor-symmetric", 4, "feature", "NCHW", (2, 3, 5, 5), 1.5, None),
+        ("lsq_pc_conv4", "lsq", "per-channel-symmetric", 4, "weight", None, (16, 8, 3, 3), 0.3, None),
+        ("lsq_pc_lin8", "lsq", "per-channel-symmetric", 8, "weight", None, (24, 40), 0.3, None),
+        ("lsq_pc_neg4", "lsq", "per-channel-symmetric", 4, "weight", None, (6, 4, 3, 3), 0.3, "negate_scale"),
+        ("lsqp_pt_a8_half", "lsq+", "per-tensor-affine", 8, "feature", "NCHW", (2, 3, 5, 5), 1.5, "zp_half"),
+        ("lsqp_pt_a8_qmin", "lsq+", "per-tensor-affine", 8, "feature", "NCHW", (2, 3, 5, 5), 1.5, "zp_qmin"),
+        ("lsqp_pt_a8_above", "lsq+", "per-tensor-affine", 8, "feature", "NCHW", (2, 3, 5, 5), 1.5, "zp_above"),
+        ("lsqp_pc_w4", "lsq+", "per-channel-symmetric", 4, "weight", None, (6, 4, 3, 3), 0.3, None),
+        ("pact_s8_a15", "pact", "per-tensor-symmetric", 8, "feature", "NCHW", (4, 3, 16, 16), 2.0, 1.5),
+        ("pact_s4_a30", "pact", "per-tensor-symmetric", 4, "feature", "NCHW", (2, 3, 5, 5), 2.5, 3.0),
+        ("pact_s8_qmax", "pact", "per-tensor-symmetric", 8, "feature", "NCHW", (2, 3, 5, 5), 1.5, alpha_qmax),
+        ("pact_u8", "pact", "per-tensor-affine", 8, "feature", "NCHW", (2, 3, 5, 5), 1.5, 1.5),
+        ("pact_u4", "pact", "per-tensor-affine", 4, "feature", "NCHW", (2, 3, 5, 5), 2.5, 3.0),
+        ("dorefa_w4", "dorefa", "per-tensor-symmetric", 4, "weight", None, (6, 4, 3, 3), 0.6, None),
+    ]
+    for name, qtype, scheme, bit, target, layout, shape, mult, setup in specs:
+        cfg = R.make_cfg(scheme, bit, target, "minmax", layout or "NCHW", qtype=qtype)
+        if qtype == "pact":
+            cfg.QUANTIZER.PACT = R._CfgNode({"ALPHA_VALUE": setup})
+        q = build_quantizer(cfg)
+        q.set_backend(Backend.VIRTUAL)
+        if name == "pact_s8_a15":  # the inputs of the worked example in SURVEY Q19: alpha.grad = 45.153
+            gp = torch.Generator().manual_seed(0)
+            x = torch.randn(shape, generator=gp) * mult
+            gy = torch.randn(shape, generator=gp)
+        else:
+            x = torch.randn(shape, generator=g) * mult
+            gy = torch.randn(shape, generator=g)
+        q.update_observer(x)
+        q.calc_qparams()
+        with torch.no_grad():
+            if setup == "negate_scale":
+                q.scale[::3] *= -1
+            elif setup in ("zp_half", "zp_qmin", "zp_above"):
+                z = {"zp_half": float(torch.round(q.zero_point).reshape(-1)[0]) + 0.5, "zp_qmin": float(q.qdesc.qmin),
+                     "zp_above": float(q.qdesc.qmax) + 9.25}[setup]
+                q.zero_point.fill_(z)
+            s_used, z_used = q._qparams_preprocess(x)
+            if qtype == "dorefa":  # ties of the normalised tensor: x = atanh(u * s * max|tanh x|), the maximum kept
+                t_ = x.tanh()
+                m = t_.abs().max()
+                u = torch.tensor([0.5, 1.5, -2.5, 6.5, -6.5, 7.0]) * q.scale.reshape(-1)[0] * m
+                keep = int(t_.abs().reshape(-1).argmax())
+                pos = [i for i in range(8) if i != keep][: u.numel()]
+                x.reshape(-1)[pos] = torch.atanh(u)
+            elif name != "pact_s8_a15":
+                ch = q.qdesc.ch_axis if q.qdesc.is_perchannel else None
+                _plant_grid_edges(x, s_used.detach(), z_used.detach(), q.qdesc.qmin, q.qdesc.qmax, ch)
+                if qtype == "pact":  # the clamp bounds themselves and one ulp either side
+                    a = np.float32(setup)
+                    lo = -a if q.qdesc.qmin < 0 else np.float32(0)
+                    bounds = [a, np.nextafter(a, np.float32(0)), np.nextafter(a, np.float32(9)), lo,
+                              np.nextafter(lo, np.float32(-9)), np.nextafter(lo, np.float32(9))]
+                    x.reshape(-1)[9:9 + len(bounds)] = torch.tensor(bounds)
+        q.enable_quant()
+        xr = x.clone().requires_grad_(True)
+        y = q(xr)
+        (y * gy).sum().backward()
+        cases.append(name)
+        qd = q.qdesc
+        out[name + "_cfg"] = np.array([qtype, scheme, target, layout or ""])
+        out[name + "_meta"] = np.array([qd.qmin, qd.qmax, qd.ch_axis, int(qd.is_perchannel), int(qd.is_symmetric), bit])
+        out[name + "_x"], out[name + "_gy"] = x.numpy(), gy.numpy()
+        out[name + "_y"], out[name + "_gx"] = y.detach().numpy(), xr.grad.numpy()
+        if qtype == "pact":
+            out[name + "_alpha"] = q.alpha.detach().numpy()
+            out[name + "_galpha"] = q.alpha.grad.numpy()
+            continue
+        out[name + "_scale"] = q.scale.detach().reshape(-1).numpy()
+        out[name + "_zp"] = q.zero_point.detach().reshape(-1).numpy()
+        if q.scale.grad is not None:
+            out[name + "_gscale"] = q.scale.grad.reshape(-1).numpy()
+        if isinstance(q.zero_point, torch.nn.Parameter) and q.zero_point.grad is not None:
+            out[name + "_gzp"] = q.zero_point.grad.reshape(-1).numpy()
+    out["cases"] = np.array(cases)
+    save("qat", **out)
+
+
 GENERATORS = {"qdq": gen_qdq, "observers": gen_observers, "sparse": gen_sparse, "gptq": gen_gptq,
               "next_rows": gen_next_rows, "calibration": gen_calibration, "bwd": gen_bwd,
-              "sparse_structured": gen_sparse_structured}
+              "sparse_structured": gen_sparse_structured, "qat": gen_qat}
 
 if __name__ == "__main__":
     torch.set_num_threads(4)

@@ -211,35 +211,6 @@ def test_row_moments_vs_fp64_numpy():
         ops.moments_update(t(batches[0]), torch.zeros(2, 5, device=dev()))  # wrong dtype / shape
 
 
-@pytest.mark.parametrize("scheme,bit", [("per-tensor-affine", 4), ("per-tensor-symmetric", 8)])
-def test_pact_fused_clamp_gradients_equal_autograd_through_clamp(scheme, bit):
-    """PACT without the separate clamp pass (pact.py:43-46): forward == the reference chain clamp -> fake-quant, and the
-    gradients of x and alpha equal what autograd derives through ``torch.clamp`` followed by the straight-through op."""
-    q = build_quantizer(sbcfg.quantizer_config(scheme, bit, "feature", "minmax", qtype="pact", pact_alpha=1.5)).to(dev())
-    q.set_backend(Backend.VIRTUAL)
-    x = torch.randn(4, 3, 32, 32, device=dev()) * 1.2
-    x.view(-1)[:4] = torch.tensor([1.5, -1.5, 0.0, 1.5000001], device=dev())  # values on the clamp bounds
-    q.update_observer(x)
-    q.calc_qparams()
-    q.enable_quant()
-    xr = x.clone().requires_grad_(True)
-    gy = torch.randn_like(x)
-    y = q(xr)
-    (y * gy).sum().backward()
-    # reference chain in plain torch: clamp, then a straight-through fake-quant whose mask is all ones on clamped data
-    alpha = q.alpha.detach().clone().requires_grad_(True)
-    lower = -alpha if q.qdesc.qmin < 0 else torch.zeros(1, device=dev())
-    x2 = x.clone().requires_grad_(True)
-    xc = torch.clamp(x2, lower, alpha)
-    scale, zp = q.calc_qparams_with_minmax(lower.detach(), alpha.detach())
-    y_ref = oqdq.qdq(xc.detach().cpu().numpy(), scale.reshape(-1).cpu().numpy(), zp.reshape(-1).cpu().numpy(), *q.qdesc.qrange)
-    assert bits_equal(y.detach().cpu().numpy(), y_ref)
-    (xc * gy).sum().backward()
-    assert torch.equal(xr.grad, x2.grad)
-    ref_ga = float(alpha.grad)
-    assert abs(float(q.alpha.grad) - ref_ga) <= 1e-5 * max(1.0, float(gy.abs().sum()) * 1e-2)
-
-
 def _dorefa_eager(x, scale, zp, qdesc_q):
     """The reference op chain on the GPU (dorefa.py:15-20): ATen tanh / abs / max / div, then STE (native QDQ)."""
     from sparsebit_b200.quantization.quantizers.quant_tensor import STE

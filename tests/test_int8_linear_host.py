@@ -201,6 +201,21 @@ def test_every_ineligible_case_gives_its_reason():
     assert "expected a QLinear" in int8_ineligibility(nn.Linear(3, 4))
 
 
+@pytest.mark.parametrize("alpha,narrowed", [(1.5, False), (3.0, False), (1.0, True)])
+def test_signed_pact_inputs_whose_clamp_narrows_the_grid_are_ineligible(alpha, narrowed):
+    """alpha / scale = 127.5 in exact arithmetic; where fp32 rounds it to 127, -alpha lands on qmin + 1 and the clamp in
+    front of the fake-quant op narrows the grid (SURVEY Q19), which the integer path does not restate."""
+    q = _qlinear(a_type="pact")
+    q.input_quantizer.dims = 2
+    q.input_quantizer.alpha = nn.Parameter(torch.tensor([alpha]))
+    s = np.float32(alpha) * np.float32(2) / np.float32(255)
+    assert (np.rint(np.float32(alpha) / s) == 127) == narrowed
+    if narrowed:
+        assert "PACT with alpha on the grid, whose clamp narrows it to [-127, 127]" in _reason(q)
+    else:
+        assert int8_ineligibility(q) is None
+
+
 def test_to_integer_linears_skips_ineligible_layers():
     model = nn.Sequential(_qlinear(w_type="dorefa"), nn.ReLU(), _qlinear(a_bit=9))
     assert to_integer_linears(model) == []

@@ -357,6 +357,33 @@ def test_exact_division_schemes_on_cpu():
     assert out["cases"] > 5_000_000 and out["fast_path_accepted"] > 1_000_000
 
 
+def test_qat_restatement_matches_reference(golden):
+    """oracle.qdq's QAT chains (lsq_grads, pact_grads, dorefa_grads, the plain STE) against the unmodified reference
+    quantizers in a train-mode step (tests/golden/make_golden.py:gen_qat): y and gx bit-exact, every parameter gradient
+    within 1e-5 of the L1 norm of the terms summed into it (the reference sums them in fp32)."""
+    from qat_ref import GRAD_KEYS, case_geometry, oracle_case, within_l1
+
+    g = golden("qat")
+    seen = set()
+    for name in g["cases"]:
+        qtype = case_geometry(g, name)[0]
+        y, gx, grads = oracle_case(g, name)
+        if qtype == "dorefa":  # numpy's tanh may differ from ATen's by an ulp: a rare value moves one grid step
+            assert np.mean(y != g[name + "_y"]) < 5e-3, name
+            assert np.mean(~np.isclose(gx, g[name + "_gx"], rtol=1e-4, atol=1e-6)) < 5e-3, name
+        else:
+            assert _eq_bits(y, g[name + "_y"]), name
+            assert _eq_bits(gx, g[name + "_gx"]), name
+        recorded = {k for k, suffix in GRAD_KEYS.items() if name + suffix in g.files}
+        assert set(grads) == recorded, (name, set(grads), recorded)
+        for k, (grad, l1) in grads.items():
+            assert within_l1(grad, g[name + GRAD_KEYS[k]], l1), (name, k, grad, g[name + GRAD_KEYS[k]])
+        seen.add(qtype)
+    assert seen == {"uniform", "lsq", "lsq+", "pact", "dorefa"}
+    # the worked example of SURVEY Q19: signed 8-bit PACT, alpha 1.5, seed 0
+    assert abs(float(g["pact_s8_a15_galpha"][0]) - 45.153) < 1e-3
+
+
 def test_ste_backward_oracle_pinned_to_reference_myste(golden):
     """oracle.qdq.ste_backward against outputs of the reference's MySTE.backward (quant_tensor.py:46-71,
     generated by tests/golden/make_golden.py:gen_bwd): gx bit-exact; the scale / zero-point gradients equal the
