@@ -450,6 +450,44 @@ int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_
                       const float* bias, float* out, int64_t m, int64_t k, int64_t n, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* ---- (5a) 2:4 structured sparsity on the integer grid (int8 sparse wgmma, sm_90a) ---------------
+ * New; the reference's L1 sparser has only unstructured and per-filter masks, and its pruned layers run dense.
+ *
+ * sb200_sparse24_mask: mask [rows, cols] uint8 0 / 1 for w [rows, cols] fp32 (weight.reshape(C_out, -1)).  Each row is
+ * walked in aligned groups of 4 from column 0; a group keeps the two elements of largest |w|: ties go to the lower
+ * index, NaN ranks above every number (so it is kept), +-0 rank as 0; a tail group of r < 4 keeps min(2, r).
+ *
+ * Compressed weight format.  d[n, k] = w_q[n, k] - w_zero[n] (w_q / w_zero as sb200_int8_quantize_rows stores them) is
+ * the centred weight grid, 0 exactly where the fake-quant weight is 0, for k < K; d = 0 for k >= K.  With K64 =
+ * round_up(K, 64), group j of row n is d[n, 4j .. 4j + 3]; it keeps two indices i0 < i1: its nonzero positions, then its
+ * lowest-index zero positions up to two (so an all-zero group, and every padding group, keeps (0, 1)).
+ *   vals [N, K64 / 2] s8: vals[n, 2j] = d[n, 4j + i0], vals[n, 2j + 1] = d[n, 4j + i1].
+ *   meta [ceil(N / 128), K64 / 64, 2, 128] uint32: word (b, s, h, t) is what thread t of consumer warpgroup h reads at
+ *     k64 step s of 128-feature tile b: feature n = 128 b + 64 h + 16 (t >> 5) + ((t & 31) >> 2) + 8 (t & 1), groups
+ *     j = 16 s + 8 ((t >> 1) & 1) + g for g = 0 .. 7 with i0 | i1 << 2 in bits [4 g, 4 g + 4).  Features n >= N hold
+ *     0x44444444 (every group (0, 1)).  This is the sparse-metadata order of wgmma .sp .s8 m64nNk64, selector 0.
+ *   dsum [N] int32 = sum_k d[n, k].
+ *   bad [N] int32 = groups of row n with more than two nonzero d, or a d outside [-128, 127]; vals then do not hold
+ *     row n and sb200_int8_sparse24_linear must not be given it.
+ * A row whose w_scale is NaN is packed as d = 0 (its output column is NaN through w_scale).
+ *
+ * sb200_int8_sparse24_pack: the format above from w_q [N, Kp] s8, w_zero [N] int32, w_scale [N] fp32; vals 16-byte
+ * aligned.  Once per weight, at conversion.
+ *
+ * sb200_int8_sparse24_linear: out [M, N] fp32 (overwritten) for x [M, K] fp32 with per-tensor device scalars x_scale /
+ * x_zero_point and [qmin_x, qmax_x], the packed weight (vals, meta 16-byte aligned; dsum) with w_scale [N] and bias [N]
+ * or NULL.  I = sum_k a d - Z_x dsum on the stored activation grid equals sb200_int8_linear's integer, and the epilogue
+ * is the same: y = fp32(fp64(I) * (fp64(s_x) * fp64(w_scale[n]))) (+ bias[n] in fp32), NaN rows from x's NaN rows.
+ * So out equals sb200_int8_linear on the dense weight bit for bit.  Argument rules, K < 2^17 and the workspace
+ * (sb200_int8_linear_workspace_bytes(m, k), the same layout) are sb200_int8_linear's.  Deterministic, graph-capturable. */
+int sb200_sparse24_mask(const float* w, uint8_t* mask, int64_t rows, int64_t cols, void* stream);
+int sb200_int8_sparse24_pack(const int8_t* w_q, const int32_t* w_zero, const float* w_scale, int8_t* vals,
+                             uint32_t* meta, int32_t* dsum, int32_t* bad, int64_t n, int64_t k, void* stream);
+int sb200_int8_sparse24_linear(const float* x, const float* x_scale, const float* x_zero_point, int qmin_x, int qmax_x,
+                               const int8_t* vals, const uint32_t* meta, const int32_t* dsum, const float* w_scale,
+                               const float* bias, float* out, int64_t m, int64_t k, int64_t n, void* workspace,
+                               size_t workspace_bytes, void* stream);
+
 /* ---- (5b) Integer-grid inference of a calibrated QConv2d (int8 wgmma, sm_90a) ----------------
  * New; the reference's QConv2d (modules/conv.py) fake-quantises x and W (QDQ x 2) and runs F.conv2d.  Lowered, the
  * convolution is the integer linear above: M = n OH OW output pixels, K = c kh kw taps in the order (c, kh, kw) of

@@ -99,6 +99,10 @@ PROTOTYPES = {
     "sb200_int8_linear_workspace_bytes": (c_sz, [c_i64, c_i64]),
     "sb200_int8_linear": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp,
                                   c_sz, c_vp]),
+    "sb200_sparse24_mask": (c_int, [c_vp, c_vp, c_i64, c_i64, c_vp]),
+    "sb200_int8_sparse24_pack": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
+    "sb200_int8_sparse24_linear": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64,
+                                           c_i64, c_vp, c_sz, c_vp]),
     "sb200_int8_im2col_quantize": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "sb200_int8_conv2d_workspace_bytes": (c_sz, [c_geom]),
     "sb200_int8_conv2d": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_sz,

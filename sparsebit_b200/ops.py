@@ -764,6 +764,79 @@ def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     return out
 
 
+def sparse24_mask(w):
+    """2:4 keep-mask of ``w`` (sb200_sparse24_mask): bool, shaped like ``w``.  Each row of ``w.reshape(w.shape[0], -1)``
+    keeps the two largest |w| of every aligned group of 4 (ties to the lower index, NaN kept, a tail of r < 4 keeps
+    min(2, r))."""
+    lib = _lib.load()
+    _req(w, "weight")
+    rows = int(w.shape[0]) if w.dim() > 0 else 1
+    mask = torch.empty(w.shape, dtype=torch.bool, device=w.device)
+    with torch.cuda.device(w.device):
+        check(lib.sb200_sparse24_mask(w.data_ptr(), mask.data_ptr(), rows, w.numel() // rows, _stream(w)))
+    return mask
+
+
+def int8_sparse24_shapes(n, k):
+    """Shapes of the packed 2:4 weight (see sb200_int8_sparse24_pack): vals [N, K64 / 2], meta [ceil(N / 128), K64 / 64,
+    2, 128], K64 = round_up(K, 64)."""
+    k64 = (int(k) + 63) // 64 * 64
+    return (int(n), k64 // 2), ((int(n) + 127) // 128, k64 // 64, 2, 128)
+
+
+def int8_sparse24_pack(w_q, w_zero, w_scale, k):
+    """Compress a weight stored by ``int8_quantize_rows`` (w_q int8 [N, Kp], w_zero int32 [N], w_scale fp32 [N]) into
+    the 2:4 operand of ``int8_sparse24_linear``: returns ``(vals, meta, dsum, bad)`` with vals int8 [N, K64 / 2], meta
+    int32 [ceil(N / 128), K64 / 64, 2, 128] (uint32 words), dsum int32 [N] = sum_k (w_q - w_zero) and bad int32 [N] =
+    the groups of each row that are not 2:4 on the centred grid or leave s8 (a nonzero row cannot be used)."""
+    lib = _lib.load()
+    _req(w_q, "w_q", torch.int8), _req(w_zero, "w_zero", torch.int32), _req(w_scale, "w_scale")
+    k = int(k)
+    if w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
+        raise SparsebitB200Error(f"int8_sparse24_pack: w_q is {tuple(w_q.shape)} (need [N, {int8_padded_k(k)}])")
+    n = w_q.shape[0]
+    if w_zero.numel() != n or w_scale.numel() != n:
+        raise SparsebitB200Error(f"int8_sparse24_pack: w_zero / w_scale need {n} elements")
+    vshape, mshape = int8_sparse24_shapes(n, k)
+    vals = torch.empty(vshape, dtype=torch.int8, device=w_q.device)
+    meta = torch.empty(mshape, dtype=torch.int32, device=w_q.device)
+    dsum = torch.empty(n, dtype=torch.int32, device=w_q.device)
+    bad = torch.empty(n, dtype=torch.int32, device=w_q.device)
+    with torch.cuda.device(w_q.device):
+        check(lib.sb200_int8_sparse24_pack(w_q.data_ptr(), w_zero.data_ptr(), w_scale.data_ptr(), vals.data_ptr(),
+                                           meta.data_ptr(), dsum.data_ptr(), bad.data_ptr(), n, k, _stream(w_q)))
+    return vals, meta, dsum, bad
+
+
+def int8_sparse24_linear(x, x_scale, x_zero_point, qmin, qmax, vals, meta, dsum, w_scale, bias=None, k=None):
+    """``int8_linear`` of a 2:4-sparse weight on the sparse int8 tensor cores (sb200_int8_sparse24_linear), from the
+    operand ``int8_sparse24_pack`` made (vals, meta, dsum; every ``bad`` entry 0) and w_scale fp32 [N].  The output
+    equals ``int8_linear`` on the dense stored weight bit for bit.  ``x`` [..., K] fp32; returns fp32 [..., N]."""
+    lib = _lib.load()
+    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+    _req(vals, "vals", torch.int8), _req(meta, "meta", torch.int32), _req(dsum, "dsum", torch.int32)
+    if bias is not None:
+        _req(bias, "bias")
+    k = x.shape[-1] if k is None else int(k)
+    n = vals.shape[0] if vals.dim() == 2 else -1
+    vshape, mshape = int8_sparse24_shapes(max(n, 1), k)
+    if x.shape[-1] != k or tuple(vals.shape) != vshape or tuple(meta.shape) != mshape:
+        raise SparsebitB200Error(f"int8_sparse24_linear: x has {x.shape[-1]} features, vals is {tuple(vals.shape)} and meta "
+                                 f"{tuple(meta.shape)} (need {vshape} and {mshape})")
+    if dsum.numel() != n or w_scale.numel() != n or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"int8_sparse24_linear: dsum / w_scale / bias need {n} elements")
+    m = x.numel() // k
+    out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
+    ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
+    ws = _int8_workspace(x.device, ws_bytes)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_sparse24_linear(x.data_ptr(), x_scale.data_ptr(), x_zero_point.data_ptr(), int(qmin), int(qmax),
+                                             vals.data_ptr(), meta.data_ptr(), dsum.data_ptr(), w_scale.data_ptr(),
+                                             bias.data_ptr() if bias is not None else None, out.data_ptr(), m, k, n,
+                                             ws.data_ptr(), ws_bytes, _stream(x)))
+    return out
+
+
 def int8_quantize_cols(x, scale, zero_point, qmin, qmax):
     """Transposed integer grid of ``x`` [..., K, N] (sb200_int8_quantize_cols): returns ``(q, col_sum, nan)`` with q int8
     [..., N, Kp], q[..., n, k] = the ``int8_quantize_rows`` grid value of x[..., k, n], the padding to Kp =

@@ -162,17 +162,12 @@ def _check_inference_only(mod, training_cls, *inputs):
                            f"keep {training_cls} for training")
 
 
-class _Int8WeightModule(nn.Module):
-    """The stored weight operand of ``QLinearInt8`` / ``QConv2dInt8``: ``w_q`` int8 [N, Kp] and ``w_rowsum`` /
-    ``w_scale`` / ``w_zero`` [N] as ``_int8_weight_rows`` stores them, the per-tensor activation ``scale`` /
-    ``zero_point`` and integer range ``qmin`` / ``qmax``, and ``bias`` (fp32 or None)."""
+class _Int8InputModule(nn.Module):
+    """What every weight-carrying integer-grid module holds besides its weight operand: the per-tensor activation
+    ``scale`` / ``zero_point`` and integer range ``qmin`` / ``qmax``, and ``bias`` (fp32 or None).  A subclass registers
+    its weight buffers, then ``_register_input``."""
 
-    def __init__(self, out_features, k, device):
-        super().__init__()
-        self.register_buffer("w_q", torch.zeros(out_features, ops.int8_padded_k(k), dtype=torch.int8, device=device))
-        self.register_buffer("w_rowsum", torch.zeros(out_features, dtype=torch.int32, device=device))
-        self.register_buffer("w_scale", torch.zeros(out_features, dtype=torch.float32, device=device))
-        self.register_buffer("w_zero", torch.zeros(out_features, dtype=torch.int32, device=device))
+    def _register_input(self, device):
         self.register_buffer("scale", torch.ones(1, dtype=torch.float32, device=device))
         self.register_buffer("zero_point", torch.zeros(1, dtype=torch.float32, device=device))
         self.register_buffer("bias", None)
@@ -183,13 +178,10 @@ class _Int8WeightModule(nn.Module):
         if reason is not None:
             raise ValueError(f"{cls.__name__}.{method}: {reason}")
 
-    def _load(self, qmod):
-        """Fills the buffers from the calibrated ``qmod`` (a ``QLinear`` or ``QConv2d``); returns ``self``."""
+    def _load_input(self, qmod):
+        """Fills the activation qparams and the bias from the calibrated ``qmod``; returns ``self``."""
         aq = qmod.input_quantizer
         with torch.no_grad():
-            for buf, v in zip((self.w_q, self.w_rowsum, self.w_scale, self.w_zero),
-                              _int8_weight_rows(qmod.weight_quantizer, qmod.weight)):
-                buf.copy_(v)
             xs, xz = _qparams(aq, None)
             self.scale.copy_(xs.reshape(1))
             self.zero_point.copy_(xz.reshape(1))
@@ -197,6 +189,28 @@ class _Int8WeightModule(nn.Module):
                 self.bias = qmod.bias.detach().float().clone().contiguous()
         self.qmin, self.qmax = aq.qdesc.qrange
         return self
+
+
+class _Int8WeightModule(_Int8InputModule):
+    """The stored weight operand of ``QLinearInt8`` / ``QConv2dInt8``: ``w_q`` int8 [N, Kp] and ``w_rowsum`` /
+    ``w_scale`` / ``w_zero`` [N] as ``_int8_weight_rows`` stores them, with the activation qparams and bias of
+    ``_Int8InputModule``."""
+
+    def __init__(self, out_features, k, device):
+        super().__init__()
+        self.register_buffer("w_q", torch.zeros(out_features, ops.int8_padded_k(k), dtype=torch.int8, device=device))
+        self.register_buffer("w_rowsum", torch.zeros(out_features, dtype=torch.int32, device=device))
+        self.register_buffer("w_scale", torch.zeros(out_features, dtype=torch.float32, device=device))
+        self.register_buffer("w_zero", torch.zeros(out_features, dtype=torch.int32, device=device))
+        self._register_input(device)
+
+    def _load(self, qmod):
+        """Fills the buffers from the calibrated ``qmod`` (a ``QLinear`` or ``QConv2d``); returns ``self``."""
+        with torch.no_grad():
+            for buf, v in zip((self.w_q, self.w_rowsum, self.w_scale, self.w_zero),
+                              _int8_weight_rows(qmod.weight_quantizer, qmod.weight)):
+                buf.copy_(v)
+        return self._load_input(qmod)
 
 
 class QLinearInt8(_Int8WeightModule):
@@ -223,6 +237,78 @@ class QLinearInt8(_Int8WeightModule):
 
     def extra_repr(self):
         return f"in_features={self.in_features}, out_features={self.out_features}, qrange=[{self.qmin}, {self.qmax}]"
+
+
+def _sparse24_operand(qlinear):
+    """The weight of ``qlinear`` on the stored grid, packed by ``ops.int8_sparse24_pack``: ``((vals, meta, dsum,
+    w_scale), reason)``, where ``reason`` names the first row and group of 4 that is not 2:4 on the centred grid
+    d = g_w - rint(zp_w), or whose d leaves s8 (None when every row packs)."""
+    w_q, _, w_scale, w_zero = _int8_weight_rows(qlinear.weight_quantizer, qlinear.weight)
+    k = qlinear.weight.shape[1]
+    vals, meta, dsum, bad = ops.int8_sparse24_pack(w_q, w_zero.contiguous(), w_scale.contiguous(), k)
+    rows = torch.nonzero(bad).reshape(-1)
+    if rows.numel() == 0:
+        return (vals, meta, dsum, w_scale.contiguous()), None
+    r = int(rows[0])
+    d = w_q[r, :k].to(torch.int32) - w_zero[r]
+    d = F.pad(d, (0, (-k) % 4)).reshape(-1, 4)
+    wrong = ((d != 0).sum(1) > 2) | ((d < -128) | (d > 127)).any(1)
+    g = int(torch.nonzero(wrong).reshape(-1)[0])
+    if bool(((d[g] < -128) | (d[g] > 127)).any()):
+        why = f"the centred weight grid g_w - rint(zp_w) leaves s8 in row {r}, group {g} (k = {4 * g} .. {4 * g + 3})"
+    else:
+        why = f"the weight is not 2:4 sparse on the grid: row {r}, group {g} (k = {4 * g} .. {4 * g + 3}) has more than two nonzeros"
+    return None, why
+
+
+def int8_sparse24_ineligibility(qlinear):
+    """Why ``QLinearSparse24Int8.from_qlinear`` cannot convert ``qlinear`` (None when it can): a rule of
+    ``int8_ineligibility``, a centred weight grid outside s8 (possible for affine 8-bit weights only), or a group of 4
+    along a row of the weight grid with more than two nonzeros."""
+    reason = int8_ineligibility(qlinear)
+    return reason if reason is not None else _sparse24_operand(qlinear)[1]
+
+
+class QLinearSparse24Int8(_Int8InputModule):
+    """Inference-only replacement of a calibrated ``QLinear`` whose weight is 2:4 sparse on the grid: the linear of
+    ``QLinearInt8`` on the sparse int8 tensor cores (``ops.int8_sparse24_linear``), bit-identical to ``QLinearInt8`` on
+    the same module.  Only the compressed weight is stored: ``vals`` int8 [N, K64 / 2] (the kept centred grid values),
+    ``meta`` (their 2-bit indices), ``dsum`` int32 [N] and ``w_scale`` fp32 [N], about 0.625 byte per weight.  fp16
+    input is up-cast and the output is fp32, as in the fake-quant op.  Built by ``from_qlinear``; no backward."""
+
+    def __init__(self, in_features, out_features, device):
+        super().__init__()
+        vshape, mshape = ops.int8_sparse24_shapes(out_features, in_features)
+        self.register_buffer("vals", torch.zeros(vshape, dtype=torch.int8, device=device))
+        self.register_buffer("meta", torch.zeros(mshape, dtype=torch.int32, device=device))
+        self.register_buffer("dsum", torch.zeros(out_features, dtype=torch.int32, device=device))
+        self.register_buffer("w_scale", torch.zeros(out_features, dtype=torch.float32, device=device))
+        self._register_input(device)
+        self.in_features, self.out_features = int(in_features), int(out_features)
+
+    @classmethod
+    def from_qlinear(cls, qlinear):
+        reason = int8_ineligibility(qlinear)
+        operand = None
+        if reason is None:
+            operand, reason = _sparse24_operand(qlinear)
+        cls._check_eligible(reason, "from_qlinear")
+        n, k = qlinear.weight.shape
+        mod = cls(k, n, qlinear.weight.device)
+        with torch.no_grad():
+            for buf, v in zip((mod.vals, mod.meta, mod.dsum, mod.w_scale), operand):
+                buf.copy_(v)
+        return mod._load_input(qlinear)
+
+    def forward(self, x_in):
+        _check_inference_only(self, "QLinear", x_in)
+        x = x_in.float() if x_in.dtype != torch.float32 else x_in
+        return ops.int8_sparse24_linear(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.vals,
+                                        self.meta, self.dsum, self.w_scale, self.bias, k=self.in_features)
+
+    def extra_repr(self):
+        return (f"in_features={self.in_features}, out_features={self.out_features}, qrange=[{self.qmin}, {self.qmax}], "
+                f"2:4 sparse")
 
 
 def resolve_conv_padding(padding, kernel_size, dilation=1, stride=1):

@@ -1,10 +1,13 @@
 """Turn a calibrated model into an integer-inference model: every eligible ``QLinear`` becomes a ``QLinearInt8``
 (``to_integer_linears``), every eligible ``QConv2d`` a ``QConv2dInt8`` (``to_integer_convs``), every eligible ``QMatMul``
 a ``QMatMulInt8`` (``to_integer_matmuls``), every eligible grouped or depthwise ``QConv2d`` a ``QConv2dGroupInt8``
-(``to_integer_group_convs``), every eligible ``QAttention`` a ``QAttentionInt8`` (``to_integer_attentions``)."""
-from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, QLinearInt8, QMatMul,
-                       QMatMulInt8, int8_attention_ineligibility, int8_conv_ineligibility, int8_group_conv_ineligibility,
-                       int8_ineligibility, int8_matmul_ineligibility)
+(``to_integer_group_convs``), every eligible ``QAttention`` a ``QAttentionInt8`` (``to_integer_attentions``), and,
+opt-in, every ``QLinear`` whose weight is 2:4 sparse on the grid a ``QLinearSparse24Int8``
+(``to_sparse24_integer_linears``)."""
+from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, QLinearInt8,
+                       QLinearSparse24Int8, QMatMul, QMatMulInt8, int8_attention_ineligibility, int8_conv_ineligibility,
+                       int8_group_conv_ineligibility, int8_ineligibility, int8_matmul_ineligibility,
+                       int8_sparse24_ineligibility)
 
 
 def _swap(model, kind, ineligibility, convert):
@@ -52,3 +55,13 @@ def to_integer_attentions(model):
     stay ``QAttention``.  Run it before ``to_integer_matmuls``, which would otherwise convert the two matmuls of each
     attention separately.  Returns the qualified names of the converted modules, in ``named_modules`` order."""
     return _swap(model, QAttention, int8_attention_ineligibility, QAttentionInt8.from_qattention)
+
+
+def to_sparse24_integer_linears(model):
+    """Swap, in place, every ``QLinear`` of ``model`` that ``QLinearSparse24Int8.from_qlinear`` accepts (its weight 2:4
+    sparse on the grid, e.g. pruned by the 2:4 sparser with the mask folded into the weight); the others stay
+    ``QLinear``, and ``int8_sparse24_ineligibility`` says why.  Opt-in: the weight format differs from ``QLinearInt8``'s,
+    and where the sparse layer beats the dense one depends on the shape.  Run it before ``to_integer_linears``, which
+    would otherwise convert the sparse layers to dense ``QLinearInt8``.  Returns the qualified names of the converted
+    modules, in ``named_modules`` order."""
+    return _swap(model, QLinear, int8_sparse24_ineligibility, QLinearSparse24Int8.from_qlinear)

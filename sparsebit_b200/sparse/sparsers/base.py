@@ -3,7 +3,7 @@ a module built from ``(config, opr)`` that turns a weight into a keep-mask via `
 operator multiplies by that mask on every forward."""
 from torch import nn
 
-_KNOWN_TYPES = ("unstructed", "structed")  # spelling of the reference's config values
+_KNOWN_TYPES = ("unstructed", "structed", "2:4")  # the reference's two config values, and 2:4 (N:M) sparsity
 
 
 class Sparser(nn.Module):

@@ -8,7 +8,9 @@ sort.  structed (:27-40): the per-filter L1 norms are one pass of the row-moment
 fp64 sums), the cut is the exact (pruned - 1)-th smallest norm from the same radix select, and the float mask is
 written by ``sb200_mask_rows_gt`` -- no ``abs().sum()`` / ``torch.sort`` / per-index CPU round trips.  The ranking
 equals the reference's whenever two filters' norms differ by more than its fp32 summation error; filters that tie
-with the cut are pruned together.
+with the cut are pruned together.  2:4 (not in the reference): every aligned group of 4 along a row of
+``w.reshape(C_out, -1)`` keeps its two largest |w| (``sb200_sparse24_mask``), the pattern the sparse tensor cores run;
+RATIO is 0 (all ones) or 0.5.
 """
 import torch
 
@@ -24,6 +26,8 @@ class Sparser(BaseSparser):
     def calc_mask(self, x):
         if self.ratio == 0.0:
             return torch.ones_like(x)
+        if self.type == "2:4" and self.ratio != 0.5:
+            raise ValueError(f"the 2:4 sparser prunes half of every group of 4: RATIO must be 0 or 0.5, got {self.ratio}")
         w = x.detach()
         if not w.is_cuda:
             if not torch.cuda.is_available():
@@ -35,6 +39,8 @@ class Sparser(BaseSparser):
             k = min(int(n * self.ratio), n - 1)
             thresh = ops.kth_value(w.reshape(-1), k, key_mode=1)
             mask = ops.mask_gt(w, thresh)
+        elif self.type == "2:4":
+            mask = ops.sparse24_mask(w)
         elif self.type == "structed":
             pruned = int(w.shape[0] * self.ratio)
             if pruned == 0:
