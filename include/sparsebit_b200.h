@@ -528,6 +528,19 @@ int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float
                       const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* sb200_int8_sparse24_conv2d: the conv2d above with a 2:4-sparse weight on the sparse int8 tensor cores.  The weight is
+ * the (5a) operand that sb200_int8_sparse24_pack made from the stored rows of weight.reshape(c_out, -1) (K = c kh kw;
+ * vals, meta 16-byte aligned, dsum, every `bad` entry 0) with w_scale [c_out] and bias [c_out] or NULL.  The input is
+ * lowered by sb200_int8_im2col_quantize, whose K order (c, kh, kw) is the order the 2:4 groups follow, and a padding tap
+ * stores rint(zero_point) - off, so I = sum_k a d - Z_x dsum is sb200_int8_conv2d's integer.  out [n, c_out, OH, OW] fp32
+ * NCHW (overwritten) equals sb200_int8_conv2d on the dense stored weight bit for bit, NaNs included.  Argument checks
+ * in sb200_int8_conv2d's order (vals and meta take w_q's alignment rule); the workspace is
+ * sb200_int8_conv2d_workspace_bytes(geom), the same layout.  Deterministic, graph-capturable. */
+int sb200_int8_sparse24_conv2d(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                               const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* vals,
+                               const uint32_t* meta, const int32_t* dsum, const float* w_scale, const float* bias,
+                               float* out, int64_t c_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- (5c) Integer-grid inference of a calibrated activation x activation matmul (int8 wgmma, sm_90a) ----
  * New; the reference's MatMul (modules/matmul.py) multiplies two fake-quantised activations (a QIdentity carrier in
  * front of each input) with an fp32 torch.matmul.  With both operands per-tensor the product is

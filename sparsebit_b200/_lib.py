@@ -107,6 +107,8 @@ PROTOTYPES = {
     "sb200_int8_conv2d_workspace_bytes": (c_sz, [c_geom]),
     "sb200_int8_conv2d": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_sz,
                                   c_vp]),
+    "sb200_int8_sparse24_conv2d": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                           c_vp, c_sz, c_vp]),
     "sb200_int8_quantize_cols": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp]),
     "sb200_int8_matmul_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64]),
     "sb200_int8_matmul": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_i64, c_i64,

@@ -23,6 +23,15 @@
 // loaded; a consumer thread reads one metadata word per 64-feature x 64-K step from shared memory.  The accumulator
 // rows are features, so the epilogue stages the tile through shared memory (the ring, free once both warpgroups are
 // done) and stores rows of out [M, N] whole.
+//
+// Conv2d.  sb200_int8_im2col_quantize lowers the input into the same workspace, one s8 row per output pixel in the K
+// order (c, kh, kw) of weight.reshape(C_out, -1), the order the 2:4 groups of a pruned conv weight follow; the same GEMM
+// (kNchw = true) then writes NCHW: out[(img N + n) P + p] for token m = img P + p, P = OH OW.  The epilogue stages the
+// tile as [feature][token] (rows of kSpTok + 4 floats), the mirror of the row-major staging; warp c of the consumers
+// stores feature rows c, c + 8, ..., lane l tokens 4 l .. 4 l + 3, whose image / pixel split and NaN flags it computes
+// once.  Four tokens at consecutive out addresses (one image, or N = 1) leave as one 16-byte store when the first is
+// 16-byte aligned, others one by one,
+// so a tile spanning images (P < 128, P = 1 at a 1 x 1 output) is stored correctly.
 #include "int8_grid.cuh"
 #include "tc_common.cuh"
 namespace sb200 {
@@ -38,10 +47,12 @@ constexpr int kSpWBytes = kSpFeat * (kSpBK / 2);   // 16 KB: 128 features x 128 
 constexpr int kSpEWords = (kSpBK / 64) * 2 * 128;  // metadata words of a stage: [k64 step][warpgroup][thread]
 constexpr int kSpStageBytes = 2 * kSpXBox + kSpWBytes + kSpEWords * 4;  // 52 KB, a multiple of 1024
 constexpr int kSpLd = kSpFeat + 4;                 // floats per staged token row: conflict-free transposed writes
+constexpr int kSpLdT = kSpTok + 4;                 // NCHW: floats per staged feature row
 constexpr long long kSpMaxK = 1LL << 17;
 constexpr uint32_t kSpPadMeta = 0x44444444u;       // every group keeps indices (0, 1)
 static_assert(kSpStageBytes % 1024 == 0, "stage tiles stay 1024-byte aligned");
 static_assert(kSpTok * kSpLd * 4 <= kSpStages * kSpStageBytes, "the output tile fits the ring");
+static_assert(kSpFeat * kSpLdT * 4 <= kSpStages * kSpStageBytes, "the NCHW output tile fits the ring");
 
 struct SpRing {
   uint64_t full[kSpStages];
@@ -151,6 +162,63 @@ __device__ __forceinline__ void wgmma_m64n128k64_sp_s8(int (&d)[64], uint64_t ad
       : "l"(adesc), "l"(bdesc), "r"(e), "r"(accumulate));
 }
 
+// NCHW epilogue of the sparse GEMM (the 256 consumer threads; the ring is free).  Thread (warp w, lane l, q = l & 3)
+// holds features f0, f0 + 8 of the tile (per-feature terms cn, sxw, bn) and, in acc[j], tokens 8 (j >> 2) + 2 q +
+// (j & 1).  The tile is staged [feature][token]; then consumer warp cw stores feature rows cw, cw + 8, ... < N - n0 and
+// lane l tokens t = 4 l .. 4 l + 3 < M - m0 of each: out[(img N + n) P + p] with m = img P + p, split once per token.
+__device__ __forceinline__ void sp_store_nchw(const int (&acc)[64], float* tile, const long long (&cn)[2],
+                                              const double (&sxw)[2], const float (&bn)[2], bool has_bias, int f0, int q,
+                                              int cw, int lane, float* __restrict__ out, const uint8_t* __restrict__ x_nan,
+                                              int m0, int n0, int M, int N, int P, int vec4) {
+#pragma unroll
+  for (int c = 0; c < 16; ++c) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float y[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const long long I = (long long)acc[4 * c + 2 * h + e] + cn[h];
+        y[e] = __double2float_rn((double)I * sxw[h]);
+        if (has_bias) y[e] = __fadd_rn(y[e], bn[h]);
+      }
+      *reinterpret_cast<float2*>(tile + (f0 + 8 * h) * kSpLdT + 8 * c + 2 * q) = make_float2(y[0], y[1]);
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  // per token of this lane: the out offset of feature 0, img N P + p, and its NaN flag
+  long long base[4];
+  bool tnan[4], live[4];
+  const int t0 = 4 * lane;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int m = m0 + t0 + i;
+    live[i] = m < M;
+    const int img = live[i] ? m / P : 0;
+    base[i] = (long long)img * N * P + (m - img * P);
+    tnan[i] = live[i] && __ldg(x_nan + m) != 0;
+  }
+  // the four tokens are live and lie in one image: consecutive pixels, consecutive out addresses
+  const bool run = live[3] && base[3] - base[0] == 3;
+  const float qnan = __int_as_float(0x7fc00000);
+  for (int r = cw; r < kSpFeat; r += 8) {
+    const int n = n0 + r;
+    if (n >= N) break;
+    const float4 v4 = *reinterpret_cast<const float4*>(tile + r * kSpLdT + t0);
+    float v[4] = {v4.x, v4.y, v4.z, v4.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (tnan[i]) v[i] = qnan;
+    const long long o = base[0] + (long long)n * P;
+    if (vec4 && run && (o & 3) == 0) {
+      *reinterpret_cast<float4*>(out + o) = make_float4(v[0], v[1], v[2], v[3]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        if (live[i]) out[base[i] + (long long)n * P] = v[i];
+    }
+  }
+}
+
 // Ring protocol (as int8_linear.cu): full[s] (count 1) completes when the producer's expect_tx and the stage's TMA loads
 // have landed; empty[s] (count 8) when each consumer warp has arrived.  Unlike the dense kernel, a consumer retires each
 // stage's wgmma group before loading the next stage's metadata words and frees the stage then (see the loop).  Every
@@ -161,13 +229,15 @@ __device__ __forceinline__ void wgmma_m64n128k64_sp_s8(int (&d)[64], uint64_t ad
 //
 // Accumulator layout of a consumer thread (warp w of its warpgroup, lane l, q = l & 3), j = 0 .. 63:
 //   acc[j] = D[feature 16 w + l / 4 + 8 ((j >> 1) & 1)][token 8 (j >> 2) + 2 q + (j & 1)]
+// kNchw = false: out is row-major [M, N].  kNchw = true: out is NCHW [M / P, N, P] (conv2d, P = OH OW pixels per image).
+template <bool kNchw>
 __global__ void __launch_bounds__(kSpThreads, 1)
 int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_v,
                           const __grid_constant__ CUtensorMap map_e, float* __restrict__ out,
                           const uint8_t* __restrict__ x_nan, const float* __restrict__ x_scale,
                           const float* __restrict__ x_zero, int x_off, const int* __restrict__ dsum,
                           const float* __restrict__ w_scale, const float* __restrict__ bias, int M, int N, int kb64,
-                          int vec4) {
+                          int vec4, int P) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   SpRing* ring = reinterpret_cast<SpRing*>(stage_base + (size_t)kSpStages * kSpStageBytes);
@@ -255,39 +325,44 @@ int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
     __syncwarp();
     if (lane == 0) mbar_arrive(&ring->empty[s]);
   }
-  // every wgmma of both warpgroups has read its stage: the ring becomes the output tile [token][feature]
+  // every wgmma of both warpgroups has read its stage: the ring becomes the output tile, [token][feature] (row-major
+  // out) or [feature][token] (NCHW out)
   asm volatile("bar.sync 1, 256;" ::: "memory");
   float* tile = reinterpret_cast<float*>(stage_base);
+  if constexpr (kNchw) {
+    sp_store_nchw(acc, tile, cn, sxw, bn, bias != nullptr, f0, q, warp - 4, lane, out, x_nan, m0, n0, M, N, P, vec4);
+  } else {
 #pragma unroll
-  for (int c = 0; c < 16; ++c) {
+    for (int c = 0; c < 16; ++c) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const long long I = (long long)acc[4 * c + 2 * h + e] + cn[h];
-        float y = __double2float_rn((double)I * sxw[h]);
-        if (bias) y = __fadd_rn(y, bn[h]);
-        tile[(8 * c + 2 * q + e) * kSpLd + f0 + 8 * h] = y;
+        for (int e = 0; e < 2; ++e) {
+          const long long I = (long long)acc[4 * c + 2 * h + e] + cn[h];
+          float y = __double2float_rn((double)I * sxw[h]);
+          if (bias) y = __fadd_rn(y, bn[h]);
+          tile[(8 * c + 2 * q + e) * kSpLd + f0 + 8 * h] = y;
+        }
       }
     }
-  }
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  // warp c of the consumers stores token rows c, c + 8, ...: lane l holds features 4 l .. 4 l + 3
-  const int cw = warp - 4, nl = 4 * lane, n = n0 + nl;
-  const float qnan = __int_as_float(0x7fc00000);
-  for (int r = cw; r < kSpTok; r += 8) {
-    const int m = m0 + r;
-    if (m >= M) break;
-    float4 v = *reinterpret_cast<const float4*>(tile + r * kSpLd + nl);
-    if (__ldg(x_nan + m)) v = make_float4(qnan, qnan, qnan, qnan);
-    float* o = out + (size_t)m * N + n;
-    if (vec4 && n + 3 < N) {
-      *reinterpret_cast<float4*>(o) = v;
-    } else {
-      const float vv[4] = {v.x, v.y, v.z, v.w};
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // warp c of the consumers stores token rows c, c + 8, ...: lane l holds features 4 l .. 4 l + 3
+    const int cw = warp - 4, nl = 4 * lane, n = n0 + nl;
+    const float qnan = __int_as_float(0x7fc00000);
+    for (int r = cw; r < kSpTok; r += 8) {
+      const int m = m0 + r;
+      if (m >= M) break;
+      float4 v = *reinterpret_cast<const float4*>(tile + r * kSpLd + nl);
+      if (__ldg(x_nan + m)) v = make_float4(qnan, qnan, qnan, qnan);
+      float* o = out + (size_t)m * N + n;
+      if (vec4 && n + 3 < N) {
+        *reinterpret_cast<float4*>(o) = v;
+      } else {
+        const float vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (n + i < N) o[i] = vv[i];
+        for (int i = 0; i < 4; ++i)
+          if (n + i < N) o[i] = vv[i];
+      }
     }
   }
 }
@@ -307,6 +382,38 @@ SpWorkspace sp_workspace(void* workspace, long long m, long long k) {
   const size_t off_sum = align_up((size_t)m * (size_t)padded_k(k), 1024);
   const size_t off_nan = off_sum + align_up((size_t)m * 4, 256);
   return {reinterpret_cast<int8_t*>(ws), reinterpret_cast<int32_t*>(ws + off_sum), ws + off_nan};
+}
+
+// The lowered activations in the workspace, written by `lower` (the row quantizer or the conv lowering), then the
+// sparse GEMM into `out` (row-major [M, N], or NCHW with P pixels per image).  Arguments are checked by the caller.
+template <bool kNchw, typename Lower>
+int sp_run(const char* fn, long long m, long long k, long long n, long long P, int qmin_x, const float* x_scale,
+           const float* x_zero_point, const int8_t* vals, const uint32_t* meta, const int32_t* dsum, const float* w_scale,
+           const float* bias, float* out, void* workspace, cudaStream_t st, Lower lower) {
+  const SpWorkspace w = sp_workspace(workspace, m, k);
+  const long long kp = padded_k(k), kb64 = k64_of(k) / 64;
+  CUtensorMap map_x, map_v, map_e;
+  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, w.xq, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, 128, kSpTok,
+                   CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_2d(&map_v, CU_TENSOR_MAP_DATA_TYPE_UINT8, vals, (uint64_t)(kb64 * 32), (uint64_t)n, (uint64_t)(kb64 * 32),
+                   128, kSpFeat, CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_3d(&map_e, CU_TENSOR_MAP_DATA_TYPE_UINT32, meta, 256, (uint64_t)kb64, (uint64_t)meta_tiles(n), 1024, 256,
+                   kSpBK / 64, CU_TENSOR_MAP_SWIZZLE_NONE)) {
+    set_error("%s: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", fn, m, k, n);
+    return SB200_E_CUDA;
+  }
+  if (const int rc = lower(w, st)) return rc;
+  const size_t smem = (size_t)kSpStages * kSpStageBytes + sizeof(SpRing) + 1024;
+  static std::atomic<int> attr_done[64];
+  SB_CUDA(ensure_dyn_smem(int8_sparse24_gemm_kernel<kNchw>, (int)smem, attr_done));
+  const long long tiles = ((m + kSpTok - 1) / kSpTok) * ((n + kSpFeat - 1) / kSpFeat);
+  // row-major: 16-byte stores of 4 features need N % 4 = 0; NCHW: each run of 4 pixels checks its own address
+  const int vec4 = (kNchw || n % 4 == 0) && aligned16(out);
+  int8_sparse24_gemm_kernel<kNchw><<<(unsigned)tiles, kSpThreads, smem, st>>>(
+      map_x, map_v, map_e, out, w.xnan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(dsum),
+      w_scale, bias, (int)m, (int)n, (int)kb64, vec4, (int)P);
+  SB_LAUNCHED();
+  return SB200_OK;
 }
 
 }  // namespace
@@ -362,29 +469,37 @@ int sb200_int8_sparse24_linear(const float* x, const float* x_scale, const float
     return SB200_E_UNSUPPORTED;
   }
   if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_linear_workspace_bytes(m, k))) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const SpWorkspace w = sp_workspace(workspace, m, k);
-  const long long kp = padded_k(k), kb64 = k64_of(k) / 64;
-  CUtensorMap map_x, map_v, map_e;
-  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, w.xq, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, 128, kSpTok,
-                   CU_TENSOR_MAP_SWIZZLE_128B) ||
-      !make_map_2d(&map_v, CU_TENSOR_MAP_DATA_TYPE_UINT8, vals, (uint64_t)(kb64 * 32), (uint64_t)n, (uint64_t)(kb64 * 32),
-                   128, kSpFeat, CU_TENSOR_MAP_SWIZZLE_128B) ||
-      !make_map_3d(&map_e, CU_TENSOR_MAP_DATA_TYPE_UINT32, meta, 256, (uint64_t)kb64, (uint64_t)meta_tiles(n), 1024, 256,
-                   kSpBK / 64, CU_TENSOR_MAP_SWIZZLE_NONE)) {
-    set_error("%s: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", fn, (long long)m, (long long)k, (long long)n);
-    return SB200_E_CUDA;
+  return sp_run<false>(fn, m, k, n, 1, qmin_x, x_scale, x_zero_point, vals, meta, dsum, w_scale, bias, out, workspace,
+                       (cudaStream_t)stream, [&](const SpWorkspace& w, cudaStream_t st) {
+                         return sb200_int8_quantize_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, w.xq, w.xsum, w.xnan,
+                                                         m, k, st);
+                       });
+}
+
+int sb200_int8_sparse24_conv2d(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                               const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* vals,
+                               const uint32_t* meta, const int32_t* dsum, const float* w_scale, const float* bias,
+                               float* out, int64_t c_out, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "sb200_int8_sparse24_conv2d";
+  SB_REQUIRE(x && geom && x_scale && x_zero_point && vals && meta && dsum && w_scale && out && workspace,
+             "%s: null pointer argument", fn);
+  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
+  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
+  long long oh = 0, ow = 0;
+  if (const int rc = int8_check_conv(fn, geom, &oh, &ow)) return rc;
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
+  SB_REQUIRE(aligned16(vals) && aligned16(meta), "%s: vals and meta must be 16-byte aligned", fn);
+  // each factor is < 2^31 (int8_check_conv): the product fits __int128
+  const __int128 k = (__int128)geom->c * geom->kh * geom->kw;
+  if (k >= kSpMaxK) {
+    set_error("%s: K >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
+    return SB200_E_UNSUPPORTED;
   }
-  if (const int rc = sb200_int8_quantize_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, w.xq, w.xsum, w.xnan, m, k, st))
-    return rc;
-  const size_t smem = (size_t)kSpStages * kSpStageBytes + sizeof(SpRing) + 1024;
-  static std::atomic<int> attr_done[64];
-  SB_CUDA(ensure_dyn_smem(int8_sparse24_gemm_kernel, (int)smem, attr_done));
-  const long long tiles = ((m + kSpTok - 1) / kSpTok) * ((n + kSpFeat - 1) / kSpFeat);
-  const int vec4 = (n % 4 == 0) && aligned16(out);
-  int8_sparse24_gemm_kernel<<<(unsigned)tiles, kSpThreads, smem, st>>>(
-      map_x, map_v, map_e, out, w.xnan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(dsum),
-      w_scale, bias, (int)m, (int)n, (int)kb64, vec4);
-  SB_LAUNCHED();
-  return SB200_OK;
+  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
+  const long long P = oh * ow, m = geom->n * P;
+  return sp_run<true>(fn, m, (long long)k, c_out, P, qmin_x, x_scale, x_zero_point, vals, meta, dsum, w_scale, bias, out,
+                      workspace, (cudaStream_t)stream, [&](const SpWorkspace& w, cudaStream_t st) {
+                        return sb200_int8_im2col_quantize(x, geom, x_scale, x_zero_point, qmin_x, qmax_x, w.xq, w.xsum,
+                                                          w.xnan, st);
+                      });
 }

@@ -1100,6 +1100,41 @@ def int8_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     return out
 
 
+def int8_sparse24_conv2d(x, x_scale, x_zero_point, qmin, qmax, vals, meta, dsum, w_scale, kernel_size, bias=None,
+                         stride=1, padding=0, dilation=1):
+    """``int8_conv2d`` of a 2:4-sparse weight on the sparse int8 tensor cores (sb200_int8_sparse24_conv2d): ``x`` [N, C,
+    H, W] fp32 is lowered as ``int8_conv2d`` lowers it and multiplied with the operand ``int8_sparse24_pack`` made from
+    the stored rows of ``weight.reshape(C_out, -1)`` (K = C KH KW; vals, meta, dsum, every ``bad`` entry 0) and w_scale
+    fp32 [C_out].  The output equals ``int8_conv2d`` on the dense stored weight bit for bit.  Returns fp32 [N, C_out, OH,
+    OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right)."""
+    lib = _lib.load()
+    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+    _req(vals, "vals", torch.int8), _req(meta, "meta", torch.int32), _req(dsum, "dsum", torch.int32)
+    if bias is not None:
+        _req(bias, "bias")
+    if x.dim() != 4:
+        raise SparsebitB200Error("int8_sparse24_conv2d: data must be [N, C, H, W]")
+    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
+    k = g.c * g.kh * g.kw
+    n = vals.shape[0] if vals.dim() == 2 else -1
+    vshape, mshape = int8_sparse24_shapes(max(n, 1), k)
+    if tuple(vals.shape) != vshape or tuple(meta.shape) != mshape:
+        raise SparsebitB200Error(f"int8_sparse24_conv2d: vals is {tuple(vals.shape)} and meta {tuple(meta.shape)}, the "
+                                 f"geometry (K = {k}) needs {vshape} and {mshape}")
+    if dsum.numel() != n or w_scale.numel() != n or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"int8_sparse24_conv2d: dsum / w_scale / bias need {n} elements")
+    oh, ow = conv2d_output_hw(g)
+    out = torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
+    ws = _int8_workspace(x.device, max(ws_bytes, 16))
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_sparse24_conv2d(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(), x_zero_point.data_ptr(),
+                                             int(qmin), int(qmax), vals.data_ptr(), meta.data_ptr(), dsum.data_ptr(),
+                                             w_scale.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                             out.data_ptr(), n, ws.data_ptr(), ws.numel(), _stream(x)))
+    return out
+
+
 def int8_group_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups, bias=None,
                       stride=1, padding=0, dilation=1):
     """The fake-quant grouped / depthwise conv2d (groups >= 2) on the integer grid (sb200_int8_group_conv2d): one direct

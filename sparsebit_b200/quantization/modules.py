@@ -239,12 +239,13 @@ class QLinearInt8(_Int8WeightModule):
         return f"in_features={self.in_features}, out_features={self.out_features}, qrange=[{self.qmin}, {self.qmax}]"
 
 
-def _sparse24_operand(qlinear):
-    """The weight of ``qlinear`` on the stored grid, packed by ``ops.int8_sparse24_pack``: ``((vals, meta, dsum,
-    w_scale), reason)``, where ``reason`` names the first row and group of 4 that is not 2:4 on the centred grid
-    d = g_w - rint(zp_w), or whose d leaves s8 (None when every row packs)."""
-    w_q, _, w_scale, w_zero = _int8_weight_rows(qlinear.weight_quantizer, qlinear.weight)
-    k = qlinear.weight.shape[1]
+def _sparse24_operand(qmod):
+    """The weight of ``qmod`` (a ``QLinear`` or ``QConv2d``) on the stored grid, rows of ``weight.reshape(C_out, -1)``
+    with K = ``weight[0].numel()``, packed by ``ops.int8_sparse24_pack``: ``((vals, meta, dsum, w_scale), reason)``,
+    where ``reason`` names the first row and group of 4 that is not 2:4 on the centred grid d = g_w - rint(zp_w), or
+    whose d leaves s8 (None when every row packs); k indexes a row of ``weight.reshape(C_out, -1)``."""
+    w_q, _, w_scale, w_zero = _int8_weight_rows(qmod.weight_quantizer, qmod.weight)
+    k = qmod.weight[0].numel()
     vals, meta, dsum, bad = ops.int8_sparse24_pack(w_q, w_zero.contiguous(), w_scale.contiguous(), k)
     rows = torch.nonzero(bad).reshape(-1)
     if rows.numel() == 0:
@@ -365,36 +366,25 @@ def int8_conv_ineligibility(qconv):
     return _int8_conv_ineligibility(qconv, _dense_conv_rule)
 
 
-class QConv2dInt8(_Int8WeightModule):
-    """Inference-only replacement of a calibrated ``QConv2d`` (groups = 1): the fake-quant conv2d computed on the
-    integer grid by ``ops.int8_conv2d`` -- the input lowered to its int8 grid in one pass, exact int8 x int8 sums on the
-    tensor cores, zero points removed in int64, then s_x s_w[n] I + bias, written NCHW.  Built by ``from_qconv2d``; the
-    weights (``weight.reshape(C_out, -1)``) are quantized once at conversion.  Takes [N, C, H, W] or unbatched
-    [C, H, W]; fp16 input is up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps
-    ``QConv2d``."""
+class _Int8Conv2dModule:
+    """The conv geometry and forward shared by the integer-grid conv modules: ``_set_geometry`` records it, a subclass
+    supplies ``_conv`` of a contiguous fp32 [N, C, H, W] input.  ``forward`` takes [N, C, H, W] or unbatched [C, H, W]
+    and up-casts fp16; the output is fp32."""
 
-    _ineligibility = staticmethod(int8_conv_ineligibility)
-
-    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device, groups=1):
-        super().__init__(out_channels, in_channels // int(groups) * kernel_size[0] * kernel_size[1], device)
+    def _set_geometry(self, in_channels, out_channels, kernel_size, stride, padding, dilation, groups=1):
         self.in_channels, self.out_channels, self.groups = int(in_channels), int(out_channels), int(groups)
         self.kernel_size, self.stride, self.dilation = tuple(kernel_size), tuple(stride), tuple(dilation)
         self.padding = tuple(padding)  # (top, bottom, left, right)
 
-    @classmethod
-    def from_qconv2d(cls, qconv):
-        cls._check_eligible(cls._ineligibility(qconv), "from_qconv2d")
+    @staticmethod
+    def _geometry_of(qconv):
+        """The constructor arguments of ``qconv``'s geometry: in / out channels, kernel, stride, resolved padding,
+        dilation, groups."""
         kw = qconv.fwd_kwargs
         c_out, c_g, kh, kwd = qconv.weight.shape
         groups = int(kw["groups"])
         padding = resolve_conv_padding(kw["padding"], (kh, kwd), kw["dilation"], kw["stride"])
-        return cls(c_g * groups, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]),
-                   device=qconv.weight.device, groups=groups)._load(qconv)
-
-    def _conv(self, x):
-        return ops.int8_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
-                               self.w_scale, self.w_zero, self.kernel_size, self.bias, self.stride, self.padding,
-                               self.dilation)
+        return c_g * groups, c_out, (kh, kwd), _pair(kw["stride"]), padding, _pair(kw["dilation"]), groups
 
     def forward(self, x_in):
         _check_inference_only(self, "QConv2d", x_in)
@@ -408,6 +398,81 @@ class QConv2dInt8(_Int8WeightModule):
     def extra_repr(self):
         return (f"{self.in_channels}, {self.out_channels}, kernel_size={self.kernel_size}, stride={self.stride}, "
                 f"padding={self.padding}, dilation={self.dilation}, qrange=[{self.qmin}, {self.qmax}]")
+
+
+class QConv2dInt8(_Int8Conv2dModule, _Int8WeightModule):
+    """Inference-only replacement of a calibrated ``QConv2d`` (groups = 1): the fake-quant conv2d computed on the
+    integer grid by ``ops.int8_conv2d`` -- the input lowered to its int8 grid in one pass, exact int8 x int8 sums on the
+    tensor cores, zero points removed in int64, then s_x s_w[n] I + bias, written NCHW.  Built by ``from_qconv2d``; the
+    weights (``weight.reshape(C_out, -1)``) are quantized once at conversion.  Takes [N, C, H, W] or unbatched
+    [C, H, W]; fp16 input is up-cast and the output is fp32, as in the fake-quant op.  There is no backward: QAT keeps
+    ``QConv2d``."""
+
+    _ineligibility = staticmethod(int8_conv_ineligibility)
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device, groups=1):
+        super().__init__(out_channels, in_channels // int(groups) * kernel_size[0] * kernel_size[1], device)
+        self._set_geometry(in_channels, out_channels, kernel_size, stride, padding, dilation, groups)
+
+    @classmethod
+    def from_qconv2d(cls, qconv):
+        cls._check_eligible(cls._ineligibility(qconv), "from_qconv2d")
+        *geometry, groups = cls._geometry_of(qconv)
+        return cls(*geometry, device=qconv.weight.device, groups=groups)._load(qconv)
+
+    def _conv(self, x):
+        return ops.int8_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
+                               self.w_scale, self.w_zero, self.kernel_size, self.bias, self.stride, self.padding,
+                               self.dilation)
+
+
+def int8_sparse24_conv_ineligibility(qconv):
+    """Why ``QConv2dSparse24Int8.from_qconv2d`` cannot convert ``qconv`` (None when it can): a rule of
+    ``int8_conv_ineligibility`` (groups >= 2 and unresolvable padding included), a centred weight grid outside s8, or a
+    group of 4 along a row of ``weight.reshape(C_out, -1)`` on the grid with more than two nonzeros."""
+    reason = int8_conv_ineligibility(qconv)
+    return reason if reason is not None else _sparse24_operand(qconv)[1]
+
+
+class QConv2dSparse24Int8(_Int8Conv2dModule, _Int8InputModule):
+    """Inference-only replacement of a calibrated ``QConv2d`` (groups = 1) whose weight is 2:4 sparse on the grid along
+    the rows of ``weight.reshape(C_out, -1)``: the conv2d of ``QConv2dInt8`` on the sparse int8 tensor cores
+    (``ops.int8_sparse24_conv2d``), bit-identical to ``QConv2dInt8`` on the same module.  Only the compressed weight
+    is stored (``vals``, ``meta``, ``dsum``, ``w_scale``, as ``QLinearSparse24Int8``), about 0.625 byte per weight.
+    Takes [N, C, H, W] or unbatched [C, H, W]; fp16 input is up-cast and the output is fp32.  Built by
+    ``from_qconv2d``; no backward."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device):
+        super().__init__()
+        vshape, mshape = ops.int8_sparse24_shapes(out_channels, in_channels * kernel_size[0] * kernel_size[1])
+        self.register_buffer("vals", torch.zeros(vshape, dtype=torch.int8, device=device))
+        self.register_buffer("meta", torch.zeros(mshape, dtype=torch.int32, device=device))
+        self.register_buffer("dsum", torch.zeros(out_channels, dtype=torch.int32, device=device))
+        self.register_buffer("w_scale", torch.zeros(out_channels, dtype=torch.float32, device=device))
+        self._register_input(device)
+        self._set_geometry(in_channels, out_channels, kernel_size, stride, padding, dilation)
+
+    @classmethod
+    def from_qconv2d(cls, qconv):
+        reason = int8_conv_ineligibility(qconv)
+        operand = None
+        if reason is None:
+            operand, reason = _sparse24_operand(qconv)
+        cls._check_eligible(reason, "from_qconv2d")
+        *geometry, _ = cls._geometry_of(qconv)
+        mod = cls(*geometry, device=qconv.weight.device)
+        with torch.no_grad():
+            for buf, v in zip((mod.vals, mod.meta, mod.dsum, mod.w_scale), operand):
+                buf.copy_(v)
+        return mod._load_input(qconv)
+
+    def _conv(self, x):
+        return ops.int8_sparse24_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.vals, self.meta,
+                                        self.dsum, self.w_scale, self.kernel_size, self.bias, self.stride, self.padding,
+                                        self.dilation)
+
+    def extra_repr(self):
+        return super().extra_repr() + ", 2:4 sparse"
 
 
 INT8_MAX_KG = 1 << 17  # sb200_int8_group_conv2d: K_g = C / groups KH KW must stay below 2^17 (exact int32 sums)

@@ -3,11 +3,11 @@
 a ``QMatMulInt8`` (``to_integer_matmuls``), every eligible grouped or depthwise ``QConv2d`` a ``QConv2dGroupInt8``
 (``to_integer_group_convs``), every eligible ``QAttention`` a ``QAttentionInt8`` (``to_integer_attentions``), and,
 opt-in, every ``QLinear`` whose weight is 2:4 sparse on the grid a ``QLinearSparse24Int8``
-(``to_sparse24_integer_linears``)."""
-from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, QLinearInt8,
-                       QLinearSparse24Int8, QMatMul, QMatMulInt8, int8_attention_ineligibility, int8_conv_ineligibility,
-                       int8_group_conv_ineligibility, int8_ineligibility, int8_matmul_ineligibility,
-                       int8_sparse24_ineligibility)
+(``to_sparse24_integer_linears``) and every such ``QConv2d`` a ``QConv2dSparse24Int8`` (``to_sparse24_integer_convs``)."""
+from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QConv2dSparse24Int8, QLinear,
+                       QLinearInt8, QLinearSparse24Int8, QMatMul, QMatMulInt8, int8_attention_ineligibility,
+                       int8_conv_ineligibility, int8_group_conv_ineligibility, int8_ineligibility,
+                       int8_matmul_ineligibility, int8_sparse24_conv_ineligibility, int8_sparse24_ineligibility)
 
 
 def _swap(model, kind, ineligibility, convert):
@@ -65,3 +65,13 @@ def to_sparse24_integer_linears(model):
     would otherwise convert the sparse layers to dense ``QLinearInt8``.  Returns the qualified names of the converted
     modules, in ``named_modules`` order."""
     return _swap(model, QLinear, int8_sparse24_ineligibility, QLinearSparse24Int8.from_qlinear)
+
+
+def to_sparse24_integer_convs(model):
+    """Swap, in place, every ``QConv2d`` of ``model`` that ``QConv2dSparse24Int8.from_qconv2d`` accepts (groups = 1, its
+    weight 2:4 sparse on the grid along the rows of ``weight.reshape(C_out, -1)``, e.g. pruned by the 2:4 sparser with
+    the mask folded into the weight); the others stay ``QConv2d``, and ``int8_sparse24_conv_ineligibility`` says why.
+    Opt-in, as ``to_sparse24_integer_linears``: where the sparse conv beats the dense one depends on the layer.  Run it
+    before ``to_integer_convs``, which would otherwise convert the sparse convs to dense ``QConv2dInt8``.  Returns the
+    qualified names of the converted modules, in ``named_modules`` order."""
+    return _swap(model, QConv2d, int8_sparse24_conv_ineligibility, QConv2dSparse24Int8.from_qconv2d)
