@@ -1,6 +1,6 @@
 // int8_grid.cuh -- the stored int8 grid of the integer-grid kernels (int8_linear.cu, int8_group_conv.cu,
-// int8_attention.cu): the one quantizer they all store an element through, the storage rules of that grid and the host
-// checks their entry points share.
+// int8_attention.cu, int8_sparse24.cu): the one quantizer they all store an element through, the storage rules of that
+// grid, the host checks their entry points share, and the lowering of an activation onto the grid (int8_linear.cu).
 #pragma once
 
 #include "common.cuh"
@@ -41,8 +41,39 @@ static inline int check_workspace(const char* fn, size_t have, size_t need) {
   return SB200_E_WORKSPACE;
 }
 
-// int8_linear.cu: the conv geometry checks of sb200_int8_conv2d that come before the range check (a non-positive
-// geometry, an empty output, M = n OH OW >= 2^31: SB200_E_INVALID); on success sets the output size.
-int int8_check_conv(const char* fn, const sb200_conv2d_geom* g, long long* oh, long long* ow);
+// |a|, |b| <= 128 on the stored grid: the s32 accumulator holds |sum a b| <= K * 2^14 for K < 2^17
+constexpr long long kI8MaxK = 1LL << 17;
+
+// Conv geometry on the device; every product is 64-bit (M Kp passes 2^31 at ResNet-50 stem sizes from batch ~1024).
+struct ConvDims {
+  long long H, W, HW, CHW;     // input plane, image
+  long long sh, sw, dh, dw;    // stride, dilation
+  long long pt, pl;            // top / left padding
+  long long OW, P, M;          // output width, pixels per image, output pixels
+  int KH, KW, K, Kp;           // taps, taps padded to 16
+};
+
+// The lowered activations of M rows of K elements in a workspace whose base is aligned up to 1024 bytes: the stored
+// grid q [M, Kp] at the base, the int32 row sums 1024-aligned behind it, the NaN flags 256-aligned behind those.
+struct I8Lowered {
+  int8_t* q;
+  int* sum;
+  uint8_t* nan;
+};
+
+// ---- int8_linear.cu
+I8Lowered i8_lowered(void* workspace, long long m, long long k);
+// K < kI8MaxK, else SB200_E_UNSUPPORTED
+int check_k(const char* fn, long long k);
+// The conv geometry checks that come before the range check (a non-positive geometry, an empty output,
+// M = n OH OW >= 2^31: SB200_E_INVALID); on success fills `d` (K saturated at kI8MaxK).
+int check_conv(const char* fn, const sb200_conv2d_geom* g, ConvDims* d);
+// The lowering launches: the row quantizer (x [rows, K], per-tensor or per-row qparams) and the conv2d lowering
+// (one row per output pixel).  Unchecked: the caller has made every check of sb200_int8_quantize_rows /
+// sb200_int8_im2col_quantize, q included (16-byte aligned).
+int launch_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax, int8_t* q,
+                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st);
+int launch_im2col(const float* x, const ConvDims& d, const float* scale, const float* zero_point, int qmin, int qmax,
+                  int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st);
 
 }  // namespace sb200

@@ -36,7 +36,6 @@ constexpr int kGcTarget = 2048;          // outputs per CTA aimed at (depthwise)
 constexpr int kGcMaxTW = 128;            // output columns per tile
 constexpr int kGcMaxMB = 64;             // output channels per CTA (kGrouped)
 constexpr long long kGcMaxGrid = 1 << 16;  // CTAs launched; a larger call loops (grid-stride over CTA tiles)
-constexpr long long kGcMaxKg = 1LL << 17;
 
 enum GcMode { kDepthwise = 0, kGrouped = 1, kDirect = 2 };
 
@@ -409,20 +408,20 @@ int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64
   SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
   SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
   SB_REQUIRE(groups >= 2, "%s: groups = %lld; a conv with groups = 1 runs on sb200_int8_conv2d", fn, (long long)groups);
-  long long oh, ow;
-  if (const int rc = int8_check_conv(fn, geom, &oh, &ow)) return rc;
+  ConvDims cd;
+  if (const int rc = check_conv(fn, geom, &cd)) return rc;
   const sb200_conv2d_geom& g = *geom;
   SB_REQUIRE(g.c % groups == 0 && c_out % groups == 0, "%s: groups = %lld does not divide c = %lld and c_out = %lld", fn,
              (long long)groups, (long long)g.c, (long long)c_out);
   if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
   const long long kg = (g.c / groups) * g.kh * g.kw;  // c, kh, kw < 2^31 each: c / groups * kh stays far below 2^63 / kw
-  if ((__int128)(g.c / groups) * g.kh * g.kw >= kGcMaxKg) {
+  if ((__int128)(g.c / groups) * g.kh * g.kw >= kI8MaxK) {
     set_error("%s: K_g = c / groups kh kw = %lld x %lld x %lld >= 2^17, the integer path supports K_g < 2^17 (|sum| <= "
               "K_g * 2^14 must fit int32)", fn, (long long)(g.c / groups), (long long)g.kh, (long long)g.kw);
     return SB200_E_UNSUPPORTED;
   }
   GcDims d{};
-  d.N = g.n, d.C = g.c, d.H = g.h, d.W = g.w, d.Cout = c_out, d.OH = oh, d.OW = ow;
+  d.N = g.n, d.C = g.c, d.H = g.h, d.W = g.w, d.Cout = c_out, d.OH = cd.P / cd.OW, d.OW = cd.OW;
   d.Cg = (int)(g.c / groups), d.Mg = (int)(c_out / groups);
   d.KH = (int)g.kh, d.KW = (int)g.kw, d.sh = (int)g.stride_h, d.sw = (int)g.stride_w;
   d.dh = (int)g.dilation_h, d.dw = (int)g.dilation_w, d.pt = (int)g.pad_top, d.pl = (int)g.pad_left;

@@ -42,7 +42,6 @@ constexpr int kI8Stages = 6;
 constexpr int kI8Threads = 384;
 constexpr int kI8TileBytes = kI8Rows * kI8BK;     // 16 KB (x tile; the weight tile has the same size)
 constexpr int kI8StageBytes = 2 * kI8TileBytes;   // 32 KB
-constexpr long long kI8MaxK = 1LL << 17;
 
 // per-feature epilogue terms of the CTA's 128 features, computed once per tile
 struct I8Col {
@@ -227,15 +226,6 @@ __global__ void __launch_bounds__(kColThreads) int8_quantize_cols_kernel(const f
 }
 
 // ---------------------------------------------------------------------------------- conv2d lowering
-// Conv geometry on the device; every product is 64-bit (M Kp passes 2^31 at ResNet-50 stem sizes from batch ~1024).
-struct ConvDims {
-  long long H, W, HW, CHW;     // input plane, image
-  long long sh, sw, dh, dw;    // stride, dilation
-  long long pt, pl;            // top / left padding
-  long long OW, P, M;          // output width, pixels per image, output pixels
-  int KH, KW, K, Kp;           // taps, taps padded to 16
-};
-
 constexpr int kLowPix = 128;              // output pixels (rows of q) per CTA
 constexpr int kLowK = 128;                // taps per chunk: one 128-byte line of each row of q
 constexpr int kLowWords = kLowK / 4 + 1;  // words per tile row, padded: the column writes are conflict-free
@@ -584,52 +574,30 @@ I8Layout i8_layout(long long M, long long K) {
   return w;
 }
 
-// |a|, |b| <= 128: the s32 accumulator holds |sum a b| <= K * 2^14 for K < 2^17
-int check_k(const char* fn, long long k) {
-  if (k < kI8MaxK) return SB200_OK;
-  set_error("%s: K >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
-  return SB200_E_UNSUPPORTED;
-}
-
-int launch_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax, int8_t* q,
-                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st) {
-  const int vec = (k % 4 == 0) && aligned16(x);
-  int8_quantize_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, scale, zero_point, per_row, (float)qmin, (float)qmax,
-                                                                      grid_offset(qmin), q, row_sum, nan_flag, rows, (int)k,
-                                                                      (int)padded_k(k), vec);
-  SB_LAUNCHED();
-  return SB200_OK;
-}
-
-
 // The lowered activations (q, row sums, NaN flags) in the workspace, written by `lower`, then the GEMM into `out`
 // (row-major [M, N], or NCHW with P pixels per image).  Arguments are checked by the caller.
 template <bool kNchw, typename Lower>
 int run_gemm(const char* fn, long long m, long long k, long long n, long long P, int qmin_x, const float* x_scale,
              const float* x_zero_point, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
              const int32_t* w_zero, const float* bias, float* out, void* workspace, cudaStream_t st, Lower lower) {
-  const I8Layout w = i8_layout(m, k);
-  unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
-  int8_t* xq = reinterpret_cast<int8_t*>(ws + w.off_q);
-  int* xsum = reinterpret_cast<int*>(ws + w.off_sum);
-  uint8_t* xnan = ws + w.off_nan;
+  const I8Lowered w = i8_lowered(workspace, m, k);
   const long long kp = padded_k(k);
 
   CUtensorMap map_x, map_w;
-  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, xq, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, kI8BK, kI8Rows,
+  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, w.q, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, kI8BK, kI8Rows,
                    CU_TENSOR_MAP_SWIZZLE_128B) ||
       !make_map_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, w_q, (uint64_t)kp, (uint64_t)n, (uint64_t)kp, kI8BK, kI8Feat,
                    CU_TENSOR_MAP_SWIZZLE_128B)) {
     set_error("%s: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", fn, m, k, n);
     return SB200_E_CUDA;
   }
-  if (const int rc = lower(xq, xsum, xnan, st)) return rc;
+  if (const int rc = lower(w.q, w.sum, w.nan, st)) return rc;
   const size_t smem = (size_t)kI8Stages * kI8StageBytes + sizeof(I8Smem) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(int8_linear_gemm_kernel<kNchw>, (int)smem, attr_done));
   const long long tiles = ((m + kI8Rows - 1) / kI8Rows) * ((n + kI8Feat - 1) / kI8Feat);
   int8_linear_gemm_kernel<kNchw><<<(unsigned)tiles, kI8Threads, smem, st>>>(
-      map_x, map_w, out, xsum, xnan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(w_rowsum),
+      map_x, map_w, out, w.sum, w.nan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(w_rowsum),
       w_scale, reinterpret_cast<const int*>(w_zero), bias, (int)m, (int)n, (int)k, (int)P);
   SB_LAUNCHED();
   return SB200_OK;
@@ -675,7 +643,31 @@ int conv_shape(const sb200_conv2d_geom& g, ConvDims* d) {
   return 0;
 }
 
-// Checks of the conv entry points that come before the range check
+}  // namespace
+
+// ---------------------------------------------------------------------------------- shared through int8_grid.cuh
+I8Lowered i8_lowered(void* workspace, long long m, long long k) {
+  const I8Layout w = i8_layout(m, k);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
+  return {reinterpret_cast<int8_t*>(ws + w.off_q), reinterpret_cast<int*>(ws + w.off_sum), ws + w.off_nan};
+}
+
+int check_k(const char* fn, long long k) {
+  if (k < kI8MaxK) return SB200_OK;
+  set_error("%s: K >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
+  return SB200_E_UNSUPPORTED;
+}
+
+int launch_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax, int8_t* q,
+                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st) {
+  const int vec = (k % 4 == 0) && aligned16(x);
+  int8_quantize_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, scale, zero_point, per_row, (float)qmin, (float)qmax,
+                                                                      grid_offset(qmin), q, row_sum, nan_flag, rows, (int)k,
+                                                                      (int)padded_k(k), vec);
+  SB_LAUNCHED();
+  return SB200_OK;
+}
+
 int check_conv(const char* fn, const sb200_conv2d_geom* g, ConvDims* d) {
   const int rule = conv_shape(*g, d);
   SB_REQUIRE(rule != 1, "%s: empty or non-positive geometry (n=%lld c=%lld h=%lld w=%lld kernel %lldx%lld stride %lldx%lld "
@@ -696,7 +688,6 @@ int launch_im2col(const float* x, const ConvDims& d, const float* scale, const f
   return SB200_OK;
 }
 
-}  // namespace
 }  // namespace sb200
 
 using namespace sb200;
@@ -821,47 +812,31 @@ int sb200_int8_matmul(const float* a, const float* b, int b_k_major, const float
   if (const int rc = check_k(fn, k)) return rc;
   if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_matmul_workspace_bytes(batch, m, k, n))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const I8Layout la = i8_layout(batch * m, k), lb = i8_layout(batch * n, k);
-  unsigned char* wa = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
-  unsigned char* wb = wa + matmul_b_offset(batch, m, k);
-  int8_t* aq = reinterpret_cast<int8_t*>(wa + la.off_q);
-  int8_t* bq = reinterpret_cast<int8_t*>(wb + lb.off_q);
-  int* asum = reinterpret_cast<int*>(wa + la.off_sum);
-  int* bsum = reinterpret_cast<int*>(wb + lb.off_sum);
+  const I8Lowered la = i8_lowered(workspace, batch * m, k);
+  const I8Lowered lb = i8_lowered(la.q + matmul_b_offset(batch, m, k), batch * n, k);
   const long long kp = padded_k(k);
   CUtensorMap map_a, map_b;
-  if (!make_map_3d(&map_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, aq, (uint64_t)kp, (uint64_t)m, (uint64_t)batch, (uint64_t)kp, kI8BK,
-                   kI8Rows, CU_TENSOR_MAP_SWIZZLE_128B) ||
-      !make_map_3d(&map_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, bq, (uint64_t)kp, (uint64_t)n, (uint64_t)batch, (uint64_t)kp, kI8BK,
+  if (!make_map_3d(&map_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, la.q, (uint64_t)kp, (uint64_t)m, (uint64_t)batch, (uint64_t)kp,
+                   kI8BK, kI8Rows, CU_TENSOR_MAP_SWIZZLE_128B) ||
+      !make_map_3d(&map_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, lb.q, (uint64_t)kp, (uint64_t)n, (uint64_t)batch, (uint64_t)kp, kI8BK,
                    kI8Feat, CU_TENSOR_MAP_SWIZZLE_128B)) {
     set_error("%s: cuTensorMapEncodeTiled failed (batch=%lld M=%lld K=%lld N=%lld)", fn, (long long)batch, (long long)m,
               (long long)k, (long long)n);
     return SB200_E_CUDA;
   }
-  if (const int rc = launch_rows(a, a_scale, a_zero_point, 0, qmin_a, qmax_a, aq, asum, wa + la.off_nan, batch * m, k, st))
+  if (const int rc = launch_rows(a, a_scale, a_zero_point, 0, qmin_a, qmax_a, la.q, la.sum, la.nan, batch * m, k, st))
     return rc;
-  if (const int rc = b_k_major ? launch_rows(b, b_scale, b_zero_point, 0, qmin_b, qmax_b, bq, bsum, wb + lb.off_nan,
-                                             batch * n, k, st)
-                               : launch_cols(b, b_scale, b_zero_point, qmin_b, qmax_b, bq, bsum, wb + lb.off_nan, batch, k,
-                                             n, st))
+  if (const int rc = b_k_major ? launch_rows(b, b_scale, b_zero_point, 0, qmin_b, qmax_b, lb.q, lb.sum, lb.nan, batch * n, k,
+                                             st)
+                               : launch_cols(b, b_scale, b_zero_point, qmin_b, qmax_b, lb.q, lb.sum, lb.nan, batch, k, n, st))
     return rc;
   const size_t smem = (size_t)kI8Stages * kI8StageBytes + sizeof(I8MmSmem) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(int8_matmul_gemm_kernel, (int)smem, attr_done));
   const int vec2 = (n % 2 == 0) && (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
   int8_matmul_gemm_kernel<<<(unsigned)tiles, kI8Threads, smem, st>>>(
-      map_a, map_b, out, asum, wa + la.off_nan, bsum, wb + lb.off_nan, a_scale, a_zero_point, grid_offset(qmin_a), b_scale,
+      map_a, map_b, out, la.sum, la.nan, lb.sum, lb.nan, a_scale, a_zero_point, grid_offset(qmin_a), b_scale,
       b_zero_point, grid_offset(qmin_b), (int)m, (int)n, (int)k, vec2);
   SB_LAUNCHED();
   return SB200_OK;
 }
-
-// ---------------------------------------------------------------------------------- shared with int8_group_conv.cu
-namespace sb200 {
-int int8_check_conv(const char* fn, const sb200_conv2d_geom* g, long long* oh, long long* ow) {
-  ConvDims d;
-  if (const int rc = check_conv(fn, g, &d)) return rc;
-  *oh = d.P / d.OW, *ow = d.OW;
-  return SB200_OK;
-}
-}  // namespace sb200

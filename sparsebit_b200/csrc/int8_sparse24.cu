@@ -24,7 +24,7 @@
 // rows are features, so the epilogue stages the tile through shared memory (the ring, free once both warpgroups are
 // done) and stores rows of out [M, N] whole.
 //
-// Conv2d.  sb200_int8_im2col_quantize lowers the input into the same workspace, one s8 row per output pixel in the K
+// Conv2d.  launch_im2col (int8_linear.cu) lowers the input into the same workspace, one s8 row per output pixel in the K
 // order (c, kh, kw) of weight.reshape(C_out, -1), the order the 2:4 groups of a pruned conv weight follow; the same GEMM
 // (kNchw = true) then writes NCHW: out[(img N + n) P + p] for token m = img P + p, P = OH OW.  The epilogue stages the
 // tile as [feature][token] (rows of kSpTok + 4 floats), the mirror of the row-major staging; warp c of the consumers
@@ -48,7 +48,6 @@ constexpr int kSpEWords = (kSpBK / 64) * 2 * 128;  // metadata words of a stage:
 constexpr int kSpStageBytes = 2 * kSpXBox + kSpWBytes + kSpEWords * 4;  // 52 KB, a multiple of 1024
 constexpr int kSpLd = kSpFeat + 4;                 // floats per staged token row: conflict-free transposed writes
 constexpr int kSpLdT = kSpTok + 4;                 // NCHW: floats per staged feature row
-constexpr long long kSpMaxK = 1LL << 17;
 constexpr uint32_t kSpPadMeta = 0x44444444u;       // every group keeps indices (0, 1)
 static_assert(kSpStageBytes % 1024 == 0, "stage tiles stay 1024-byte aligned");
 static_assert(kSpTok * kSpLd * 4 <= kSpStages * kSpStageBytes, "the output tile fits the ring");
@@ -370,30 +369,16 @@ int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
 long long k64_of(long long k) { return (k + 63) / 64 * 64; }
 long long meta_tiles(long long n) { return (n + kSpFeat - 1) / kSpFeat; }
 
-// sb200_int8_linear's workspace layout (int8_linear.cu i8_layout): the activation grid [M, Kp] at 0, the row sums
-// 1024-aligned behind it, the NaN flags 256-aligned behind those
-struct SpWorkspace {
-  int8_t* xq;
-  int32_t* xsum;
-  uint8_t* xnan;
-};
-SpWorkspace sp_workspace(void* workspace, long long m, long long k) {
-  unsigned char* ws = reinterpret_cast<unsigned char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
-  const size_t off_sum = align_up((size_t)m * (size_t)padded_k(k), 1024);
-  const size_t off_nan = off_sum + align_up((size_t)m * 4, 256);
-  return {reinterpret_cast<int8_t*>(ws), reinterpret_cast<int32_t*>(ws + off_sum), ws + off_nan};
-}
-
 // The lowered activations in the workspace, written by `lower` (the row quantizer or the conv lowering), then the
 // sparse GEMM into `out` (row-major [M, N], or NCHW with P pixels per image).  Arguments are checked by the caller.
 template <bool kNchw, typename Lower>
 int sp_run(const char* fn, long long m, long long k, long long n, long long P, int qmin_x, const float* x_scale,
            const float* x_zero_point, const int8_t* vals, const uint32_t* meta, const int32_t* dsum, const float* w_scale,
            const float* bias, float* out, void* workspace, cudaStream_t st, Lower lower) {
-  const SpWorkspace w = sp_workspace(workspace, m, k);
+  const I8Lowered w = i8_lowered(workspace, m, k);
   const long long kp = padded_k(k), kb64 = k64_of(k) / 64;
   CUtensorMap map_x, map_v, map_e;
-  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, w.xq, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, 128, kSpTok,
+  if (!make_map_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, w.q, (uint64_t)kp, (uint64_t)m, (uint64_t)kp, 128, kSpTok,
                    CU_TENSOR_MAP_SWIZZLE_128B) ||
       !make_map_2d(&map_v, CU_TENSOR_MAP_DATA_TYPE_UINT8, vals, (uint64_t)(kb64 * 32), (uint64_t)n, (uint64_t)(kb64 * 32),
                    128, kSpFeat, CU_TENSOR_MAP_SWIZZLE_128B) ||
@@ -402,7 +387,7 @@ int sp_run(const char* fn, long long m, long long k, long long n, long long P, i
     set_error("%s: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", fn, m, k, n);
     return SB200_E_CUDA;
   }
-  if (const int rc = lower(w, st)) return rc;
+  if (const int rc = lower(w.q, w.sum, w.nan, st)) return rc;
   const size_t smem = (size_t)kSpStages * kSpStageBytes + sizeof(SpRing) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(int8_sparse24_gemm_kernel<kNchw>, (int)smem, attr_done));
@@ -410,7 +395,7 @@ int sp_run(const char* fn, long long m, long long k, long long n, long long P, i
   // row-major: 16-byte stores of 4 features need N % 4 = 0; NCHW: each run of 4 pixels checks its own address
   const int vec4 = (kNchw || n % 4 == 0) && aligned16(out);
   int8_sparse24_gemm_kernel<kNchw><<<(unsigned)tiles, kSpThreads, smem, st>>>(
-      map_x, map_v, map_e, out, w.xnan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(dsum),
+      map_x, map_v, map_e, out, w.nan, x_scale, x_zero_point, grid_offset(qmin_x), reinterpret_cast<const int*>(dsum),
       w_scale, bias, (int)m, (int)n, (int)kb64, vec4, (int)P);
   SB_LAUNCHED();
   return SB200_OK;
@@ -439,7 +424,7 @@ int sb200_int8_sparse24_pack(const int8_t* w_q, const int32_t* w_zero, const flo
   SB_REQUIRE(w_q && w_zero && w_scale && vals && meta && dsum && bad, "%s: null pointer argument", fn);
   SB_REQUIRE(n > 0 && k > 0, "%s: empty operand (N=%lld K=%lld)", fn, (long long)n, (long long)k);
   SB_REQUIRE(n < (1LL << 31), "%s: dimension too large (N=%lld)", fn, (long long)n);
-  SB_REQUIRE(k < kSpMaxK, "%s: K >= 2^17, the integer path supports K < 2^17", fn);
+  SB_REQUIRE(k < kI8MaxK, "%s: K >= 2^17, the integer path supports K < 2^17", fn);
   SB_REQUIRE(aligned16(vals), "%s: vals must be 16-byte aligned", fn);
   cudaStream_t st = (cudaStream_t)stream;
   SB_CUDA(cudaMemsetAsync(dsum, 0, (size_t)n * 4, st));
@@ -464,15 +449,11 @@ int sb200_int8_sparse24_linear(const float* x, const float* x_scale, const float
   SB_REQUIRE(m < (1LL << 31) && n < (1LL << 31), "%s: dimension too large", fn);
   if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
   SB_REQUIRE(aligned16(vals) && aligned16(meta), "%s: vals and meta must be 16-byte aligned", fn);
-  if (k >= kSpMaxK) {
-    set_error("%s: K >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
-    return SB200_E_UNSUPPORTED;
-  }
+  if (const int rc = check_k(fn, k)) return rc;
   if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_linear_workspace_bytes(m, k))) return rc;
   return sp_run<false>(fn, m, k, n, 1, qmin_x, x_scale, x_zero_point, vals, meta, dsum, w_scale, bias, out, workspace,
-                       (cudaStream_t)stream, [&](const SpWorkspace& w, cudaStream_t st) {
-                         return sb200_int8_quantize_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, w.xq, w.xsum, w.xnan,
-                                                         m, k, st);
+                       (cudaStream_t)stream, [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                         return launch_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, xq, xsum, xnan, m, k, st);
                        });
 }
 
@@ -485,21 +466,14 @@ int sb200_int8_sparse24_conv2d(const float* x, const sb200_conv2d_geom* geom, co
              "%s: null pointer argument", fn);
   SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
   SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
-  long long oh = 0, ow = 0;
-  if (const int rc = int8_check_conv(fn, geom, &oh, &ow)) return rc;
+  ConvDims d;
+  if (const int rc = check_conv(fn, geom, &d)) return rc;
   if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
   SB_REQUIRE(aligned16(vals) && aligned16(meta), "%s: vals and meta must be 16-byte aligned", fn);
-  // each factor is < 2^31 (int8_check_conv): the product fits __int128
-  const __int128 k = (__int128)geom->c * geom->kh * geom->kw;
-  if (k >= kSpMaxK) {
-    set_error("%s: K >= 2^17, the integer path supports K < 2^17 (|sum| <= K * 2^14 must fit int32)", fn);
-    return SB200_E_UNSUPPORTED;
-  }
+  if (const int rc = check_k(fn, d.K)) return rc;
   if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
-  const long long P = oh * ow, m = geom->n * P;
-  return sp_run<true>(fn, m, (long long)k, c_out, P, qmin_x, x_scale, x_zero_point, vals, meta, dsum, w_scale, bias, out,
-                      workspace, (cudaStream_t)stream, [&](const SpWorkspace& w, cudaStream_t st) {
-                        return sb200_int8_im2col_quantize(x, geom, x_scale, x_zero_point, qmin_x, qmax_x, w.xq, w.xsum,
-                                                          w.xnan, st);
+  return sp_run<true>(fn, d.M, d.K, c_out, d.P, qmin_x, x_scale, x_zero_point, vals, meta, dsum, w_scale, bias, out,
+                      workspace, (cudaStream_t)stream, [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                        return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st);
                       });
 }

@@ -689,19 +689,20 @@ def _check_per_tensor(fn, *qparams):
         raise SparsebitB200Error(f"{fn}: the qparams are per-tensor (1 element each)")
 
 
-def _req_int8_operands(x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias):
-    """The dtypes of a per-tensor fp32 activation and of the weight operand ``int8_quantize_rows`` stores."""
+def _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, **weight):
+    """The dtypes of a per-tensor fp32 activation, the fp32 ``w_scale`` and ``bias``, and the integer tensors of the
+    weight operand by name: int8 ``w_q`` / ``vals``, the others int32."""
     _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
-    _req(w_q, "w_q", torch.int8), _req(w_rowsum, "w_rowsum", torch.int32), _req(w_zero, "w_zero", torch.int32)
+    for name, t in weight.items():
+        _req(t, name, torch.int8 if name in ("w_q", "vals") else torch.int32)
     if bias is not None:
         _req(bias, "bias")
 
 
-def _int8_weight_rows(fn, w_q, w_rowsum, w_scale, w_zero, bias):
-    """N, the rows of the stored weight operand (w_q [N, Kp]), which each per-row term must match."""
-    n = w_q.shape[0]
-    if w_rowsum.numel() != n or w_scale.numel() != n or w_zero.numel() != n or (bias is not None and bias.numel() != n):
-        raise SparsebitB200Error(f"{fn}: w_rowsum / w_scale / w_zero / bias need {n} elements")
+def _int8_weight_rows(fn, n, bias, **per_row):
+    """``n``, the rows of the weight operand, which each per-row term (by name) and the bias must match."""
+    if any(t.numel() != n for t in per_row.values()) or (bias is not None and bias.numel() != n):
+        raise SparsebitB200Error(f"{fn}: {' / '.join(per_row)} / bias need {n} elements")
     return n
 
 
@@ -747,11 +748,11 @@ def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     int32 [N], w_scale fp32 [N], w_zero int32 [N] = rint(zero point) - int8_grid_offset).  ``x`` [..., K] fp32; returns
     fp32 [..., N].  ``k`` defaults to x.shape[-1]."""
     lib = _lib.load()
-    _req_int8_operands(x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias)
+    _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero)
     k = x.shape[-1] if k is None else int(k)
     if x.shape[-1] != k or w_q.dim() != 2 or w_q.shape[1] != int8_padded_k(k):
         raise SparsebitB200Error(f"int8_linear: x has {x.shape[-1]} features, w_q is {tuple(w_q.shape)} (need [N, {int8_padded_k(k)}])")
-    n = _int8_weight_rows("int8_linear", w_q, w_rowsum, w_scale, w_zero, bias)
+    n = _int8_weight_rows("int8_linear", w_q.shape[0], bias, w_rowsum=w_rowsum, w_scale=w_scale, w_zero=w_zero)
     m = x.numel() // k
     out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
     ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
@@ -813,18 +814,14 @@ def int8_sparse24_linear(x, x_scale, x_zero_point, qmin, qmax, vals, meta, dsum,
     operand ``int8_sparse24_pack`` made (vals, meta, dsum; every ``bad`` entry 0) and w_scale fp32 [N].  The output
     equals ``int8_linear`` on the dense stored weight bit for bit.  ``x`` [..., K] fp32; returns fp32 [..., N]."""
     lib = _lib.load()
-    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
-    _req(vals, "vals", torch.int8), _req(meta, "meta", torch.int32), _req(dsum, "dsum", torch.int32)
-    if bias is not None:
-        _req(bias, "bias")
+    _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, vals=vals, meta=meta, dsum=dsum)
     k = x.shape[-1] if k is None else int(k)
     n = vals.shape[0] if vals.dim() == 2 else -1
     vshape, mshape = int8_sparse24_shapes(max(n, 1), k)
     if x.shape[-1] != k or tuple(vals.shape) != vshape or tuple(meta.shape) != mshape:
         raise SparsebitB200Error(f"int8_sparse24_linear: x has {x.shape[-1]} features, vals is {tuple(vals.shape)} and meta "
                                  f"{tuple(meta.shape)} (need {vshape} and {mshape})")
-    if dsum.numel() != n or w_scale.numel() != n or (bias is not None and bias.numel() != n):
-        raise SparsebitB200Error(f"int8_sparse24_linear: dsum / w_scale / bias need {n} elements")
+    _int8_weight_rows("int8_sparse24_linear", n, bias, dsum=dsum, w_scale=w_scale)
     m = x.numel() // k
     out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
     ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
@@ -1038,21 +1035,38 @@ def conv2d_output_hw(g):
     return oh, ow
 
 
-def _int8_conv_prelude(fn, x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups, bias, stride,
+def _int8_conv_rows(fn, k, w_scale, bias, w_q, w_rowsum, w_zero):
+    """C_out of the weight operand ``int8_quantize_rows`` stores, for K = C / groups KH KW."""
+    kp = int8_padded_k(k)
+    if w_q.dim() != 2 or w_q.shape[1] != kp:
+        raise SparsebitB200Error(f"{fn}: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {kp}]")
+    return _int8_weight_rows(fn, w_q.shape[0], bias, w_rowsum=w_rowsum, w_scale=w_scale, w_zero=w_zero)
+
+
+def _sparse24_conv_rows(fn, k, w_scale, bias, vals, meta, dsum):
+    """C_out of the 2:4 operand ``int8_sparse24_pack`` made, for K = C KH KW."""
+    n = vals.shape[0] if vals.dim() == 2 else -1
+    vshape, mshape = int8_sparse24_shapes(max(n, 1), k)
+    if tuple(vals.shape) != vshape or tuple(meta.shape) != mshape:
+        raise SparsebitB200Error(f"{fn}: vals is {tuple(vals.shape)} and meta {tuple(meta.shape)}, the geometry (K = {k}) "
+                                 f"needs {vshape} and {mshape}")
+    return _int8_weight_rows(fn, n, bias, dsum=dsum, w_scale=w_scale)
+
+
+def _int8_conv_prelude(fn, x, x_scale, x_zero_point, w_scale, bias, weight_rows, weight, kernel_size, groups, stride,
                        padding, dilation):
-    """The argument checks of ``int8_conv2d`` (groups = 1) and ``int8_group_conv2d``: returns the ``Conv2dGeom``, C_out
-    and the fp32 [N, C_out, OH, OW] output (one pixel when the kernel does not fit, which the C entry points reject)."""
-    _req_int8_operands(x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias)
+    """The argument checks of the integer-grid conv wrappers, ``weight`` being the integer tensors of the weight
+    operand by name and ``weight_rows`` its ``_int8_conv_rows`` / ``_sparse24_conv_rows``: returns the
+    ``Conv2dGeom``, C_out and the fp32 [N, C_out, OH, OW] output (one pixel when the kernel does not fit, which the C
+    entry points reject)."""
+    _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, **weight)
     if x.dim() != 4:
         raise SparsebitB200Error(f"{fn}: data must be [N, C, H, W]")
     groups = int(groups)
     g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
     if groups < 1 or g.c % groups:
         raise SparsebitB200Error(f"{fn}: groups = {groups} does not divide C = {g.c}")
-    kp = int8_padded_k(g.c // groups * g.kh * g.kw)
-    if w_q.dim() != 2 or w_q.shape[1] != kp:
-        raise SparsebitB200Error(f"{fn}: w_q is {tuple(w_q.shape)}, the geometry needs [C_out, {kp}]")
-    n = _int8_weight_rows(fn, w_q, w_rowsum, w_scale, w_zero, bias)
+    n = weight_rows(fn, g.c // groups * g.kh * g.kw, w_scale, bias, **weight)
     oh, ow = conv2d_output_hw(g)
     return g, n, torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
 
@@ -1088,8 +1102,9 @@ def int8_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     ``int8_linear``.  Returns fp32 [N, C_out, OH, OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left,
     right)."""
     lib = _lib.load()
-    g, n, out = _int8_conv_prelude("int8_conv2d", x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, kernel_size, 1,
-                                   bias, stride, padding, dilation)
+    g, n, out = _int8_conv_prelude("int8_conv2d", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
+                                   dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, 1, stride, padding,
+                                   dilation)
     ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     ws = _int8_workspace(x.device, max(ws_bytes, 16))
     with torch.cuda.device(x.device):
@@ -1108,23 +1123,8 @@ def int8_sparse24_conv2d(x, x_scale, x_zero_point, qmin, qmax, vals, meta, dsum,
     fp32 [C_out].  The output equals ``int8_conv2d`` on the dense stored weight bit for bit.  Returns fp32 [N, C_out, OH,
     OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right)."""
     lib = _lib.load()
-    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
-    _req(vals, "vals", torch.int8), _req(meta, "meta", torch.int32), _req(dsum, "dsum", torch.int32)
-    if bias is not None:
-        _req(bias, "bias")
-    if x.dim() != 4:
-        raise SparsebitB200Error("int8_sparse24_conv2d: data must be [N, C, H, W]")
-    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
-    k = g.c * g.kh * g.kw
-    n = vals.shape[0] if vals.dim() == 2 else -1
-    vshape, mshape = int8_sparse24_shapes(max(n, 1), k)
-    if tuple(vals.shape) != vshape or tuple(meta.shape) != mshape:
-        raise SparsebitB200Error(f"int8_sparse24_conv2d: vals is {tuple(vals.shape)} and meta {tuple(meta.shape)}, the "
-                                 f"geometry (K = {k}) needs {vshape} and {mshape}")
-    if dsum.numel() != n or w_scale.numel() != n or (bias is not None and bias.numel() != n):
-        raise SparsebitB200Error(f"int8_sparse24_conv2d: dsum / w_scale / bias need {n} elements")
-    oh, ow = conv2d_output_hw(g)
-    out = torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    g, n, out = _int8_conv_prelude("int8_sparse24_conv2d", x, x_scale, x_zero_point, w_scale, bias, _sparse24_conv_rows,
+                                   dict(vals=vals, meta=meta, dsum=dsum), kernel_size, 1, stride, padding, dilation)
     ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     ws = _int8_workspace(x.device, max(ws_bytes, 16))
     with torch.cuda.device(x.device):
@@ -1143,8 +1143,9 @@ def int8_group_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_sca
     round_up(C / groups KH KW, 16), w_rowsum int32, w_scale fp32, w_zero int32 [C_out]).  Returns fp32 [N, C_out, OH,
     OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right).  No workspace."""
     lib = _lib.load()
-    g, n, out = _int8_conv_prelude("int8_group_conv2d", x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero,
-                                   kernel_size, groups, bias, stride, padding, dilation)
+    g, n, out = _int8_conv_prelude("int8_group_conv2d", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
+                                   dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, groups, stride, padding,
+                                   dilation)
     with torch.cuda.device(x.device):
         check(lib.sb200_int8_group_conv2d(x.data_ptr(), ctypes.byref(g), int(groups), x_scale.data_ptr(),
                                           x_zero_point.data_ptr(), int(qmin), int(qmax), w_q.data_ptr(),

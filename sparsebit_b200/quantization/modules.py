@@ -262,15 +262,49 @@ def _sparse24_operand(qmod):
     return None, why
 
 
+def _sparse24_checked(qmod, dense_reason):
+    """``_sparse24_operand(qmod)`` on top of a dense rule: ``(None, dense_reason)`` when that rule refuses ``qmod``."""
+    return (None, dense_reason) if dense_reason is not None else _sparse24_operand(qmod)
+
+
 def int8_sparse24_ineligibility(qlinear):
     """Why ``QLinearSparse24Int8.from_qlinear`` cannot convert ``qlinear`` (None when it can): a rule of
     ``int8_ineligibility``, a centred weight grid outside s8 (possible for affine 8-bit weights only), or a group of 4
     along a row of the weight grid with more than two nonzeros."""
-    reason = int8_ineligibility(qlinear)
-    return reason if reason is not None else _sparse24_operand(qlinear)[1]
+    return _sparse24_checked(qlinear, int8_ineligibility(qlinear))[1]
 
 
-class QLinearSparse24Int8(_Int8InputModule):
+class _Sparse24WeightModule(_Int8InputModule):
+    """The compressed 2:4 weight operand of ``QLinearSparse24Int8`` / ``QConv2dSparse24Int8``: ``vals`` int8
+    [N, K64 / 2] (the kept centred grid values), ``meta`` (their 2-bit indices), ``dsum`` int32 [N] and ``w_scale``
+    fp32 [N] as ``_sparse24_operand`` packs them, with the activation qparams and bias of ``_Int8InputModule``."""
+
+    def __init__(self, out_features, k, device):
+        super().__init__()
+        vshape, mshape = ops.int8_sparse24_shapes(out_features, k)
+        self.register_buffer("vals", torch.zeros(vshape, dtype=torch.int8, device=device))
+        self.register_buffer("meta", torch.zeros(mshape, dtype=torch.int32, device=device))
+        self.register_buffer("dsum", torch.zeros(out_features, dtype=torch.int32, device=device))
+        self.register_buffer("w_scale", torch.zeros(out_features, dtype=torch.float32, device=device))
+        self._register_input(device)
+
+    @classmethod
+    def _eligible_operand(cls, qmod, dense_reason, method):
+        """The packed weight of the calibrated ``qmod``; raises the class-named ``ValueError`` when the dense rule's
+        ``dense_reason`` or the 2:4 rule refuses it."""
+        operand, reason = _sparse24_checked(qmod, dense_reason)
+        cls._check_eligible(reason, method)
+        return operand
+
+    def _load(self, qmod, operand):
+        """Fills the buffers from ``_eligible_operand``'s ``operand`` and the calibrated ``qmod``; returns ``self``."""
+        with torch.no_grad():
+            for buf, v in zip((self.vals, self.meta, self.dsum, self.w_scale), operand):
+                buf.copy_(v)
+        return self._load_input(qmod)
+
+
+class QLinearSparse24Int8(_Sparse24WeightModule):
     """Inference-only replacement of a calibrated ``QLinear`` whose weight is 2:4 sparse on the grid: the linear of
     ``QLinearInt8`` on the sparse int8 tensor cores (``ops.int8_sparse24_linear``), bit-identical to ``QLinearInt8`` on
     the same module.  Only the compressed weight is stored: ``vals`` int8 [N, K64 / 2] (the kept centred grid values),
@@ -278,28 +312,14 @@ class QLinearSparse24Int8(_Int8InputModule):
     input is up-cast and the output is fp32, as in the fake-quant op.  Built by ``from_qlinear``; no backward."""
 
     def __init__(self, in_features, out_features, device):
-        super().__init__()
-        vshape, mshape = ops.int8_sparse24_shapes(out_features, in_features)
-        self.register_buffer("vals", torch.zeros(vshape, dtype=torch.int8, device=device))
-        self.register_buffer("meta", torch.zeros(mshape, dtype=torch.int32, device=device))
-        self.register_buffer("dsum", torch.zeros(out_features, dtype=torch.int32, device=device))
-        self.register_buffer("w_scale", torch.zeros(out_features, dtype=torch.float32, device=device))
-        self._register_input(device)
+        super().__init__(out_features, in_features, device)
         self.in_features, self.out_features = int(in_features), int(out_features)
 
     @classmethod
     def from_qlinear(cls, qlinear):
-        reason = int8_ineligibility(qlinear)
-        operand = None
-        if reason is None:
-            operand, reason = _sparse24_operand(qlinear)
-        cls._check_eligible(reason, "from_qlinear")
+        operand = cls._eligible_operand(qlinear, int8_ineligibility(qlinear), "from_qlinear")
         n, k = qlinear.weight.shape
-        mod = cls(k, n, qlinear.weight.device)
-        with torch.no_grad():
-            for buf, v in zip((mod.vals, mod.meta, mod.dsum, mod.w_scale), operand):
-                buf.copy_(v)
-        return mod._load_input(qlinear)
+        return cls(k, n, qlinear.weight.device)._load(qlinear, operand)
 
     def forward(self, x_in):
         _check_inference_only(self, "QLinear", x_in)
@@ -430,11 +450,10 @@ def int8_sparse24_conv_ineligibility(qconv):
     """Why ``QConv2dSparse24Int8.from_qconv2d`` cannot convert ``qconv`` (None when it can): a rule of
     ``int8_conv_ineligibility`` (groups >= 2 and unresolvable padding included), a centred weight grid outside s8, or a
     group of 4 along a row of ``weight.reshape(C_out, -1)`` on the grid with more than two nonzeros."""
-    reason = int8_conv_ineligibility(qconv)
-    return reason if reason is not None else _sparse24_operand(qconv)[1]
+    return _sparse24_checked(qconv, int8_conv_ineligibility(qconv))[1]
 
 
-class QConv2dSparse24Int8(_Int8Conv2dModule, _Int8InputModule):
+class QConv2dSparse24Int8(_Int8Conv2dModule, _Sparse24WeightModule):
     """Inference-only replacement of a calibrated ``QConv2d`` (groups = 1) whose weight is 2:4 sparse on the grid along
     the rows of ``weight.reshape(C_out, -1)``: the conv2d of ``QConv2dInt8`` on the sparse int8 tensor cores
     (``ops.int8_sparse24_conv2d``), bit-identical to ``QConv2dInt8`` on the same module.  Only the compressed weight
@@ -443,28 +462,14 @@ class QConv2dSparse24Int8(_Int8Conv2dModule, _Int8InputModule):
     ``from_qconv2d``; no backward."""
 
     def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, device):
-        super().__init__()
-        vshape, mshape = ops.int8_sparse24_shapes(out_channels, in_channels * kernel_size[0] * kernel_size[1])
-        self.register_buffer("vals", torch.zeros(vshape, dtype=torch.int8, device=device))
-        self.register_buffer("meta", torch.zeros(mshape, dtype=torch.int32, device=device))
-        self.register_buffer("dsum", torch.zeros(out_channels, dtype=torch.int32, device=device))
-        self.register_buffer("w_scale", torch.zeros(out_channels, dtype=torch.float32, device=device))
-        self._register_input(device)
+        super().__init__(out_channels, in_channels * kernel_size[0] * kernel_size[1], device)
         self._set_geometry(in_channels, out_channels, kernel_size, stride, padding, dilation)
 
     @classmethod
     def from_qconv2d(cls, qconv):
-        reason = int8_conv_ineligibility(qconv)
-        operand = None
-        if reason is None:
-            operand, reason = _sparse24_operand(qconv)
-        cls._check_eligible(reason, "from_qconv2d")
+        operand = cls._eligible_operand(qconv, int8_conv_ineligibility(qconv), "from_qconv2d")
         *geometry, _ = cls._geometry_of(qconv)
-        mod = cls(*geometry, device=qconv.weight.device)
-        with torch.no_grad():
-            for buf, v in zip((mod.vals, mod.meta, mod.dsum, mod.w_scale), operand):
-                buf.copy_(v)
-        return mod._load_input(qconv)
+        return cls(*geometry, device=qconv.weight.device)._load(qconv, operand)
 
     def _conv(self, x):
         return ops.int8_sparse24_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.vals, self.meta,

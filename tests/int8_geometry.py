@@ -21,7 +21,7 @@ GEMM_FEAT = 128         # :39 kI8Feat
 GEMM_BK = 128           # :40 kI8BK
 STAGES = 6              # :41 kI8Stages
 WG_ROWS = 64            # :456 rows per consumer warpgroup
-MAX_K = 1 << 17         # :45 kI8MaxK
+MAX_K = 1 << 17         # kI8MaxK (int8_grid.cuh)
 
 
 def cdiv(a, b):

@@ -13,18 +13,18 @@ TARGET = 2048           # :35 kGcTarget
 MAX_TW = 128            # :36 kGcMaxTW
 MAX_MB = 64             # :37 kGcMaxMB
 MAX_GRID = 1 << 16      # :38 kGcMaxGrid
-MAX_KG = 1 << 17        # :39 kGcMaxKg
+MAX_KG = 1 << 17        # kI8MaxK (int8_grid.cuh)
 
 
 def smem_bytes(mode, cb, ob, c4, tih, tiw, kh, kw):
-    """gc_smem_bytes, :345-349."""
+    """gc_smem_bytes, :344-348."""
     if mode == "depthwise":
         return cb * tih * tiw + 16 + ob * kh * kw
     return 4 * c4 * tih * tiw + 4 * cdiv(ob, 4) * 4 * kh * kw * c4
 
 
 def plan(n, c, h, w, c_out, groups, kernel, stride=1, padding=0, dilation=1, x_off=0):
-    """gc_plan, :358-396, with the output shape of the entry point."""
+    """gc_plan, :357-395, with the output shape of the entry point."""
     (kh, kw), (sh, sw), (dh, dw) = _pair(kernel), _pair(stride), _pair(dilation)
     pt, pb, pl, pr = _pads(padding)
     oh = (h + pt + pb - dh * (kh - 1) - 1) // sh + 1
@@ -72,39 +72,39 @@ def branches(n, c, h, w, c_out, groups, kernel, stride=1, padding=0, dilation=1,
     p = plan(n, c, h, w, c_out, groups, kernel, stride, padding, dilation, x_off)
     (kh, kw), (sh, sw), (dh, dw) = _pair(kernel), _pair(stride), _pair(dilation)
     pt, pb, pl, pr = _pads(padding)
-    b = {"path." + p["mode"], "bias" if bias else "no_bias"}  # :65
+    b = {"path." + p["mode"], "bias" if bias else "no_bias"}  # :64
     if nan:
-        b.add("nan.rescan")  # :281 / :325 a CTA whose tile holds a NaN re-reads each window
-    # a window reaching into the padding: :110 / :128 (staged), :174 (direct)
+        b.add("nan.rescan")  # :280 / :324 a CTA whose tile holds a NaN re-reads each window
+    # a window reaching into the padding: :109 / :127 (staged), :173 (direct)
     pad_h = any(not 0 <= o * sh - pt + t * dh < h for o in range(p["oh"]) for t in range(kh))
     pad_w = any(not 0 <= o * sw - pl + t * dw < w for o in range(p["ow"]) for t in range(kw))
     if pad_h or pad_w:
         b.add("pad_taps")
     if p["mode"] == "direct":
         if cdiv(p["total"], THREADS) > MAX_GRID:
-            b.add("grid.loop")  # :160
+            b.add("grid.loop")  # :159
         return b
-    b.add("load." + ("vec" if p["vec"] else "scalar"))  # :95, :393
+    b.add("load." + ("vec" if p["vec"] else "scalar"))  # :94, :392
     if p["ctas"] > MAX_GRID:
-        b.add("grid.loop")  # :188
+        b.add("grid.loop")  # :187
     if p["oh"] % p["th"]:
-        b.add("tile.partial_h")  # :279 / :324
+        b.add("tile.partial_h")  # :278 / :323
     if p["ow"] % p["tw"]:
         b.add("tile.partial_w")
     if p["shrunk"]:
-        b.add("tile.shrunk")  # :377-380 the first tile did not fit kGcSmemMax
+        b.add("tile.shrunk")  # :376-379 the first tile did not fit kGcSmemMax
     if p["mode"] == "depthwise":
         if c % p["cb"]:
-            b.add("dw.cb_partial")  # :103 channels past C stage 0
+            b.add("dw.cb_partial")  # :102 channels past C stage 0
         if p["mg"] > 1:
             b.add("dw.multiplier")
     else:
         if p["cg"] % 4:
-            b.add("grp.c4_pad")  # :103 channels past C_g stage 0
+            b.add("grp.c4_pad")  # :102 channels past C_g stage 0
         if p["mg"] % p["ob"]:
             b.add("grp.mb_partial")
         if any(min(p["ob"], p["mg"] - i * p["ob"]) % 4 for i in range(p["mblocks"])):
-            b.add("grp.quad_partial")  # :329
+            b.add("grp.quad_partial")  # :328
     return b
 
 

@@ -17,7 +17,8 @@ from int8_linear_ref import BOUND, integer_terms, truth
 from sparsebit_b200 import _lib
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.common import Backend
-from sparsebit_b200.quantization.modules import QLinear, QLinearInt8, int8_ineligibility
+from sparsebit_b200.quantization.modules import (QConv2dSparse24Int8, QLinear, QLinearInt8, QLinearSparse24Int8,
+                                                 int8_ineligibility)
 from sparsebit_b200.quantization.tools import to_integer_linears
 
 E_INVALID, E_UNSUPPORTED, E_WORKSPACE = -1, -3, -4
@@ -232,3 +233,27 @@ def test_qlinear_int8_module_contract():
     assert repr(mod) == "QLinearInt8(in_features=20, out_features=6, qrange=[-128, 127])"
     with pytest.raises(RuntimeError, match=r"^QLinearInt8 is inference-only and has no backward; .* keep QLinear for"):
         mod(torch.zeros(2, 20, requires_grad=True))
+
+
+def test_sparse24_int8_module_contract():
+    """Both 2:4 modules store the same compressed operand, registered before the activation qparams."""
+    lin = QLinearSparse24Int8(20, 6, torch.device("cpu"))
+    conv = QConv2dSparse24Int8(3, 5, (3, 2), (1, 2), (1, 0, 1, 1), (2, 1), torch.device("cpu"))
+    for mod, n in ((lin, 6), (conv, 5)):  # K = 20 and K = 3 * 3 * 2 = 18: K64 = 64
+        buffers = [(name, b.dtype, tuple(b.shape)) for name, b in mod.named_buffers()]
+        assert buffers == [("vals", torch.int8, (n, 32)), ("meta", torch.int32, (1, 1, 2, 128)), ("dsum", torch.int32, (n,)),
+                           ("w_scale", torch.float32, (n,)), ("scale", torch.float32, (1,)),
+                           ("zero_point", torch.float32, (1,))]
+        assert list(mod.state_dict()) == [name for name, _, _ in buffers]
+        assert "bias" in mod._buffers and mod.bias is None and (mod.qmin, mod.qmax) == (-128, 127)
+    assert (lin.in_features, lin.out_features) == (20, 6)
+    assert repr(lin) == "QLinearSparse24Int8(in_features=20, out_features=6, qrange=[-128, 127], 2:4 sparse)"
+    assert (conv.in_channels, conv.out_channels) == (3, 5)
+    assert (conv.kernel_size, conv.stride, conv.padding, conv.dilation) == ((3, 2), (1, 2), (1, 0, 1, 1), (2, 1))
+    assert repr(conv) == ("QConv2dSparse24Int8(3, 5, kernel_size=(3, 2), stride=(1, 2), padding=(1, 0, 1, 1), "
+                          "dilation=(2, 1), qrange=[-128, 127], 2:4 sparse)")
+    with pytest.raises(RuntimeError, match=r"^QLinearSparse24Int8 is inference-only and has no backward; .* keep QLinear for"):
+        lin(torch.zeros(2, 20, requires_grad=True))
+    for x in (torch.zeros(1, 3, 6, 6, requires_grad=True), torch.zeros(3, 6, 6, requires_grad=True)):
+        with pytest.raises(RuntimeError, match=r"^QConv2dSparse24Int8 is inference-only and has no backward; .* keep QConv2d for"):
+            conv(x)
