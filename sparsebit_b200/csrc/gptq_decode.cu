@@ -38,9 +38,6 @@ constexpr int kDecBlockK = 128;
 // packed rows a quarter-warp reads with one LDS.128 then fall into disjoint bank groups.
 constexpr int kSlabRowBytes = kDecCols * 4 + 32;
 constexpr int kSlabGroupBytes = (kDecBlockK / 8) * kSlabRowBytes;
-__device__ __forceinline__ void dec_mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 
 template <uint32_t MASK>
 __device__ __forceinline__ uint32_t dec_and_or(uint32_t x, uint32_t c) {
@@ -164,7 +161,7 @@ __global__ void __launch_bounds__(kDecThreads) gptq4_decode_kernel(const __grid_
         tma_bulk_g2s(dst, qw + (size_t)row * N + col0, bytes, &s_bar[bl]);
       } else {  // K % 128 != 0: rows past the packed matrix contribute nothing
         for (int j = 0; j < kDecCols / 4; ++j) reinterpret_cast<uint4*>(dst)[j] = make_uint4(0u, 0u, 0u, 0u);
-        dec_mbar_arrive(&s_bar[bl]);
+        mbar_arrive(&s_bar[bl]);
       }
     }
   } else {

@@ -179,11 +179,6 @@ int launch_simt(const float* go, const int32_t* qweight, float* grad_in, const f
 constexpr int kDgStages = 5;
 constexpr int kDgChunk = 8;  // 64-n stages per restart of the MMA accumulator (512 n)
 
-struct DgSmem {
-  uint64_t full[kDgStages];
-  uint64_t empty[kDgStages];
-};
-
 // qweight[KW, N] (8 nibbles along k) -> qT[N/8, K] (8 nibbles along n).  CTA = 64 k x 64 n.
 __global__ void __launch_bounds__(256) dgrad_repack_kernel(const uint32_t* __restrict__ qw, uint32_t* __restrict__ qT, int K,
                                                            int N, int KW) {
@@ -255,8 +250,8 @@ gptq4_dgrad_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_c
                       const float4* __restrict__ tab, const float* __restrict__ gscale, const int* __restrict__ need_lo_flag,
                       int M, int K, int N, int group_size, int N8p, int backoff_ns) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  DgSmem* sm = reinterpret_cast<DgSmem*>(stage_base + (size_t)kDgStages * kWgStageBytes);
+  unsigned char* stage_base = smem_align1024(smem_raw);
+  auto& ring = *reinterpret_cast<StageRing<kDgStages>*>(stage_base + (size_t)kDgStages * kWgStageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + kWgTok - 1) / kWgTok;
   const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kWgTok, k0 = (int)(blockIdx.x / (unsigned)tiles_m) * kWgFeat;
@@ -264,13 +259,10 @@ gptq4_dgrad_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_c
   const bool need_lo = need_lo_flag[0] != 0;  // uniform: some gradient has a non-zero fp16 low part
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    for (int s = 0; s < kDgStages; ++s) {
-      mbar_init(&sm->full[s], 1);
-      mbar_init(&sm->empty[s], 8);
-    }
+    prefetch_tensormap(&map_hi);
+    prefetch_tensormap(&map_lo);
+    prefetch_tensormap(&map_q);
+    ring.init();
     mbar_fence_init();
   }
   __syncthreads();
@@ -278,7 +270,7 @@ gptq4_dgrad_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_c
   if (warp < 4) {
     reg_dec<40>();
     if (threadIdx.x == 0)
-      wg_produce(stage_base, sm->full, sm->empty, kDgStages, &map_hi, &map_lo, &map_q, m0, k0, num_nb, need_lo, backoff_ns);
+      wg_produce(stage_base, ring, &map_hi, &map_lo, &map_q, m0, k0, num_nb, need_lo, backoff_ns);
     return;
   }
   reg_inc<232>();
@@ -295,13 +287,11 @@ gptq4_dgrad_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_c
   for (int nb = 0; nb < num_nb;) {
     const int nb_end = min(num_nb, nb + kDgChunk);
     for (bool first = true; nb < nb_end; ++nb, first = false) {
-      const int s = nb % kDgStages;
-      const uint32_t ph = (uint32_t)(nb / kDgStages) & 1u;
       // the stage's 8 packed rows p -> fragment pairs (n, n + 4) = 64 nb + 8 p + (q, q + 4)
       float4 t[8];
 #pragma unroll
       for (int p = 0; p < 8; ++p) t[p] = __ldg(tg + (size_t)(nb * 8 + p) * 4);
-      mbar_wait_relaxed(&sm->full[s], ph, 0);
+      const int s = ring.wait(nb);
       const uint32_t* bq = reinterpret_cast<const uint32_t*>(stage_base + (size_t)s * kWgStageBytes + 2 * kWgXBytes);
       uint32_t H[4][4], L[4][4];
 #pragma unroll
@@ -330,8 +320,7 @@ gptq4_dgrad_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_c
       }
       wgmma_commit();
       wgmma_wait_all(c);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm->empty[s]);
+      ring.release(nb, lane);
     }
 #pragma unroll
     for (int j = 0; j < 64; ++j) acc[j] += c[j];
@@ -436,7 +425,7 @@ int gptq4_dgrad_tc(const float* go, const int32_t* qweight, float* grad_in, cons
     set_error("sb200_gptq_matmul_dgrad: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", M, K, N);
     return SB200_E_CUDA;
   }
-  const size_t smem = (size_t)kDgStages * kWgStageBytes + sizeof(DgSmem) + 1024;
+  const size_t smem = (size_t)kDgStages * kWgStageBytes + sizeof(StageRing<kDgStages>) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(gptq4_dgrad_tc_kernel, (int)smem, attr_done));
   const long long tiles = ((M + kWgTok - 1) / kWgTok) * ((K + kWgFeat - 1) / kWgFeat);

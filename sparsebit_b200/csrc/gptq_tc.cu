@@ -30,11 +30,6 @@ namespace sb200 {
 constexpr int kTcStages = 5;
 constexpr int kGroupK = 128;  // fold granularity (= the reference's BLOCKLEN)
 
-struct TcSmem {
-  uint64_t full[kTcStages];   // TMA data of the stage landed
-  uint64_t empty[kTcStages];  // the 8 consumer warps' wgmmas reading the stage completed
-};
-
 // ---------------------------------------------------------------------------------- prologue kernel
 // Row m of x -> A_hi[m, :], A_lo[m, :] (fp16, K order permuted inside every 8 as 0,4,1,5,2,6,3,7 to
 // match the nibble pairs the unpacker extracts with one AND per pair), xsum[m, g] = sum of the scaled
@@ -152,8 +147,8 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                 int G128, int group_size, int backoff_ns, __half* __restrict__ out_h, const float* __restrict__ bias) {
   extern __shared__ unsigned char smem_raw[];
   // stage buffers first (1024-byte aligned for SWIZZLE_128B), bookkeeping after them
-  unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  TcSmem* sm = reinterpret_cast<TcSmem*>(stage_base + (size_t)kTcStages * kWgStageBytes);
+  unsigned char* stage_base = smem_align1024(smem_raw);
+  auto& ring = *reinterpret_cast<StageRing<kTcStages>*>(stage_base + (size_t)kTcStages * kWgStageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + kWgTok - 1) / kWgTok;
   const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kWgTok, n0 = (int)(blockIdx.x / (unsigned)tiles_m) * kWgFeat;
@@ -162,13 +157,10 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
   const bool need_lo = int_zero_flag[1] != 0;   // uniform: some activation has a non-zero fp16 low part
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    for (int s = 0; s < kTcStages; ++s) {
-      mbar_init(&sm->full[s], 1);
-      mbar_init(&sm->empty[s], 8);  // one arrival per consumer warp
-    }
+    prefetch_tensormap(&map_hi);
+    prefetch_tensormap(&map_lo);
+    prefetch_tensormap(&map_q);
+    ring.init();
     mbar_fence_init();
   }
   __syncthreads();
@@ -177,7 +169,7 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
     // ================================================================== TMA producer
     reg_dec<40>();
     if (threadIdx.x == 0)
-      wg_produce(stage_base, sm->full, sm->empty, kTcStages, &map_hi, &map_lo, &map_q, m0, n0, num_kb, need_lo, backoff_ns);
+      wg_produce(stage_base, ring, &map_hi, &map_lo, &map_q, m0, n0, num_kb, need_lo, backoff_ns);
     return;
   }
   // ==================================================================== consumers: 64 features x 128 tokens each
@@ -192,8 +184,6 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
 #pragma unroll
   for (int j = 0; j < 64; ++j) acc[j] = 0.f;
   for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % kTcStages;
-    const uint32_t ph = (uint32_t)(kb / kTcStages) & 1u;
     const int g = kb >> 1;                                            // 128-K group
     const int gq = (int)((long long)g * kGroupK / group_size);        // quantisation group
     // this group's parameters, requested before the wait for the stage
@@ -205,7 +195,7 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
     const float za = (int_zero && live_a) ? __half2float(zint[(size_t)na * Gq + gq]) : 0.f;
     const float zb = (int_zero && live_b) ? __half2float(zint[(size_t)nb * Gq + gq]) : 0.f;
     const __half2 offa = unpack.offset(za), offb = unpack.offset(zb);
-    mbar_wait_relaxed(&sm->full[s], ph, 0);
+    const int s = ring.wait(kb);
     const uint32_t* bq = reinterpret_cast<const uint32_t*>(stage_base + (size_t)s * kWgStageBytes + 2 * kWgXBytes);
     uint32_t a[4][4];
 #pragma unroll
@@ -225,8 +215,7 @@ gptq4_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
     }
     wgmma_commit();
     wgmma_wait_all(part);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&sm->empty[s]);
+    ring.release(kb, lane);
     if ((kb & 1) == 1 || kb == num_kb - 1) {
       // acc[n, m] += s[n] * part (- z[n] * xsum[m, g]);  d[j]: feature f0 + 8 * ((j >> 1) & 1), token 8 (j >> 2) + 2q + (j & 1)
       if (int_zero) {
@@ -344,7 +333,7 @@ int gptq4_tc(const float* x, const int32_t* qweight, float* out, const float* sc
     set_error("gptq4_tc: cuTensorMapEncodeTiled failed (M=%lld K=%lld N=%lld)", M, K, N);
     return SB200_E_CUDA;
   }
-  const size_t smem = (size_t)kTcStages * kWgStageBytes + sizeof(TcSmem) + 1024;
+  const size_t smem = (size_t)kTcStages * kWgStageBytes + sizeof(StageRing<kTcStages>) + 1024;
   auto* const kernel = x_h ? gptq4_tc_kernel<true> : gptq4_tc_kernel<false>;
   static std::atomic<int> attr_done[2][64];
   SB_CUDA(ensure_dyn_smem(kernel, (int)smem, attr_done[x_h ? 1 : 0]));

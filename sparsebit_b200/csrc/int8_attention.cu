@@ -7,7 +7,7 @@
 //
 // CTA = 128 query rows of one batch entry: warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 own 64
 // rows each.  The q tile is loaded once; k blocks (128 keys) and v^T blocks (128 keys of all dv <= 128 columns) stream
-// through a ring of kAtStages stages.  The key blocks are walked twice:
+// through the stage ring of tc_common.cuh.  The key blocks are walked twice, with one load index running over both:
 //   pass 1  (k only)   s = the scores of the block; per row a running max m and sum l = sum exp(s - m) in fp64
 //   pass 2  (k and v)  the same scores again; p = exp(s - m) * RN32(1 / l) in fp32, quantized by the QDQ rule
 //                      (stored_grid, int8_grid.cuh) into a SWIZZLE_128B s8 tile in shared memory, which is the K-major
@@ -117,11 +117,11 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                       const __grid_constant__ CUtensorMap map_v, const __grid_constant__ AtParams a,
                       const __grid_constant__ AtMask mk) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* q_tile = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  unsigned char* q_tile = smem_align1024(smem_raw);
   unsigned char* stages = q_tile + kAtTile;
   unsigned char* p_tiles = stages + (size_t)kAtStages * kAtStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(p_tiles + 2 * kAtPBytes);  // full[kAtStages] | empty[kAtStages] | q
-  uint64_t *full = bars, *empty = bars + kAtStages, *qbar = bars + 2 * kAtStages;
+  auto& ring = *reinterpret_cast<StageRing<kAtStages>*>(p_tiles + 2 * kAtPBytes);
+  uint64_t* qbar = reinterpret_cast<uint64_t*>(&ring + 1);  // the q tile's barrier
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned tiles_q = (unsigned)(a.Tq + kAtRows - 1) / kAtRows;
   int m0 = (int)(blockIdx.x % tiles_q) * kAtRows, batch = (int)(blockIdx.x / tiles_q);
@@ -135,12 +135,9 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   }
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    for (int s = 0; s < kAtStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);  // one arrival per consumer warp
-    }
+    prefetch_tensormap(&map_k);
+    prefetch_tensormap(&map_v);
+    ring.init();
     mbar_init(qbar, 1);
     mbar_fence_init();
   }
@@ -153,14 +150,11 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
       tma_load_3d(q_tile, &map_q, 0, m0, batch, qbar);
       // block i < nvb: pass 1 (k block i); i >= nvb: pass 2 (k and v^T block i - nvb)
       for (int i = 0; i < 2 * nvb; ++i) {
-        const int s = i % kAtStages;
-        const uint32_t ph = (uint32_t)(i / kAtStages) & 1u;
         const int kb = i < nvb ? i : i - nvb;
-        mbar_wait_relaxed(&empty[s], ph ^ 1u, 0);
+        const int s = ring.acquire(i, (uint32_t)(i < nvb ? kAtTile : kAtStageBytes));
         unsigned char* st = stages + (size_t)s * kAtStageBytes;
-        mbar_expect_tx(&full[s], (uint32_t)(i < nvb ? kAtTile : kAtStageBytes));
-        tma_load_3d(st, &map_k, 0, kb * kAtKeys, batch, &full[s]);
-        if (i >= nvb) tma_load_3d(st + kAtTile, &map_v, kb * kAtKeys, 0, batch, &full[s]);
+        tma_load_3d(st, &map_k, 0, kb * kAtKeys, batch, &ring.full[s]);
+        if (i >= nvb) tma_load_3d(st + kAtTile, &map_v, kb * kAtKeys, 0, batch, &ring.full[s]);
       }
     }
     return;
@@ -208,11 +202,9 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   double l[2] = {0.0, 0.0};
   bool knan = false, knr[2] = {false, false};  // knr: the masked kernel's per-row NaN key
   for (int kb = 0; kb < nvb; ++kb) {
-    const int s = kb % kAtStages;
-    mbar_wait_relaxed(&full[s], (uint32_t)(kb / kAtStages) & 1u, 0);
+    const int s = ring.wait(kb);
     qk_mma(acc, dq, gmma_desc_sw128(stage0 + (uint32_t)s * kAtStageBytes), nk32);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
+    ring.release(kb, lane);
     float bm[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j = 0; j < 64; j += 2) {  // acc[j], acc[j + 1]: keys 8 (j >> 2) + 2 q4 + {0, 1}, row h = (j >> 1) & 1
@@ -280,8 +272,7 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   int psum[2] = {0, 0};
   bool pnan[2] = {false, false};
   for (int kb = 0; kb < nvb; ++kb) {
-    const int i = nvb + kb, s = i % kAtStages;
-    mbar_wait_relaxed(&full[s], (uint32_t)(i / kAtStages) & 1u, 0);
+    const int s = ring.wait(nvb + kb);
     const uint32_t st = stage0 + (uint32_t)s * kAtStageBytes;
     qk_mma(acc, dq, gmma_desc_sw128(st), nk32);
 #pragma unroll
@@ -321,8 +312,7 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     for (int j = 0; j < 4; ++j) wgmma_m64n128k32_s8(o, dp_desc + 2 * j, gmma_desc_sw128(st + kAtTile) + 2 * j, 1);
     wgmma_commit();
     wgmma_wait_s32<0>(o);  // the stage and the p tile are free again
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
+    ring.release(nvb + kb, lane);
   }
   if constexpr (kMasked) {  // the skipped keys' p is 0 (NaN in a row without a visible key): its grid into p_q
     if (a.p_q != nullptr) {

@@ -50,12 +50,8 @@ struct I8Col {
   int zw;
   float bias;
 };
-struct I8Ring {
-  uint64_t full[kI8Stages];
-  uint64_t empty[kI8Stages];
-};
 struct I8Smem {
-  I8Ring ring;
+  StageRing<kI8Stages> ring;
   I8Col col[kI8Feat];
 };
 // the matmul's per-column terms: both scales and zero points are scalars
@@ -64,7 +60,7 @@ struct I8MmCol {
   int nan;       // the column of b holds a NaN
 };
 struct I8MmSmem {
-  I8Ring ring;
+  StageRing<kI8Stages> ring;
   I8MmCol col[kI8Feat];
 };
 
@@ -336,53 +332,35 @@ __global__ void __launch_bounds__(kLowThreads) int8_im2col_quantize_kernel(const
 //
 // Exactness.  |a|, |b| <= 128 on the stored grid, so every product is at most 2^14 in magnitude and the s32 sum over
 // K < 2^17 products cannot overflow; the zero points come out afterwards in int64.
-//
-// Ring protocol of the mainloop below.  Stage s holds one 128-row tile of each operand.  full[s] (count 1) completes
-// when the producer's expect_tx and both TMA loads have landed; empty[s] (count 8) completes when each of the eight
-// consumer warps has arrived, one lane per warp.  Stage s is reused every kI8Stages k blocks with alternating
-// parity; the consumers keep one wgmma group in flight, so they free the stage of the previous k block, not the
-// current one.  The parity of k block kb at its stage is (kb / kI8Stages) & 1; the producer waits on the opposite
-// parity of empty[s], so the first lap over the ring does not wait.
 
 // ---- the mainloop shared by the linear / conv2d kernel and the batched matmul kernel
-// thread 0, before the CTA-wide barrier
-__device__ __forceinline__ void i8_ring_init(I8Ring* ring, const CUtensorMap* map_a, const CUtensorMap* map_b) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(map_a) : "memory");
-  asm volatile("prefetch.tensormap [%0];" ::"l"(map_b) : "memory");
-  for (int s = 0; s < kI8Stages; ++s) {
-    mbar_init(&ring->full[s], 1);
-    mbar_init(&ring->empty[s], 8);  // one arrival per consumer warp
-  }
-  mbar_fence_init();
-}
+// Load kb of the stage ring (tc_common.cuh) is k block kb: one 128-row tile of each operand.  The consumers keep one
+// wgmma group in flight, so they release the previous k block's stage, not the current one.
 // TMA producer (one thread): rows m0.. of map_a and n0.. of map_b, 128 K per stage.  kBatched: the maps are
 // (Kp, rows, batch) and `batch` picks the matrix.
 template <bool kBatched>
-__device__ __forceinline__ void i8_produce(unsigned char* stage_base, I8Ring* ring, const CUtensorMap* map_a,
-                                           const CUtensorMap* map_b, int m0, int n0, int batch, int num_kb) {
+__device__ __forceinline__ void i8_produce(unsigned char* stage_base, StageRing<kI8Stages>& ring,
+                                           const CUtensorMap* map_a, const CUtensorMap* map_b, int m0, int n0, int batch,
+                                           int num_kb) {
   for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % kI8Stages;
-    const uint32_t ph = (uint32_t)(kb / kI8Stages) & 1u;
-    mbar_wait_relaxed(&ring->empty[s], ph ^ 1u, 0);
+    const int s = ring.acquire(kb, (uint32_t)kI8StageBytes);
     unsigned char* st = stage_base + (size_t)s * kI8StageBytes;
-    mbar_expect_tx(&ring->full[s], (uint32_t)kI8StageBytes);
     if constexpr (kBatched) {
-      tma_load_3d(st, map_a, kb * kI8BK, m0, batch, &ring->full[s]);
-      tma_load_3d(st + kI8TileBytes, map_b, kb * kI8BK, n0, batch, &ring->full[s]);
+      tma_load_3d(st, map_a, kb * kI8BK, m0, batch, &ring.full[s]);
+      tma_load_3d(st + kI8TileBytes, map_b, kb * kI8BK, n0, batch, &ring.full[s]);
     } else {
-      tma_load_2d(st, map_a, kb * kI8BK, m0, &ring->full[s]);
-      tma_load_2d(st + kI8TileBytes, map_b, kb * kI8BK, n0, &ring->full[s]);
+      tma_load_2d(st, map_a, kb * kI8BK, m0, &ring.full[s]);
+      tma_load_2d(st + kI8TileBytes, map_b, kb * kI8BK, n0, &ring.full[s]);
     }
   }
 }
 // Consumer warpgroup wg: acc = rows 64 wg .. 64 wg + 63 of the a tile times the 128 rows of the b tile, over all of K.
-__device__ __forceinline__ void i8_consume(int (&acc)[64], uint32_t stage0, I8Ring* ring, int wg, int lane, int num_kb) {
+__device__ __forceinline__ void i8_consume(int (&acc)[64], uint32_t stage0, StageRing<kI8Stages>& ring, int wg, int lane,
+                                           int num_kb) {
 #pragma unroll
   for (int j = 0; j < 64; ++j) acc[j] = 0;
   for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % kI8Stages;
-    const uint32_t ph = (uint32_t)(kb / kI8Stages) & 1u;
-    mbar_wait_relaxed(&ring->full[s], ph, 0);
+    const int s = ring.wait(kb);
     const uint32_t xa = stage0 + (uint32_t)s * kI8StageBytes;
     const uint64_t da = gmma_desc_sw128(xa + (uint32_t)wg * (64 * kI8BK)), db = gmma_desc_sw128(xa + kI8TileBytes);
     wgmma_fence();
@@ -391,8 +369,7 @@ __device__ __forceinline__ void i8_consume(int (&acc)[64], uint32_t stage0, I8Ri
     wgmma_commit();
     // one group stays in flight: the stage of the previous k block is free once this wait returns
     wgmma_wait_s32<1>(acc);
-    __syncwarp();
-    if (kb > 0 && lane == 0) mbar_arrive(&ring->empty[(kb + kI8Stages - 1) % kI8Stages]);
+    if (kb > 0) ring.release(kb - 1, lane);
   }
   wgmma_wait_s32<0>(acc);
 }
@@ -407,19 +384,24 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
                         const int* __restrict__ w_sum, const float* __restrict__ w_scale, const int* __restrict__ w_zero,
                         const float* __restrict__ bias, int M, int N, int K, int P) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  unsigned char* stage_base = smem_align1024(smem_raw);
   I8Smem* sm = reinterpret_cast<I8Smem*>(stage_base + (size_t)kI8Stages * kI8StageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + kI8Rows - 1) / kI8Rows;
   const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kI8Rows, n0 = (int)(blockIdx.x / (unsigned)tiles_m) * kI8Feat;
   const int num_kb = (K + kI8BK - 1) / kI8BK;
 
-  if (threadIdx.x == 0) i8_ring_init(&sm->ring, &map_x, &map_w);
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&map_x);
+    prefetch_tensormap(&map_w);
+    sm->ring.init();
+    mbar_fence_init();
+  }
   __syncthreads();
 
   if (warp < 4) {
     reg_dec<40>();
-    if (threadIdx.x == 0) i8_produce<false>(stage_base, &sm->ring, &map_x, &map_w, m0, n0, 0, num_kb);
+    if (threadIdx.x == 0) i8_produce<false>(stage_base, sm->ring, &map_x, &map_w, m0, n0, 0, num_kb);
     return;
   }
   reg_inc<232>();
@@ -455,7 +437,7 @@ int8_linear_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
     }
   }
   int acc[64];
-  i8_consume(acc, stage0, &sm->ring, wg, lane, num_kb);
+  i8_consume(acc, stage0, sm->ring, wg, lane, num_kb);
   asm volatile("bar.sync 1, 256;" ::: "memory");  // sm->col written by both consumer warpgroups
 
   // acc[j]: row r0 + 8 ((j >> 1) & 1), feature n0 + 8 (j >> 2) + 2 q + (j & 1)
@@ -490,7 +472,7 @@ int8_matmul_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
                         const float* __restrict__ a_zero, int a_off, const float* __restrict__ b_scale,
                         const float* __restrict__ b_zero, int b_off, int M, int N, int K, int vec2) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  unsigned char* stage_base = smem_align1024(smem_raw);
   I8MmSmem* sm = reinterpret_cast<I8MmSmem*>(stage_base + (size_t)kI8Stages * kI8StageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned tiles_m = (unsigned)(M + kI8Rows - 1) / kI8Rows, tiles_n = (unsigned)(N + kI8Feat - 1) / kI8Feat;
@@ -499,12 +481,17 @@ int8_matmul_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
   const int batch = (int)(tile_n / tiles_n);
   const int num_kb = (K + kI8BK - 1) / kI8BK;
 
-  if (threadIdx.x == 0) i8_ring_init(&sm->ring, &map_a, &map_b);
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&map_a);
+    prefetch_tensormap(&map_b);
+    sm->ring.init();
+    mbar_fence_init();
+  }
   __syncthreads();
 
   if (warp < 4) {
     reg_dec<40>();
-    if (threadIdx.x == 0) i8_produce<true>(stage_base, &sm->ring, &map_a, &map_b, m0, n0, batch, num_kb);
+    if (threadIdx.x == 0) i8_produce<true>(stage_base, sm->ring, &map_a, &map_b, m0, n0, batch, num_kb);
     return;
   }
   reg_inc<232>();
@@ -533,7 +520,7 @@ int8_matmul_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
     rnan[h] = m < M && __ldg(a_nan + arow + m) != 0;
   }
   int acc[64];
-  i8_consume(acc, smem_u32(stage_base), &sm->ring, wg, lane, num_kb);
+  i8_consume(acc, smem_u32(stage_base), sm->ring, wg, lane, num_kb);
   asm volatile("bar.sync 1, 256;" ::: "memory");  // sm->col written by both consumer warpgroups
 
   // acc[j]: row r0 + 8 ((j >> 1) & 1), column n0 + 8 (j >> 2) + 2 q + (j & 1)

@@ -53,11 +53,6 @@ static_assert(kSpStageBytes % 1024 == 0, "stage tiles stay 1024-byte aligned");
 static_assert(kSpTok * kSpLd * 4 <= kSpStages * kSpStageBytes, "the output tile fits the ring");
 static_assert(kSpFeat * kSpLdT * 4 <= kSpStages * kSpStageBytes, "the NCHW output tile fits the ring");
 
-struct SpRing {
-  uint64_t full[kSpStages];
-  uint64_t empty[kSpStages];
-};
-
 // ---------------------------------------------------------------------------------- 2:4 mask
 // |a| ranks above |b|: NaN above every number, +-0 as 0
 __device__ __forceinline__ bool sp_above(float a, float b) {
@@ -218,13 +213,13 @@ __device__ __forceinline__ void sp_store_nchw(const int (&acc)[64], float* tile,
   }
 }
 
-// Ring protocol (as int8_linear.cu): full[s] (count 1) completes when the producer's expect_tx and the stage's TMA loads
-// have landed; empty[s] (count 8) when each consumer warp has arrived.  Unlike the dense kernel, a consumer retires each
-// stage's wgmma group before loading the next stage's metadata words and frees the stage then (see the loop).  Every
-// stage issues four k64 steps, so that no branch separates the wgmmas (a branch there makes ptxas serialise them).  Past K64 the last stage's steps multiply zeros: the weight box is
-// zero-filled beyond the vals, their metadata word is the padding word (indices 0, 1), and the second activation box,
-// loaded only when one of the stage's steps = min(4, kb64 - 4 kb) real steps reads it, holds whatever an earlier
-// stage left there, which the zero weights cancel exactly.  No box lies wholly beyond its operand.
+// Load kb of the stage ring (tc_common.cuh) holds K block kb, 256 K of both operands.  Unlike the dense kernel, a consumer
+// retires each stage's wgmma group before it loads the next stage's metadata words, and releases the stage then (see the
+// loop).  Every stage issues four k64 steps, so that no branch separates the wgmmas (a branch there makes ptxas
+// serialise them).  Past K64 the last stage's steps multiply zeros: the weight box is zero-filled beyond the vals, their
+// metadata word is the padding word (indices 0, 1), and the second activation box, loaded only when one of the stage's
+// steps = min(4, kb64 - 4 kb) real steps reads it, holds whatever an earlier stage left there, which the zero weights
+// cancel exactly.  No box lies wholly beyond its operand.
 //
 // Accumulator layout of a consumer thread (warp w of its warpgroup, lane l, q = l & 3), j = 0 .. 63:
 //   acc[j] = D[feature 16 w + l / 4 + 8 ((j >> 1) & 1)][token 8 (j >> 2) + 2 q + (j & 1)]
@@ -238,21 +233,18 @@ int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
                           const float* __restrict__ w_scale, const float* __restrict__ bias, int M, int N, int kb64,
                           int vec4, int P) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* stage_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  SpRing* ring = reinterpret_cast<SpRing*>(stage_base + (size_t)kSpStages * kSpStageBytes);
+  unsigned char* stage_base = smem_align1024(smem_raw);
+  auto& ring = *reinterpret_cast<StageRing<kSpStages>*>(stage_base + (size_t)kSpStages * kSpStageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + kSpTok - 1) / kSpTok;
   const int m0 = (int)(blockIdx.x % (unsigned)tiles_m) * kSpTok, n0 = (int)(blockIdx.x / (unsigned)tiles_m) * kSpFeat;
   const int num_kb = (kb64 + 3) / 4;
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_e) : "memory");
-    for (int s = 0; s < kSpStages; ++s) {
-      mbar_init(&ring->full[s], 1);
-      mbar_init(&ring->empty[s], 8);  // one arrival per consumer warp
-    }
+    prefetch_tensormap(&map_x);
+    prefetch_tensormap(&map_v);
+    prefetch_tensormap(&map_e);
+    ring.init();
     mbar_fence_init();
   }
   __syncthreads();
@@ -261,15 +253,13 @@ int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
     reg_dec<40>();
     if (threadIdx.x == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kSpStages;
-        mbar_wait_relaxed(&ring->empty[s], ((uint32_t)(kb / kSpStages) & 1u) ^ 1u, 0);
-        unsigned char* st = stage_base + (size_t)s * kSpStageBytes;
         const bool hi = kb64 - 4 * kb > 2;
-        mbar_expect_tx(&ring->full[s], (uint32_t)(kSpStageBytes - (hi ? 0 : kSpXBox)));
-        tma_load_2d(st, &map_x, kb * kSpBK, m0, &ring->full[s]);
-        if (hi) tma_load_2d(st + kSpXBox, &map_x, kb * kSpBK + 128, m0, &ring->full[s]);
-        tma_load_2d(st + 2 * kSpXBox, &map_v, kb * (kSpBK / 2), n0, &ring->full[s]);
-        tma_load_3d(st + 2 * kSpXBox + kSpWBytes, &map_e, 0, 4 * kb, n0 / kSpFeat, &ring->full[s]);
+        const int s = ring.acquire(kb, (uint32_t)(kSpStageBytes - (hi ? 0 : kSpXBox)));
+        unsigned char* st = stage_base + (size_t)s * kSpStageBytes;
+        tma_load_2d(st, &map_x, kb * kSpBK, m0, &ring.full[s]);
+        if (hi) tma_load_2d(st + kSpXBox, &map_x, kb * kSpBK + 128, m0, &ring.full[s]);
+        tma_load_2d(st + 2 * kSpXBox, &map_v, kb * (kSpBK / 2), n0, &ring.full[s]);
+        tma_load_3d(st + 2 * kSpXBox + kSpWBytes, &map_e, 0, 4 * kb, n0 / kSpFeat, &ring.full[s]);
       }
     }
     return;
@@ -299,8 +289,7 @@ int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
   for (int j = 0; j < 64; ++j) acc[j] = 0;
   const uint32_t stage_e = smem_u32(stage_base) + 2 * kSpXBox + kSpWBytes + (uint32_t)(wg * 128 + wt) * 4;
   for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % kSpStages;
-    mbar_wait_relaxed(&ring->full[s], (uint32_t)(kb / kSpStages) & 1u, 0);
+    const int s = ring.wait(kb);
     const uint32_t st = stage0 + (uint32_t)s * kSpStageBytes;
     const uint64_t da = gmma_desc_sw128(st + 2 * kSpXBox + (uint32_t)wg * (64 * 128));
     const int steps = min(4, kb64 - 4 * kb);
@@ -321,8 +310,7 @@ int8_sparse24_gemm_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
     // The sparse wgmma reads its metadata register when it executes, not when it issues, and ptxas does not guard
     // that register across the loop's back edge: the group retires before the next stage's words are loaded.
     wgmma_wait_s32<0>(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&ring->empty[s]);
+    ring.release(kb, lane);
   }
   // every wgmma of both warpgroups has read its stage: the ring becomes the output tile, [token][feature] (row-major
   // out) or [feature][token] (NCHW out)
@@ -388,7 +376,7 @@ int sp_run(const char* fn, long long m, long long k, long long n, long long P, i
     return SB200_E_CUDA;
   }
   if (const int rc = lower(w.q, w.sum, w.nan, st)) return rc;
-  const size_t smem = (size_t)kSpStages * kSpStageBytes + sizeof(SpRing) + 1024;
+  const size_t smem = (size_t)kSpStages * kSpStageBytes + sizeof(StageRing<kSpStages>) + 1024;
   static std::atomic<int> attr_done[64];
   SB_CUDA(ensure_dyn_smem(int8_sparse24_gemm_kernel<kNchw>, (int)smem, attr_done));
   const long long tiles = ((m + kSpTok - 1) / kSpTok) * ((n + kSpFeat - 1) / kSpFeat);

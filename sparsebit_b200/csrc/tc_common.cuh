@@ -1,6 +1,6 @@
-// tc_common.cuh -- pieces shared by the wgmma kernels (gptq_tc.cu, gptq_dgrad.cu, int8_linear.cu): mbarrier / TMA /
-// wgmma PTX wrappers, setmaxnreg, the in-register int4 -> fp16 fragment unpack, the TMA producer role,
-// cuTensorMapEncodeTiled.
+// tc_common.cuh -- pieces shared by the warp-specialised wgmma kernels (gptq_tc.cu, gptq_dgrad.cu, int8_linear.cu,
+// int8_sparse24.cu, int8_attention.cu): TMA / wgmma PTX wrappers, setmaxnreg, the TMA stage ring between the producer
+// and the consumers, the in-register int4 -> fp16 fragment unpack, the GPTQ TMA producer role, cuTensorMapEncodeTiled.
 //
 // The GPTQ kernels compute the transposed product D[n, m] = sum_k W[n, k] * x'[m, k] with one warpgroup-wide
 // wgmma.m64n128k16 per 16 K: the weights are the A operand, unpacked by every consumer thread straight into its own
@@ -27,8 +27,8 @@ constexpr int kWgQBytes = (kWgBK / 8) * kWgFeat * 4;         // 4 KB   packed wo
 constexpr int kWgStageBytes = 2 * kWgXBytes + kWgQBytes;     // 36 KB  (a multiple of 1024: every tile stays aligned)
 
 // ---------------------------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
@@ -44,22 +44,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
       : "memory");
 }
-// mbarrier wait with an optional back-off between polls (sb200_gptq4_set_wait_backoff; 0 = poll continuously)
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, int backoff_ns) {
-  for (;;) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (done) return;
-    if (backoff_ns > 0) __nanosleep((unsigned)backoff_ns);
-  }
-}
-
 // Register re-balancing between warpgroups (384 threads launch with 168 registers each; the producer needs few, the
 // consumers hold two 64-float accumulators plus the weight fragments).
 template <int N>
@@ -123,6 +107,56 @@ __device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
 
+// ---------------------------------------------------------------------------------- TMA stage ring
+// The producer / consumer pipeline of every warp-specialised wgmma kernel.  Warpgroup 0 is the producer: one thread
+// issues the TMA loads.  The eight warps of warpgroups 1 and 2 consume them.  Load i (counted from 0 over the whole
+// kernel) goes to stage i % S, and each stage has two barriers:
+//   full[s]   count 1.  Completes when acquire()'s expect_tx has armed it and the load's TMA bytes have landed.  The
+//             consumers wait on it with parity (i / S) & 1 (wait).
+//   empty[s]  count 8.  Completes when lane 0 of each consumer warp has arrived, once its warp is done reading the
+//             stage (release).  The producer waits on it with the opposite parity before it refills the stage
+//             (acquire), so its first lap over the ring does not wait.
+// The producer and the consumers must count the same loads, and every consumer warp must release every load once: a
+// wrong parity or a missing arrival does not produce a wrong number, it hangs the CTA.  When a consumer releases a load
+// (right after its wgmma group retires, or one load later while a group stays in flight) is the kernel's choice.
+// Thread 0 runs init(), any barrier init of the kernel's own, then mbar_fence_init(), all before the CTA-wide barrier.
+template <int S>
+struct StageRing {
+  uint64_t full[S];
+  uint64_t empty[S];
+
+  __device__ __forceinline__ void init() {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);  // one arrival per consumer warp
+    }
+  }
+  // producer: wait until load i may overwrite its stage, arm full with the load's TMA bytes; returns the stage
+  __device__ __forceinline__ int acquire(int i, uint32_t bytes, int backoff_ns = 0) {
+    const int s = i % S;
+    mbar_wait_relaxed(&empty[s], ((uint32_t)(i / S) & 1u) ^ 1u, backoff_ns);
+    mbar_expect_tx(&full[s], bytes);
+    return s;
+  }
+  // consumers: wait until load i has landed; returns the stage
+  __device__ __forceinline__ int wait(int i) {
+    const int s = i % S;
+    mbar_wait_relaxed(&full[s], (uint32_t)(i / S) & 1u, 0);
+    return s;
+  }
+  // consumers: this warp is done with load i's stage
+  __device__ __forceinline__ void release(int i, int lane) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[i % S]);
+  }
+};
+
+// The dynamic shared memory from its first 1024-byte boundary, the alignment SWIZZLE_128B tiles need (every launch
+// requests 1024 bytes of slack for it).
+__device__ __forceinline__ unsigned char* smem_align1024(unsigned char* smem) {
+  return smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
+}
+
 // ---------------------------------------------------------------------------------- int4 -> fp16 fragment unpack
 // One packed word = 8 nibbles along K.  With the activations permuted inside every 8 K as 0,4,1,5,2,6,3,7, the two
 // fp16 values a thread with (lane & 3) == q needs from a word (K positions 2q, 2q+1 of the fragment layout) are the
@@ -148,21 +182,21 @@ struct NibblePair {
 };
 __device__ __forceinline__ uint32_t h2u(__half2 v) { return *reinterpret_cast<const uint32_t*>(&v); }
 
-// ---------------------------------------------------------------------------------- TMA producer role
+// ---------------------------------------------------------------------------------- GPTQ TMA producer role
 // Stage s of a tile: x_hi [128 tok][64 K] | x_lo [128 tok][64 K] (only when need_lo) | packed words [8][128 features].
-__device__ __forceinline__ void wg_produce(unsigned char* stage_base, uint64_t* full, uint64_t* empty, int stages,
-                                           const CUtensorMap* map_hi, const CUtensorMap* map_lo, const CUtensorMap* map_q,
-                                           int m0, int n0, int num_kb, bool need_lo, int backoff_ns) {
+// Load kb is K block kb.  Unlike the int8 producers, this one may sleep backoff_ns between polls of a full ring
+// (sb200_gptq4_set_wait_backoff).
+template <int S>
+__device__ __forceinline__ void wg_produce(unsigned char* stage_base, StageRing<S>& ring, const CUtensorMap* map_hi,
+                                           const CUtensorMap* map_lo, const CUtensorMap* map_q, int m0, int n0,
+                                           int num_kb, bool need_lo, int backoff_ns) {
   const uint32_t tx = (uint32_t)(kWgXBytes + kWgQBytes + (need_lo ? kWgXBytes : 0));
   for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % stages;
-    const uint32_t ph = (uint32_t)(kb / stages) & 1u;
-    mbar_wait_relaxed(&empty[s], ph ^ 1u, backoff_ns);
+    const int s = ring.acquire(kb, tx, backoff_ns);
     unsigned char* st = stage_base + (size_t)s * kWgStageBytes;
-    mbar_expect_tx(&full[s], tx);
-    tma_load_2d(st, map_hi, kb * kWgBK, m0, &full[s]);
-    if (need_lo) tma_load_2d(st + kWgXBytes, map_lo, kb * kWgBK, m0, &full[s]);
-    tma_load_2d(st + 2 * kWgXBytes, map_q, n0, kb * (kWgBK / 8), &full[s]);
+    tma_load_2d(st, map_hi, kb * kWgBK, m0, &ring.full[s]);
+    if (need_lo) tma_load_2d(st + kWgXBytes, map_lo, kb * kWgBK, m0, &ring.full[s]);
+    tma_load_2d(st + 2 * kWgXBytes, map_q, n0, kb * (kWgBK / 8), &ring.full[s]);
   }
 }
 

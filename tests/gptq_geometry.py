@@ -19,8 +19,8 @@ SIMT_CTAS_PER_SM = 8        # gptq_simt.cu:202
 SIMT_STAGED_K = 1024        # gptq_simt.cu:205 s_cap = 1024 / kBlockK
 DEC_COLS = 128              # gptq_decode.cu:31 kDecCols
 DEC_BLOCK_K = 128           # gptq_decode.cu:32 kDecBlockK
-DEC_DEFAULT_PER_SM = 5      # gptq_decode.cu:459
-DEC_DEFAULT_MODE = 6        # gptq_decode.cu:419 g_dec_mode
+DEC_DEFAULT_PER_SM = 5      # gptq_decode.cu:456
+DEC_DEFAULT_MODE = 6        # gptq_decode.cu:416 g_dec_mode
 DEC_MAX_PROBLEMS = 4        # gptq_launch.cuh:15 kDecMaxProblems
 TC_MIN_M = 32               # gptq.cu:96 auto dispatch takes the wgmma kernel from this M on
 TC_STAGES = 5               # gptq_tc.cu:30 kTcStages
@@ -33,8 +33,9 @@ DG_TC_MIN_M = 48            # gptq.cu:225 kDgradTcMinM
 DG_COLS = 128               # gptq_dgrad.cu:40 kDgCols
 DG_UNIT_K = 32              # gptq_dgrad.cu:41 kDgUnitK
 DG_TARGET_CTAS = 1024       # gptq_dgrad.cu:42 kDgTargetCtas
+DG_STAGES = 5               # gptq_dgrad.cu:179 kDgStages
 DG_CHUNK = 8                # gptq_dgrad.cu:180 kDgChunk
-DG_C_CLAMP = 100            # gptq_dgrad.cu:233
+DG_C_CLAMP = 100            # gptq_dgrad.cu:228
 
 
 def _cdiv(a, b):
@@ -57,7 +58,7 @@ def packed_rows(bits, k):
 
 # ----------------------------------------------------------------------------------------------- dispatch (gptq.cu)
 def tc_refusal(k, n, gs, x_off=0, qw_off=0):
-    """gptq4_tc_supported, gptq_tc.cu:294-304: None, or the first reason it refuses."""
+    """gptq4_tc_supported, gptq_tc.cu:284-294: None, or the first reason it refuses."""
     if k % 8:
         return "k8"
     if n % 4:
@@ -72,7 +73,7 @@ def tc_refusal(k, n, gs, x_off=0, qw_off=0):
 
 
 def decode_supported(n, qw_off=0):
-    """gptq4_decode_supported, gptq_decode.cu:413."""
+    """gptq4_decode_supported, gptq_decode.cu:410."""
     return n % 4 == 0 and _a16(qw_off)
 
 
@@ -140,7 +141,7 @@ def simt_branches(bits, m, k, n, kw, sm):
 
 # ----------------------------------------------------------------------------------------------- decode (gptq_decode.cu)
 def dec_plan(problems, m, mode, sm):
-    """dec_run, gptq_decode.cu:443-480.  problems: [(k, n, kw)]."""
+    """dec_run, gptq_decode.cu:440-477.  problems: [(k, n, kw)]."""
     colblocks = sum(_cdiv(n, DEC_COLS) for _, n, _ in problems)
     nblk_max = max(_cdiv(k, DEC_BLOCK_K) for k, _, _ in problems)
     nbk = 1 if m <= 8 else (2 if m <= 16 else 4)
@@ -159,7 +160,7 @@ def dec_branches(problems, m, mode, sm, static_flag=False, f16=False):
     s, mt = p["S"], p["mt"]
     b = {f"dec.nbk{p['nbk']}"}
     if m > mt:
-        b.add("dec.mpass")  # gptq_decode.cu:211, reached through forced impl 1 (M > 32)
+        b.add("dec.mpass")  # gptq_decode.cu:208, reached through forced impl 1 (M > 32)
     if p["capped"]:
         b.add("dec.smax")
     if p["nblk_max"] % s:
@@ -174,24 +175,24 @@ def dec_branches(problems, m, mode, sm, static_flag=False, f16=False):
         for y in range(p["slices"]):
             b0 = y * s
             if b0 >= nblk:
-                b.add("dec.batch.short_k")  # gptq_decode.cu:119
+                b.add("dec.batch.short_k")  # gptq_decode.cu:116
                 continue
             nbs.append(min(b0 + s, nblk) - b0)
         if slab:
             if nblk * (DEC_BLOCK_K // 8) > kw:
-                b.add("dec.slab.zero_fill")  # gptq_decode.cu:165-168
+                b.add("dec.slab.zero_fill")  # gptq_decode.cu:162-165
             if n % DEC_COLS:
-                b.add("dec.slab.n_tail")  # gptq_decode.cu:161
+                b.add("dec.slab.n_tail")  # gptq_decode.cu:158
     if 1 in nbs:
         b.add("dec.nb1")
     if slab:
         b.add("dec.slab")
         if m % mt:
-            b.add("dec.slab.trow_alias")  # x_rows < MT in some pass, gptq_decode.cu:290
+            b.add("dec.slab.trow_alias")  # x_rows < MT in some pass, gptq_decode.cu:287
     else:
         b.add("dec.reg")
         if prefetch and any(nb > 2 for nb in nbs):
-            b.add("dec.prefetch")  # gptq_decode.cu:173-188
+            b.add("dec.prefetch")  # gptq_decode.cu:170-185
     b.add(("dec.wait.static" if static else "dec.wait.strict") if pdl else "dec.no_pdl")
     if len(problems) > 1:
         b.add("dec.batch")
@@ -200,15 +201,15 @@ def dec_branches(problems, m, mode, sm, static_flag=False, f16=False):
     if f16:
         b.add("dec.f16")
         if p["slices"] >= 4:
-            b.add("dec.f16.unroll4")  # gptq_decode.cu:399
+            b.add("dec.f16.unroll4")  # gptq_decode.cu:396
         if p["slices"] % 4:
-            b.add("dec.f16.rem")  # gptq_decode.cu:404
+            b.add("dec.f16.rem")  # gptq_decode.cu:401
     return b
 
 
 # ----------------------------------------------------------------------------------------------- wgmma prefill (gptq_tc.cu)
 def tc_live_a_only(n):
-    """Some consumer thread of the last feature tile has na = n0 + f0 < N <= nb = na + 8 (gptq_tc.cu:184-186):
+    """Some consumer thread of the last feature tile has na = n0 + f0 < N <= nb = na + 8 (gptq_tc.cu:176-178):
     f0 = 64 a + 16 b + l (l < 8), so with r = N % 128 some f0 in [r - 8, r - 1] has l < 8 iff r % 16 != 0."""
     r = n % WG_FEAT
     return r != 0 and r % 16 != 0
@@ -222,7 +223,7 @@ def tc_branches(m, k, n, kw, gs, f16=False, bias=True):
     if k % WG_BK:
         b.add("tc.k64_tail")  # the TMA zero-fills the last stage
     if num_kb % 2:
-        b.add("tc.odd_kb")  # gptq_tc.cu:228: fold on the last stage
+        b.add("tc.odd_kb")  # gptq_tc.cu:219: fold on the last stage
     if num_kb > TC_STAGES:
         b.add("tc.ring_wrap")
     if num_kb > 2 * TC_STAGES:
@@ -234,14 +235,14 @@ def tc_branches(m, k, n, kw, gs, f16=False, bias=True):
     if tc_live_a_only(n):
         b.add("tc.live_a_only")
     if gs != TC_GROUP_K:
-        b.add("tc.gq_ne_g")  # gptq_tc.cu:196
+        b.add("tc.gq_ne_g")  # gptq_tc.cu:187
     if kw > _cdiv(k, 8):
         b.add("tc.kw_extra")
     return b
 
 
 def zero_probe(scales, zeros):
-    """gptq_zero_probe_kernel, gptq_tc.cu:130-139, on numpy fp32 arrays: the set of reasons the integer-zero epilogue is
+    """gptq_zero_probe_kernel, gptq_tc.cu:125-134, on numpy fp32 arrays: the set of reasons the integer-zero epilogue is
     refused (empty: integer zero points)."""
     import numpy as np
 
@@ -263,7 +264,7 @@ def zero_probe(scales, zeros):
 
 
 def split_need_lo(x):
-    """gptq_split_kernel, gptq_tc.cu:61-94, with the exponent clamped at -126: does some row-scaled element keep a non-zero
+    """gptq_split_kernel, gptq_tc.cu:56-89, with the exponent clamped at -126: does some row-scaled element keep a non-zero
     fp16 low part?  x: [M, K] fp32."""
     import numpy as np
 
@@ -336,7 +337,7 @@ def dgrad_simt_plan(m, k, n):
 
 
 def dgrad_tc_ok(bits, k, n, gs, go_off=0):
-    """gptq.cu:243 and gptq_dgrad_tc_supported / tc_shape_ok, gptq_dgrad.cu:371-389 (workspace given)."""
+    """gptq.cu:243 and gptq_dgrad_tc_supported / tc_shape_ok, gptq_dgrad.cu:360-378 (workspace given)."""
     return bits == 4 and n % 8 == 0 and k % 4 == 0 and (gs % 128 == 0 or gs == k) and _a16(go_off)
 
 
@@ -354,11 +355,15 @@ def dgrad_branches(bits, m, k, n, kw, gs, impl, go_off=0):
         b.add("dg.tc")
         num_nb = _cdiv(n, WG_BK)
         if kw % 8:
-            b.add("dg.tc.kw_tail")  # dgrad_repack_kernel, gptq_dgrad.cu:196
+            b.add("dg.tc.kw_tail")  # dgrad_repack_kernel, gptq_dgrad.cu:191
         if n % 64:
             b.add("dg.tc.n_tail")  # repack and table padding of the last 64-n stage
+        if num_nb > DG_STAGES:
+            b.add("dg.tc.ring_wrap")  # gptq_dgrad.cu:294, 323: stage reuse with alternating parity
+        if num_nb > 2 * DG_STAGES:
+            b.add("dg.tc.ring_wrap2")
         if num_nb > DG_CHUNK:
-            b.add("dg.tc.chunk_restart")  # gptq_dgrad.cu:295-338
+            b.add("dg.tc.chunk_restart")  # gptq_dgrad.cu:287-327
             if num_nb % DG_CHUNK == 0:
                 b.add("dg.tc.chunk_exact")
         if gs == k and k % 128:
@@ -378,7 +383,7 @@ def dgrad_branches(bits, m, k, n, kw, gs, impl, go_off=0):
 
 
 def dgrad_table_c(scales, zeros):
-    """dgrad_table_kernel, gptq_dgrad.cu:219-233: the per-group exponent c, before and after its clamp."""
+    """dgrad_table_kernel, gptq_dgrad.cu:214-228: the per-group exponent c, before and after its clamp."""
     import numpy as np
 
     s = np.asarray(scales, np.float32)

@@ -47,7 +47,7 @@ def sel_seg(rows, row_len, sm):
 
 
 def strided_finish_threads(tpr, nval):
-    """common.cuh:294-301."""
+    """common.cuh:312-319."""
     t = max((tpr + 3) // 4, 1) * nval
     if t > 1024:
         t = (1024 // nval) * nval

@@ -19,11 +19,11 @@ element a kernel skips fails.  Packed values past K are random, not zero: they m
   dispatch.auto.simt              gptq.cu:102            refuse_n4: N = 250 (no decode either)
   dispatch.auto.ws_null           gptq.cu:89-90          ws_null: M = 64 without a workspace -> decode
   dispatch.auto.ws_small          gptq.cu:90             ws_small: one byte short -> decode
-  dispatch.refuse.k8              gptq_tc.cu:299         refuse_k8: K = 1004
-  dispatch.refuse.n4              gptq_tc.cu:299         refuse_n4: N = 250
-  dispatch.refuse.group128        gptq_tc.cu:300         refuse_group128: one group of K = 1000
-  dispatch.refuse.x_misaligned    gptq_tc.cu:301         refuse_x_misaligned: x at float offset 1
-  dispatch.refuse.qw_misaligned   gptq_tc.cu:301         refuse_qw_misaligned: qweight at word offset 1 -> SIMT
+  dispatch.refuse.k8              gptq_tc.cu:289         refuse_k8: K = 1004
+  dispatch.refuse.n4              gptq_tc.cu:289         refuse_n4: N = 250
+  dispatch.refuse.group128        gptq_tc.cu:290         refuse_group128: one group of K = 1000
+  dispatch.refuse.x_misaligned    gptq_tc.cu:291         refuse_x_misaligned: x at float offset 1
+  dispatch.refuse.qw_misaligned   gptq_tc.cu:291         refuse_qw_misaligned: qweight at word offset 1 -> SIMT
   dispatch.impl1.decode           gptq.cu:100            dec_mpass_slab (forced, M = 70)
   dispatch.impl1.simt_fallback    gptq.cu:100-102        impl1_simt_fallback: N = 250
   dispatch.impl2.tc               gptq.cu:96             tc_odd_wrap2_frac (process-wide impl 2)
@@ -44,29 +44,29 @@ SIMT (launch_simt), for b = 2, 3, 4:
   simt3.straddle                  gptq_unpack.cuh        every 3-bit case (values 10 and 21 of a unit span two words)
 
 Decode (dec_run):
-  dec.nbk1, dec.reg, dec.prefetch, dec.wait.strict   gptq_decode.cu:455-458   dec_nbk1_default: M = 1, 4096 x 11008
+  dec.nbk1, dec.reg, dec.prefetch, dec.wait.strict   gptq_decode.cu:452-455   dec_nbk1_default: M = 1, 4096 x 11008
   dec.nbk2, dec.slab, dec.slab.trow_alias, dec.slab.zero_fill, dec.slab.n_tail, dec.nb1, dec.wait.static
-                                  gptq_decode.cu:152-168, 290   dec_slab_alias: M = 12, K = 1000, N = 260, mode 11
-  dec.nbk4, dec.mpass, dec.no_pdl gptq_decode.cu:211     dec_mpass_slab: forced impl 1, M = 70, mode 1
-  dec.smax, dec.short_slice       gptq_decode.cu:466-468 dec_smax: M = 20, 10880 x 4096 (S 5 > 2, 85 blocks)
-  dec.per_sm                      gptq_decode.cu:459     dec_per_sm: mode 0x82
-  dec.need_lo, dec.no_lo (data)   gptq_decode.cu:276-279 dec_nbk1_default (fp32); dec_per_sm (fp16-exact activations)
-  dec.batch, dec.batch.diff_n, dec.batch.short_k     gptq_decode.cu:107, 119   batch_3: N 512 / 132 / 256, one K 512
-  dec.batch (4 problems)          gptq_decode.cu:107     batch_4: M = 32
-  dec.f16, dec.f16.unroll4        gptq_decode.cu:382-410 f16_single: M = 1, 4096 x 4096 (16 slices)
-  dec.f16.rem                     gptq_decode.cu:404     f16_single_rem_nobias: 9 slices
-  dec.f16.counter_reset (data)    gptq_decode.cu:408     f16_single, f16_single_rem_nobias: three calls on one state
+                                  gptq_decode.cu:149-165, 287   dec_slab_alias: M = 12, K = 1000, N = 260, mode 11
+  dec.nbk4, dec.mpass, dec.no_pdl gptq_decode.cu:208     dec_mpass_slab: forced impl 1, M = 70, mode 1
+  dec.smax, dec.short_slice       gptq_decode.cu:463-465 dec_smax: M = 20, 10880 x 4096 (S 5 > 2, 85 blocks)
+  dec.per_sm                      gptq_decode.cu:456     dec_per_sm: mode 0x82
+  dec.need_lo, dec.no_lo (data)   gptq_decode.cu:273-276 dec_nbk1_default (fp32); dec_per_sm (fp16-exact activations)
+  dec.batch, dec.batch.diff_n, dec.batch.short_k     gptq_decode.cu:104, 116   batch_3: N 512 / 132 / 256, one K 512
+  dec.batch (4 problems)          gptq_decode.cu:104     batch_4: M = 32
+  dec.f16, dec.f16.unroll4        gptq_decode.cu:379-407 f16_single: M = 1, 4096 x 4096 (16 slices)
+  dec.f16.rem                     gptq_decode.cu:401     f16_single_rem_nobias: 9 slices
+  dec.f16.counter_reset (data)    gptq_decode.cu:405     f16_single, f16_single_rem_nobias: three calls on one state
 
 wgmma prefill (gptq4_tc):
   tc.f32, tc.k64_tail, tc.ring_wrap, tc.ring_wrap2, tc.m_tail, tc.n_tail, tc.live_a_only, tc.kw_extra
-                                  gptq_tc.cu:158-263     tc_tail_wrap: M = 300, K = 1000, N = 264, 3 extra rows
-  tc.odd_kb, tc.gq_ne_g           gptq_tc.cu:196, 228    tc_odd_wrap2_frac: K = 704 (11 stages), group 384
-  tc.int_zero, tc.two_pass (data) gptq_tc.cu:159-160     tc_tail_wrap
-  tc.general.fractional, tc.one_pass (data)   gptq_tc.cu:136   tc_odd_wrap2_frac (fp16-exact activations)
-  tc.general.big_zero (data)      gptq_tc.cu:136         tc_big_zero: some |zero| = 1100
-  tc.general.scale0 (data)        gptq_tc.cu:136         tc_scale0: one scale 0
-  tc.f16_out, tc.f16_out.bias     gptq_tc.cu:243-251     f16_tc: M = 800, N = 260
-  tc.f16_out.nobias               gptq_tc.cu:244         f16_tc_nobias: M = 768
+                                  gptq_tc.cu:153-252     tc_tail_wrap: M = 300, K = 1000, N = 264, 3 extra rows
+  tc.odd_kb, tc.gq_ne_g           gptq_tc.cu:187, 219    tc_odd_wrap2_frac: K = 704 (11 stages), group 384
+  tc.int_zero, tc.two_pass (data) gptq_tc.cu:154-155     tc_tail_wrap
+  tc.general.fractional, tc.one_pass (data)   gptq_tc.cu:131   tc_odd_wrap2_frac (fp16-exact activations)
+  tc.general.big_zero (data)      gptq_tc.cu:131         tc_big_zero: some |zero| = 1100
+  tc.general.scale0 (data)        gptq_tc.cu:131         tc_scale0: one scale 0
+  tc.f16_out, tc.f16_out.bias     gptq_tc.cu:232-240     f16_tc: M = 800, N = 260
+  tc.f16_out.nobias               gptq_tc.cu:233         f16_tc_nobias: M = 768
 
 fp16 linear (sb200_gptq4_linear_f16_ex):
   f16.tc                          gptq.cu:182            f16_tc, f16_tc_nobias
@@ -80,17 +80,18 @@ Input gradient (sb200_gptq_matmul_dgrad):
   dg.auto.small_m, dg.simt.slices, dg.simt.k_tail, dg.simt.mt4, dg.simt.m_tiles, dg.simt.b4
                                   gptq.cu:250, gptq_dgrad.cu:135-175   dg_small_m: M = 40, K = 1000, N = 2512
   dg.auto.tc, dg.tc, dg.tc.kw_tail, dg.tc.n_tail, dg.tc.one_group_k128, dg.tc.m_tail, dg.tc.k_tail
-                                  gptq_dgrad.cu:188-209  dg_tc_tails: M = 300, K = 516 (one group), N = 264
+                                  gptq_dgrad.cu:183-204  dg_tc_tails: M = 300, K = 516 (one group), N = 264
   dg.auto.unsupported, dg.simt.b3 gptq.cu:243            dg_auto_3bit: 3-bit
   dg.impl1, dg.simt.mt1, dg.simt.one_slice, dg.simt.b2   gptq.cu:253   dg_impl1_mt1: 2-bit, M = 1, N = 61
   dg.simt.mt2                     gptq_dgrad.cu:137      dg_impl1_mt2: M = 2, N = 2516 (5 slices)
-  dg.impl2, dg.tc.chunk_restart   gptq_dgrad.cu:295-338  dg_chunk_restart: N = 1032 (17 stages)
-  dg.tc.chunk_exact               gptq_dgrad.cu:296      dg_chunk_exact: N = 1024 (16 stages)
+  dg.impl2, dg.tc.chunk_restart, dg.tc.ring_wrap, dg.tc.ring_wrap2
+                                  gptq_dgrad.cu:287-327  dg_chunk_restart: N = 1032 (17 stages)
+  dg.tc.chunk_exact               gptq_dgrad.cu:288      dg_chunk_exact: N = 1024 (16 stages)
   dg.impl2.error                  gptq.cu:245-249        dg_impl2_error: K = 126
-  dg.tc.c_clamp (data)            gptq_dgrad.cu:233      dg_c_clamp: group 0 scales ~1e-28 (c = 104 -> 100)
-  dg.tc.need_lo, dg.tc.no_lo (data)   gptq_dgrad.cu:264  dg_tc_tails (fp32); dg_chunk_exact (fp16-exact gradients)
+  dg.tc.c_clamp (data)            gptq_dgrad.cu:228      dg_c_clamp: group 0 scales ~1e-28 (c = 104 -> 100)
+  dg.tc.need_lo, dg.tc.no_lo (data)   gptq_dgrad.cu:259  dg_tc_tails (fp32); dg_chunk_exact (fp16-exact gradients)
 
-Split-kernel data edges (gptq_split_kernel, gptq_tc.cu:42-95), in tiny_fwd_tc, tiny_dgrad_tc and tiny_fwd_decode:
+Split-kernel data edges (gptq_split_kernel, gptq_tc.cu:37-90), in tiny_fwd_tc, tiny_dgrad_tc and tiny_fwd_decode:
   split.zero_row, split.nonfinite_row, split.tiny_row, split.subnormal_row   (data)
 Rows r * 2^-j with max |r| in [1, 2): for j <= 112 the wgmma forward and input gradient and the one-slice decode launch
 give exactly y * 2^-j, bit for bit wherever that is a normal number; below (max |x| < 2^-112, subnormal rows) the result
@@ -246,7 +247,8 @@ DGRAD_CASES = [
     C("dg_impl1_mt1", "dgrad", ["dg.impl1", "dg.simt.mt1", "dg.simt.one_slice", "dg.simt.b2", "dg.simt.k_tail"],
       bits=2, m=1, k=6661, n=61, gs=0, impl=1),
     C("dg_impl1_mt2", "dgrad", ["dg.impl1", "dg.simt.mt2", "dg.simt.slices"], m=2, k=256, n=2516, gs=128, impl=1),
-    C("dg_chunk_restart", "dgrad", ["dg.impl2", "dg.tc.chunk_restart"], m=64, k=512, n=1032, gs=128, impl=2),
+    C("dg_chunk_restart", "dgrad", ["dg.impl2", "dg.tc.chunk_restart", "dg.tc.ring_wrap", "dg.tc.ring_wrap2"],
+      m=64, k=512, n=1032, gs=128, impl=2),
     C("dg_chunk_exact", "dgrad", ["dg.auto.tc", "dg.tc.chunk_exact"], ["dg.tc.no_lo"], m=128, k=256, n=1024, gs=128,
       impl=0, data="f16x"),
     C("dg_impl2_error", "dgrad", ["dg.impl2.error"], m=64, k=126, n=64, gs=0, impl=2),
@@ -274,8 +276,8 @@ REQUIRED = {
     "dg.auto.small_m", "dg.auto.tc", "dg.auto.unsupported", "dg.impl1", "dg.impl2", "dg.impl2.error", "dg.tc",
     "dg.simt.mt1", "dg.simt.mt2", "dg.simt.mt4", "dg.simt.one_slice", "dg.simt.slices", "dg.simt.k_tail",
     "dg.simt.m_tiles", "dg.simt.b2", "dg.simt.b3", "dg.simt.b4", "dg.tc.kw_tail", "dg.tc.n_tail", "dg.tc.chunk_restart",
-    "dg.tc.chunk_exact", "dg.tc.one_group_k128", "dg.tc.m_tail", "dg.tc.k_tail", "dg.tc.c_clamp", "dg.tc.need_lo",
-    "dg.tc.no_lo", *SPLIT_DATA,
+    "dg.tc.chunk_exact", "dg.tc.one_group_k128", "dg.tc.m_tail", "dg.tc.k_tail", "dg.tc.ring_wrap", "dg.tc.ring_wrap2",
+    "dg.tc.c_clamp", "dg.tc.need_lo", "dg.tc.no_lo", *SPLIT_DATA,
 }
 
 

@@ -314,7 +314,7 @@ def test_geometry_matches_documented_launches():
 
 
 def test_finish_has_several_slices_below_17_values():
-    """strided_finish_threads (common.cuh:294-301) rounds the block up to whole warps, so it never launches fewer than 32
+    """strided_finish_threads (common.cuh:312-319) rounds the block up to whole warps, so it never launches fewer than 32
     threads and S = blockDim / nval >= 2 for nval <= 16: with the moments' 5 values S >= 6, so moments.finish.S1 cannot
     run.  Exhaustive over the tile counts up to 2^17 and a spread of larger ones."""
     tprs = list(range(1, 1 << 17)) + [10**6, 10**9, 10**12]

@@ -879,7 +879,7 @@ def _qp_state(rng, c, qmin, qmax):
         if kind == 0:
             keys[j] = (0xFFFFFFFF, 0x00000000)  # never observed (minmax_init)
         elif kind == 1:
-            keys[j] = (0xFFFFFFFF, 0xFFFFFFFF)  # a NaN was observed (common.cuh:258-266)
+            keys[j] = (0xFFFFFFFF, 0xFFFFFFFF)  # a NaN was observed (common.cuh:276-284)
         elif kind == 2:
             keys[j] = enc(np.array([-np.inf, np.inf], F32))
         elif kind == 3:
