@@ -602,6 +602,37 @@ int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64
                             const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
                             void* stream);
 
+/* ---- (5f) Channels-last (NHWC) integer-grid convs ----------------------------------------------------------------
+ * The entry points of (5b) and (5d) for an x stored NHWC: geom keeps its meaning (n, c, h, w) -- only the storage of x,
+ * x[((img h + ih) w + iw) c + ch], and of out, out[((img OH + oh) OW + ow) c_out + n], changes.  Each takes the argument
+ * list of its NCHW counterpart, makes the same checks in the same order with the same codes before any CUDA call, and
+ * computes the same values: the lowered q / row_sum / nan_flag byte for byte, every output bit for bit, NaNs
+ * included.  The weights are the same stored rows (K order (c, kh, kw)), so one stored weight serves both layouts.
+ *
+ * sb200_int8_im2col_quantize_nhwc: sb200_int8_im2col_quantize of an NHWC x.  A stride-1, unpadded 1 x 1 conv with
+ * c >= 256 is the row quantizer over x as [n h w, c]; otherwise each window's channels are read with 16-byte loads when c % 4 = 0 and
+ * x is 16-byte aligned.
+ * sb200_int8_conv2d_nhwc, sb200_int8_sparse24_conv2d_nhwc: the lowering above, then the GEMM of sb200_int8_conv2d /
+ * sb200_int8_sparse24_conv2d with its row-major [n OH OW, c_out] epilogue, which is out stored NHWC.  Workspace:
+ * sb200_int8_conv2d_workspace_bytes(geom), as for NCHW.
+ * sb200_int8_group_conv2d_nhwc: sb200_int8_group_conv2d, one direct kernel reading the channels of each tap with
+ * vector loads; no workspace.  All deterministic and graph-capturable. */
+int sb200_int8_im2col_quantize_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* scale,
+                                    const float* zero_point, int qmin, int qmax, int8_t* q, int32_t* row_sum,
+                                    uint8_t* nan_flag, void* stream);
+int sb200_int8_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                           const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                           const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
+                           void* workspace, size_t workspace_bytes, void* stream);
+int sb200_int8_sparse24_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                                    const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* vals,
+                                    const uint32_t* meta, const int32_t* dsum, const float* w_scale, const float* bias,
+                                    float* out, int64_t c_out, void* workspace, size_t workspace_bytes, void* stream);
+int sb200_int8_group_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                                 const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q,
+                                 const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* bias,
+                                 float* out, int64_t c_out, void* stream);
+
 /* ---- (5e) Integer-grid inference of a calibrated attention, fused (int8 wgmma, sm_90a) ----
  * New; the reference runs MatMul -> Softmax -> MatMul with a QIdentity carrier in front of every matmul input, so q,
  * k, the softmax output p and v are each fake-quantised per tensor.  Per batch entry, with q [tq, d], k [tk, d] and

@@ -115,6 +115,13 @@ PROTOTYPES = {
                                   c_i64, c_i64, c_vp, c_sz, c_vp]),
     "sb200_int8_group_conv2d": (c_int, [c_vp, c_geom, c_i64, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                         c_i64, c_vp]),
+    "sb200_int8_im2col_quantize_nhwc": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "sb200_int8_conv2d_nhwc": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp,
+                                       c_sz, c_vp]),
+    "sb200_int8_sparse24_conv2d_nhwc": (c_int, [c_vp, c_geom, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                c_i64, c_vp, c_sz, c_vp]),
+    "sb200_int8_group_conv2d_nhwc": (c_int, [c_vp, c_geom, c_i64, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                             c_vp, c_i64, c_vp]),
     "sb200_int8_attention_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_i64]),
     "sb200_int8_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int,
                                      c_int, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,

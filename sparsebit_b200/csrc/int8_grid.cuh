@@ -75,5 +75,8 @@ int launch_rows(const float* x, const float* scale, const float* zero_point, int
                 int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st);
 int launch_im2col(const float* x, const ConvDims& d, const float* scale, const float* zero_point, int qmin, int qmax,
                   int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st);
+// The same lowering of an x stored NHWC with c channels; a stride-1, unpadded 1 x 1 conv runs the row quantizer.
+int launch_im2col_nhwc(const float* x, const ConvDims& d, int c, const float* scale, const float* zero_point, int qmin,
+                       int qmax, int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st);
 
 }  // namespace sb200

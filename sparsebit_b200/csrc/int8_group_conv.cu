@@ -393,10 +393,318 @@ int gc_plan(GcDims* d, const float* x) {
   return mode;
 }
 
+// ---------------------------------------------------------------------------------- NHWC
+// x [n, h, w, c] and out [n, OH, OW, c_out] stored NHWC: the channels of one pixel are contiguous, so a thread owns a
+// quad of 4 adjacent output channels n0 .. n0 + 3 at a few output pixels and reads each tap's channels with vector
+// loads, straight from x (L1 / L2 serve the overlap of neighbouring windows); no staged input tile.  A CTA covers a
+// block of 4 QB output channels (QB quads, QB a power of two <= 16) and 256 / QB x kNhRounds consecutive output
+// pixels; its weights are staged in shared memory, re-laid out from w_q [c_out, Kp] for the path:
+//   kNhDw    C_g = 1, M_g = 1 (depthwise): word [tap][quad] packs the quad's 4 weights of the tap; the quad's 4
+//            channels are one float4 (vec) and 4 independent outputs, plain integer MACs.
+//   kNhQuad  M_g % 4 = 0: the quad lies in one group and shares its window; word [output][tap][c4] packs channels
+//            4 c4 .. 4 c4 + 3 (0 past C_g) and a float4 of the group's channels (vec: C_g % 4 = 0) quantizes straight
+//            into one __dp4a word.
+//   kNhAny   any other grouping, or weights that do not fit kGcSmemMax: each output of the quad reads its own group's
+//            window and w_q directly.
+// An output's NaN flag is set by exactly the elements of its group's window, its epilogue is gc_epilogue: outputs are
+// bit-identical to the NCHW kernel.  No workspace, no atomics: deterministic and graph-capturable.
+constexpr int kNhMaxQuads = 16;
+constexpr int kNhRounds = 4;  // pixels per thread
+
+enum NhMode { kNhDw = 0, kNhQuad = 1, kNhAny = 2 };
+
+struct NhDims {
+  long long M, P, OW, H, W, C, Cout;
+  int Cg, Mg, KH, KW, sh, sw, dh, dw, pt, pl, Kg, Kp, C4;
+  int QB, pix;                     // output-channel quads, output pixels per CTA
+  long long pblocks, nblocks, ctas;
+  int vec, vec_out;
+};
+
+__device__ __forceinline__ void nh_store(float* __restrict__ out, const NhDims& d, long long m, long long n0,
+                                         const float (&y)[4]) {
+  float* o = out + m * d.Cout + n0;
+  if (d.vec_out && n0 + 3 < d.Cout) {
+    *reinterpret_cast<float4*>(o) = make_float4(y[0], y[1], y[2], y[3]);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (n0 + j < d.Cout) o[j] = y[j];
+  }
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const float* __restrict__ x, NhDims d,
+                                                                          const float* __restrict__ x_scale,
+                                                                          const float* __restrict__ x_zero, float qmin,
+                                                                          float qmax, int off,
+                                                                          const int8_t* __restrict__ w_q,
+                                                                          const int* __restrict__ w_sum,
+                                                                          const float* __restrict__ w_scale,
+                                                                          const int* __restrict__ w_zero,
+                                                                          const float* __restrict__ bias,
+                                                                          float* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char gc_smem[];
+  uint32_t* ws = reinterpret_cast<uint32_t*>(gc_smem);
+  QP p;
+  p.set(__ldg(x_scale), __ldg(x_zero));
+  p.qmin = qmin;
+  p.qmax = qmax;
+  const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
+  const float sx = __ldg(x_scale);
+  const long long zx = (long long)rintf(__ldg(x_zero)) - off;
+  const int taps = d.KH * d.KW;
+  const int ql = threadIdx.x % d.QB, slot = threadIdx.x / d.QB, pstride = kGcThreads / d.QB;
+  long long staged = -1;
+  for (long long tile = blockIdx.x; tile < d.ctas; tile += gridDim.x) {
+    // pixel block fastest: neighbouring CTAs share the weight block and their windows' rows in L2
+    const long long pb = tile % d.pblocks, nb = tile / d.pblocks;
+    const long long nbase = nb * 4 * d.QB;
+    if constexpr (kMode != kNhAny) {
+      if (nb != staged) {
+        __syncthreads();  // the previous block's weights have been read
+        if constexpr (kMode == kNhDw) {
+          for (int i = threadIdx.x; i < taps * d.QB; i += kGcThreads) {
+            const int k = i / d.QB, qq = i - k * d.QB;
+            uint32_t wv = 0u;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const long long n = nbase + 4 * qq + j;
+              if (n < d.Cout) wv |= (uint32_t)(uint8_t)__ldg(w_q + n * d.Kp + k) << (8 * j);
+            }
+            ws[i] = wv;
+          }
+        } else {
+          for (int i = threadIdx.x; i < 4 * d.QB * taps * d.C4; i += kGcThreads) {
+            const int ol = i / (taps * d.C4), rem = i - ol * (taps * d.C4), k = rem / d.C4, c4 = rem - k * d.C4;
+            const long long n = nbase + ol;
+            uint32_t wv = 0u;
+            if (n < d.Cout) {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int c = 4 * c4 + j;
+                if (c < d.Cg) wv |= (uint32_t)(uint8_t)__ldg(w_q + n * d.Kp + c * taps + k) << (8 * j);
+              }
+            }
+            ws[i] = wv;
+          }
+        }
+        __syncthreads();
+        staged = nb;
+      }
+    }
+    const long long n0 = nbase + 4 * ql;  // the thread's quad of output channels
+    if (n0 >= d.Cout) continue;
+    for (int r = 0; r < kNhRounds; ++r) {
+      const long long m = pb * d.pix + slot + (long long)r * pstride;
+      if (m >= d.M) break;
+      const long long img = m / d.P, pp = m - img * d.P, oh = pp / d.OW, ow = pp - oh * d.OW;
+      const long long ih0 = oh * d.sh - d.pt, iw0 = ow * d.sw - d.pl;
+      const float* xi = x + img * d.H * d.W * d.C;
+      float y[4];
+      if constexpr (kMode == kNhDw) {
+        int acc[4] = {0, 0, 0, 0}, sa[4] = {0, 0, 0, 0};
+        bool nan[4] = {false, false, false, false};
+        for (int kh = 0; kh < d.KH; ++kh) {
+          const long long ih = ih0 + (long long)kh * d.dh;
+          for (int kw = 0; kw < d.KW; ++kw) {
+            const long long iw = iw0 + (long long)kw * d.dw;
+            int a[4];
+            if ((unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W) {
+              const float* xp = xi + (ih * d.W + iw) * d.C + n0;
+              float v[4];
+              if (d.vec) {
+                const float4 f = __ldg(reinterpret_cast<const float4*>(xp));
+                v[0] = f.x, v[1] = f.y, v[2] = f.z, v[3] = f.w;
+              } else {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) v[j] = n0 + j < d.C ? __ldg(xp + j) : 0.f;
+              }
+#pragma unroll
+              for (int j = 0; j < 4; ++j) a[j] = (int)(int8_t)stored_grid(v[j], p, off, nan[j]);
+            } else {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) a[j] = (int)(int8_t)pad;
+            }
+            const uint32_t wv = ws[(kh * d.KW + kw) * d.QB + ql];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              acc[j] += a[j] * (int)(int8_t)(wv >> (8 * j));
+              sa[j] += a[j];
+            }
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          y[j] = n0 + j < d.Cout ? gc_epilogue(acc[j], sa[j], (int)(n0 + j), zx, sx, d.Kg, w_sum, w_scale, w_zero, bias,
+                                               nan[j])
+                                 : 0.f;
+      } else if constexpr (kMode == kNhQuad) {
+        const long long c0 = n0 / d.Mg * d.Cg;  // M_g % 4 = 0: the quad's one group
+        const uint32_t* wt = ws + (size_t)4 * ql * taps * d.C4;
+        const int wstride = taps * d.C4;
+        int acc[4] = {0, 0, 0, 0}, sa = 0;
+        bool nan = false;
+        for (int kh = 0; kh < d.KH; ++kh) {
+          const long long ih = ih0 + (long long)kh * d.dh;
+          for (int kw = 0; kw < d.KW; ++kw) {
+            const long long iw = iw0 + (long long)kw * d.dw;
+            const bool in = (unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W;
+            const float* xp = xi + (ih * d.W + iw) * d.C + c0;
+            const int k = kh * d.KW + kw;
+            for (int c4 = 0; c4 < d.C4; ++c4) {
+              uint32_t a4 = 0u;
+              const int live = min(4, d.Cg - 4 * c4);  // channels of the quad inside the group
+              if (in) {
+                float4 f;
+                if (d.vec) {
+                  f = __ldg(reinterpret_cast<const float4*>(xp + 4 * c4));
+                } else {
+                  f.x = __ldg(xp + 4 * c4);
+                  f.y = live > 1 ? __ldg(xp + 4 * c4 + 1) : 0.f;
+                  f.z = live > 2 ? __ldg(xp + 4 * c4 + 2) : 0.f;
+                  f.w = live > 3 ? __ldg(xp + 4 * c4 + 3) : 0.f;
+                }
+                a4 = ((uint32_t)stored_grid(f.x, p, off, nan) & 0xFFu);
+                if (live > 1) a4 |= ((uint32_t)stored_grid(f.y, p, off, nan) & 0xFFu) << 8;
+                if (live > 2) a4 |= ((uint32_t)stored_grid(f.z, p, off, nan) & 0xFFu) << 16;
+                if (live > 3) a4 |= ((uint32_t)stored_grid(f.w, p, off, nan) & 0xFFu) << 24;
+              } else {
+                a4 = ((uint32_t)pad & 0xFFu) * 0x01010101u;
+                if (live < 4) a4 &= 0xFFFFFFFFu >> (8 * (4 - live));
+              }
+              sa = __dp4a((int)a4, 0x01010101, sa);
+#pragma unroll
+              for (int j = 0; j < 4; ++j) acc[j] = __dp4a((int)a4, (int)wt[j * wstride + k * d.C4 + c4], acc[j]);
+            }
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          y[j] = n0 + j < d.Cout ? gc_epilogue(acc[j], sa, (int)(n0 + j), zx, sx, d.Kg, w_sum, w_scale, w_zero, bias, nan)
+                                 : 0.f;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const long long n = n0 + j;
+          y[j] = 0.f;
+          if (n >= d.Cout) continue;
+          const long long c0 = n / d.Mg * d.Cg;
+          const int8_t* wr = w_q + n * d.Kp;
+          int acc = 0, sa = 0;
+          bool nan = false;
+          for (int kh = 0; kh < d.KH; ++kh) {
+            const long long ih = ih0 + (long long)kh * d.dh;
+            for (int kw = 0; kw < d.KW; ++kw) {
+              const long long iw = iw0 + (long long)kw * d.dw;
+              const bool in = (unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W;
+              const float* xp = xi + (ih * d.W + iw) * d.C + c0;
+              const int k = kh * d.KW + kw;
+              for (int c = 0; c < d.Cg; ++c) {
+                const int a = (int)(int8_t)(in ? stored_grid(__ldg(xp + c), p, off, nan) : pad);
+                acc += a * (int)__ldg(wr + c * taps + k);
+                sa += a;
+              }
+            }
+          }
+          y[j] = gc_epilogue(acc, sa, (int)n, zx, sx, d.Kg, w_sum, w_scale, w_zero, bias, nan);
+        }
+      }
+      nh_store(out, d, m, n0, y);
+    }
+  }
+}
+
+long long nh_smem_bytes(int mode, const NhDims& d) {
+  const long long taps = (long long)d.KH * d.KW;
+  if (mode == kNhDw) return 4 * taps * d.QB;
+  if (mode == kNhQuad) return 16LL * d.QB * taps * d.C4;
+  return 0;
+}
+
+// The NHWC launch plan: path and channel block.  Returns the path.
+int nh_plan(NhDims* d, const float* x, const float* out) {
+  int mode = d->Cg == 1 && d->Mg == 1 ? kNhDw : d->Mg % 4 == 0 ? kNhQuad : kNhAny;
+  d->C4 = (d->Cg + 3) / 4;
+  int qb = 1;
+  while (qb < kNhMaxQuads && 4LL * qb < d->Cout) qb *= 2;
+  if (mode != kNhAny) {
+    for (;;) {
+      d->QB = qb;
+      if (nh_smem_bytes(mode, *d) <= kGcSmemMax) break;
+      if (qb == 1) {
+        mode = kNhAny;
+        break;
+      }
+      qb /= 2;
+    }
+  }
+  d->QB = qb;
+  d->pix = kGcThreads / qb * kNhRounds;
+  d->pblocks = cdiv(d->M, d->pix);
+  d->nblocks = cdiv(d->Cout, 4LL * qb);
+  d->ctas = d->pblocks * d->nblocks;
+  d->vec = (mode == kNhDw ? d->C % 4 == 0 : d->Cg % 4 == 0) && aligned16(x);
+  d->vec_out = d->Cout % 4 == 0 && aligned16(out);
+  return mode;
+}
+
 }  // namespace
 }  // namespace sb200
 
 using namespace sb200;
+
+int sb200_int8_group_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                                 const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q,
+                                 const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* bias,
+                                 float* out, int64_t c_out, void* stream) {
+  const char* fn = "sb200_int8_group_conv2d_nhwc";
+  SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out,
+             "%s: null pointer argument", fn);
+  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
+  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
+  SB_REQUIRE(groups >= 2, "%s: groups = %lld; a conv with groups = 1 runs on sb200_int8_conv2d_nhwc", fn,
+             (long long)groups);
+  ConvDims cd;
+  if (const int rc = check_conv(fn, geom, &cd)) return rc;
+  const sb200_conv2d_geom& g = *geom;
+  SB_REQUIRE(g.c % groups == 0 && c_out % groups == 0, "%s: groups = %lld does not divide c = %lld and c_out = %lld", fn,
+             (long long)groups, (long long)g.c, (long long)c_out);
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
+  const long long kg = (g.c / groups) * g.kh * g.kw;
+  if ((__int128)(g.c / groups) * g.kh * g.kw >= kI8MaxK) {
+    set_error("%s: K_g = c / groups kh kw = %lld x %lld x %lld >= 2^17, the integer path supports K_g < 2^17 (|sum| <= "
+              "K_g * 2^14 must fit int32)", fn, (long long)(g.c / groups), (long long)g.kh, (long long)g.kw);
+    return SB200_E_UNSUPPORTED;
+  }
+  NhDims d{};
+  d.M = cd.M, d.P = cd.P, d.OW = cd.OW, d.H = g.h, d.W = g.w, d.C = g.c, d.Cout = c_out;
+  d.Cg = (int)(g.c / groups), d.Mg = (int)(c_out / groups);
+  d.KH = (int)g.kh, d.KW = (int)g.kw, d.sh = (int)g.stride_h, d.sw = (int)g.stride_w;
+  d.dh = (int)g.dilation_h, d.dw = (int)g.dilation_w, d.pt = (int)g.pad_top, d.pl = (int)g.pad_left;
+  d.Kg = (int)kg, d.Kp = (int)padded_k(kg);
+  const int mode = nh_plan(&d, x, out);
+  const unsigned grid = (unsigned)min(d.ctas, kGcMaxGrid);
+  const size_t smem = (size_t)nh_smem_bytes(mode, d);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int off = grid_offset(qmin_x);
+  const int* wsum = reinterpret_cast<const int*>(w_rowsum);
+  const int* wzero = reinterpret_cast<const int*>(w_zero);
+  if (mode == kNhDw)
+    int8_group_conv_nhwc_kernel<kNhDw><<<grid, kGcThreads, smem, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
+                                                                      (float)qmax_x, off, w_q, wsum, w_scale, wzero, bias,
+                                                                      out);
+  else if (mode == kNhQuad)
+    int8_group_conv_nhwc_kernel<kNhQuad><<<grid, kGcThreads, smem, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
+                                                                        (float)qmax_x, off, w_q, wsum, w_scale, wzero,
+                                                                        bias, out);
+  else
+    int8_group_conv_nhwc_kernel<kNhAny><<<grid, kGcThreads, 0, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
+                                                                    (float)qmax_x, off, w_q, wsum, w_scale, wzero, bias,
+                                                                    out);
+  SB_LAUNCHED();
+  return SB200_OK;
+}
 
 int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
                             const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,

@@ -317,6 +317,107 @@ __global__ void __launch_bounds__(kLowThreads) int8_im2col_quantize_kernel(const
   }
 }
 
+// ---------------------------------------------------------------------------------- conv2d lowering, NHWC
+constexpr int kNhPix = 64;        // output pixels (rows of q) per CTA
+constexpr int kNhMaxKC = 640;     // K bytes per chunk at most: the tile is kNhPix x kc <= 40 KB of dynamic shared memory
+constexpr int kNhThreads = 256;
+constexpr int kNhRowsMinK = 256;  // a stride-1 unpadded 1 x 1 conv with c >= this runs the row quantizer
+
+// The same q, row sums and NaN flags as int8_im2col_quantize_kernel, read from the NHWC storage of x.  One CTA per 64
+// consecutive output pixels; K in chunks [k0, k0 + kc) of a multiple of 16 bytes, normally whole blocks of channels
+// (kc = cb KH KW).  A work item is (tap, pixel, channel quad): it reads the quad's 4 channels of one input pixel
+// (vec: one 16-byte load; otherwise 4 guarded scalar loads) -- a warp reads 8 pixels x 4 quads, whole 64-byte runs of
+// channels -- and stores each element whose k = c KH KW + tap lies in the chunk into the pixel's row of the shared
+// tile, adding it to the pixel's row sum (integer, so the order of the shared-memory adds does not matter).  The tile
+// then leaves as 16-byte pieces of rows of q, K padding zeroed.
+__global__ void __launch_bounds__(kNhThreads) int8_im2col_quantize_nhwc_kernel(const float* __restrict__ x, ConvDims d,
+                                                                                int C, int kcmax,
+                                                                                const float* __restrict__ scale,
+                                                                                const float* __restrict__ zero_point,
+                                                                                float qmin, float qmax, int off,
+                                                                                int8_t* __restrict__ q,
+                                                                                int* __restrict__ row_sum,
+                                                                                uint8_t* __restrict__ nan_flag, int vec) {
+  extern __shared__ __align__(16) unsigned char nh_tile[];
+  __shared__ long long pix_org[kNhPix], pix_ih[kNhPix], pix_iw[kNhPix];  // x offset of the window's top-left, row, col
+  __shared__ int rsum[kNhPix];
+  __shared__ int rnan[kNhPix];
+  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  const long long m0 = (long long)blockIdx.x * kNhPix;
+  const int pix = (int)min((long long)kNhPix, d.M - m0);
+  if (t < pix) {
+    const long long m = m0 + t, img = m / d.P, pp = m - img * d.P;
+    const long long oh = pp / d.OW, ow = pp - oh * d.OW;
+    pix_ih[t] = oh * d.sh - d.pt;
+    pix_iw[t] = ow * d.sw - d.pl;
+    pix_org[t] = ((img * d.H + pix_ih[t]) * d.W + pix_iw[t]) * C;
+    rsum[t] = 0;
+    rnan[t] = 0;
+  }
+  QP p;
+  p.set(__ldg(scale), __ldg(zero_point));
+  p.qmin = qmin;
+  p.qmax = qmax;
+  const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
+  const int taps = d.KH * d.KW;
+  __syncthreads();
+  for (int k0 = 0; k0 < d.Kp; k0 += kcmax) {
+    const int kc = min(kcmax, d.Kp - k0);
+    const int klive = min(kc, d.K - k0);  // bytes of the chunk below K
+    if (klive > 0) {
+      const int q0 = k0 / taps / 4, nq = (k0 + klive - 1) / taps / 4 - q0 + 1;  // channel quads the chunk touches
+      const int items = taps * pix * nq;
+      for (int i = t; i < items; i += kNhThreads) {
+        const int qi = i % nq, r = i / nq, px = r % pix, tap = r / pix;
+        const int c = 4 * (q0 + qi), kh = tap / d.KW, kw = tap - kh * d.KW;
+        const long long ih = pix_ih[px] + (long long)kh * d.dh, iw = pix_iw[px] + (long long)kw * d.dw;
+        const bool in = (unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W;
+        const float* xp = x + pix_org[px] + ((long long)kh * d.dh * d.W + (long long)kw * d.dw) * C + c;
+        float v[4];
+        if (in && vec) {
+          const float4 f = __ldg(reinterpret_cast<const float4*>(xp));
+          v[0] = f.x, v[1] = f.y, v[2] = f.z, v[3] = f.w;
+        } else {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) v[j] = in && c + j < C ? __ldg(xp + j) : 0.f;
+        }
+        int s = 0;
+        bool nan = false;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int k = (c + j) * taps + tap - k0;
+          if (c + j < C && k >= 0 && k < klive) {
+            const int e = in ? stored_grid(v[j], p, off, nan) : pad;
+            s += e;
+            nh_tile[px * kcmax + k] = (unsigned char)e;
+          }
+        }
+        if (s) atomicAdd(&rsum[px], s);
+        if (nan) rnan[px] = 1;
+      }
+    }
+    __syncthreads();
+    // warp w stores rows w, w + 8, ...; bytes at or past K are the K padding
+    const int pieces = kc / 16;
+    for (int r = warp; r < pix; r += kNhThreads / 32) {
+      int8_t* qr = q + (m0 + r) * d.Kp + k0;
+      for (int j = lane; j < pieces; j += 32) {
+        uint4 u = *reinterpret_cast<const uint4*>(nh_tile + r * kcmax + 16 * j);
+        uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int b = 0; b < 16; ++b)
+          if (16 * j + b >= klive) w[b >> 2] &= ~(0xFFu << (8 * (b & 3)));
+        *reinterpret_cast<uint4*>(qr + 16 * j) = make_uint4(w[0], w[1], w[2], w[3]);
+      }
+    }
+    __syncthreads();  // the tile has been read
+  }
+  if (t < pix) {
+    row_sum[m0 + t] = rsum[t];
+    nan_flag[m0 + t] = rnan[t] ? 1 : 0;
+  }
+}
+
 // ---------------------------------------------------------------------------------- GEMM
 // The atom of every GEMM of this file is wgmma_m64n128k32_s8 of tc_common.cuh, which the fused attention kernel
 // (int8_attention.cu) shares: D[64 x 128] (+)= A[64 x 32] * B[32 x 128], s8 x s8 -> s32, both operands K-major
@@ -675,6 +776,27 @@ int launch_im2col(const float* x, const ConvDims& d, const float* scale, const f
   return SB200_OK;
 }
 
+int nhwc_chunk(const ConvDims& d) {
+  const int taps = d.KH * d.KW;
+  const long long cb = 16LL * max(1, 8 / taps);  // channels per chunk: a multiple of 16, so that c0 KH KW is too
+  return (int)min(min(cb * taps, (long long)kNhMaxKC), (long long)d.Kp);
+}
+
+int launch_im2col_nhwc(const float* x, const ConvDims& d, int c, const float* scale, const float* zero_point, int qmin,
+                       int qmax, int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st) {
+  // a stride-1, unpadded 1 x 1 conv: x is already the [n h w, c] row matrix of the lowering.  The row quantizer gives
+  // each row one warp, 16 elements per lane, so it takes rows of c >= kNhRowsMinK; shorter rows would leave most lanes
+  // idle, and the NHWC kernel below (one tap, 64 rows per CTA) quantizes them.
+  if (d.KH == 1 && d.KW == 1 && d.sh == 1 && d.sw == 1 && d.pt == 0 && d.pl == 0 && d.P == d.HW && d.K >= kNhRowsMinK)
+    return launch_rows(x, scale, zero_point, 0, qmin, qmax, q, row_sum, nan_flag, d.M, d.K, st);
+  const int kc = nhwc_chunk(d);
+  const int vec = (c % 4 == 0) && aligned16(x);
+  int8_im2col_quantize_nhwc_kernel<<<(unsigned)((d.M + kNhPix - 1) / kNhPix), kNhThreads, (size_t)kNhPix * kc, st>>>(
+      x, d, c, kc, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, row_sum, nan_flag, vec);
+  SB_LAUNCHED();
+  return SB200_OK;
+}
+
 }  // namespace sb200
 
 using namespace sb200;
@@ -757,6 +879,44 @@ int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float
                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
                           return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st);
                         });
+}
+
+int sb200_int8_im2col_quantize_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* scale,
+                                    const float* zero_point, int qmin, int qmax, int8_t* q, int32_t* row_sum,
+                                    uint8_t* nan_flag, void* stream) {
+  const char* fn = "sb200_int8_im2col_quantize_nhwc";
+  SB_REQUIRE(x && geom && scale && zero_point && q && row_sum && nan_flag, "%s: null pointer argument", fn);
+  ConvDims d;
+  if (const int rc = check_conv(fn, geom, &d)) return rc;
+  if (const int rc = check_range(fn, qmin, qmax)) return rc;
+  SB_REQUIRE(aligned16(q), "%s: q must be 16-byte aligned", fn);
+  if (const int rc = check_k(fn, d.K)) return rc;
+  return launch_im2col_nhwc(x, d, (int)geom->c, scale, zero_point, qmin, qmax, q, reinterpret_cast<int*>(row_sum),
+                            nan_flag, (cudaStream_t)stream);
+}
+
+int sb200_int8_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                           const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                           const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
+                           void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "sb200_int8_conv2d_nhwc";
+  SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out && workspace,
+             "%s: null pointer argument", fn);
+  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
+  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
+  ConvDims d;
+  if (const int rc = check_conv(fn, geom, &d)) return rc;
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
+  SB_REQUIRE(aligned16(w_q), "%s: w_q must be 16-byte aligned", fn);
+  if (const int rc = check_k(fn, d.K)) return rc;
+  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
+  // the row-major [n OH OW, c_out] output of the linear is the NHWC storage of [n, c_out, OH, OW]
+  return run_gemm<false>(fn, d.M, d.K, c_out, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
+                         out, workspace, (cudaStream_t)stream,
+                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                           return launch_im2col_nhwc(x, d, (int)geom->c, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum,
+                                                     xnan, st);
+                         });
 }
 
 size_t sb200_int8_matmul_workspace_bytes(int64_t batch, int64_t m, int64_t k, int64_t n) {

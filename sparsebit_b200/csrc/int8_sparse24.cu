@@ -465,3 +465,26 @@ int sb200_int8_sparse24_conv2d(const float* x, const sb200_conv2d_geom* geom, co
                         return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st);
                       });
 }
+
+int sb200_int8_sparse24_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                                    const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* vals,
+                                    const uint32_t* meta, const int32_t* dsum, const float* w_scale, const float* bias,
+                                    float* out, int64_t c_out, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* fn = "sb200_int8_sparse24_conv2d_nhwc";
+  SB_REQUIRE(x && geom && x_scale && x_zero_point && vals && meta && dsum && w_scale && out && workspace,
+             "%s: null pointer argument", fn);
+  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
+  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
+  ConvDims d;
+  if (const int rc = check_conv(fn, geom, &d)) return rc;
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
+  SB_REQUIRE(aligned16(vals) && aligned16(meta), "%s: vals and meta must be 16-byte aligned", fn);
+  if (const int rc = check_k(fn, d.K)) return rc;
+  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
+  // the row-major [n OH OW, c_out] output of the linear is the NHWC storage of [n, c_out, OH, OW]
+  return sp_run<false>(fn, d.M, d.K, c_out, 1, qmin_x, x_scale, x_zero_point, vals, meta, dsum, w_scale, bias, out,
+                       workspace, (cudaStream_t)stream, [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                         return launch_im2col_nhwc(x, d, (int)geom->c, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum,
+                                                   xnan, st);
+                       });
+}

@@ -16,7 +16,7 @@ def _stream(t):
     return torch.cuda.current_stream(t.device).cuda_stream
 
 
-def _req(t, name, dtype=torch.float32):
+def _req(t, name, dtype=torch.float32, memory_format=torch.contiguous_format):
     if not isinstance(t, torch.Tensor):
         raise SparsebitB200Error(f"{name}: expected a torch.Tensor")
     if not t.is_cuda:
@@ -25,7 +25,9 @@ def _req(t, name, dtype=torch.float32):
         raise SparsebitB200Error(f"Kernel Failure, Invalid dtype of Input tensor: {name}(Expect to be {dtype})")
     if t.numel() == 0:
         raise SparsebitB200Error(f"Kernel Failure, Tensor is empty: {name}")
-    if not t.is_contiguous():
+    if not t.is_contiguous(memory_format=memory_format):
+        if memory_format == torch.channels_last:
+            raise SparsebitB200Error(f"{name}: expected a 4-D channels-last (NHWC) contiguous tensor")
         raise SparsebitB200Error(f"{name}: expected a contiguous tensor")
     return t
 
@@ -689,10 +691,10 @@ def _check_per_tensor(fn, *qparams):
         raise SparsebitB200Error(f"{fn}: the qparams are per-tensor (1 element each)")
 
 
-def _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, **weight):
-    """The dtypes of a per-tensor fp32 activation, the fp32 ``w_scale`` and ``bias``, and the integer tensors of the
-    weight operand by name: int8 ``w_q`` / ``vals``, the others int32."""
-    _req(x, "data"), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
+def _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, x_format=torch.contiguous_format, **weight):
+    """The dtypes of a per-tensor fp32 activation (contiguous in ``x_format``), the fp32 ``w_scale`` and ``bias``, and the
+    integer tensors of the weight operand by name: int8 ``w_q`` / ``vals``, the others int32."""
+    _req(x, "data", memory_format=x_format), _req(x_scale, "x_scale"), _req(x_zero_point, "x_zero_point"), _req(w_scale, "w_scale")
     for name, t in weight.items():
         _req(t, name, torch.int8 if name in ("w_q", "vals") else torch.int32)
     if bias is not None:
@@ -1054,12 +1056,14 @@ def _sparse24_conv_rows(fn, k, w_scale, bias, vals, meta, dsum):
 
 
 def _int8_conv_prelude(fn, x, x_scale, x_zero_point, w_scale, bias, weight_rows, weight, kernel_size, groups, stride,
-                       padding, dilation):
+                       padding, dilation, memory_format=torch.contiguous_format):
     """The argument checks of the integer-grid conv wrappers, ``weight`` being the integer tensors of the weight
     operand by name and ``weight_rows`` its ``_int8_conv_rows`` / ``_sparse24_conv_rows``: returns the
-    ``Conv2dGeom``, C_out and the fp32 [N, C_out, OH, OW] output (one pixel when the kernel does not fit, which the C
-    entry points reject)."""
-    _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, **weight)
+    ``Conv2dGeom``, C_out and the fp32 [N, C_out, OH, OW] output in ``memory_format``, the layout x must have (one
+    pixel when the kernel does not fit, which the C entry points reject)."""
+    if memory_format == torch.channels_last and isinstance(x, torch.Tensor) and x.dim() != 4:
+        raise SparsebitB200Error(f"{fn}: data must be [N, C, H, W] stored channels-last")
+    _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, x_format=memory_format, **weight)
     if x.dim() != 4:
         raise SparsebitB200Error(f"{fn}: data must be [N, C, H, W]")
     groups = int(groups)
@@ -1068,7 +1072,8 @@ def _int8_conv_prelude(fn, x, x_scale, x_zero_point, w_scale, bias, weight_rows,
         raise SparsebitB200Error(f"{fn}: groups = {groups} does not divide C = {g.c}")
     n = weight_rows(fn, g.c // groups * g.kh * g.kw, w_scale, bias, **weight)
     oh, ow = conv2d_output_hw(g)
-    return g, n, torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device)
+    return g, n, torch.empty(g.n, n, max(oh, 1), max(ow, 1), dtype=torch.float32, device=x.device,
+                             memory_format=memory_format)
 
 
 def int8_im2col_quantize(x, kernel_size, scale, zero_point, qmin, qmax, stride=1, padding=0, dilation=1):
@@ -1152,6 +1157,84 @@ def int8_group_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_sca
                                           w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                           bias.data_ptr() if bias is not None else None, out.data_ptr(), n, _stream(x)))
     return out
+
+
+# ----------------------------------------------------------------------------- channels-last (NHWC) convs
+def int8_im2col_quantize_nhwc(x, kernel_size, scale, zero_point, qmin, qmax, stride=1, padding=0, dilation=1):
+    """``int8_im2col_quantize`` of a channels-last ``x`` (sb200_int8_im2col_quantize_nhwc): ``x`` [N, C, H, W] fp32
+    with ``x.is_contiguous(memory_format=torch.channels_last)``; the same ``(q, row_sum, nan)`` byte for byte."""
+    lib = _lib.load()
+    if isinstance(x, torch.Tensor) and x.dim() != 4:
+        raise SparsebitB200Error("int8_im2col_quantize_nhwc: data must be [N, C, H, W] stored channels-last")
+    _req(x, "data", memory_format=torch.channels_last), _req(scale, "scale"), _req(zero_point, "zero_point")
+    _check_per_tensor("int8_im2col_quantize_nhwc", scale, zero_point)
+    g = conv2d_geometry(x.shape, kernel_size, stride, padding, dilation)
+    oh, ow = conv2d_output_hw(g)
+    m = g.n * max(oh, 0) * max(ow, 0)
+    q = torch.empty(max(m, 1), int8_padded_k(g.c * g.kh * g.kw), dtype=torch.int8, device=x.device)
+    row_sum = torch.empty(max(m, 1), dtype=torch.int32, device=x.device)
+    nan = torch.empty(max(m, 1), dtype=torch.bool, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_im2col_quantize_nhwc(x.data_ptr(), ctypes.byref(g), scale.data_ptr(), zero_point.data_ptr(),
+                                                  int(qmin), int(qmax), q.data_ptr(), row_sum.data_ptr(), nan.data_ptr(),
+                                                  _stream(x)))
+    return q, row_sum, nan
+
+
+def int8_conv2d_nhwc(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, bias=None,
+                     stride=1, padding=0, dilation=1):
+    """``int8_conv2d`` of a channels-last ``x`` (sb200_int8_conv2d_nhwc), with the same stored weights: returns a
+    channels-last fp32 [N, C_out, OH, OW] whose values equal ``int8_conv2d`` on ``x.contiguous()`` bit for bit."""
+    lib = _lib.load()
+    g, n, out = _int8_conv_prelude("int8_conv2d_nhwc", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
+                                   dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, 1, stride, padding,
+                                   dilation, torch.channels_last)
+    ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
+    ws = _int8_workspace(x.device, max(ws_bytes, 16))
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_conv2d_nhwc(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(), x_zero_point.data_ptr(),
+                                         int(qmin), int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(),
+                                         w_zero.data_ptr(), bias.data_ptr() if bias is not None else None, out.data_ptr(),
+                                         n, ws.data_ptr(), ws.numel(), _stream(x)))
+    return out
+
+
+def int8_sparse24_conv2d_nhwc(x, x_scale, x_zero_point, qmin, qmax, vals, meta, dsum, w_scale, kernel_size, bias=None,
+                              stride=1, padding=0, dilation=1):
+    """``int8_sparse24_conv2d`` of a channels-last ``x`` (sb200_int8_sparse24_conv2d_nhwc): returns a channels-last fp32
+    [N, C_out, OH, OW] whose values equal ``int8_sparse24_conv2d`` on ``x.contiguous()`` bit for bit."""
+    lib = _lib.load()
+    g, n, out = _int8_conv_prelude("int8_sparse24_conv2d_nhwc", x, x_scale, x_zero_point, w_scale, bias,
+                                   _sparse24_conv_rows, dict(vals=vals, meta=meta, dsum=dsum), kernel_size, 1, stride,
+                                   padding, dilation, torch.channels_last)
+    ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
+    ws = _int8_workspace(x.device, max(ws_bytes, 16))
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_sparse24_conv2d_nhwc(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(),
+                                                  x_zero_point.data_ptr(), int(qmin), int(qmax), vals.data_ptr(),
+                                                  meta.data_ptr(), dsum.data_ptr(), w_scale.data_ptr(),
+                                                  bias.data_ptr() if bias is not None else None, out.data_ptr(), n,
+                                                  ws.data_ptr(), ws.numel(), _stream(x)))
+    return out
+
+
+def int8_group_conv2d_nhwc(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups,
+                           bias=None, stride=1, padding=0, dilation=1):
+    """``int8_group_conv2d`` of a channels-last ``x`` (sb200_int8_group_conv2d_nhwc), with the same stored weights:
+    returns a channels-last fp32 [N, C_out, OH, OW] whose values equal ``int8_group_conv2d`` on ``x.contiguous()`` bit
+    for bit.  No workspace."""
+    lib = _lib.load()
+    g, n, out = _int8_conv_prelude("int8_group_conv2d_nhwc", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
+                                   dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, groups, stride, padding,
+                                   dilation, torch.channels_last)
+    with torch.cuda.device(x.device):
+        check(lib.sb200_int8_group_conv2d_nhwc(x.data_ptr(), ctypes.byref(g), int(groups), x_scale.data_ptr(),
+                                               x_zero_point.data_ptr(), int(qmin), int(qmax), w_q.data_ptr(),
+                                               w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
+                                               bias.data_ptr() if bias is not None else None, out.data_ptr(), n,
+                                               _stream(x)))
+    return out
+
 
 def gptq_matmul_dgrad(grad_out, qweight, grad_in, scales, zeros, bits, group_size=0, impl=None):
     """In-place ``grad_in += grad_out @ dequant(qweight).T``: the input gradient of ``gptq_matmul`` for 2 / 3 / 4-bit

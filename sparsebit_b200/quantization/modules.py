@@ -388,8 +388,11 @@ def int8_conv_ineligibility(qconv):
 
 class _Int8Conv2dModule:
     """The conv geometry and forward shared by the integer-grid conv modules: ``_set_geometry`` records it, a subclass
-    supplies ``_conv`` of a contiguous fp32 [N, C, H, W] input.  ``forward`` takes [N, C, H, W] or unbatched [C, H, W]
-    and up-casts fp16; the output is fp32."""
+    supplies ``_conv(x, nhwc)`` of an fp32 [N, C, H, W] input, contiguous (NCHW) or, with ``nhwc``, channels-last.
+    ``forward`` takes [N, C, H, W] or unbatched [C, H, W] and up-casts fp16; the output is fp32.  A batched input that is
+    channels-last (and not also NCHW-contiguous) runs the channels-last kernels and gets a channels-last output, as
+    ``F.conv2d`` returns; every other input, an unbatched one whatever its strides included, is made contiguous and
+    gets a contiguous output, as ``F.conv2d`` returns for it.  The values are the same."""
 
     def _set_geometry(self, in_channels, out_channels, kernel_size, stride, padding, dilation, groups=1):
         self.in_channels, self.out_channels, self.groups = int(in_channels), int(out_channels), int(groups)
@@ -412,7 +415,10 @@ class _Int8Conv2dModule:
         unbatched = x.dim() == 3
         if unbatched:
             x = x.unsqueeze(0)
-        y = self._conv(x.contiguous())
+        if not unbatched and x.dim() == 4 and x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous():
+            y = self._conv(x, True)
+        else:
+            y = self._conv(x.contiguous(), False)
         return y.squeeze(0) if unbatched else y
 
     def extra_repr(self):
@@ -440,10 +446,10 @@ class QConv2dInt8(_Int8Conv2dModule, _Int8WeightModule):
         *geometry, groups = cls._geometry_of(qconv)
         return cls(*geometry, device=qconv.weight.device, groups=groups)._load(qconv)
 
-    def _conv(self, x):
-        return ops.int8_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
-                               self.w_scale, self.w_zero, self.kernel_size, self.bias, self.stride, self.padding,
-                               self.dilation)
+    def _conv(self, x, nhwc):
+        op = ops.int8_conv2d_nhwc if nhwc else ops.int8_conv2d
+        return op(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum, self.w_scale, self.w_zero,
+                  self.kernel_size, self.bias, self.stride, self.padding, self.dilation)
 
 
 def int8_sparse24_conv_ineligibility(qconv):
@@ -471,10 +477,10 @@ class QConv2dSparse24Int8(_Int8Conv2dModule, _Sparse24WeightModule):
         *geometry, _ = cls._geometry_of(qconv)
         return cls(*geometry, device=qconv.weight.device)._load(qconv, operand)
 
-    def _conv(self, x):
-        return ops.int8_sparse24_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.vals, self.meta,
-                                        self.dsum, self.w_scale, self.kernel_size, self.bias, self.stride, self.padding,
-                                        self.dilation)
+    def _conv(self, x, nhwc):
+        op = ops.int8_sparse24_conv2d_nhwc if nhwc else ops.int8_sparse24_conv2d
+        return op(x, self.scale, self.zero_point, self.qmin, self.qmax, self.vals, self.meta, self.dsum, self.w_scale,
+                  self.kernel_size, self.bias, self.stride, self.padding, self.dilation)
 
     def extra_repr(self):
         return super().extra_repr() + ", 2:4 sparse"
@@ -509,10 +515,10 @@ class QConv2dGroupInt8(QConv2dInt8):
     def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation, groups, device):
         super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, device, groups)
 
-    def _conv(self, x):
-        return ops.int8_group_conv2d(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
-                                     self.w_scale, self.w_zero, self.kernel_size, self.groups, self.bias, self.stride,
-                                     self.padding, self.dilation)
+    def _conv(self, x, nhwc):
+        op = ops.int8_group_conv2d_nhwc if nhwc else ops.int8_group_conv2d
+        return op(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum, self.w_scale, self.w_zero,
+                  self.kernel_size, self.groups, self.bias, self.stride, self.padding, self.dilation)
 
     def extra_repr(self):
         return super().extra_repr() + f", groups={self.groups}"
