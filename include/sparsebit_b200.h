@@ -697,6 +697,42 @@ int sb200_int8_attention_masked(const float* q, const float* k, const float* v, 
                                 int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* ---- (5g) Integer-grid layers with a DoReFa input ------------------------------------------------------------------
+ * Replaces the chain of sparsebit/quantization/quantizers/dorefa.py:15-20 (t = tanh(x); x_n = t / max |t|; QDQ(x_n))
+ * feeding F.linear / F.conv2d when the layer's input quantizer is DoReFa: the lowering (or the grouped kernel) quantizes
+ * x_n = tanh(x) / *x_absmax in registers, with the op sequence of sb200_dorefa_fwd (libdevice tanhf, a true division),
+ * so that every output is bit-identical to the plain entry point run on sb200_dorefa_fwd(x, x_absmax, quantize = 0),
+ * NaNs included.  x_absmax: device, one float, max |tanh(x)| over the layer's whole input as sb200_dorefa_absmax writes
+ * it (the caller zeroes it and launches sb200_dorefa_absmax first, on the same stream).  A NaN in x makes *x_absmax
+ * NaN and an all-zero x makes it 0 (0 / 0 = NaN): either way every output is NaN, as in the fake-quant op.  Padding
+ * taps stay at the grid point of a real 0.
+ *
+ * Each takes its plain counterpart's arguments with x_absmax inserted after x_zero_point, makes the counterpart's checks
+ * in the same order with the same codes, then rejects a null x_absmax (SB200_E_INVALID), all before any CUDA call.  The
+ * workspace queries and layout are the counterpart's. */
+int sb200_int8_linear_dorefa(const float* x, const float* x_scale, const float* x_zero_point, const float* x_absmax,
+                             int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                             const int32_t* w_zero, const float* bias, float* out, int64_t m, int64_t k, int64_t n,
+                             void* workspace, size_t workspace_bytes, void* stream);
+int sb200_int8_conv2d_dorefa(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                             const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x, const int8_t* w_q,
+                             const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* bias,
+                             float* out, int64_t c_out, void* workspace, size_t workspace_bytes, void* stream);
+int sb200_int8_conv2d_nhwc_dorefa(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                                  const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x,
+                                  const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                                  const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+int sb200_int8_group_conv2d_dorefa(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                                   const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x,
+                                   const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                                   const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* stream);
+int sb200_int8_group_conv2d_nhwc_dorefa(const float* x, const sb200_conv2d_geom* geom, int64_t groups,
+                                        const float* x_scale, const float* x_zero_point, const float* x_absmax,
+                                        int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                                        const float* w_scale, const int32_t* w_zero, const float* bias, float* out,
+                                        int64_t c_out, void* stream);
+
 /* Force a GPTQ implementation for sb200_gptq4_matmul (process-wide; tests / benchmarking only -- prefer the
  * per-call sb200_gptq4_matmul_ex): 0 = auto, 1 = small-M path, 2 = wgmma kernel, 4 = scalar kernel; 3 is invalid. */
 int sb200_gptq4_set_impl(int impl);

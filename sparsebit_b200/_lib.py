@@ -122,6 +122,16 @@ PROTOTYPES = {
                                                 c_i64, c_vp, c_sz, c_vp]),
     "sb200_int8_group_conv2d_nhwc": (c_int, [c_vp, c_geom, c_i64, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
                                              c_vp, c_i64, c_vp]),
+    "sb200_int8_linear_dorefa": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64,
+                                         c_i64, c_vp, c_sz, c_vp]),
+    "sb200_int8_conv2d_dorefa": (c_int, [c_vp, c_geom, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                         c_i64, c_vp, c_sz, c_vp]),
+    "sb200_int8_conv2d_nhwc_dorefa": (c_int, [c_vp, c_geom, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                              c_vp, c_i64, c_vp, c_sz, c_vp]),
+    "sb200_int8_group_conv2d_dorefa": (c_int, [c_vp, c_geom, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                                               c_vp, c_vp, c_i64, c_vp]),
+    "sb200_int8_group_conv2d_nhwc_dorefa": (c_int, [c_vp, c_geom, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp,
+                                                    c_vp, c_vp, c_vp, c_i64, c_vp]),
     "sb200_int8_attention_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_i64]),
     "sb200_int8_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int,
                                      c_int, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,

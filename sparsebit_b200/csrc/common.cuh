@@ -189,6 +189,33 @@ __device__ __forceinline__ float qdq1(float x, const QP& p, int rounding) {
   return __fmul_rn(__fsub_rn(v, p.zp), p.s);
 }
 
+// DoReFa's normalised value tanh(x) / m (dorefa.py:16-17), m = max |tanh| over the tensor: libdevice tanhf (what
+// ATen's CUDA tanh calls), then the IEEE quotient (`tensor / 0-dim tensor` is a true division in ATen).  The one
+// sequence of the DoReFa kernels (dorefa.cu) and of the integer-grid kernels' DoReFa inputs (int8_grid.cuh); `t`
+// receives tanh(x).
+//
+// The quotient is RN32(RN64(t * rm)), rm = dorefa_rcp(m) hoisted out of the loop, as div_exact above: a binary32
+// quotient lies at least 2^-49 (relative) from every binary32 rounding midpoint, and rm is 1 / m within 2^-51 for every
+// finite nonzero m (a normal double even for a subnormal float m), so the product rounds to RN32(t / m) for every t,
+// zero, subnormal, infinite and NaN included.  rm comes from the approximate reciprocal and two Newton steps (error
+// 2^-20 -> 2^-40 -> under 2^-51) rather than rcp.rn / div.rn, whose slow-path calls make the integer-grid kernels spill
+// registers; the exact reciprocals of +-0 (+-inf) and +-inf (+-0) are set apart, and a NaN m gives a NaN rm.  So the
+// quotient equals __fdiv_rn(t, m) for every float m, not only the 0, (0, 1] or NaN that a max |tanh| can be.
+__device__ __forceinline__ double dorefa_rcp(float m) {
+  const double md = (double)m;
+  double r;
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(md));
+  r = __fma_rn(r, __fma_rn(-md, r, 1.0), r);
+  r = __fma_rn(r, __fma_rn(-md, r, 1.0), r);
+  if (m == 0.f) r = copysign(__longlong_as_double(0x7ff0000000000000LL), md);
+  if (isinf(m)) r = copysign(0.0, md);
+  return r;
+}
+__device__ __forceinline__ float dorefa_norm(float x, double rm, float& t) {
+  t = tanhf(x);
+  return __double2float_rn(__dmul_rn((double)t, rm));
+}
+
 // ---------------------------------------------------------------- mbarrier + TMA bulk copy (sm_90+)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {

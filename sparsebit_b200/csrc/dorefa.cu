@@ -9,7 +9,8 @@
 //   sb200_dorefa_fwd      y = QDQ(tanh(x) / m)  (or tanh(x) / m alone for the observer)   8 B/elem
 //   sb200_dorefa_bwd      gx = ((gy * [qmin <= round(xn / s) + zp <= qmax]) / m) * (1 - t^2)   12 B/elem
 // Same IEEE op sequence as the eager chain: libdevice tanhf (what ATen's CUDA tanh calls), a true division by m
-// (`tensor / 0-dim tensor` is a real division in ATen, not a reciprocal multiply), then quant_tensor.py:181-184.
+// (`tensor / 0-dim tensor` is a real division in ATen, not a reciprocal multiply: dorefa_norm of common.cuh gives that
+// IEEE quotient), then quant_tensor.py:181-184.
 // Weights are small (<= a few M elements), so these are plain chunked grid-stride kernels like adaround.cu.
 #include "common.cuh"
 
@@ -51,9 +52,9 @@ __global__ void __launch_bounds__(kThreads) dorefa_absmax_kernel(const float* __
 // OP 1: out = QDQ(tanh(x) / m)       (dorefa.py:15-20)
 // OP 2: out = d loss / d x given gy  (autograd of the same chain; scale / zero_point are buffers there: no gs / gzp)
 template <int OP>
-__device__ __forceinline__ float one_elem(float x, float gy, const QP& p, float m) {
-  const float t = tanhf(x);
-  const float xn = __fdiv_rn(t, m);
+__device__ __forceinline__ float one_elem(float x, float gy, const QP& p, float m, double rm) {
+  float t;
+  const float xn = dorefa_norm(x, rm, t);
   if (OP == 0) return xn;
   if (OP == 1) return qdq1<0>(xn, p, 0);
   const float vq = __fadd_rn(round_q<0>(div_exact(xn, p), 0), p.zp);
@@ -71,6 +72,7 @@ __global__ void __launch_bounds__(kThreads) dorefa_kernel(const float* __restric
   const long long chunks_per_row = (inner + kChunk - 1) / kChunk;
   const long long total = rows * chunks_per_row;
   const float m = __ldg(absmax);
+  const double rm = dorefa_rcp(m);
   for (long long tix = blockIdx.x; tix < total; tix += gridDim.x) {
     const long long row = tix / chunks_per_row;
     const long long k0 = (tix - row * chunks_per_row) * kChunk;
@@ -86,15 +88,15 @@ __global__ void __launch_bounds__(kThreads) dorefa_kernel(const float* __restric
         const float4 xv = *reinterpret_cast<const float4*>(x + base + k);
         float4 gv = make_float4(0.f, 0.f, 0.f, 0.f), o;
         if (OP == 2) gv = *reinterpret_cast<const float4*>(gy + base + k);
-        o.x = one_elem<OP>(xv.x, gv.x, p, m); o.y = one_elem<OP>(xv.y, gv.y, p, m);
-        o.z = one_elem<OP>(xv.z, gv.z, p, m); o.w = one_elem<OP>(xv.w, gv.w, p, m);
+        o.x = one_elem<OP>(xv.x, gv.x, p, m, rm); o.y = one_elem<OP>(xv.y, gv.y, p, m, rm);
+        o.z = one_elem<OP>(xv.z, gv.z, p, m, rm); o.w = one_elem<OP>(xv.w, gv.w, p, m, rm);
         *reinterpret_cast<float4*>(out + base + k) = o;
       }
     } else {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const long long k = threadIdx.x + (long long)j * kThreads;
-        if (k < left) out[base + k] = one_elem<OP>(x[base + k], OP == 2 ? gy[base + k] : 0.f, p, m);
+        if (k < left) out[base + k] = one_elem<OP>(x[base + k], OP == 2 ? gy[base + k] : 0.f, p, m, rm);
       }
     }
   }

@@ -18,6 +18,20 @@ __device__ __forceinline__ int stored_grid(float v, const QP& p, int off, bool& 
   return (int)g - off;
 }
 
+// The stored grid value of an activation element v: stored_grid(v), or, kDoReFa, stored_grid of DoReFa's normalised
+// tanh(v) / m (dorefa_norm of common.cuh, the op sequence of sb200_dorefa_fwd), m = max |tanh| over the whole input,
+// rm = dorefa_rcp(m).
+// A NaN m, or m = 0 (an all-zero input: 0 / 0), makes every element NaN, as in the fake-quant op.  Padding taps are
+// not elements: they stay at the grid point of a real 0.
+template <bool kDoReFa>
+__device__ __forceinline__ int input_grid(float v, double rm, const QP& p, int off, bool& nan) {
+  if constexpr (kDoReFa) {
+    float t;
+    v = dorefa_norm(v, rm, t);
+  }
+  return stored_grid(v, p, off, nan);
+}
+
 // The s8 storage offset: a grid value g is stored as g - off, off = 128 for unsigned ranges and 0 otherwise.
 static inline int grid_offset(int qmin) { return qmin >= 0 ? 128 : 0; }
 
@@ -39,6 +53,13 @@ static inline int check_workspace(const char* fn, size_t have, size_t need) {
   if (have >= need) return SB200_OK;
   set_error("%s: workspace too small (%zu bytes, need %zu)", fn, have, need);
   return SB200_E_WORKSPACE;
+}
+
+// The _dorefa entry points make every check of their plain counterpart, then this one: a null x_absmax is
+// SB200_E_INVALID (dorefa = false: the plain entry point, nothing to check).
+static inline int check_absmax(const char* fn, bool dorefa, const float* x_absmax) {
+  SB_REQUIRE(!dorefa || x_absmax, "%s: null x_absmax", fn);
+  return SB200_OK;
 }
 
 // |a|, |b| <= 128 on the stored grid: the s32 accumulator holds |sum a b| <= K * 2^14 for K < 2^17
@@ -70,13 +91,16 @@ int check_k(const char* fn, long long k);
 int check_conv(const char* fn, const sb200_conv2d_geom* g, ConvDims* d);
 // The lowering launches: the row quantizer (x [rows, K], per-tensor or per-row qparams) and the conv2d lowering
 // (one row per output pixel).  Unchecked: the caller has made every check of sb200_int8_quantize_rows /
-// sb200_int8_im2col_quantize, q included (16-byte aligned).
+// sb200_int8_im2col_quantize, q included (16-byte aligned).  x_absmax: NULL, or the device m of a DoReFa input
+// (input_grid<true>).
 int launch_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax, int8_t* q,
-                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st);
+                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st,
+                const float* x_absmax = nullptr);
 int launch_im2col(const float* x, const ConvDims& d, const float* scale, const float* zero_point, int qmin, int qmax,
-                  int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st);
+                  int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st, const float* x_absmax = nullptr);
 // The same lowering of an x stored NHWC with c channels; a stride-1, unpadded 1 x 1 conv runs the row quantizer.
 int launch_im2col_nhwc(const float* x, const ConvDims& d, int c, const float* scale, const float* zero_point, int qmin,
-                       int qmax, int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st);
+                       int qmax, int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st,
+                       const float* x_absmax = nullptr);
 
 }  // namespace sb200

@@ -67,7 +67,8 @@ __device__ __forceinline__ float gc_epilogue(int acc, int sa, int n, long long z
 }
 
 // Does the window of output (img, oh, ow) over channels [c0, c0 + cn) hold an element whose grid value is NaN?
-__device__ bool gc_window_nan(const float* __restrict__ x, const GcDims& d, const QP& p, int off, long long img,
+template <bool kDoReFa>
+__device__ bool gc_window_nan(const float* __restrict__ x, const GcDims& d, const QP& p, int off, double xm, long long img,
                               long long c0, int cn, long long oh, long long ow) {
   bool nan = false;
   for (int c = 0; c < cn; ++c) {
@@ -77,7 +78,8 @@ __device__ bool gc_window_nan(const float* __restrict__ x, const GcDims& d, cons
       if ((unsigned long long)ih >= (unsigned long long)d.H) continue;
       for (int kw = 0; kw < d.KW; ++kw) {
         const long long iw = ow * d.sw - d.pl + (long long)kw * d.dw;
-        if ((unsigned long long)iw < (unsigned long long)d.W) (void)stored_grid(__ldg(xc + ih * d.W + iw), p, off, nan);
+        if ((unsigned long long)iw < (unsigned long long)d.W)
+          (void)input_grid<kDoReFa>(__ldg(xc + ih * d.W + iw), xm, p, off, nan);
       }
     }
   }
@@ -86,9 +88,9 @@ __device__ bool gc_window_nan(const float* __restrict__ x, const GcDims& d, cons
 
 // Stage the stored grid of the input window [ih_lo, ih_lo + TIH) x [iw_lo, iw_lo + TIW) of `cq` channels: put(cl, r,
 // col, value) stores one element; channel cl is real when cl < creal (else it stores 0); c0 is the first channel.
-template <typename Put>
-__device__ __forceinline__ bool gc_stage(const float* __restrict__ x, const GcDims& d, const QP& p, int off, int pad,
-                                         long long img, long long c0, int cq, int creal, long long ih_lo, long long iw_lo,
+template <bool kDoReFa, typename Put>
+__device__ __forceinline__ bool gc_stage(const float* __restrict__ x, const GcDims& d, const QP& p, int off, double xm,
+                                         int pad, long long img, long long c0, int cq, int creal, long long ih_lo, long long iw_lo,
                                          Put put) {
   bool nan = false;
   if (d.vec) {
@@ -103,8 +105,8 @@ __device__ __forceinline__ bool gc_stage(const float* __restrict__ x, const GcDi
         e[0] = e[1] = e[2] = e[3] = 0;
       } else if ((unsigned long long)ih < (unsigned long long)d.H && gc >= 0 && gc < d.W) {
         const float4 f = __ldg(reinterpret_cast<const float4*>(x + ((img * d.C + c0 + cl) * d.H + ih) * d.W + gc));
-        e[0] = stored_grid(f.x, p, off, nan), e[1] = stored_grid(f.y, p, off, nan);
-        e[2] = stored_grid(f.z, p, off, nan), e[3] = stored_grid(f.w, p, off, nan);
+        e[0] = input_grid<kDoReFa>(f.x, xm, p, off, nan), e[1] = input_grid<kDoReFa>(f.y, xm, p, off, nan);
+        e[2] = input_grid<kDoReFa>(f.z, xm, p, off, nan), e[3] = input_grid<kDoReFa>(f.w, xm, p, off, nan);
       } else {
         e[0] = e[1] = e[2] = e[3] = pad;
       }
@@ -122,7 +124,7 @@ __device__ __forceinline__ bool gc_stage(const float* __restrict__ x, const GcDi
       int e = 0;
       if (cl < creal) {
         if ((unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W)
-          e = stored_grid(__ldg(x + ((img * d.C + c0 + cl) * d.H + ih) * d.W + iw), p, off, nan);
+          e = input_grid<kDoReFa>(__ldg(x + ((img * d.C + c0 + cl) * d.H + ih) * d.W + iw), xm, p, off, nan);
         else
           e = pad;
       }
@@ -132,8 +134,11 @@ __device__ __forceinline__ bool gc_stage(const float* __restrict__ x, const GcDi
   return nan;
 }
 
-template <int kMode>
-__global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float* __restrict__ x, GcDims d,
+// kDoReFa: x is a DoReFa input normalised by *x_absmax (input_grid of int8_grid.cuh), in every path.
+// The DoReFa kGrouped instantiation asks for 4 CTAs per SM (64 registers, as the plain one): without the hint ptxas
+// spills a few words of it to reach its own occupancy target.  Every other instantiation has no hint.
+template <int kMode, bool kDoReFa>
+__global__ void __launch_bounds__(kGcThreads, kDoReFa && kMode == kGrouped ? 4 : 0) int8_group_conv_kernel(const float* __restrict__ x, GcDims d,
                                                                      const float* __restrict__ x_scale,
                                                                      const float* __restrict__ x_zero, float qmin,
                                                                      float qmax, int off, const int8_t* __restrict__ w_q,
@@ -141,7 +146,8 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
                                                                      const float* __restrict__ w_scale,
                                                                      const int* __restrict__ w_zero,
                                                                      const float* __restrict__ bias,
-                                                                     float* __restrict__ out) {
+                                                                     float* __restrict__ out,
+                                                                     const float* __restrict__ x_absmax) {
   extern __shared__ __align__(16) unsigned char gc_smem[];
   QP p;
   p.set(__ldg(x_scale), __ldg(x_zero));
@@ -150,6 +156,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
   const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
   const float sx = __ldg(x_scale);
   const long long zx = (long long)rintf(__ldg(x_zero)) - off;
+  const double xm = kDoReFa ? dorefa_rcp(__ldg(x_absmax)) : 0.0;  // 1 / m of a DoReFa input
   const int taps = d.KH * d.KW;
   const long long plane = d.OH * d.OW;
 
@@ -172,7 +179,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
             const long long iw = ow * d.sw - d.pl + (long long)kw * d.dw;
             int a = pad;
             if ((unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W)
-              a = stored_grid(__ldg(xc + ih * d.W + iw), p, off, nan);
+              a = input_grid<kDoReFa>(__ldg(xc + ih * d.W + iw), xm, p, off, nan);
             a = (int)(int8_t)a;  // the s8 the staged paths and the conv2d lowering store
             acc += a * (int)__ldg(wr + c * taps + kh * d.KW + kw);
             sa += a;
@@ -218,7 +225,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
           const int ol = i / taps, k = i - ol * taps;
           ws[i] = __ldg(w_q + (n0 + ol) * d.Kp + k);
         }
-        nan = gc_stage(x, d, p, off, pad, img, c0, d.CB, creal, ih_lo, iw_lo,
+        nan = gc_stage<kDoReFa>(x, d, p, off, xm, pad, img, c0, d.CB, creal, ih_lo, iw_lo,
                        [&](int cl, int r, int col, int e) { xs[cl * tplane + r * d.TIW + col] = (int8_t)e; });
       } else {
         uint32_t* xs = reinterpret_cast<uint32_t*>(gc_smem);
@@ -238,7 +245,8 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
           ws[i] = wv;
         }
         unsigned char* xb = gc_smem;
-        nan = gc_stage(x, d, p, off, pad, img, c0, 4 * d.C4, creal, ih_lo, iw_lo, [&](int cl, int r, int col, int e) {
+        nan = gc_stage<kDoReFa>(x, d, p, off, xm, pad, img, c0, 4 * d.C4, creal, ih_lo, iw_lo,
+                                [&](int cl, int r, int col, int e) {
           xb[(((cl >> 2) * tplane + r * d.TIW + col) << 2) + (cl & 3)] = (unsigned char)e;
         });
       }
@@ -277,7 +285,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
             const long long oh = oh0 + ph, ow = ow0 + pw;
             if (oh >= d.OH || ow >= d.OW) continue;
             const long long n = n0 + ol[r];
-            const bool wn = any_nan && gc_window_nan(x, d, p, off, img, c0 + ol[r] / d.Mg, 1, oh, ow);
+            const bool wn = any_nan && gc_window_nan<kDoReFa>(x, d, p, off, xm, img, c0 + ol[r] / d.Mg, 1, oh, ow);
             out[((img * d.Cout + n) * d.OH + oh) * d.OW + ow] =
                 gc_epilogue(acc[r], sa[r], (int)n, zx, sx, d.Kg, w_sum, w_scale, w_zero, bias, wn);
           }
@@ -321,7 +329,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_kernel(const float
             const int px = i - oq[r] * tile_pix, ph = px / d.TW, pw = px - ph * d.TW;
             const long long oh = oh0 + ph, ow = ow0 + pw;
             if (oh >= d.OH || ow >= d.OW) continue;
-            const bool wn = any_nan && gc_window_nan(x, d, p, off, img, c0, d.Cg, oh, ow);
+            const bool wn = any_nan && gc_window_nan<kDoReFa>(x, d, p, off, xm, img, c0, d.Cg, oh, ow);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
               const int ol = 4 * oq[r] + j;
@@ -433,8 +441,10 @@ __device__ __forceinline__ void nh_store(float* __restrict__ out, const NhDims& 
   }
 }
 
-template <int kMode>
-__global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const float* __restrict__ x, NhDims d,
+// The DoReFa kNhAny instantiation asks for 3 CTAs per SM (72 registers, as the plain one), which keeps ptxas from
+// spilling it to a smaller register count; every other instantiation has no hint.
+template <int kMode, bool kDoReFa>
+__global__ void __launch_bounds__(kGcThreads, kDoReFa && kMode == kNhAny ? 3 : 0) int8_group_conv_nhwc_kernel(const float* __restrict__ x, NhDims d,
                                                                           const float* __restrict__ x_scale,
                                                                           const float* __restrict__ x_zero, float qmin,
                                                                           float qmax, int off,
@@ -443,7 +453,8 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const 
                                                                           const float* __restrict__ w_scale,
                                                                           const int* __restrict__ w_zero,
                                                                           const float* __restrict__ bias,
-                                                                          float* __restrict__ out) {
+                                                                          float* __restrict__ out,
+                                                                          const float* __restrict__ x_absmax) {
   extern __shared__ __align__(16) unsigned char gc_smem[];
   uint32_t* ws = reinterpret_cast<uint32_t*>(gc_smem);
   QP p;
@@ -453,6 +464,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const 
   const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
   const float sx = __ldg(x_scale);
   const long long zx = (long long)rintf(__ldg(x_zero)) - off;
+  const double xm = kDoReFa ? dorefa_rcp(__ldg(x_absmax)) : 0.0;  // 1 / m of a DoReFa input
   const int taps = d.KH * d.KW;
   const int ql = threadIdx.x % d.QB, slot = threadIdx.x / d.QB, pstride = kGcThreads / d.QB;
   long long staged = -1;
@@ -521,7 +533,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const 
                 for (int j = 0; j < 4; ++j) v[j] = n0 + j < d.C ? __ldg(xp + j) : 0.f;
               }
 #pragma unroll
-              for (int j = 0; j < 4; ++j) a[j] = (int)(int8_t)stored_grid(v[j], p, off, nan[j]);
+              for (int j = 0; j < 4; ++j) a[j] = (int)(int8_t)input_grid<kDoReFa>(v[j], xm, p, off, nan[j]);
             } else {
 #pragma unroll
               for (int j = 0; j < 4; ++j) a[j] = (int)(int8_t)pad;
@@ -565,10 +577,10 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const 
                   f.z = live > 2 ? __ldg(xp + 4 * c4 + 2) : 0.f;
                   f.w = live > 3 ? __ldg(xp + 4 * c4 + 3) : 0.f;
                 }
-                a4 = ((uint32_t)stored_grid(f.x, p, off, nan) & 0xFFu);
-                if (live > 1) a4 |= ((uint32_t)stored_grid(f.y, p, off, nan) & 0xFFu) << 8;
-                if (live > 2) a4 |= ((uint32_t)stored_grid(f.z, p, off, nan) & 0xFFu) << 16;
-                if (live > 3) a4 |= ((uint32_t)stored_grid(f.w, p, off, nan) & 0xFFu) << 24;
+                a4 = ((uint32_t)input_grid<kDoReFa>(f.x, xm, p, off, nan) & 0xFFu);
+                if (live > 1) a4 |= ((uint32_t)input_grid<kDoReFa>(f.y, xm, p, off, nan) & 0xFFu) << 8;
+                if (live > 2) a4 |= ((uint32_t)input_grid<kDoReFa>(f.z, xm, p, off, nan) & 0xFFu) << 16;
+                if (live > 3) a4 |= ((uint32_t)input_grid<kDoReFa>(f.w, xm, p, off, nan) & 0xFFu) << 24;
               } else {
                 a4 = ((uint32_t)pad & 0xFFu) * 0x01010101u;
                 if (live < 4) a4 &= 0xFFFFFFFFu >> (8 * (4 - live));
@@ -601,7 +613,7 @@ __global__ void __launch_bounds__(kGcThreads) int8_group_conv_nhwc_kernel(const 
               const float* xp = xi + (ih * d.W + iw) * d.C + c0;
               const int k = kh * d.KW + kw;
               for (int c = 0; c < d.Cg; ++c) {
-                const int a = (int)(int8_t)(in ? stored_grid(__ldg(xp + c), p, off, nan) : pad);
+                const int a = (int)(int8_t)(in ? input_grid<kDoReFa>(__ldg(xp + c), xm, p, off, nan) : pad);
                 acc += a * (int)__ldg(wr + c * taps + k);
                 sa += a;
               }
@@ -654,29 +666,43 @@ int nh_plan(NhDims* d, const float* x, const float* out) {
 
 using namespace sb200;
 
-int sb200_int8_group_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
-                                 const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q,
-                                 const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* bias,
-                                 float* out, int64_t c_out, void* stream) {
-  const char* fn = "sb200_int8_group_conv2d_nhwc";
+// The checks of sb200_int8_group_conv2d{,_nhwc}, in order, then (dorefa) check_absmax; fills the conv geometry and K_g.
+static int group_conv_checks(const char* fn, const char* dense_fn, bool dorefa, const float* x,
+                             const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                             const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x, const int8_t* w_q,
+                             const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* out,
+                             int64_t c_out, ConvDims* cd, long long* kg) {
   SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out,
              "%s: null pointer argument", fn);
   SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
   SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
-  SB_REQUIRE(groups >= 2, "%s: groups = %lld; a conv with groups = 1 runs on sb200_int8_conv2d_nhwc", fn,
-             (long long)groups);
-  ConvDims cd;
-  if (const int rc = check_conv(fn, geom, &cd)) return rc;
+  SB_REQUIRE(groups >= 2, "%s: groups = %lld; a conv with groups = 1 runs on %s", fn, (long long)groups, dense_fn);
+  if (const int rc = check_conv(fn, geom, cd)) return rc;
   const sb200_conv2d_geom& g = *geom;
   SB_REQUIRE(g.c % groups == 0 && c_out % groups == 0, "%s: groups = %lld does not divide c = %lld and c_out = %lld", fn,
              (long long)groups, (long long)g.c, (long long)c_out);
   if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
-  const long long kg = (g.c / groups) * g.kh * g.kw;
+  *kg = (g.c / groups) * g.kh * g.kw;  // c, kh, kw < 2^31 each: c / groups * kh stays far below 2^63 / kw
   if ((__int128)(g.c / groups) * g.kh * g.kw >= kI8MaxK) {
     set_error("%s: K_g = c / groups kh kw = %lld x %lld x %lld >= 2^17, the integer path supports K_g < 2^17 (|sum| <= "
               "K_g * 2^14 must fit int32)", fn, (long long)(g.c / groups), (long long)g.kh, (long long)g.kw);
     return SB200_E_UNSUPPORTED;
   }
+  return check_absmax(fn, dorefa, x_absmax);
+}
+
+// sb200_int8_group_conv2d_nhwc (dorefa = false) and sb200_int8_group_conv2d_nhwc_dorefa
+static int group_conv_nhwc_entry(const char* fn, bool dorefa, const float* x, const sb200_conv2d_geom* geom,
+                                 int64_t groups, const float* x_scale, const float* x_zero_point, const float* x_absmax,
+                                 int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                                 const float* w_scale, const int32_t* w_zero, const float* bias, float* out,
+                                 int64_t c_out, void* stream) {
+  ConvDims cd;
+  long long kg;
+  if (const int rc = group_conv_checks(fn, "sb200_int8_conv2d_nhwc", dorefa, x, geom, groups, x_scale, x_zero_point,
+                                       x_absmax, qmin_x, qmax_x, w_q, w_rowsum, w_scale, w_zero, out, c_out, &cd, &kg))
+    return rc;
+  const sb200_conv2d_geom& g = *geom;
   NhDims d{};
   d.M = cd.M, d.P = cd.P, d.OW = cd.OW, d.H = g.h, d.W = g.w, d.C = g.c, d.Cout = c_out;
   d.Cg = (int)(g.c / groups), d.Mg = (int)(c_out / groups);
@@ -686,48 +712,29 @@ int sb200_int8_group_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, 
   const int mode = nh_plan(&d, x, out);
   const unsigned grid = (unsigned)min(d.ctas, kGcMaxGrid);
   const size_t smem = (size_t)nh_smem_bytes(mode, d);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int off = grid_offset(qmin_x);
-  const int* wsum = reinterpret_cast<const int*>(w_rowsum);
-  const int* wzero = reinterpret_cast<const int*>(w_zero);
-  if (mode == kNhDw)
-    int8_group_conv_nhwc_kernel<kNhDw><<<grid, kGcThreads, smem, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
-                                                                      (float)qmax_x, off, w_q, wsum, w_scale, wzero, bias,
-                                                                      out);
-  else if (mode == kNhQuad)
-    int8_group_conv_nhwc_kernel<kNhQuad><<<grid, kGcThreads, smem, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
-                                                                        (float)qmax_x, off, w_q, wsum, w_scale, wzero,
-                                                                        bias, out);
-  else
-    int8_group_conv_nhwc_kernel<kNhAny><<<grid, kGcThreads, 0, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
-                                                                    (float)qmax_x, off, w_q, wsum, w_scale, wzero, bias,
-                                                                    out);
+  const bool df = x_absmax != nullptr;
+  const auto kernel = mode == kNhDw    ? (df ? int8_group_conv_nhwc_kernel<kNhDw, true> : int8_group_conv_nhwc_kernel<kNhDw, false>)
+                      : mode == kNhQuad ? (df ? int8_group_conv_nhwc_kernel<kNhQuad, true> : int8_group_conv_nhwc_kernel<kNhQuad, false>)
+                                        : (df ? int8_group_conv_nhwc_kernel<kNhAny, true> : int8_group_conv_nhwc_kernel<kNhAny, false>);
+  kernel<<<grid, kGcThreads, smem, (cudaStream_t)stream>>>(x, d, x_scale, x_zero_point, (float)qmin_x, (float)qmax_x,
+                                                           grid_offset(qmin_x), w_q, reinterpret_cast<const int*>(w_rowsum),
+                                                           w_scale, reinterpret_cast<const int*>(w_zero), bias, out,
+                                                           x_absmax);
   SB_LAUNCHED();
   return SB200_OK;
 }
 
-int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
-                            const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
-                            const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
-                            void* stream) {
-  const char* fn = "sb200_int8_group_conv2d";
-  SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out,
-             "%s: null pointer argument", fn);
-  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
-  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
-  SB_REQUIRE(groups >= 2, "%s: groups = %lld; a conv with groups = 1 runs on sb200_int8_conv2d", fn, (long long)groups);
+// sb200_int8_group_conv2d (dorefa = false) and sb200_int8_group_conv2d_dorefa
+static int group_conv_entry(const char* fn, bool dorefa, const float* x, const sb200_conv2d_geom* geom, int64_t groups,
+                            const float* x_scale, const float* x_zero_point, const float* x_absmax, int qmin_x,
+                            int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                            const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* stream) {
   ConvDims cd;
-  if (const int rc = check_conv(fn, geom, &cd)) return rc;
+  long long kg;
+  if (const int rc = group_conv_checks(fn, "sb200_int8_conv2d", dorefa, x, geom, groups, x_scale, x_zero_point, x_absmax,
+                                       qmin_x, qmax_x, w_q, w_rowsum, w_scale, w_zero, out, c_out, &cd, &kg))
+    return rc;
   const sb200_conv2d_geom& g = *geom;
-  SB_REQUIRE(g.c % groups == 0 && c_out % groups == 0, "%s: groups = %lld does not divide c = %lld and c_out = %lld", fn,
-             (long long)groups, (long long)g.c, (long long)c_out);
-  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
-  const long long kg = (g.c / groups) * g.kh * g.kw;  // c, kh, kw < 2^31 each: c / groups * kh stays far below 2^63 / kw
-  if ((__int128)(g.c / groups) * g.kh * g.kw >= kI8MaxK) {
-    set_error("%s: K_g = c / groups kh kw = %lld x %lld x %lld >= 2^17, the integer path supports K_g < 2^17 (|sum| <= "
-              "K_g * 2^14 must fit int32)", fn, (long long)(g.c / groups), (long long)g.kh, (long long)g.kw);
-    return SB200_E_UNSUPPORTED;
-  }
   GcDims d{};
   d.N = g.n, d.C = g.c, d.H = g.h, d.W = g.w, d.Cout = c_out, d.OH = cd.P / cd.OW, d.OW = cd.OW;
   d.Cg = (int)(g.c / groups), d.Mg = (int)(c_out / groups);
@@ -735,26 +742,55 @@ int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64
   d.dh = (int)g.dilation_h, d.dw = (int)g.dilation_w, d.pt = (int)g.pad_top, d.pl = (int)g.pad_left;
   d.Kg = (int)kg, d.Kp = (int)padded_k(kg);
   const int mode = gc_plan(&d, x);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int off = grid_offset(qmin_x);
+  unsigned grid;
+  size_t smem = 0;
   if (mode == kDirect) {
-    const long long total = d.N * d.Cout * d.OH * d.OW;
-    const unsigned grid = (unsigned)min(cdiv(total, kGcThreads), kGcMaxGrid);
-    int8_group_conv_kernel<kDirect><<<grid, kGcThreads, 0, st>>>(x, d, x_scale, x_zero_point, (float)qmin_x,
-                                                                (float)qmax_x, off, w_q, reinterpret_cast<const int*>(w_rowsum),
-                                                                w_scale, reinterpret_cast<const int*>(w_zero), bias, out);
+    grid = (unsigned)min(cdiv(d.N * d.Cout * d.OH * d.OW, kGcThreads), kGcMaxGrid);
   } else {
-    const unsigned grid = (unsigned)min(d.ctas, kGcMaxGrid);
-    const size_t smem = (size_t)gc_smem_bytes(mode, d);
-    if (mode == kDepthwise)
-      int8_group_conv_kernel<kDepthwise><<<grid, kGcThreads, smem, st>>>(
-          x, d, x_scale, x_zero_point, (float)qmin_x, (float)qmax_x, off, w_q, reinterpret_cast<const int*>(w_rowsum),
-          w_scale, reinterpret_cast<const int*>(w_zero), bias, out);
-    else
-      int8_group_conv_kernel<kGrouped><<<grid, kGcThreads, smem, st>>>(
-          x, d, x_scale, x_zero_point, (float)qmin_x, (float)qmax_x, off, w_q, reinterpret_cast<const int*>(w_rowsum),
-          w_scale, reinterpret_cast<const int*>(w_zero), bias, out);
+    grid = (unsigned)min(d.ctas, kGcMaxGrid);
+    smem = (size_t)gc_smem_bytes(mode, d);
   }
+  const bool df = x_absmax != nullptr;
+  const auto kernel = mode == kDirect      ? (df ? int8_group_conv_kernel<kDirect, true> : int8_group_conv_kernel<kDirect, false>)
+                      : mode == kDepthwise ? (df ? int8_group_conv_kernel<kDepthwise, true> : int8_group_conv_kernel<kDepthwise, false>)
+                                           : (df ? int8_group_conv_kernel<kGrouped, true> : int8_group_conv_kernel<kGrouped, false>);
+  kernel<<<grid, kGcThreads, smem, (cudaStream_t)stream>>>(x, d, x_scale, x_zero_point, (float)qmin_x, (float)qmax_x,
+                                                           grid_offset(qmin_x), w_q, reinterpret_cast<const int*>(w_rowsum),
+                                                           w_scale, reinterpret_cast<const int*>(w_zero), bias, out,
+                                                           x_absmax);
   SB_LAUNCHED();
   return SB200_OK;
+}
+
+int sb200_int8_group_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                                 const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q,
+                                 const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* bias,
+                                 float* out, int64_t c_out, void* stream) {
+  return group_conv_nhwc_entry("sb200_int8_group_conv2d_nhwc", false, x, geom, groups, x_scale, x_zero_point, nullptr,
+                               qmin_x, qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, stream);
+}
+
+int sb200_int8_group_conv2d_nhwc_dorefa(const float* x, const sb200_conv2d_geom* geom, int64_t groups,
+                                        const float* x_scale, const float* x_zero_point, const float* x_absmax,
+                                        int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                                        const float* w_scale, const int32_t* w_zero, const float* bias, float* out,
+                                        int64_t c_out, void* stream) {
+  return group_conv_nhwc_entry("sb200_int8_group_conv2d_nhwc_dorefa", true, x, geom, groups, x_scale, x_zero_point,
+                               x_absmax, qmin_x, qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, stream);
+}
+
+int sb200_int8_group_conv2d(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                            const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                            const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
+                            void* stream) {
+  return group_conv_entry("sb200_int8_group_conv2d", false, x, geom, groups, x_scale, x_zero_point, nullptr, qmin_x,
+                          qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, stream);
+}
+
+int sb200_int8_group_conv2d_dorefa(const float* x, const sb200_conv2d_geom* geom, int64_t groups, const float* x_scale,
+                                   const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x,
+                                   const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                                   const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* stream) {
+  return group_conv_entry("sb200_int8_group_conv2d_dorefa", true, x, geom, groups, x_scale, x_zero_point, x_absmax,
+                          qmin_x, qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, stream);
 }

@@ -77,13 +77,17 @@ struct I8MmSmem {
 // column quantizer and the conv2d lowering are the same per element.
 
 // 8 warps per CTA, one row per warp; lane l handles the 16-element chunks starting at 16 l, 16 (l + 32), ...
+// kDoReFa: x is a DoReFa input normalised by *x_absmax (input_grid), as in every lowering below.
+template <bool kDoReFa>
 __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __restrict__ x, const float* __restrict__ scale,
                                                                  const float* __restrict__ zero_point, int per_row, float qmin,
                                                                  float qmax, int off, int8_t* __restrict__ q,
                                                                  int* __restrict__ row_sum, uint8_t* __restrict__ nan_flag,
-                                                                 long long rows, int K, int Kp, int vec) {
+                                                                 long long rows, int K, int Kp, int vec,
+                                                                 const float* __restrict__ x_absmax) {
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= rows) return;
+  const double xm = kDoReFa ? dorefa_rcp(__ldg(x_absmax)) : 0.0;  // 1 / m of a DoReFa input
   const int lane = threadIdx.x & 31;
   QP p;
   const long long pi = per_row ? row : 0;
@@ -110,7 +114,7 @@ __global__ void __launch_bounds__(256) int8_quantize_rows_kernel(const float* __
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       int e = 0;  // K padding stays zero
-      if (c + i < K) e = stored_grid(v[i], p, off, nan);
+      if (c + i < K) e = input_grid<kDoReFa>(v[i], xm, p, off, nan);
       sum += e;
       packed[i >> 2] |= ((uint32_t)e & 0xFFu) << (8 * (i & 3));
     }
@@ -231,13 +235,17 @@ constexpr int kLowThreads = 256;
 // group of 4 taps of the chunk: a warp reads one tap of 32 consecutive pixels (consecutive ow: coalesced along the
 // row of x), packs 4 taps per word into a shared tile, and the tile leaves as whole 16-byte pieces of rows of q.
 // Row sums and NaN flags stay in registers across the chunks.
-__global__ void __launch_bounds__(kLowThreads) int8_im2col_quantize_kernel(const float* __restrict__ x, ConvDims d,
+// kDoReFa: at least 5 CTAs per SM (48 registers).  Left to its own occupancy target ptxas holds the DoReFa instantiation
+// at 40 registers and spills a few loop-invariant words; the plain one (minimum 0: no hint) is unchanged.
+template <bool kDoReFa>
+__global__ void __launch_bounds__(kLowThreads, kDoReFa ? 5 : 0) int8_im2col_quantize_kernel(const float* __restrict__ x, ConvDims d,
                                                                            const float* __restrict__ scale,
                                                                            const float* __restrict__ zero_point,
                                                                            float qmin, float qmax, int off,
                                                                            int8_t* __restrict__ q,
                                                                            int* __restrict__ row_sum,
-                                                                           uint8_t* __restrict__ nan_flag) {
+                                                                           uint8_t* __restrict__ nan_flag,
+                                                                           const float* __restrict__ x_absmax) {
   __shared__ uint32_t tile[kLowPix * kLowWords];
   __shared__ long long tap_off[kLowK], tap_dh[kLowK], tap_dw[kLowK];  // per tap of the chunk: x offset, row, column
   __shared__ int part_sum[kLowThreads];
@@ -258,6 +266,7 @@ __global__ void __launch_bounds__(kLowThreads) int8_im2col_quantize_kernel(const
   p.qmin = qmin;
   p.qmax = qmax;
   const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
+  const double xm = kDoReFa ? dorefa_rcp(__ldg(x_absmax)) : 0.0;  // 1 / m of a DoReFa input
   int sum = 0;
   bool nan = false;
   for (int k0 = 0; k0 < d.Kp; k0 += kLowK) {
@@ -284,7 +293,7 @@ __global__ void __launch_bounds__(kLowThreads) int8_im2col_quantize_kernel(const
         if (live && k0 + kl < d.K) {
           const long long ih = ih0 + tap_dh[kl], iw = iw0 + tap_dw[kl];
           if ((unsigned long long)ih < (unsigned long long)d.H && (unsigned long long)iw < (unsigned long long)d.W)
-            e = stored_grid(__ldg(x + org + tap_off[kl]), p, off, nan);
+            e = input_grid<kDoReFa>(__ldg(x + org + tap_off[kl]), xm, p, off, nan);
           else
             e = pad;
         }
@@ -330,6 +339,7 @@ constexpr int kNhRowsMinK = 256;  // a stride-1 unpadded 1 x 1 conv with c >= th
 // channels -- and stores each element whose k = c KH KW + tap lies in the chunk into the pixel's row of the shared
 // tile, adding it to the pixel's row sum (integer, so the order of the shared-memory adds does not matter).  The tile
 // then leaves as 16-byte pieces of rows of q, K padding zeroed.
+template <bool kDoReFa>
 __global__ void __launch_bounds__(kNhThreads) int8_im2col_quantize_nhwc_kernel(const float* __restrict__ x, ConvDims d,
                                                                                 int C, int kcmax,
                                                                                 const float* __restrict__ scale,
@@ -337,7 +347,8 @@ __global__ void __launch_bounds__(kNhThreads) int8_im2col_quantize_nhwc_kernel(c
                                                                                 float qmin, float qmax, int off,
                                                                                 int8_t* __restrict__ q,
                                                                                 int* __restrict__ row_sum,
-                                                                                uint8_t* __restrict__ nan_flag, int vec) {
+                                                                                uint8_t* __restrict__ nan_flag, int vec,
+                                                                                const float* __restrict__ x_absmax) {
   extern __shared__ __align__(16) unsigned char nh_tile[];
   __shared__ long long pix_org[kNhPix], pix_ih[kNhPix], pix_iw[kNhPix];  // x offset of the window's top-left, row, col
   __shared__ int rsum[kNhPix];
@@ -359,6 +370,7 @@ __global__ void __launch_bounds__(kNhThreads) int8_im2col_quantize_nhwc_kernel(c
   p.qmin = qmin;
   p.qmax = qmax;
   const int pad = (int)p.zp - off;  // the grid point v = 0 of the fake-quant input's zero padding
+  const double xm = kDoReFa ? dorefa_rcp(__ldg(x_absmax)) : 0.0;  // 1 / m of a DoReFa input
   const int taps = d.KH * d.KW;
   __syncthreads();
   for (int k0 = 0; k0 < d.Kp; k0 += kcmax) {
@@ -387,7 +399,7 @@ __global__ void __launch_bounds__(kNhThreads) int8_im2col_quantize_nhwc_kernel(c
         for (int j = 0; j < 4; ++j) {
           const int k = (c + j) * taps + tap - k0;
           if (c + j < C && k >= 0 && k < klive) {
-            const int e = in ? stored_grid(v[j], p, off, nan) : pad;
+            const int e = in ? input_grid<kDoReFa>(v[j], xm, p, off, nan) : pad;
             s += e;
             nh_tile[px * kcmax + k] = (unsigned char)e;
           }
@@ -747,11 +759,12 @@ int check_k(const char* fn, long long k) {
 }
 
 int launch_rows(const float* x, const float* scale, const float* zero_point, int per_row, int qmin, int qmax, int8_t* q,
-                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st) {
+                int* row_sum, uint8_t* nan_flag, long long rows, long long k, cudaStream_t st, const float* x_absmax) {
   const int vec = (k % 4 == 0) && aligned16(x);
-  int8_quantize_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, scale, zero_point, per_row, (float)qmin, (float)qmax,
-                                                                      grid_offset(qmin), q, row_sum, nan_flag, rows, (int)k,
-                                                                      (int)padded_k(k), vec);
+  const auto kernel = x_absmax ? int8_quantize_rows_kernel<true> : int8_quantize_rows_kernel<false>;
+  kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, scale, zero_point, per_row, (float)qmin, (float)qmax,
+                                                     grid_offset(qmin), q, row_sum, nan_flag, rows, (int)k,
+                                                     (int)padded_k(k), vec, x_absmax);
   SB_LAUNCHED();
   return SB200_OK;
 }
@@ -769,9 +782,10 @@ int check_conv(const char* fn, const sb200_conv2d_geom* g, ConvDims* d) {
 }
 
 int launch_im2col(const float* x, const ConvDims& d, const float* scale, const float* zero_point, int qmin, int qmax,
-                  int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st) {
-  int8_im2col_quantize_kernel<<<(unsigned)((d.M + kLowPix - 1) / kLowPix), kLowThreads, 0, st>>>(
-      x, d, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, row_sum, nan_flag);
+                  int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st, const float* x_absmax) {
+  const auto kernel = x_absmax ? int8_im2col_quantize_kernel<true> : int8_im2col_quantize_kernel<false>;
+  kernel<<<(unsigned)((d.M + kLowPix - 1) / kLowPix), kLowThreads, 0, st>>>(
+      x, d, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, row_sum, nan_flag, x_absmax);
   SB_LAUNCHED();
   return SB200_OK;
 }
@@ -783,16 +797,17 @@ int nhwc_chunk(const ConvDims& d) {
 }
 
 int launch_im2col_nhwc(const float* x, const ConvDims& d, int c, const float* scale, const float* zero_point, int qmin,
-                       int qmax, int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st) {
+                       int qmax, int8_t* q, int* row_sum, uint8_t* nan_flag, cudaStream_t st, const float* x_absmax) {
   // a stride-1, unpadded 1 x 1 conv: x is already the [n h w, c] row matrix of the lowering.  The row quantizer gives
   // each row one warp, 16 elements per lane, so it takes rows of c >= kNhRowsMinK; shorter rows would leave most lanes
   // idle, and the NHWC kernel below (one tap, 64 rows per CTA) quantizes them.
   if (d.KH == 1 && d.KW == 1 && d.sh == 1 && d.sw == 1 && d.pt == 0 && d.pl == 0 && d.P == d.HW && d.K >= kNhRowsMinK)
-    return launch_rows(x, scale, zero_point, 0, qmin, qmax, q, row_sum, nan_flag, d.M, d.K, st);
+    return launch_rows(x, scale, zero_point, 0, qmin, qmax, q, row_sum, nan_flag, d.M, d.K, st, x_absmax);
   const int kc = nhwc_chunk(d);
   const int vec = (c % 4 == 0) && aligned16(x);
-  int8_im2col_quantize_nhwc_kernel<<<(unsigned)((d.M + kNhPix - 1) / kNhPix), kNhThreads, (size_t)kNhPix * kc, st>>>(
-      x, d, c, kc, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, row_sum, nan_flag, vec);
+  const auto kernel = x_absmax ? int8_im2col_quantize_nhwc_kernel<true> : int8_im2col_quantize_nhwc_kernel<false>;
+  kernel<<<(unsigned)((d.M + kNhPix - 1) / kNhPix), kNhThreads, (size_t)kNhPix * kc, st>>>(
+      x, d, c, kc, scale, zero_point, (float)qmin, (float)qmax, grid_offset(qmin), q, row_sum, nan_flag, vec, x_absmax);
   SB_LAUNCHED();
   return SB200_OK;
 }
@@ -818,25 +833,42 @@ int sb200_int8_quantize_rows(const float* x, const float* scale, const float* ze
                      (cudaStream_t)stream);
 }
 
+// sb200_int8_linear (dorefa = false) and sb200_int8_linear_dorefa
+static int int8_linear_entry(const char* fn, bool dorefa, const float* x, const float* x_scale, const float* x_zero_point,
+                             const float* x_absmax, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
+                             const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t m,
+                             int64_t k, int64_t n, void* workspace, size_t workspace_bytes, void* stream) {
+  SB_REQUIRE(x && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out && workspace,
+             "%s: null pointer argument", fn);
+  SB_REQUIRE(m > 0 && k > 0 && n > 0, "%s: empty operand (M=%lld K=%lld N=%lld)", fn, (long long)m, (long long)k,
+             (long long)n);
+  SB_REQUIRE(m < (1LL << 31) && n < (1LL << 31), "%s: dimension too large", fn);
+  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
+  SB_REQUIRE(aligned16(w_q), "%s: w_q must be 16-byte aligned", fn);
+  if (const int rc = check_k(fn, k)) return rc;
+  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_linear_workspace_bytes(m, k))) return rc;
+  if (const int rc = check_absmax(fn, dorefa, x_absmax)) return rc;
+  return run_gemm<false>(fn, m, k, n, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias, out,
+                         workspace, (cudaStream_t)stream, [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                           return launch_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, xq, xsum, xnan, m, k, st,
+                                              x_absmax);
+                         });
+}
+
 int sb200_int8_linear(const float* x, const float* x_scale, const float* x_zero_point, int qmin_x, int qmax_x,
                       const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero,
                       const float* bias, float* out, int64_t m, int64_t k, int64_t n, void* workspace,
                       size_t workspace_bytes, void* stream) {
-  SB_REQUIRE(x && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out && workspace,
-             "sb200_int8_linear: null pointer argument");
-  SB_REQUIRE(m > 0 && k > 0 && n > 0, "sb200_int8_linear: empty operand (M=%lld K=%lld N=%lld)", (long long)m, (long long)k,
-             (long long)n);
-  SB_REQUIRE(m < (1LL << 31) && n < (1LL << 31), "sb200_int8_linear: dimension too large");
-  if (const int rc = check_range("sb200_int8_linear", qmin_x, qmax_x)) return rc;
-  SB_REQUIRE(aligned16(w_q), "sb200_int8_linear: w_q must be 16-byte aligned");
-  if (const int rc = check_k("sb200_int8_linear", k)) return rc;
-  if (const int rc = check_workspace("sb200_int8_linear", workspace_bytes, sb200_int8_linear_workspace_bytes(m, k)))
-    return rc;
-  return run_gemm<false>("sb200_int8_linear", m, k, n, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero,
-                         bias, out, workspace, (cudaStream_t)stream,
-                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
-                           return launch_rows(x, x_scale, x_zero_point, 0, qmin_x, qmax_x, xq, xsum, xnan, m, k, st);
-                         });
+  return int8_linear_entry("sb200_int8_linear", false, x, x_scale, x_zero_point, nullptr, qmin_x, qmax_x, w_q, w_rowsum,
+                           w_scale, w_zero, bias, out, m, k, n, workspace, workspace_bytes, stream);
+}
+
+int sb200_int8_linear_dorefa(const float* x, const float* x_scale, const float* x_zero_point, const float* x_absmax,
+                             int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                             const int32_t* w_zero, const float* bias, float* out, int64_t m, int64_t k, int64_t n,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  return int8_linear_entry("sb200_int8_linear_dorefa", true, x, x_scale, x_zero_point, x_absmax, qmin_x, qmax_x, w_q,
+                           w_rowsum, w_scale, w_zero, bias, out, m, k, n, workspace, workspace_bytes, stream);
 }
 
 size_t sb200_int8_conv2d_workspace_bytes(const sb200_conv2d_geom* geom) {
@@ -859,11 +891,13 @@ int sb200_int8_im2col_quantize(const float* x, const sb200_conv2d_geom* geom, co
                        (cudaStream_t)stream);
 }
 
-int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float* x_scale, const float* x_zero_point,
-                      int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
-                      const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
-                      size_t workspace_bytes, void* stream) {
-  const char* fn = "sb200_int8_conv2d";
+// sb200_int8_conv2d{,_nhwc} (dorefa = false) and their _dorefa entry points
+template <bool kNhwc>
+static int int8_conv2d_entry(const char* fn, bool dorefa, const float* x, const sb200_conv2d_geom* geom,
+                             const float* x_scale, const float* x_zero_point, const float* x_absmax, int qmin_x,
+                             int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                             const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
+                             size_t workspace_bytes, void* stream) {
   SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out && workspace,
              "%s: null pointer argument", fn);
   SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
@@ -874,11 +908,40 @@ int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float
   SB_REQUIRE(aligned16(w_q), "%s: w_q must be 16-byte aligned", fn);
   if (const int rc = check_k(fn, d.K)) return rc;
   if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
-  return run_gemm<true>(fn, d.M, d.K, c_out, d.P, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
-                        out, workspace, (cudaStream_t)stream,
-                        [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
-                          return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st);
-                        });
+  if (const int rc = check_absmax(fn, dorefa, x_absmax)) return rc;
+  if constexpr (kNhwc) {
+    // the row-major [n OH OW, c_out] output of the linear is the NHWC storage of [n, c_out, OH, OW]
+    return run_gemm<false>(fn, d.M, d.K, c_out, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
+                           out, workspace, (cudaStream_t)stream,
+                           [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                             return launch_im2col_nhwc(x, d, (int)geom->c, x_scale, x_zero_point, qmin_x, qmax_x, xq,
+                                                       xsum, xnan, st, x_absmax);
+                           });
+  } else {
+    return run_gemm<true>(fn, d.M, d.K, c_out, d.P, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
+                          out, workspace, (cudaStream_t)stream,
+                          [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
+                            return launch_im2col(x, d, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum, xnan, st,
+                                                 x_absmax);
+                          });
+  }
+}
+
+int sb200_int8_conv2d(const float* x, const sb200_conv2d_geom* geom, const float* x_scale, const float* x_zero_point,
+                      int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                      const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  return int8_conv2d_entry<false>("sb200_int8_conv2d", false, x, geom, x_scale, x_zero_point, nullptr, qmin_x, qmax_x,
+                                  w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, workspace, workspace_bytes, stream);
+}
+
+int sb200_int8_conv2d_dorefa(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                             const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x, const int8_t* w_q,
+                             const int32_t* w_rowsum, const float* w_scale, const int32_t* w_zero, const float* bias,
+                             float* out, int64_t c_out, void* workspace, size_t workspace_bytes, void* stream) {
+  return int8_conv2d_entry<false>("sb200_int8_conv2d_dorefa", true, x, geom, x_scale, x_zero_point, x_absmax, qmin_x,
+                                  qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, workspace, workspace_bytes,
+                                  stream);
 }
 
 int sb200_int8_im2col_quantize_nhwc(const float* x, const sb200_conv2d_geom* geom, const float* scale,
@@ -899,24 +962,19 @@ int sb200_int8_conv2d_nhwc(const float* x, const sb200_conv2d_geom* geom, const 
                            const float* x_zero_point, int qmin_x, int qmax_x, const int8_t* w_q, const int32_t* w_rowsum,
                            const float* w_scale, const int32_t* w_zero, const float* bias, float* out, int64_t c_out,
                            void* workspace, size_t workspace_bytes, void* stream) {
-  const char* fn = "sb200_int8_conv2d_nhwc";
-  SB_REQUIRE(x && geom && x_scale && x_zero_point && w_q && w_rowsum && w_scale && w_zero && out && workspace,
-             "%s: null pointer argument", fn);
-  SB_REQUIRE(c_out > 0, "%s: empty operand (c_out=%lld)", fn, (long long)c_out);
-  SB_REQUIRE(c_out < (1LL << 31), "%s: dimension too large (c_out=%lld)", fn, (long long)c_out);
-  ConvDims d;
-  if (const int rc = check_conv(fn, geom, &d)) return rc;
-  if (const int rc = check_range(fn, qmin_x, qmax_x)) return rc;
-  SB_REQUIRE(aligned16(w_q), "%s: w_q must be 16-byte aligned", fn);
-  if (const int rc = check_k(fn, d.K)) return rc;
-  if (const int rc = check_workspace(fn, workspace_bytes, sb200_int8_conv2d_workspace_bytes(geom))) return rc;
-  // the row-major [n OH OW, c_out] output of the linear is the NHWC storage of [n, c_out, OH, OW]
-  return run_gemm<false>(fn, d.M, d.K, c_out, 1, qmin_x, x_scale, x_zero_point, w_q, w_rowsum, w_scale, w_zero, bias,
-                         out, workspace, (cudaStream_t)stream,
-                         [&](int8_t* xq, int* xsum, uint8_t* xnan, cudaStream_t st) {
-                           return launch_im2col_nhwc(x, d, (int)geom->c, x_scale, x_zero_point, qmin_x, qmax_x, xq, xsum,
-                                                     xnan, st);
-                         });
+  return int8_conv2d_entry<true>("sb200_int8_conv2d_nhwc", false, x, geom, x_scale, x_zero_point, nullptr, qmin_x,
+                                 qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, workspace, workspace_bytes,
+                                 stream);
+}
+
+int sb200_int8_conv2d_nhwc_dorefa(const float* x, const sb200_conv2d_geom* geom, const float* x_scale,
+                                  const float* x_zero_point, const float* x_absmax, int qmin_x, int qmax_x,
+                                  const int8_t* w_q, const int32_t* w_rowsum, const float* w_scale,
+                                  const int32_t* w_zero, const float* bias, float* out, int64_t c_out, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return int8_conv2d_entry<true>("sb200_int8_conv2d_nhwc_dorefa", true, x, geom, x_scale, x_zero_point, x_absmax,
+                                 qmin_x, qmax_x, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, workspace,
+                                 workspace_bytes, stream);
 }
 
 size_t sb200_int8_matmul_workspace_bytes(int64_t batch, int64_t m, int64_t k, int64_t n) {

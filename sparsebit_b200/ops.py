@@ -708,6 +708,19 @@ def _int8_weight_rows(fn, n, bias, **per_row):
     return n
 
 
+def _x_absmax_args(fn, x, x_absmax):
+    """The entry-point suffix and extra argument of an integer-grid op's optional DoReFa input: ``("", [])`` without
+    ``x_absmax``, else ``("_dorefa", [pointer])`` once it is checked to be the one-element fp32 tensor on x's device that
+    ``dorefa_absmax(x)`` returns (max |tanh(x)|; the kernels quantize tanh(x) / x_absmax)."""
+    if x_absmax is None:
+        return "", []
+    _req(x_absmax, "x_absmax")
+    if x_absmax.numel() != 1 or x_absmax.device != x.device:
+        raise SparsebitB200Error(f"{fn}: x_absmax must be one fp32 element on x's device, as dorefa_absmax(x) returns "
+                                 f"(got {x_absmax.numel()} on {x_absmax.device})")
+    return "_dorefa", [x_absmax.data_ptr()]
+
+
 def int8_quantize_rows(x, scale, zero_point, qmin, qmax):
     """Integer grid of every row of ``x`` [rows, K] (sb200_int8_quantize_rows): returns ``(q, row_sum, nan)`` with
     q int8 [rows, Kp] = clamp(round(x / s) + rint(zp), qmin, qmax) - int8_grid_offset(qmin), the padding to
@@ -744,11 +757,13 @@ def _int8_workspace(device, nbytes):
     return _int8_workspaces.get((device, torch.cuda.current_stream(device).cuda_stream), device, nbytes)
 
 
-def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias=None, k=None):
+def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias=None, k=None, x_absmax=None):
     """``y = s_x s_w[n] sum_k v_x v_w + bias`` on the int8 tensor cores (sb200_int8_linear): the fake-quant linear of
     per-tensor activations [qmin, qmax] with the weights stored by ``int8_quantize_rows`` (w_q int8 [N, Kp], w_rowsum
     int32 [N], w_scale fp32 [N], w_zero int32 [N] = rint(zero point) - int8_grid_offset).  ``x`` [..., K] fp32; returns
-    fp32 [..., N].  ``k`` defaults to x.shape[-1]."""
+    fp32 [..., N].  ``k`` defaults to x.shape[-1].  ``x_absmax``: ``dorefa_absmax(x)`` of a DoReFa input, whose
+    tanh(x) / x_absmax is quantized (sb200_int8_linear_dorefa; the plain op on ``dorefa_forward(x, x_absmax)``, bit for
+    bit)."""
     lib = _lib.load()
     _req_int8_operands(x, x_scale, x_zero_point, w_scale, bias, w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero)
     k = x.shape[-1] if k is None else int(k)
@@ -757,11 +772,12 @@ def int8_linear(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_
     n = _int8_weight_rows("int8_linear", w_q.shape[0], bias, w_rowsum=w_rowsum, w_scale=w_scale, w_zero=w_zero)
     m = x.numel() // k
     out = torch.empty(x.shape[:-1] + (n,), dtype=torch.float32, device=x.device)
+    sfx, am = _x_absmax_args("int8_linear", x, x_absmax)
     ws_bytes = int(lib.sb200_int8_linear_workspace_bytes(m, k))
     ws = _int8_workspace(x.device, ws_bytes)
     with torch.cuda.device(x.device):
-        check(lib.sb200_int8_linear(x.data_ptr(), x_scale.data_ptr(), x_zero_point.data_ptr(), int(qmin), int(qmax),
-                                    w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
+        check(getattr(lib, "sb200_int8_linear" + sfx)(x.data_ptr(), x_scale.data_ptr(), x_zero_point.data_ptr(), *am,
+                                    int(qmin), int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                     bias.data_ptr() if bias is not None else None, out.data_ptr(), m, k, n, ws.data_ptr(),
                                     ws_bytes, _stream(x)))
     return out
@@ -1100,21 +1116,23 @@ def int8_im2col_quantize(x, kernel_size, scale, zero_point, qmin, qmax, stride=1
 
 
 def int8_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, bias=None, stride=1,
-                padding=0, dilation=1):
+                padding=0, dilation=1, x_absmax=None):
     """The fake-quant conv2d (groups = 1) on the int8 tensor cores (sb200_int8_conv2d): ``x`` [N, C, H, W] fp32 is
     lowered to its integer grid and multiplied with the weights stored by ``int8_quantize_rows`` from
     ``weight.reshape(C_out, -1)`` (w_q int8 [C_out, Kp], w_rowsum int32, w_scale fp32, w_zero int32 [C_out]), as in
     ``int8_linear``.  Returns fp32 [N, C_out, OH, OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left,
-    right)."""
+    right).  ``x_absmax``: a DoReFa input's ``dorefa_absmax(x)``, as ``int8_linear`` takes it
+    (sb200_int8_conv2d_dorefa)."""
     lib = _lib.load()
     g, n, out = _int8_conv_prelude("int8_conv2d", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
                                    dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, 1, stride, padding,
                                    dilation)
+    sfx, am = _x_absmax_args("int8_conv2d", x, x_absmax)
     ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     ws = _int8_workspace(x.device, max(ws_bytes, 16))
     with torch.cuda.device(x.device):
-        check(lib.sb200_int8_conv2d(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(), x_zero_point.data_ptr(), int(qmin),
-                                    int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
+        check(getattr(lib, "sb200_int8_conv2d" + sfx)(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(),
+                                    x_zero_point.data_ptr(), *am, int(qmin), int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                     bias.data_ptr() if bias is not None else None, out.data_ptr(), n, ws.data_ptr(),
                                     ws.numel(), _stream(x)))
     return out
@@ -1141,19 +1159,21 @@ def int8_sparse24_conv2d(x, x_scale, x_zero_point, qmin, qmax, vals, meta, dsum,
 
 
 def int8_group_conv2d(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups, bias=None,
-                      stride=1, padding=0, dilation=1):
+                      stride=1, padding=0, dilation=1, x_absmax=None):
     """The fake-quant grouped / depthwise conv2d (groups >= 2) on the integer grid (sb200_int8_group_conv2d): one direct
     int8 kernel that quantizes its input tile on the fly.  ``x`` [N, C, H, W] fp32; the weights as ``int8_conv2d``
     takes them, stored by ``int8_quantize_rows`` from ``weight.reshape(C_out, -1)`` (w_q int8 [C_out, Kp] with Kp =
     round_up(C / groups KH KW, 16), w_rowsum int32, w_scale fp32, w_zero int32 [C_out]).  Returns fp32 [N, C_out, OH,
-    OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right).  No workspace."""
+    OW].  ``padding``: an int, (pad_h, pad_w) or (top, bottom, left, right).  No workspace.  ``x_absmax``: a DoReFa
+    input's ``dorefa_absmax(x)``, as ``int8_linear`` takes it (sb200_int8_group_conv2d_dorefa)."""
     lib = _lib.load()
     g, n, out = _int8_conv_prelude("int8_group_conv2d", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
                                    dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, groups, stride, padding,
                                    dilation)
+    sfx, am = _x_absmax_args("int8_group_conv2d", x, x_absmax)
     with torch.cuda.device(x.device):
-        check(lib.sb200_int8_group_conv2d(x.data_ptr(), ctypes.byref(g), int(groups), x_scale.data_ptr(),
-                                          x_zero_point.data_ptr(), int(qmin), int(qmax), w_q.data_ptr(),
+        check(getattr(lib, "sb200_int8_group_conv2d" + sfx)(x.data_ptr(), ctypes.byref(g), int(groups), x_scale.data_ptr(),
+                                          x_zero_point.data_ptr(), *am, int(qmin), int(qmax), w_q.data_ptr(),
                                           w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                           bias.data_ptr() if bias is not None else None, out.data_ptr(), n, _stream(x)))
     return out
@@ -1182,18 +1202,20 @@ def int8_im2col_quantize_nhwc(x, kernel_size, scale, zero_point, qmin, qmax, str
 
 
 def int8_conv2d_nhwc(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, bias=None,
-                     stride=1, padding=0, dilation=1):
+                     stride=1, padding=0, dilation=1, x_absmax=None):
     """``int8_conv2d`` of a channels-last ``x`` (sb200_int8_conv2d_nhwc), with the same stored weights: returns a
-    channels-last fp32 [N, C_out, OH, OW] whose values equal ``int8_conv2d`` on ``x.contiguous()`` bit for bit."""
+    channels-last fp32 [N, C_out, OH, OW] whose values equal ``int8_conv2d`` on ``x.contiguous()`` bit for bit.
+    ``x_absmax``: as ``int8_conv2d`` takes it (sb200_int8_conv2d_nhwc_dorefa)."""
     lib = _lib.load()
     g, n, out = _int8_conv_prelude("int8_conv2d_nhwc", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
                                    dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, 1, stride, padding,
                                    dilation, torch.channels_last)
+    sfx, am = _x_absmax_args("int8_conv2d_nhwc", x, x_absmax)
     ws_bytes = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     ws = _int8_workspace(x.device, max(ws_bytes, 16))
     with torch.cuda.device(x.device):
-        check(lib.sb200_int8_conv2d_nhwc(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(), x_zero_point.data_ptr(),
-                                         int(qmin), int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(),
+        check(getattr(lib, "sb200_int8_conv2d_nhwc" + sfx)(x.data_ptr(), ctypes.byref(g), x_scale.data_ptr(),
+                                         x_zero_point.data_ptr(), *am, int(qmin), int(qmax), w_q.data_ptr(), w_rowsum.data_ptr(), w_scale.data_ptr(),
                                          w_zero.data_ptr(), bias.data_ptr() if bias is not None else None, out.data_ptr(),
                                          n, ws.data_ptr(), ws.numel(), _stream(x)))
     return out
@@ -1219,17 +1241,18 @@ def int8_sparse24_conv2d_nhwc(x, x_scale, x_zero_point, qmin, qmax, vals, meta, 
 
 
 def int8_group_conv2d_nhwc(x, x_scale, x_zero_point, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, kernel_size, groups,
-                           bias=None, stride=1, padding=0, dilation=1):
+                           bias=None, stride=1, padding=0, dilation=1, x_absmax=None):
     """``int8_group_conv2d`` of a channels-last ``x`` (sb200_int8_group_conv2d_nhwc), with the same stored weights:
     returns a channels-last fp32 [N, C_out, OH, OW] whose values equal ``int8_group_conv2d`` on ``x.contiguous()`` bit
-    for bit.  No workspace."""
+    for bit.  No workspace.  ``x_absmax``: as ``int8_group_conv2d`` takes it (sb200_int8_group_conv2d_nhwc_dorefa)."""
     lib = _lib.load()
     g, n, out = _int8_conv_prelude("int8_group_conv2d_nhwc", x, x_scale, x_zero_point, w_scale, bias, _int8_conv_rows,
                                    dict(w_q=w_q, w_rowsum=w_rowsum, w_zero=w_zero), kernel_size, groups, stride, padding,
                                    dilation, torch.channels_last)
+    sfx, am = _x_absmax_args("int8_group_conv2d_nhwc", x, x_absmax)
     with torch.cuda.device(x.device):
-        check(lib.sb200_int8_group_conv2d_nhwc(x.data_ptr(), ctypes.byref(g), int(groups), x_scale.data_ptr(),
-                                               x_zero_point.data_ptr(), int(qmin), int(qmax), w_q.data_ptr(),
+        check(getattr(lib, "sb200_int8_group_conv2d_nhwc" + sfx)(x.data_ptr(), ctypes.byref(g), int(groups),
+                                               x_scale.data_ptr(), x_zero_point.data_ptr(), *am, int(qmin), int(qmax), w_q.data_ptr(),
                                                w_rowsum.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(),
                                                bias.data_ptr() if bias is not None else None, out.data_ptr(), n,
                                                _stream(x)))

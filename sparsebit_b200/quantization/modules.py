@@ -76,8 +76,9 @@ def _qparams(quantizer, x):
     return scale.detach().float().reshape(-1), zero_point.detach().float().reshape(-1)
 
 
-def _int8_plain_qdq_reason(role, q):
-    """Why quantizer ``q`` does not run the plain <= 8-bit fake-quant op that the integer path restates (None if it does)."""
+def _int8_plain_qdq_reason(role, q, types=_PLAIN_QDQ_TYPES):
+    """Why quantizer ``q`` does not run the plain <= 8-bit fake-quant op that the integer path restates (None if it does);
+    ``types``: the quantizer types the caller restates."""
     if q is None:
         return f"the {role} quantizer is missing"
     if q.fake_fused:
@@ -86,7 +87,7 @@ def _int8_plain_qdq_reason(role, q):
         return f"the {role} quantizer is not enabled"
     if q.export_onnx:
         return f"the {role} quantizer is in export_onnx mode"
-    if q.TYPE.lower() not in _PLAIN_QDQ_TYPES:
+    if q.TYPE.lower() not in types:
         return f"the {role} quantizer is {q.TYPE}, whose forward is not the plain fake-quant op"
     if q.bit > 8:
         return f"the {role} quantizer has {q.bit} bits (at most 8)"
@@ -114,12 +115,12 @@ def _int8_qparams_reason(role, q, x, counts):
     return None
 
 
-def _int8_quantizer_ineligibility(mod):
+def _int8_quantizer_ineligibility(mod, input_types=_PLAIN_QDQ_TYPES, weight_types=_PLAIN_QDQ_TYPES):
     """The quantizer rules of the integer path, shared by ``QLinear`` and ``QConv2d``: ``mod`` has an input and a
     weight quantizer and a weight whose axis 0 is the output channels."""
     n = mod.weight.shape[0]
-    for role, q in (("input", mod.input_quantizer), ("weight", mod.weight_quantizer)):
-        reason = _int8_plain_qdq_reason(role, q)
+    for role, q, types in (("input", mod.input_quantizer, input_types), ("weight", mod.weight_quantizer, weight_types)):
+        reason = _int8_plain_qdq_reason(role, q, types)
         if reason is not None:
             return reason
     aq, wq = mod.input_quantizer, mod.weight_quantizer
@@ -141,11 +142,26 @@ def int8_ineligibility(qlinear):
     return _int8_quantizer_ineligibility(qlinear)
 
 
+def _grid_source(wq, weight):
+    """The tensor whose plain QDQ grid under ``wq``'s qparams is ``wq``'s grid: the weight itself, DoReFa's normalised
+    tanh(w) / max |tanh(w)| (the fake-quant op's own sequence, ``DoReFaSTE``), or AdaRound's eval-mode (hard rounding)
+    output RN((q - zp) s), which re-quantizes to q exactly under the preconditions ``dorefa_adaround_ineligibility``
+    enforces."""
+    kind = wq.TYPE.lower()
+    if kind == "dorefa":
+        w = weight.detach().float().contiguous()
+        return ops.dorefa_forward(w, ops.dorefa_absmax(w))
+    if kind == "adaround":
+        return wq(weight.detach())
+    return weight.detach()
+
+
 def _int8_weight_rows(wq, weight):
     """The weights on the stored integer grid, one row per output channel (``weight.reshape(N, -1)``):
     ``(w_q, w_rowsum, w_scale, w_zero)`` as ``ops.int8_linear`` / ``ops.int8_conv2d`` take them.  A weight row holding a
-    NaN gets ``w_scale = NaN``, which makes its output channel NaN, as in the fake-quant op."""
-    rows = weight.detach().reshape(weight.shape[0], -1)
+    NaN gets ``w_scale = NaN``, which makes its output channel NaN, as in the fake-quant op (a DoReFa weight holding a
+    NaN makes every row NaN: its max |tanh| is global)."""
+    rows = _grid_source(wq, weight).reshape(weight.shape[0], -1)
     n = rows.shape[0]
     ws, wz = _qparams(wq, weight)
     wqmin, wqmax = wq.qdesc.qrange
@@ -166,6 +182,10 @@ class _Int8InputModule(nn.Module):
     """What every weight-carrying integer-grid module holds besides its weight operand: the per-tensor activation
     ``scale`` / ``zero_point`` and integer range ``qmin`` / ``qmax``, and ``bias`` (fp32 or None).  A subclass registers
     its weight buffers, then ``_register_input``."""
+
+    def _x_absmax(self, x):
+        """The ``x_absmax`` the ops take for input ``x``: None, the input is quantized as it is (see ``_DoReFaInput``)."""
+        return None
 
     def _register_input(self, device):
         self.register_buffer("scale", torch.ones(1, dtype=torch.float32, device=device))
@@ -226,14 +246,19 @@ class QLinearInt8(_Int8WeightModule):
     @classmethod
     def from_qlinear(cls, qlinear):
         cls._check_eligible(int8_ineligibility(qlinear), "from_qlinear")
+        return cls._build(qlinear)
+
+    @classmethod
+    def _build(cls, qlinear):
         n, k = qlinear.weight.shape
         return cls(k, n, qlinear.weight.device)._load(qlinear)
 
     def forward(self, x_in):
         _check_inference_only(self, "QLinear", x_in)
         x = x_in.float() if x_in.dtype != torch.float32 else x_in
-        return ops.int8_linear(x.contiguous(), self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
-                               self.w_scale, self.w_zero, self.bias, k=self.in_features)
+        x = x.contiguous()
+        return ops.int8_linear(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum,
+                               self.w_scale, self.w_zero, self.bias, k=self.in_features, x_absmax=self._x_absmax(x))
 
     def extra_repr(self):
         return f"in_features={self.in_features}, out_features={self.out_features}, qrange=[{self.qmin}, {self.qmax}]"
@@ -357,12 +382,12 @@ def resolve_conv_padding(padding, kernel_size, dilation=1, stride=1):
     return (ph, ph, pw, pw)
 
 
-def _int8_conv_ineligibility(qconv, groups_rule):
+def _int8_conv_ineligibility(qconv, groups_rule, quantizer_rule=_int8_quantizer_ineligibility):
     """The conversion rules of a ``QConv2d`` in the order they are reported: the quantizer rules, then
     ``groups_rule(groups, K_g)`` (a reason or None; K_g = C / groups KH KW), then the padding."""
     if not isinstance(qconv, QConv2d):
         return f"expected a QConv2d, got {type(qconv).__name__}"
-    reason = _int8_quantizer_ineligibility(qconv)
+    reason = quantizer_rule(qconv)
     if reason is not None:
         return reason
     kw = qconv.fwd_kwargs
@@ -443,13 +468,17 @@ class QConv2dInt8(_Int8Conv2dModule, _Int8WeightModule):
     @classmethod
     def from_qconv2d(cls, qconv):
         cls._check_eligible(cls._ineligibility(qconv), "from_qconv2d")
+        return cls._build(qconv)
+
+    @classmethod
+    def _build(cls, qconv):
         *geometry, groups = cls._geometry_of(qconv)
         return cls(*geometry, device=qconv.weight.device, groups=groups)._load(qconv)
 
     def _conv(self, x, nhwc):
         op = ops.int8_conv2d_nhwc if nhwc else ops.int8_conv2d
         return op(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum, self.w_scale, self.w_zero,
-                  self.kernel_size, self.bias, self.stride, self.padding, self.dilation)
+                  self.kernel_size, self.bias, self.stride, self.padding, self.dilation, x_absmax=self._x_absmax(x))
 
 
 def int8_sparse24_conv_ineligibility(qconv):
@@ -518,10 +547,108 @@ class QConv2dGroupInt8(QConv2dInt8):
     def _conv(self, x, nhwc):
         op = ops.int8_group_conv2d_nhwc if nhwc else ops.int8_group_conv2d
         return op(x, self.scale, self.zero_point, self.qmin, self.qmax, self.w_q, self.w_rowsum, self.w_scale, self.w_zero,
-                  self.kernel_size, self.groups, self.bias, self.stride, self.padding, self.dilation)
+                  self.kernel_size, self.groups, self.bias, self.stride, self.padding, self.dilation,
+                  x_absmax=self._x_absmax(x))
 
     def extra_repr(self):
         return super().extra_repr() + f", groups={self.groups}"
+
+
+# ----------------------------------------------------------------------------- DoReFa and AdaRound layers
+ADAROUND_SCALE_RANGE = (2.0 ** -126, 2.0 ** 119)  # |s|: (q - zp) s for |q - zp| <= 255 stays normal and finite
+
+
+def _is(q, *types):
+    return q is not None and q.TYPE.lower() in types
+
+
+def _adaround_reason(wq, weight):
+    """Why an AdaRound weight quantizer's eval-mode output does not re-quantize to its grid exactly (None if it does):
+    RN((q - zp) s) / s rounds back to q when zp is integral, |q - zp| <= 255 (zp inside the integer range, which the
+    shared rules check) and 2^-126 <= |s| <= 2^119."""
+    if wq.training:
+        return "the weight quantizer is AdaRound in training mode, whose soft rounding lies off the grid"
+    if getattr(wq, "v", None) is None:
+        return "the weight quantizer is AdaRound without its rounding variables v (run the reconstruction first)"
+    scale, zero_point = _qparams(wq, weight)
+    if not bool(torch.equal(zero_point, torch.round(zero_point))):
+        return "the weight quantizer is AdaRound with a non-integral zero point"
+    lo, hi = ADAROUND_SCALE_RANGE
+    a = scale.abs()
+    if not bool(((a >= lo) & (a <= hi)).all()):
+        return "the weight quantizer is AdaRound with a scale outside [2^-126, 2^119] in magnitude"
+    return None
+
+
+def dorefa_adaround_ineligibility(qmod):
+    """Why ``from_dorefa_adaround`` cannot convert ``qmod`` (None when it can): a ``QLinear`` or a ``QConv2d`` of any
+    ``groups`` whose input quantizer is DoReFa, or whose weight quantizer is DoReFa or AdaRound (a layer with neither
+    belongs to ``to_integer_linears`` / ``to_integer_convs`` / ``to_integer_group_convs``), and that meets every other
+    rule of the matching plain converter.  DoReFa on a per-channel input and AdaRound on an input are refused; an
+    AdaRound weight must be in eval mode with its ``v``, an integral zero point and 2^-126 <= |s| <= 2^119."""
+    if not isinstance(qmod, (QLinear, QConv2d)):
+        return f"expected a QLinear or a QConv2d, got {type(qmod).__name__}"
+    for role, q in (("input", qmod.input_quantizer), ("weight", qmod.weight_quantizer)):
+        if q is None:
+            return f"the {role} quantizer is missing"
+    aq, wq = qmod.input_quantizer, qmod.weight_quantizer
+    if not (_is(aq, "dorefa") or _is(wq, "dorefa", "adaround")):
+        return ("neither quantizer is DoReFa or AdaRound: use to_integer_linears / to_integer_convs / "
+                "to_integer_group_convs")
+    rule = lambda m: _int8_quantizer_ineligibility(m, _PLAIN_QDQ_TYPES + ("dorefa",),  # noqa: E731
+                                                  _PLAIN_QDQ_TYPES + ("dorefa", "adaround"))
+    if isinstance(qmod, QLinear):
+        reason = rule(qmod)
+    else:
+        groups = int(qmod.fwd_kwargs["groups"])
+        reason = _int8_conv_ineligibility(qmod, _dense_conv_rule if groups == 1 else _group_conv_rule, rule)
+    if reason is None and _is(wq, "adaround"):
+        reason = _adaround_reason(wq, qmod.weight)
+    return reason
+
+
+class _DoReFaInput:
+    """A layer whose input quantizer is DoReFa: ``forward`` computes m = ``ops.dorefa_absmax`` over the whole input, the
+    tensor the fake-quant quantizer sees, and the kernels quantize tanh(x) / m.  Same buffers as the plain layer."""
+
+    def _x_absmax(self, x):
+        # max |tanh| does not depend on the order: a channels-last x is read in its NHWC storage order
+        return ops.dorefa_absmax(x if x.is_contiguous() else x.permute(0, 2, 3, 1))
+
+    def extra_repr(self):
+        return super().extra_repr() + ", input=DoReFa"
+
+
+class QLinearDoReFaInt8(_DoReFaInput, QLinearInt8):
+    """``QLinearInt8`` of a ``QLinear`` whose input quantizer is DoReFa (per-tensor); built by ``from_dorefa_adaround``."""
+
+
+class QConv2dDoReFaInt8(_DoReFaInput, QConv2dInt8):
+    """``QConv2dInt8`` of a ``QConv2d`` (groups = 1) whose input quantizer is DoReFa (per-tensor); built by
+    ``from_dorefa_adaround``."""
+
+
+class QConv2dGroupDoReFaInt8(_DoReFaInput, QConv2dGroupInt8):
+    """``QConv2dGroupInt8`` of a grouped or depthwise ``QConv2d`` whose input quantizer is DoReFa (per-tensor); built by
+    ``from_dorefa_adaround``."""
+
+
+def from_dorefa_adaround(qmod):
+    """The integer-grid layer of a calibrated ``QLinear`` / ``QConv2d`` that ``dorefa_adaround_ineligibility`` accepts:
+    the weights stored on the weight quantizer's grid (``_grid_source``), and ``QLinearDoReFaInt8`` /
+    ``QConv2dDoReFaInt8`` / ``QConv2dGroupDoReFaInt8`` when the input quantizer is DoReFa, else the plain
+    ``QLinearInt8`` / ``QConv2dInt8`` / ``QConv2dGroupInt8``.  Raises ``ValueError`` with the reason otherwise."""
+    reason = dorefa_adaround_ineligibility(qmod)
+    if reason is not None:
+        raise ValueError(f"from_dorefa_adaround: {reason}")
+    dorefa = _is(qmod.input_quantizer, "dorefa")
+    if isinstance(qmod, QLinear):
+        cls = QLinearDoReFaInt8 if dorefa else QLinearInt8
+    elif int(qmod.fwd_kwargs["groups"]) == 1:
+        cls = QConv2dDoReFaInt8 if dorefa else QConv2dInt8
+    else:
+        cls = QConv2dGroupDoReFaInt8 if dorefa else QConv2dGroupInt8
+    return cls._build(qmod)
 
 
 class QReLU(QuantOpr):

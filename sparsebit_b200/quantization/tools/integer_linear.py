@@ -3,11 +3,14 @@
 a ``QMatMulInt8`` (``to_integer_matmuls``), every eligible grouped or depthwise ``QConv2d`` a ``QConv2dGroupInt8``
 (``to_integer_group_convs``), every eligible ``QAttention`` a ``QAttentionInt8`` (``to_integer_attentions``), and,
 opt-in, every ``QLinear`` whose weight is 2:4 sparse on the grid a ``QLinearSparse24Int8``
-(``to_sparse24_integer_linears``) and every such ``QConv2d`` a ``QConv2dSparse24Int8`` (``to_sparse24_integer_convs``)."""
-from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QConv2dSparse24Int8, QLinear,
-                       QLinearInt8, QLinearSparse24Int8, QMatMul, QMatMulInt8, int8_attention_ineligibility,
-                       int8_conv_ineligibility, int8_group_conv_ineligibility, int8_ineligibility,
-                       int8_matmul_ineligibility, int8_sparse24_conv_ineligibility, int8_sparse24_ineligibility)
+(``to_sparse24_integer_linears``) and every such ``QConv2d`` a ``QConv2dSparse24Int8`` (``to_sparse24_integer_convs``),
+and every ``QLinear`` / ``QConv2d`` with a DoReFa or AdaRound quantizer its integer-grid layer
+(``to_integer_dorefa_adaround``)."""
+from ..modules import (QAttention, QAttentionInt8, QConv2d, QConv2dGroupInt8, QConv2dInt8, QConv2dSparse24Int8,
+                       QLinear, QLinearInt8, QLinearSparse24Int8, QMatMul, QMatMulInt8, dorefa_adaround_ineligibility,
+                       from_dorefa_adaround, int8_attention_ineligibility, int8_conv_ineligibility,
+                       int8_group_conv_ineligibility, int8_ineligibility, int8_matmul_ineligibility,
+                       int8_sparse24_conv_ineligibility, int8_sparse24_ineligibility)
 
 
 def _swap(model, kind, ineligibility, convert):
@@ -75,3 +78,12 @@ def to_sparse24_integer_convs(model):
     before ``to_integer_convs``, which would otherwise convert the sparse convs to dense ``QConv2dInt8``.  Returns the
     qualified names of the converted modules, in ``named_modules`` order."""
     return _swap(model, QConv2d, int8_sparse24_conv_ineligibility, QConv2dSparse24Int8.from_qconv2d)
+
+
+def to_integer_dorefa_adaround(model):
+    """Swap, in place, every ``QLinear`` / ``QConv2d`` of ``model`` that ``from_dorefa_adaround`` accepts: its input
+    quantizer is DoReFa, or its weight quantizer DoReFa or AdaRound (the DoReFa and PACT QAT recipes, AdaRound PTQ).
+    The others stay, and ``dorefa_adaround_ineligibility`` says why.  Opt-in: the plain converters keep refusing these
+    layers, and this one refuses every layer they convert, so the converters can run in any order.  Returns the
+    qualified names of the converted modules, in ``named_modules`` order."""
+    return _swap(model, (QLinear, QConv2d), dorefa_adaround_ineligibility, from_dorefa_adaround)
