@@ -1,9 +1,23 @@
 import zlib
 
 import numpy as np
+import pytest
 import torch
 
 from sparsebit_b200 import _lib
+
+
+def _tf32_off():
+    """TF32 off for cuDNN convs and cuBLAS matmuls over a test, so that the fp32 comparison paths round as fp32."""
+    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    yield
+    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
+
+
+# ``no_tf32`` for the tests that ask for it; a module that imports ``no_tf32_autouse`` has it on every test
+no_tf32 = pytest.fixture(_tf32_off, name="no_tf32")
+no_tf32_autouse = pytest.fixture(_tf32_off, autouse=True, name="no_tf32_autouse")
 
 
 def dev():

@@ -6,6 +6,7 @@ import torch
 import torch.nn as nn
 
 from gpu_util import bits_equal, dev, t
+from gpu_util import no_tf32_autouse  # noqa: F401 -- TF32 off on every test
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import QConv2d, QLinear, QReLU
 from sparsebit_b200.quantization.tools import CalibrationRunner, trace_quant_model
@@ -42,14 +43,6 @@ class Tiny(nn.Module):
         x = self.relu1(self.conv1(x))
         x = self.relu2(self.conv2(x))
         return self.fc(torch.flatten(x, 1))
-
-
-@pytest.fixture(autouse=True)
-def _no_tf32():
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
 
 
 def _calibrate(g, case, streaming=True, asym=False, **kw):

@@ -64,7 +64,6 @@ row blocks.  Each GPU test states its device-memory need and skips when the devi
 backward cases, hold x, gy and gx (25.8 GB) plus one chunk of the fp64 reference.  The host refusal of a per-tensor QDQ
 that needs more than 2^31 - 1 chunk CTAs is checked on the CPU with fake pointers.
 """
-import ctypes
 import functools
 import gc
 
@@ -78,6 +77,7 @@ import qdq_geometry as qgeo
 import weight_geometry as wgeo
 from branch_cases import C, assert_table_covers, check_reach, params
 from gpu_util import bits_equal, dev, real_sm, seed_of, stream
+from int8_harness import E_INVALID, buf
 from oracle import observers as oobs
 from oracle import qdq as oqdq
 from sparsebit_b200 import _lib, ops
@@ -90,7 +90,6 @@ SUB = 1 << 28          # elements per sub-range launch at most
 WIN = 1 << 16          # elements per oracle window, about
 SENTINEL = 0x7FA5A5A5  # a NaN no kernel writes
 GIB = 1 << 30
-E_INVALID = -1
 # gy past element 2^31 is scaled by this, so that those few thousand elements move gs / gzp / g_hi / g_lo by far more
 # than the 1e-5-of-L1 bar (at unit scale they would be below it)
 TAIL_GY = 4096.0
@@ -260,18 +259,13 @@ def test_channel_last_grid_y_cap_cannot_bind():
         assert qgeo.cols_row_blocks(outer, c, sm) <= 8 * sm * 2
 
 
-def _buf(nbytes=4096):
-    b = ctypes.create_string_buffer(nbytes + 16)
-    return b, (ctypes.addressof(b) + 15) // 16 * 16
-
-
 def test_pertensor_refuses_more_than_2_31_chunks_on_the_host():
     """launch_chunks (qdq.cu) refuses a per-tensor QDQ whose chunk grid would pass 2^31 - 1 CTAs with SB200_E_INVALID,
     before any CUDA call (there is no device here): check_common, use_tma and launch_chunks read only the arguments and
     the variant switch up to that check.  At the boundary: 4 x 1024 elements per CTA on the 128-bit path, 1024 on the
     scalar one (a pointer off 16-byte alignment)."""
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     refused = [(p, 1 << 43), (p, (1 << 43) - 4092), (p + 4, (1 << 41) - 1023), (p + 4, 1 << 43)]
     try:
         for variant in (0, 1):

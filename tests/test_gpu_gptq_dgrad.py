@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import dev, t
+from gpu_util import dev, no_tf32, t  # noqa: F401 -- no_tf32: a fixture
 from gptq_dgrad_ref import dequant_weight
 from oracle import gptq as ogptq
 from sparsebit_b200 import _lib, ops
@@ -180,14 +180,6 @@ def _quant_linear(k, n, bit, gs, seed):
     ql = QuantLinear(k, n, bit, gs)
     ql.pack(lin, scale, zero)
     return ql.to(dev()), lin.to(dev())
-
-
-@pytest.fixture
-def no_tf32():
-    old = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32 = old
 
 
 @pytest.mark.parametrize("bit,gs", [(4, 128), (3, -1), (2, 64)])

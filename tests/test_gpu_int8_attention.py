@@ -19,47 +19,21 @@ import torch.nn as nn
 
 import int8_attention_ref as ref
 from gpu_util import dev, t
+from gpu_util import no_tf32_autouse  # noqa: F401 -- TF32 off on every test
+from int8_harness import attention_operand, calibrated, cfg, operands_of, p_qparams, scalar
 from sparsebit_b200 import SparsebitB200Error, launch_count, ops
-from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import QAttention, QAttentionInt8, QLinear, QLinearInt8, QMatMul
-from sparsebit_b200.quantization.tools import (CalibrationRunner, to_integer_attentions, to_integer_linears,
-                                               to_integer_matmuls, trace_quant_model)
+from sparsebit_b200.quantization.tools import to_integer_attentions, to_integer_linears, to_integer_matmuls
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
 
 
-@pytest.fixture(autouse=True)
-def _no_tf32():
-    old = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32 = old
-
-
-def _scalar(v):
-    return t(np.array([v], F32))
-
-
-def _operand(rng, shape, pow2, spread=1.0, qrange=(-128, 127)):
-    x = (rng.standard_normal(shape) * spread).astype(F32)
-    qmin, qmax = qrange
-    s = F32(2.0 ** np.round(np.log2(spread * 4 / (qmax - qmin)))) if pow2 else F32(np.abs(x).max() / (0.49 * (qmax - qmin)))
-    z = F32(0 if qmin < 0 else rng.integers(qmin, qmin + 20))
-    return x, s, z, qmin, qmax
-
-
-def _p_qparams(unsigned, pow2):
-    if unsigned:
-        return (F32(2.0 ** -8) if pow2 else F32(1.0 / 255 * 1.37), F32(0), 0, 255)
-    return (F32(2.0 ** -7) if pow2 else F32(1.0 / 127 * 0.93), F32(0), -128, 127)
-
-
 def _run(q, k, v, p, scale=None, return_p=True):
-    qp = [(_scalar(o[1]), _scalar(o[2]), o[3:]) for o in (q, k)]
-    pp = (_scalar(p[0]), _scalar(p[1]), p[2:])
-    vp = (_scalar(v[1]), _scalar(v[2]), v[3:])
+    qp = [(scalar(o[1]), scalar(o[2]), o[3:]) for o in (q, k)]
+    pp = (scalar(p[0]), scalar(p[1]), p[2:])
+    vp = (scalar(v[1]), scalar(v[2]), v[3:])
     return ops.int8_attention(t(q[0]), t(k[0]), t(v[0]), qp[0], qp[1], pp, vp, scale=scale, return_p=return_p)
 
 
@@ -101,34 +75,34 @@ GEOMS = [(2, 1, 1, 8, 8), (3, 31, 64, 40, 8), (2, 64, 31, 64, 40), (2, 65, 65, 8
 def test_geometry_matrix(geom, unsigned_p, scaled, pow2):
     b, tq, tk, d, dv = geom
     rng = np.random.default_rng(abs(hash((geom, unsigned_p, scaled, pow2))) % 2**32)
-    q = _operand(rng, (b, tq, d), pow2, 2.0)
-    k = _operand(rng, (b, tk, d), pow2, 2.0, (0, 255) if d == 40 else (-128, 127))
-    v = _operand(rng, (b, tk, dv), pow2, 1.0, (0, 255) if dv == 64 else (-128, 127))
+    q = attention_operand(rng, (b, tq, d), pow2, 2.0)
+    k = attention_operand(rng, (b, tk, d), pow2, 2.0, (0, 255) if d == 40 else (-128, 127))
+    v = attention_operand(rng, (b, tk, dv), pow2, 1.0, (0, 255) if dv == 64 else (-128, 127))
     scale = (2.0 ** -3 if pow2 else d ** -0.5) if scaled else None
-    _check(q, k, v, _p_qparams(unsigned_p, pow2), scale, f"{geom} unsigned_p={unsigned_p} scale={scale} pow2={pow2}")
+    _check(q, k, v, p_qparams(unsigned_p, pow2), scale, f"{geom} unsigned_p={unsigned_p} scale={scale} pow2={pow2}")
 
 
 def test_scores_are_those_of_the_integer_matmul():
     """With the kernel's p grid fed to int8_matmul as an exact operand, the fused output is int8_matmul's p @ v."""
     rng = np.random.default_rng(3)
-    q, k, v = (_operand(rng, (4, 197, 64), False, 2.0) for _ in range(3))
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, (4, 197, 64), False, 2.0) for _ in range(3))
+    p = p_qparams(True, False)
     y, pq = _run(q, k, v, p, 0.125)
-    s_mm = ops.int8_matmul(t(q[0]), _scalar(q[1]), _scalar(q[2]), q[3:], t(k[0]).transpose(-2, -1), _scalar(k[1]),
-                           _scalar(k[2]), k[3:])
+    s_mm = ops.int8_matmul(t(q[0]), scalar(q[1]), scalar(q[2]), q[3:], t(k[0]).transpose(-2, -1), scalar(k[1]),
+                           scalar(k[2]), k[3:])
     s_ref, _ = ref.scores(q, k)
     assert np.array_equal(s_mm.cpu().numpy(), s_ref)  # the reference's scores are QMatMulInt8's, bit for bit
     # p @ v through int8_matmul on the kernel's grid dequantized to g s_p, which int8_matmul quantizes back to g
     fp = ((pq[..., :197].float() + 128 - p[1]) * float(p[0]))
-    y_mm = ops.int8_matmul(fp, _scalar(p[0]), _scalar(p[1]), p[2:], t(v[0]), _scalar(v[1]), _scalar(v[2]), v[3:])
+    y_mm = ops.int8_matmul(fp, scalar(p[0]), scalar(p[1]), p[2:], t(v[0]), scalar(v[1]), scalar(v[2]), v[3:])
     assert torch.equal(y, y_mm)
 
 
 def test_nan_placement_and_batch_isolation():
     rng = np.random.default_rng(4)
     b, tq, tk, d, dv = 4, 70, 150, 64, 40
-    q, k, v = _operand(rng, (b, tq, d), False), _operand(rng, (b, tk, d), False), _operand(rng, (b, tk, dv), False)
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, shape, False) for shape in ((b, tq, d), (b, tk, d), (b, tk, dv)))
+    p = p_qparams(True, False)
     clean = _run(q, k, v, p, 0.125, return_p=False).cpu().numpy()
     assert np.isfinite(clean).all()
     q[0][1, 5, 3] = np.nan  # row 5 of entry 1
@@ -155,11 +129,11 @@ def test_nan_placement_and_batch_isolation():
 
 def test_determinism_and_graph_replay_after_growth():
     rng = np.random.default_rng(5)
-    q, k, v = (_operand(rng, (6, 197, 64), False) for _ in range(3))
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, (6, 197, 64), False) for _ in range(3))
+    p = p_qparams(True, False)
     qt, kt, vt = t(q[0]), t(k[0]), t(v[0])
-    qp = [(_scalar(o[1]), _scalar(o[2]), o[3:]) for o in (q, k)]
-    pp, vp = (_scalar(p[0]), _scalar(p[1]), p[2:]), (_scalar(v[1]), _scalar(v[2]), v[3:])
+    qp = [(scalar(o[1]), scalar(o[2]), o[3:]) for o in (q, k)]
+    pp, vp = (scalar(p[0]), scalar(p[1]), p[2:]), (scalar(v[1]), scalar(v[2]), v[3:])
 
     def call(x, y, z):
         return ops.int8_attention(x, y, z, qp[0], qp[1], pp, vp, scale=0.125)
@@ -224,10 +198,6 @@ def test_16k_tokens_without_a_t_squared_allocation():
 
 
 # ---------------------------------------------------------------------------------------------- the DeiT-tiny block
-def _cfg(scheme, target, **kw):
-    return sbcfg.quantizer_config(scheme, 8, target, layout="NLC", **kw)
-
-
 class Attention(nn.Module):
     """The attention of a DeiT-tiny block around QAttention: fused qkv projection, the quantized attention, output
     projection."""
@@ -235,12 +205,12 @@ class Attention(nn.Module):
     def __init__(self, dim=192, heads=3):
         super().__init__()
         self.heads, self.head_dim = heads, dim // heads
-        self.qkv = QLinear(nn.Linear(dim, 3 * dim)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                     _cfg("per-channel-symmetric", "weight"))
-        self.attn = QAttention(scale=self.head_dim ** -0.5).build_quantizer(
-            _cfg("per-tensor-symmetric", "feature"), _cfg("per-tensor-affine", "feature"))  # p: unsigned, Z = 0 ... 255
-        self.proj = QLinear(nn.Linear(dim, dim)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                 _cfg("per-channel-symmetric", "weight"))
+        self.qkv = QLinear(nn.Linear(dim, 3 * dim)).build_quantizer(
+            cfg("per-tensor-symmetric", "feature", layout="NLC"), cfg("per-channel-symmetric", "weight"))
+        self.attn = QAttention(scale=self.head_dim ** -0.5).build_quantizer(  # p: unsigned, Z = 0 ... 255
+            cfg("per-tensor-symmetric", "feature", layout="NLC"), cfg("per-tensor-affine", "feature", layout="NLC"))
+        self.proj = QLinear(nn.Linear(dim, dim)).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC"),
+                                                                 cfg("per-channel-symmetric", "weight"))
 
     def forward(self, x):
         qkv = self.qkv(x).reshape(x.shape[0], x.shape[1], 3, self.heads, self.head_dim).permute(2, 0, 3, 1, 4)
@@ -248,37 +218,11 @@ class Attention(nn.Module):
         return self.proj(out)
 
 
-def _calibrated(model, batches, replay):
-    model = model.to(dev())
-    driven = trace_quant_model(model) if replay else model
-    runner = CalibrationRunner(driven, streaming=not replay)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for b in batches:
-            driven(b)
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if getattr(m, "input_quantizer", None) is not None:
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
-def _operands_of(qattn, q, k, v):
-    out = []
-    for carrier, x in ((qattn.qk.left, q), (qattn.qk.right, k), (qattn.pv.right, v)):
-        qz = carrier.input_quantizer
-        s, z = (w.detach().reshape(-1).cpu().numpy() for w in qz._qparams_preprocess(x))
-        out.append((x.float().cpu().numpy(), F32(s[0]), F32(z[0]), *qz.qdesc.qrange))
-    pq = qattn.pv.left.input_quantizer
-    s, z = (w.detach().reshape(-1).cpu().numpy() for w in pq._qparams_preprocess(None))
-    return out, (F32(s[0]), F32(z[0]), *pq.qdesc.qrange)
-
-
 @pytest.mark.parametrize("replay", [False, True])
 def test_deit_tiny_block_converts_and_meets_the_bounds(replay):
     torch.manual_seed(0)
     batches = [torch.randn(4, 197, 192, device=dev()) for _ in range(3)]
-    model = _calibrated(Attention(), batches, replay)
+    model = calibrated(Attention(), batches, streaming=not replay, record_inputs=None, replay=replay)
     original = model.attn
     for carrier in (original.qk.left, original.qk.right, original.pv.left, original.pv.right):
         s = float(carrier.input_quantizer.scale.reshape(-1)[0])
@@ -295,7 +239,7 @@ def test_deit_tiny_block_converts_and_meets_the_bounds(replay):
         for x in batches[:2]:
             model(x)
             (qx, kx, vx), y = seen["attn"]
-            (q, k, v), p = _operands_of(original, qx, kx, vx)
+            (q, k, v), p = operands_of(original, qx, kx, vx)
             T, g64, mm, _ = ref.truth(q, k, v, p, original.scale)
             s, _ = ref.scores(q, k, original.scale)
             lo, hi = ref.admissible_range(ref.softmax64(s), p)
@@ -332,7 +276,7 @@ def test_deit_tiny_block_converts_and_meets_the_bounds(replay):
 
 def test_module_input_forms_and_errors():
     torch.manual_seed(1)
-    qa = QAttention(scale=0.25).build_quantizer(_cfg("per-tensor-symmetric", "feature")).to(dev())
+    qa = QAttention(scale=0.25).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC")).to(dev())
     xs = [torch.randn(2, 3, 20, 16, device=dev()) for _ in range(3)]
     for carrier, x in ((qa.qk.left, xs[0]), (qa.qk.right, xs[1].transpose(-2, -1)), (qa.pv.right, xs[2]),
                        (qa.pv.left, torch.rand(2, 3, 20, 20, device=dev()))):

@@ -20,50 +20,23 @@ import torch.nn as nn
 import int8_attention_mask_ref as mref
 import int8_attention_ref as ref
 from gpu_util import dev, t
+from gpu_util import no_tf32_autouse  # noqa: F401 -- TF32 off on every test
+from int8_harness import attention_operand, calibrated, cfg, check_p, operands_of, p_qparams, scalar
 from int8_matmul_ref import BOUND
 from oracle import qdq as oqdq
 from sparsebit_b200 import launch_count, ops
-from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import QAttention, QAttentionInt8, QLinear, QLinearInt8
-from sparsebit_b200.quantization.tools import (CalibrationRunner, to_integer_attentions, to_integer_linears,
-                                               trace_quant_model)
-from test_gpu_int8_attention_mask_branches import check_p
+from sparsebit_b200.quantization.tools import to_integer_attentions, to_integer_linears
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
 
 
-@pytest.fixture(autouse=True)
-def _no_tf32():
-    old = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32 = old
-
-
-def _scalar(v):
-    return t(np.array([v], F32))
-
-
-def _operand(rng, shape, pow2, spread=1.0, qrange=(-128, 127)):
-    x = (rng.standard_normal(shape) * spread).astype(F32)
-    qmin, qmax = qrange
-    s = F32(2.0 ** np.round(np.log2(spread * 4 / (qmax - qmin)))) if pow2 else F32(np.abs(x).max() / (0.49 * (qmax - qmin)))
-    z = F32(0 if qmin < 0 else rng.integers(qmin, qmin + 20))
-    return x, s, z, qmin, qmax
-
-
-def _p_qparams(unsigned, pow2):
-    if unsigned:
-        return (F32(2.0 ** -8) if pow2 else F32(1.0 / 255 * 1.37), F32(0), 0, 255)
-    return (F32(2.0 ** -7) if pow2 else F32(1.0 / 127 * 0.93), F32(0), -128, 127)
-
-
 def _run(q, k, v, p, scale=None, mask=None, causal=False, return_p=True):
-    qp = [(_scalar(o[1]), _scalar(o[2]), o[3:]) for o in (q, k)]
-    pp = (_scalar(p[0]), _scalar(p[1]), p[2:])
-    vp = (_scalar(v[1]), _scalar(v[2]), v[3:])
+    qp = [(scalar(o[1]), scalar(o[2]), o[3:]) for o in (q, k)]
+    pp = (scalar(p[0]), scalar(p[1]), p[2:])
+    vp = (scalar(v[1]), scalar(v[2]), v[3:])
     m = None if mask is None else (mask if isinstance(mask, torch.Tensor) else t(mask))
     return ops.int8_attention(t(q[0]), t(k[0]), t(v[0]), qp[0], qp[1], pp, vp, scale=scale, return_p=return_p,
                               attn_mask=m, causal=causal)
@@ -116,19 +89,19 @@ MASKS = ["pad_1e4", "pad_inf", "full", "causal", "causal_pad"]
 def test_geometry_matrix(geom, kind, unsigned_p, pow2):
     lead, tq, tk, d, dv = geom
     rng = np.random.default_rng(abs(hash((geom, kind, unsigned_p, pow2))) % 2**32)
-    q = _operand(rng, lead + (tq, d), pow2, 2.0)
-    k = _operand(rng, lead + (tk, d), pow2, 2.0, (0, 255) if d == 40 else (-128, 127))
-    v = _operand(rng, lead + (tk, dv), pow2, 1.0, (0, 255) if dv == 64 else (-128, 127))
+    q = attention_operand(rng, lead + (tq, d), pow2, 2.0)
+    k = attention_operand(rng, lead + (tk, d), pow2, 2.0, (0, 255) if d == 40 else (-128, 127))
+    v = attention_operand(rng, lead + (tk, dv), pow2, 1.0, (0, 255) if dv == 64 else (-128, 127))
     scale = 2.0 ** -3 if pow2 else d ** -0.5
     mask, causal = _mask(kind, rng, lead, tq, tk)
-    _check(q, k, v, _p_qparams(unsigned_p, pow2), scale, mask, causal, f"{geom} {kind} unsigned_p={unsigned_p}")
+    _check(q, k, v, p_qparams(unsigned_p, pow2), scale, mask, causal, f"{geom} {kind} unsigned_p={unsigned_p}")
 
 
 def test_mask_identities():
     rng = np.random.default_rng(11)
     lead, tq, tk = (2, 3), 300, 300
-    q, k, v = (_operand(rng, lead + (tq, 64), False, 2.0) for _ in range(3))
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, lead + (tq, 64), False, 2.0) for _ in range(3))
+    p = p_qparams(True, False)
     y0, g0 = _run(q, k, v, p, 0.125)
     yz, gz = _run(q, k, v, p, 0.125, mask=np.zeros((lead[0], 1, 1, tk), F32))  # the masked kernel with a zero mask
     assert torch.equal(y0, yz) and torch.equal(g0, gz)
@@ -149,8 +122,8 @@ def test_mask_identities():
 def test_nan_placement():
     rng = np.random.default_rng(12)
     lead, tq, tk, d, dv = (3,), 260, 260, 64, 40
-    q, k, v = _operand(rng, lead + (tq, d), False), _operand(rng, lead + (tk, d), False), _operand(rng, lead + (tk, dv), False)
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, shape, False) for shape in (lead + (tq, d), lead + (tk, d), lead + (tk, dv)))
+    p = p_qparams(True, False)
     clean = _run(q, k, v, p, 0.125, causal=True, return_p=False).cpu().numpy()
     assert np.isfinite(clean).all()
     k[0][0, 150, 2] = np.nan  # entry 0: rows >= 150 see key 150
@@ -164,8 +137,8 @@ def test_nan_placement():
     assert np.array_equal(np.isnan(y), expect)
     assert np.array_equal(y[~expect], clean[~expect])
     # rows without a visible key: causal with Tq > Tk, and an all -inf mask row
-    q2 = _operand(rng, (2, 200, d), False)
-    k2, v2 = _operand(rng, (2, 50, d), False), _operand(rng, (2, 50, dv), False)
+    q2 = attention_operand(rng, (2, 200, d), False)
+    k2, v2 = attention_operand(rng, (2, 50, d), False), attention_operand(rng, (2, 50, dv), False)
     m = np.zeros((2, 1, 50), F32)
     m[1, 0, :] = -np.inf
     y2 = _run(q2, k2, v2, p, 0.125, mask=m, return_p=False).cpu().numpy()
@@ -177,8 +150,8 @@ def test_nan_placement():
 def test_batch_isolation_through_a_broadcast_mask():
     rng = np.random.default_rng(13)
     b, h, tq, tk, d = 4, 3, 128, 333, 64
-    q, k, v = (_operand(rng, (b, h, n, d), False) for n in (tq, tk, tk))
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, (b, h, n, d), False) for n in (tq, tk, tk))
+    p = p_qparams(True, False)
     lens = [333, 200, 1, 129]
     m = np.zeros((b, 1, 1, tk), F32)
     for e, n in enumerate(lens):
@@ -193,13 +166,13 @@ def test_batch_isolation_through_a_broadcast_mask():
 def test_determinism_and_graph_replay_after_growth():
     rng = np.random.default_rng(15)
     lead = (2, 3)
-    q, k, v = (_operand(rng, lead + (300, 64), False) for _ in range(3))
-    p = _p_qparams(True, False)
+    q, k, v = (attention_operand(rng, lead + (300, 64), False) for _ in range(3))
+    p = p_qparams(True, False)
     qt, kt, vt = t(q[0]), t(k[0]), t(v[0])
     mask = torch.zeros(2, 1, 1, 300, device=dev())
     mask[1, ..., 250:] = -10000.0
-    qp = [(_scalar(o[1]), _scalar(o[2]), o[3:]) for o in (q, k)]
-    pp, vp = (_scalar(p[0]), _scalar(p[1]), p[2:]), (_scalar(v[1]), _scalar(v[2]), v[3:])
+    qp = [(scalar(o[1]), scalar(o[2]), o[3:]) for o in (q, k)]
+    pp, vp = (scalar(p[0]), scalar(p[1]), p[2:]), (scalar(v[1]), scalar(v[2]), v[3:])
 
     def call(x, y, z, m=mask):
         return ops.int8_attention(x, y, z, qp[0], qp[1], pp, vp, scale=0.125, attn_mask=m, causal=True)
@@ -271,10 +244,6 @@ def test_16k_tokens_causal_padded_without_a_t_squared_allocation():
 
 
 # ---------------------------------------------------------------------------------------------- the synthetic blocks
-def _cfg(scheme, target, **kw):
-    return sbcfg.quantizer_config(scheme, 8, target, layout="NLC", **kw)
-
-
 class Block(nn.Module):
     """A transformer attention around QAttention: fused qkv projection, the quantized attention with a mask, output
     projection.  ``causal=False``: BERT-style, a [B, 1, 1, T] key-padding mask (1 - m) * -10000; ``causal=True``:
@@ -283,44 +252,18 @@ class Block(nn.Module):
     def __init__(self, causal, dim=192, heads=3):
         super().__init__()
         self.causal, self.heads, self.head_dim = causal, heads, dim // heads
-        self.qkv = QLinear(nn.Linear(dim, 3 * dim)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                     _cfg("per-channel-symmetric", "weight"))
+        self.qkv = QLinear(nn.Linear(dim, 3 * dim)).build_quantizer(
+            cfg("per-tensor-symmetric", "feature", layout="NLC"), cfg("per-channel-symmetric", "weight"))
         self.attn = QAttention(scale=self.head_dim ** -0.5).build_quantizer(
-            _cfg("per-tensor-symmetric", "feature"), _cfg("per-tensor-affine", "feature"))
-        self.proj = QLinear(nn.Linear(dim, dim)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                 _cfg("per-channel-symmetric", "weight"))
+            cfg("per-tensor-symmetric", "feature", layout="NLC"), cfg("per-tensor-affine", "feature", layout="NLC"))
+        self.proj = QLinear(nn.Linear(dim, dim)).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC"),
+                                                                 cfg("per-channel-symmetric", "weight"))
 
     def forward(self, x, keep):
         mask = (1.0 - keep[:, None, None, :]) * -10000.0
         qkv = self.qkv(x).reshape(x.shape[0], x.shape[1], 3, self.heads, self.head_dim).permute(2, 0, 3, 1, 4)
         out = self.attn(qkv[0], qkv[1], qkv[2], attn_mask=mask, causal=self.causal)
         return self.proj(out.transpose(1, 2).reshape(x.shape[0], x.shape[1], -1))
-
-
-def _calibrated(model, batches, replay):
-    model = model.to(dev())
-    driven = trace_quant_model(model) if replay else model
-    runner = CalibrationRunner(driven, streaming=not replay)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for x, keep in batches:
-            driven(x, keep)
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if getattr(m, "input_quantizer", None) is not None:
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
-def _operands_of(qattn, q, k, v):
-    out = []
-    for carrier, x in ((qattn.qk.left, q), (qattn.qk.right, k), (qattn.pv.right, v)):
-        qz = carrier.input_quantizer
-        s, z = (w.detach().reshape(-1).cpu().numpy() for w in qz._qparams_preprocess(x))
-        out.append((x.float().cpu().numpy(), F32(s[0]), F32(z[0]), *qz.qdesc.qrange))
-    pq = qattn.pv.left.input_quantizer
-    s, z = (w.detach().reshape(-1).cpu().numpy() for w in pq._qparams_preprocess(None))
-    return out, (F32(s[0]), F32(z[0]), *pq.qdesc.qrange)
 
 
 @pytest.mark.parametrize("causal", [False, True], ids=["bert_padding", "gpt2_causal"])
@@ -334,7 +277,7 @@ def test_synthetic_block_converts_and_meets_the_bounds(causal, replay):
         keep[1, t_len - 40:] = 0
         keep[3, t_len // 2:] = 0
         batches.append((torch.randn(4, t_len, 192, device=dev()), keep))
-    model = _calibrated(Block(causal), batches, replay)
+    model = calibrated(Block(causal), batches, streaming=not replay, record_inputs=None, replay=replay)
     original = model.attn
     for carrier in (original.qk.left, original.qk.right, original.pv.left, original.pv.right):
         s = float(carrier.input_quantizer.scale.reshape(-1)[0])
@@ -351,7 +294,7 @@ def test_synthetic_block_converts_and_meets_the_bounds(causal, replay):
             (qx, kx, vx), kw, y = seen["attn"]
             mask = kw["attn_mask"]
             assert kw["causal"] == causal
-            (q, k, v), p = _operands_of(original, qx, kx, vx)
+            (q, k, v), p = operands_of(original, qx, kx, vx)
             m = mask.cpu().numpy()
             T, g64, mm, _ = mref.truth(q, k, v, p, original.scale, m, causal)
             s, bad = mref.scores(q, k, original.scale, m, causal)
@@ -384,7 +327,7 @@ def test_synthetic_block_converts_and_meets_the_bounds(causal, replay):
 
 def test_module_masks():
     torch.manual_seed(1)
-    qa = QAttention(scale=0.25).build_quantizer(_cfg("per-tensor-symmetric", "feature")).to(dev())
+    qa = QAttention(scale=0.25).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC")).to(dev())
     xs = [torch.randn(2, 3, 20, 16, device=dev()) for _ in range(3)]
     for carrier, x in ((qa.qk.left, xs[0]), (qa.qk.right, xs[1].transpose(-2, -1)), (qa.pv.right, xs[2]),
                        (qa.pv.left, torch.rand(2, 3, 20, 20, device=dev()))):

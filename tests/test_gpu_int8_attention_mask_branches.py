@@ -12,6 +12,7 @@ import int8_attention_mask_ref as mref
 import int8_attention_ref as ref
 from gpu_util import dev, t
 from int8_attention_ref import PSENT, SENTINEL, TAIL
+from int8_harness import check_p
 from sparsebit_b200 import _lib, ops
 
 F32 = np.float32
@@ -51,23 +52,6 @@ def _inputs(name):
         v[-1, -1, 220, 5] = np.nan
     p = (F32(1 / 255), F32(0), 0, 255)
     return lead, ref.case_operands(q, k, v), p, 0.125, mask, causal, p_q
-
-
-def check_p(g, s, bad, p, tq, tk, causal, label):
-    """g [..., Tq, >= Tk] the kernel's stored p grid: admissible on the rows without NaN, the grid of 0 where the
-    composition's p is exactly 0 (a -inf score, which covers the skipped keys), 0 (the grid of NaN) on rows without a
-    visible key, the padding 0."""
-    assert not g[..., tk:].any(), label
-    gg = g[..., :tk].astype(np.int64)
-    lo, hi = ref.admissible_range(mref.softmax64(s), p)
-    assert np.all(((gg >= lo) & (gg <= hi))[~bad]), label
-    zero = (s == -np.inf) & ~bad[..., None]
-    assert np.all(gg[zero] == mref.p_zero_grid(p)), label
-    with np.errstate(invalid="ignore"):
-        empty = np.where(np.isnan(s), F32(0), s).max(-1) == -np.inf
-    assert not gg[empty].any(), label
-    sk = np.broadcast_to(mref.skipped(tq, tk, causal), gg.shape)
-    assert np.all(gg[sk & ~empty[..., None]] == mref.p_zero_grid(p)), label
 
 
 @pytest.mark.gpu

@@ -55,7 +55,7 @@ import torch
 
 import int8_geometry as geo
 from branch_cases import C, assert_table_covers, check_reach, params
-from gpu_util import dev, on_device, seed, stream
+from gpu_util import dev, no_tf32, on_device, seed, stream  # noqa: F401 -- no_tf32: a fixture
 from int8_conv_ref import integer_terms as conv_integer_terms
 from int8_conv_ref import lowered, to_nchw
 from int8_conv_ref import truth as conv_truth
@@ -307,15 +307,6 @@ def within_truth(y, t, bound):
     ok = ~np.isnan(t)
     err = np.abs(y[ok] - t[ok])
     assert np.all(err <= bound[ok]), f"max error {err.max():.3g} over the 2^-21 bound"
-
-
-@pytest.fixture
-def no_tf32():
-    """The fp64 truths run on the CPU; a test that compares against a device matmul must not get TF32 either."""
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
 
 
 # -------------------------------------------------------------------------------------------------- quantizers

@@ -15,24 +15,17 @@ import torch
 import torch.nn as nn
 
 from gpu_util import dev, t
-from int8_conv_ref import BOUND, grid_offset, lowered, truth
+from gpu_util import no_tf32_autouse  # noqa: F401 -- TF32 off on every test
+from int8_conv_ref import lowered, truth
+from int8_harness import calibrated, cfg, check_converted, layer_qparams, qrange, stored_rows, wrap_quantized
 from oracle import observers as oobs
 from sparsebit_b200 import SparsebitB200Error, ops
-from sparsebit_b200 import config as sbcfg
-from sparsebit_b200.quantization.modules import QConv2d, QConv2dInt8, QLinear, QReLU, resolve_conv_padding
-from sparsebit_b200.quantization.tools import CalibrationRunner, to_integer_convs
+from sparsebit_b200.quantization.modules import QConv2d, QConv2dInt8, QLinear, QReLU
+from sparsebit_b200.quantization.tools import to_integer_convs
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
-
-
-@pytest.fixture(autouse=True)
-def _no_tf32():
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
 
 
 # ---------------------------------------------------------------------------------------------- the lowering
@@ -114,26 +107,12 @@ def test_lowering_far_end_of_a_workspace_past_2_31():
 
 
 # ---------------------------------------------------------------------------------------------- the conv
-def _weights(w, ws, wz, wqmin, wqmax):
-    c_out = w.shape[0]
-    ws = np.broadcast_to(np.asarray(ws, F32).reshape(-1), (c_out,)).copy()
-    wz = np.broadcast_to(np.asarray(wz, F32).reshape(-1), (c_out,)).copy()
-    w_q, w_sum, w_nan = ops.int8_quantize_rows(t(w.reshape(c_out, -1)), t(ws), t(wz), wqmin, wqmax)
-    w_scale = torch.where(w_nan, torch.full_like(t(ws), float("nan")), t(ws))
-    w_zero = t((np.rint(wz) - grid_offset(wqmin)).astype(np.int32))
-    return w_q, w_sum, w_scale, w_zero
-
-
 def _run(args, bias=None, stride=1, padding=0, dilation=1):
     x, xs, xz, xqmin, xqmax, w, ws, wz, wqmin, wqmax = args
-    w_q, w_sum, w_scale, w_zero = _weights(w, ws, wz, wqmin, wqmax)
+    w_q, w_sum, w_scale, w_zero = stored_rows(w, ws, wz, wqmin, wqmax)
     y = ops.int8_conv2d(t(x), t(np.array([xs], F32)), t(np.array([xz], F32)), xqmin, xqmax, w_q, w_sum, w_scale, w_zero,
                         w.shape[2:], None if bias is None else t(bias), stride, padding, dilation)
     return y.cpu().numpy()
-
-
-def _range(bits, affine):
-    return (0, (1 << bits) - 1) if affine else (-(1 << (bits - 1)), (1 << (bits - 1)) - 1)
 
 
 CONVS = [
@@ -149,8 +128,8 @@ CONVS = [
 
 
 @pytest.mark.parametrize("conv", CONVS)
-@pytest.mark.parametrize("xr,wr", [((-128, 127), (-128, 127)), ((0, 255), (-128, 127)), (_range(4, True), _range(4, False)),
-                                   (_range(2, False), _range(2, True))])
+@pytest.mark.parametrize("xr,wr", [((-128, 127), (-128, 127)), ((0, 255), (-128, 127)), (qrange(4, True), qrange(4, False)),
+                                   (qrange(2, False), qrange(2, True))])
 def test_exact_mode(conv, xr, wr):
     n, c, h, w, c_out, kernel, stride, padding, dilation = conv
     kh, kw = (kernel, kernel) if isinstance(kernel, int) else kernel
@@ -205,9 +184,8 @@ def _qconv_from(args, bias, stride, padding):
         conv.weight.copy_(torch.from_numpy(wt))
         if bias is not None:
             conv.bias.copy_(torch.from_numpy(bias))
-    q = QConv2d(conv).build_quantizer(sbcfg.quantizer_config("per-tensor-affine" if xqmin >= 0 else "per-tensor-symmetric", 8,
-                                                             "feature"),
-                                      sbcfg.quantizer_config("per-channel-symmetric", 8, "weight")).to(dev())
+    q = QConv2d(conv).build_quantizer(cfg("per-tensor-affine" if xqmin >= 0 else "per-tensor-symmetric", "feature"),
+                                      cfg("per-channel-symmetric", "weight")).to(dev())
     q.input_quantizer.scale = t(np.array([xs], F32))
     q.input_quantizer.zero_point = t(np.array([xz], F32))
     q.weight_quantizer.scale = t(np.asarray(ws, F32).reshape(-1, 1, 1, 1))
@@ -254,7 +232,7 @@ def test_deterministic_and_graph_replay():
     rng = np.random.default_rng(23)
     args, bias = _minmax_case(rng, 4, 64, 28, 28, 96, 3, 3, True, True)
     x, xs, xz, xqmin, xqmax, wt, ws, wz, wqmin, wqmax = args
-    w_q, w_sum, w_scale, w_zero = _weights(wt, ws, wz, wqmin, wqmax)
+    w_q, w_sum, w_scale, w_zero = stored_rows(wt, ws, wz, wqmin, wqmax)
     xt, xst, xzt, bt = t(x), t(np.array([xs], F32)), t(np.array([xz], F32)), t(bias)
 
     def call():
@@ -290,27 +268,23 @@ def test_k_limit_is_unsupported():
 
 
 # ---------------------------------------------------------------------------------------------- modules
-def _cfg(scheme, target, **kw):
-    return sbcfg.quantizer_config(scheme, 8, target, layout="NCHW", **kw)
-
-
 class CnnHead(nn.Module):
     """A stem conv (symmetric), an affine-activation padded 3x3 conv, a strided 1x1 conv, a grouped conv (not
     eligible) and a classifier."""
 
     def __init__(self):
         super().__init__()
-        self.conv1 = QConv2d(nn.Conv2d(3, 16, 3, stride=2)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                            _cfg("per-channel-symmetric", "weight"))
-        self.relu = QReLU().build_quantizer(_cfg("per-tensor-symmetric", "feature", disable=True))
-        self.conv2 = QConv2d(nn.Conv2d(16, 32, 3, padding=1)).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                              _cfg("per-channel-symmetric", "weight"))
+        self.conv1 = QConv2d(nn.Conv2d(3, 16, 3, stride=2)).build_quantizer(cfg("per-tensor-symmetric", "feature"),
+                                                                            cfg("per-channel-symmetric", "weight"))
+        self.relu = QReLU().build_quantizer(cfg("per-tensor-symmetric", "feature", disable=True))
+        self.conv2 = QConv2d(nn.Conv2d(16, 32, 3, padding=1)).build_quantizer(cfg("per-tensor-affine", "feature"),
+                                                                              cfg("per-channel-symmetric", "weight"))
         self.conv3 = QConv2d(nn.Conv2d(32, 24, 1, stride=2, bias=False)).build_quantizer(
-            _cfg("per-tensor-affine", "feature"), _cfg("per-tensor-symmetric", "weight"))
-        self.dw = QConv2d(nn.Conv2d(24, 24, 3, padding=1, groups=24)).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                                      _cfg("per-channel-symmetric", "weight"))
-        self.fc = QLinear(nn.Linear(24, 10)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                             _cfg("per-tensor-symmetric", "weight"))
+            cfg("per-tensor-affine", "feature"), cfg("per-tensor-symmetric", "weight"))
+        self.dw = QConv2d(nn.Conv2d(24, 24, 3, padding=1, groups=24)).build_quantizer(cfg("per-tensor-affine", "feature"),
+                                                                                      cfg("per-channel-symmetric", "weight"))
+        self.fc = QLinear(nn.Linear(24, 10)).build_quantizer(cfg("per-tensor-symmetric", "feature"),
+                                                             cfg("per-tensor-symmetric", "weight"))
 
     def forward(self, x):
         x = self.relu(self.conv2(self.conv1(x)))  # conv2 sees signed input: affine activations with Z != 0, padded
@@ -318,70 +292,27 @@ class CnnHead(nn.Module):
         return self.fc(self.dw(x).mean(dim=(2, 3)))
 
 
-def _calibrated(model, batches, streaming=True):
-    model = model.to(dev())
-    runner = CalibrationRunner(model, streaming=streaming, record_inputs=False)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for b in batches:
-            model(b)
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if hasattr(m, "set_quant") and callable(m.set_quant) and getattr(m, "input_quantizer", None) is not None:
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
-def _layer_truth(qconv, x):
-    aq, wq = qconv.input_quantizer, qconv.weight_quantizer
-    xs, xz = (v.detach().reshape(-1).cpu().numpy() for v in aq._qparams_preprocess(x))
-    ws, wz = (v.detach().reshape(-1).cpu().numpy() for v in wq._qparams_preprocess(qconv.weight))
-    b = qconv.bias.detach().cpu().numpy() if qconv.bias is not None else None
-    kw = qconv.fwd_kwargs
-    pad = resolve_conv_padding(kw["padding"], qconv.weight.shape[2:], kw["dilation"], kw["stride"])
-    return truth(x.cpu().numpy(), xs[0], xz[0], *aq.qdesc.qrange, qconv.weight.detach().cpu().numpy(), ws, wz,
-                 *wq.qdesc.qrange, bias=b, stride=kw["stride"], padding=pad, dilation=kw["dilation"])
-
-
-def _check_converted(model, originals, inputs, names, compare_fake_quant=True):
-    seen = {}
-    hooks = [model.get_submodule(nm).register_forward_hook(lambda mod, i, o, nm=nm: seen.__setitem__(nm, (i[0], o)))
-             for nm in names]
-    with torch.no_grad():
-        for x in inputs:
-            model(x)
-            for nm in names:
-                xin, y = seen[nm]
-                assert isinstance(model.get_submodule(nm), QConv2dInt8)
-                t_, bound = _layer_truth(originals[nm], xin)
-                y = y.cpu().numpy()
-                err = np.abs(y - t_)
-                assert np.all(err <= bound), (nm, float((err / bound).max()))
-                if compare_fake_quant:  # QDQ + cuDNN fp32 conv: within its own fp32 accumulation error of the truth
-                    ref = originals[nm](xin).cpu().numpy()
-                    k = originals[nm].weight[0].numel()
-                    assert np.all(np.abs(ref - t_) <= 2.0 ** -22 * k * bound / BOUND), nm
-                    print(f"{nm}: int8 max |y - T| = {err.max():.3e}, fake-quant max |y - T| = {np.abs(ref - t_).max():.3e}")
-    for h in hooks:
-        h.remove()
+def _truth_of(qconv, x):
+    return truth(**layer_qparams(qconv, x))
 
 
 def test_cnn_head_converts_and_meets_the_bound():
     torch.manual_seed(0)
     batches = [torch.randn(8, 3, 33, 33, device=dev()) for _ in range(3)]
-    model = _calibrated(CnnHead(), batches)
+    model = calibrated(CnnHead(), batches, streaming=True, record_inputs=False)
     names = ["conv1", "conv2", "conv3"]
     originals = {nm: getattr(model, nm) for nm in names}
     assert to_integer_convs(model) == names
     assert isinstance(model.dw, QConv2d) and isinstance(model.fc, QLinear)  # grouped conv and the linear stay
     assert model.conv2.qmin == 0 and float(model.conv2.zero_point) != 0  # affine activations, padded
-    _check_converted(model, originals, batches[:2], names)
+    check_converted(model, originals, batches[:2], names, expected_cls=QConv2dInt8, layer_truth=_truth_of,
+                    compare_fake_quant=True)
 
 
 def test_module_input_forms():
     torch.manual_seed(2)
     batches = [torch.randn(4, 3, 33, 33, device=dev())]
-    model = _calibrated(CnnHead(), batches)
+    model = calibrated(CnnHead(), batches, streaming=True, record_inputs=False)
     to_integer_convs(model)
     conv = model.conv2
     x = torch.randn(3, 16, 16, 16, device=dev())
@@ -400,34 +331,18 @@ def test_module_input_forms():
         conv(xg)
 
 
-def _wrapped_resnet18():
+def test_resnet18_converts_every_conv_and_meets_the_bound():
     import torchvision
 
     torch.manual_seed(0)
-    net = torchvision.models.resnet18(weights=None).eval()
-
-    def wrap(module):
-        for name, child in list(module.named_children()):
-            if isinstance(child, nn.Conv2d):
-                setattr(module, name, QConv2d(child).build_quantizer(sbcfg.quantizer_config("per-tensor-affine", 8, "feature"),
-                                                                     sbcfg.quantizer_config("per-channel-symmetric", 8, "weight")))
-            elif isinstance(child, nn.Linear):
-                setattr(module, name, QLinear(child).build_quantizer(sbcfg.quantizer_config("per-tensor-affine", 8, "feature"),
-                                                                     sbcfg.quantizer_config("per-channel-symmetric", 8, "weight")))
-            else:
-                wrap(child)
-
-    wrap(net)
-    return net
-
-
-def test_resnet18_converts_every_conv_and_meets_the_bound():
-    qnet = _wrapped_resnet18()
+    qnet = wrap_quantized(torchvision.models.resnet18(weights=None).eval(), cfg("per-tensor-affine", "feature"),
+                          cfg("per-channel-symmetric", "weight"))
     torch.manual_seed(1)
     batches = [torch.randn(4, 3, 112, 112, device=dev()) for _ in range(2)]
-    qnet = _calibrated(qnet, batches)
+    qnet = calibrated(qnet, batches, streaming=True, record_inputs=False)
     originals = {nm: m for nm, m in qnet.named_modules() if isinstance(m, QConv2d)}
     names = to_integer_convs(qnet)
     assert len(names) == 20 and names == list(originals)
     assert isinstance(qnet.fc, QLinear)
-    _check_converted(qnet, originals, [batches[0][:2]], names, compare_fake_quant=False)
+    check_converted(qnet, originals, [batches[0][:2]], names, expected_cls=QConv2dInt8, layer_truth=_truth_of,
+                    compare_fake_quant=False)

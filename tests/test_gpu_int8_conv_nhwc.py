@@ -11,11 +11,10 @@ import torch.nn as nn
 
 import int8_sparse24_ref as ref
 from gpu_util import bits_equal, dev, on_device, t
-from int8_conv_ref import grid_offset
+from int8_harness import calibrated, cfg, stored_rows, wrap_quantized
 from sparsebit_b200 import _lib, ops
-from sparsebit_b200 import config as sbcfg
-from sparsebit_b200.quantization.modules import QConv2d, QConv2dGroupInt8, QConv2dInt8, QConv2dSparse24Int8, QLinear
-from sparsebit_b200.quantization.tools import CalibrationRunner, to_integer_convs, to_integer_group_convs
+from sparsebit_b200.quantization.modules import QConv2d, QConv2dInt8
+from sparsebit_b200.quantization.tools import to_integer_convs, to_integer_group_convs
 
 pytestmark = pytest.mark.gpu
 
@@ -125,14 +124,6 @@ def test_lowering_far_end_of_a_workspace_past_2_31(n, c, h, kernel, padding):
 
 
 # ---------------------------------------------------------------------------------------------- dense and 2:4 conv
-def _stored(w, ws, wr):
-    rows = w.reshape(w.shape[0], -1)
-    w_q, w_sum, w_nan = ops.int8_quantize_rows(t(rows), t(ws), t(np.zeros_like(ws)), *wr)
-    w_scale = torch.where(w_nan, torch.full_like(t(ws), float("nan")), t(ws))
-    w_zero = torch.full((w.shape[0],), -grid_offset(wr[0]), dtype=torch.int32, device=dev())
-    return w_q, w_sum, w_scale, w_zero
-
-
 def _nhwc_into_sentinel(fn, xc, g, args, c_out, oh, ow, workspace=True):
     out = torch.full((g.n, c_out, oh, ow), SENTINEL, device=dev()).to(memory_format=torch.channels_last)
     lib = _lib.load()
@@ -175,7 +166,7 @@ def test_dense_and_sparse_conv_equal_the_nchw_entry_points(geom):
     wt[c_out // 2, 0, 0, 0] = np.nan  # a NaN weight row
     bias = rng.standard_normal(c_out).astype(F32)
     s, z = t(np.array([2.0 ** -4], F32)), t(np.array([0.0 if xr[0] < 0 else 131.0], F32))
-    w_q, w_sum, w_scale, w_zero = _stored(wt, ws, wr)
+    w_q, w_sum, w_scale, w_zero = stored_rows(wt, ws, np.zeros_like(ws), *wr)
     bt = t(bias)
     y0 = ops.int8_conv2d(t(x), s, z, *xr, w_q, w_sum, w_scale, w_zero, (kh, kw), bt, stride, padding, dilation)
     g = _geom(x.shape, (kh, kw), stride, padding, dilation)
@@ -232,7 +223,7 @@ def test_group_conv_equals_the_nchw_entry_point(geom):
     ws = (rng.uniform(0.5, 2.0, c_out) * 2.0 ** -6).astype(F32)
     wt = (rng.uniform(-0.45, 0.45, (c_out, c // groups, kernel, kernel)) * 255 * ws[:, None, None, None]).astype(F32)
     s, z = t(np.array([2.0 ** -4], F32)), t(np.array([0.0 if xr[0] < 0 else 131.0], F32))
-    w_q, w_sum, w_scale, w_zero = _stored(wt, ws, wr)
+    w_q, w_sum, w_scale, w_zero = stored_rows(wt, ws, np.zeros_like(ws), *wr)
     for bt in (t(rng.standard_normal(c_out).astype(F32)), None):
         y0 = ops.int8_group_conv2d(t(x), s, z, *xr, w_q, w_sum, w_scale, w_zero, kernel, groups, bt, stride, padding,
                                    dilation)
@@ -258,9 +249,9 @@ def test_deterministic_and_graph_replay():
     wd = (rng.uniform(-0.45, 0.45, (64, 64, 3, 3)) * 255 * 2.0 ** -6).astype(F32)
     wd = np.where(ref.mask24(rng.standard_normal(wd.shape).astype(F32)), wd, F32(0))
     wg = (rng.uniform(-0.45, 0.45, (64, 1, 3, 3)) * 255 * 2.0 ** -6).astype(F32)
-    dq, dsm, dsc, dz = _stored(wd, ws, SIGNED)
+    dq, dsm, dsc, dz = stored_rows(wd, ws, np.zeros_like(ws), *SIGNED)
     vals, meta, dsum, _ = ops.int8_sparse24_pack(dq, dz, dsc, 64 * 9)
-    gq, gsm, gsc, gz = _stored(wg, ws, SIGNED)
+    gq, gsm, gsc, gz = stored_rows(wg, ws, np.zeros_like(ws), *SIGNED)
     calls = [
         lambda: ops.int8_im2col_quantize_nhwc(x, 3, s, z, -128, 127, 1, 1)[0],
         lambda: ops.int8_conv2d_nhwc(x, s, z, -128, 127, dq, dsm, dsc, dz, 3, None, 1, 1),
@@ -285,40 +276,6 @@ def test_deterministic_and_graph_replay():
 
 
 # ---------------------------------------------------------------------------------------------- modules and models
-def _cfg(scheme, target):
-    return sbcfg.quantizer_config(scheme, 8, target, layout="NCHW")
-
-
-def _calibrated(model, batches):
-    model = model.to(dev())
-    runner = CalibrationRunner(model, streaming=True, record_inputs=False)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for b in batches:
-            model(b)
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if hasattr(m, "set_quant") and callable(m.set_quant) and getattr(m, "input_quantizer", None) is not None:
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
-def _wrapped(net):
-    def wrap(module):
-        for name, child in list(module.named_children()):
-            if isinstance(child, nn.Conv2d):
-                setattr(module, name, QConv2d(child).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                     _cfg("per-channel-symmetric", "weight")))
-            elif isinstance(child, nn.Linear):
-                setattr(module, name, QLinear(child).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                     _cfg("per-channel-symmetric", "weight")))
-            else:
-                wrap(child)
-
-    wrap(net)
-    return net
-
-
 def _outputs(model, x, names):
     seen = {}
     hooks = [model.get_submodule(nm).register_forward_hook(lambda mod, i, o, nm=nm: seen.__setitem__(nm, o))
@@ -335,9 +292,10 @@ def test_converted_model_channels_last_equals_nchw(arch):
     import torchvision
 
     torch.manual_seed(3)
-    qnet = _wrapped(getattr(torchvision.models, arch)(weights=None).eval())
+    qnet = wrap_quantized(getattr(torchvision.models, arch)(weights=None).eval(), cfg("per-tensor-affine", "feature"),
+                          cfg("per-channel-symmetric", "weight"))
     batches = [torch.randn(2, 3, 96, 96, device=dev()) for _ in range(2)]
-    qnet = _calibrated(qnet, batches)
+    qnet = calibrated(qnet, batches, streaming=True, record_inputs=False)
     names = to_integer_convs(qnet) + to_integer_group_convs(qnet)
     assert len(names) == (20 if arch == "resnet18" else 52)
     x = batches[0]
@@ -351,9 +309,9 @@ def test_converted_model_channels_last_equals_nchw(arch):
 
 def test_module_routes_by_memory_format():
     torch.manual_seed(4)
-    q = QConv2d(nn.Conv2d(16, 32, 3, padding=1)).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                 _cfg("per-channel-symmetric", "weight"))
-    q = _calibrated(q, [torch.randn(4, 16, 12, 12, device=dev())])
+    q = QConv2d(nn.Conv2d(16, 32, 3, padding=1)).build_quantizer(cfg("per-tensor-affine", "feature"),
+                                                                 cfg("per-channel-symmetric", "weight"))
+    q = calibrated(q, [torch.randn(4, 16, 12, 12, device=dev())], streaming=True, record_inputs=False)
     conv = QConv2dInt8.from_qconv2d(q)
     x = torch.randn(3, 16, 12, 12, device=dev())
     with torch.no_grad():

@@ -15,7 +15,8 @@ import test_gpu_int8_branches as lin_suite
 import test_gpu_int8_conv_nhwc_branches as nhwc_suite
 import test_gpu_int8_group_branches as grp_suite
 from gpu_util import bits_equal, dev, seed
-from sparsebit_b200 import SparsebitB200Error, config as sbcfg, ops
+from int8_harness import calibrated, cfg, wrap_quantized
+from sparsebit_b200 import SparsebitB200Error, ops
 from sparsebit_b200.quantization.modules import (QConv2d, QConv2dDoReFaInt8, QConv2dGroupDoReFaInt8, QConv2dGroupInt8,
                                                  QConv2dInt8, QLinear, QLinearDoReFaInt8, QLinearInt8,
                                                  dorefa_adaround_ineligibility, from_dorefa_adaround)
@@ -153,17 +154,13 @@ def test_x_absmax_is_checked():
 
 
 # ----------------------------------------------------------------------------- layers
-def _cfg(qtype, target, scheme, bit=4):
-    return sbcfg.quantizer_config(scheme, bit, target, qtype=qtype)
-
-
 def _layer(kind, a_type, w_type, groups=1, bit=4, w_scheme="per-channel-symmetric", a_scheme="per-tensor-affine", seed_=0):
     torch.manual_seed(seed_)
     if kind == "linear":
         mod = QLinear(nn.Linear(40, 24))
     else:
         mod = QConv2d(nn.Conv2d(16, 16 if groups > 1 else 24, 3, padding=1, groups=groups))
-    mod.build_quantizer(_cfg(a_type, "feature", a_scheme, bit), _cfg(w_type, "weight", w_scheme, bit))
+    mod.build_quantizer(cfg(a_scheme, "feature", bit, qtype=a_type), cfg(w_scheme, "weight", bit, qtype=w_type))
     mod = mod.to(dev()).eval()
     x = torch.randn(4, 40, device=dev()) if kind == "linear" else torch.randn(2, 16, 10, 10, device=dev())
     for q, v in ((mod.input_quantizer, x), (mod.weight_quantizer, mod.weight)):
@@ -288,44 +285,20 @@ def test_deterministic_and_graph_replay():
 
 
 # ----------------------------------------------------------------------------- models
-def _wrap(model, a_type, w_type, bit):
-    for name, child in list(model.named_children()):
-        if isinstance(child, nn.Conv2d):
-            setattr(model, name, QConv2d(child).build_quantizer(_cfg(a_type, "feature", "per-tensor-affine", bit),
-                                                                _cfg(w_type, "weight", "per-channel-symmetric", bit)))
-        elif isinstance(child, nn.Linear):
-            setattr(model, name, QLinear(child).build_quantizer(_cfg(a_type, "feature", "per-tensor-affine", bit),
-                                                                _cfg(w_type, "weight", "per-channel-symmetric", bit)))
-        else:
-            _wrap(child, a_type, w_type, bit)
-    return model
-
-
-def _calibrate(model, x):
-    from sparsebit_b200.quantization.tools import CalibrationRunner
-    runner = CalibrationRunner(model, record_inputs=False)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        model(x)
-    runner.layerwise_calibration(dev())
-    model.eval()
-    for m in model.modules():
-        if isinstance(m, (QConv2d, QLinear)):
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
 @pytest.mark.parametrize("arch,convs", [("resnet18", 20), ("mobilenet_v2", 52)])
 @pytest.mark.parametrize("recipe", [("dorefa", "dorefa"), ("pact", "dorefa")])
 def test_model_converts_every_layer(arch, convs, recipe):
     tv = pytest.importorskip("torchvision")
     torch.manual_seed(0)
-    model = _wrap(getattr(tv.models, arch)(num_classes=10), *recipe, 4).to(dev())
+    a_type, w_type = recipe
+    model = wrap_quantized(getattr(tv.models, arch)(num_classes=10), cfg("per-tensor-affine", "feature", 4, qtype=a_type),
+                           cfg("per-channel-symmetric", "weight", 4, qtype=w_type)).to(dev())
     x = torch.randn(2, 3, 64, 64, device=dev())
-    _calibrate(model, x)
+    calibrated(model, [x], streaming=True, record_inputs=False).eval()
     _check_converted(model, x, convs + 1)
 
 
+# not int8_harness.check_converted: each layer runs on the input its fake-quant layer saw, captured before conversion
 def _check_converted(model, x, layers):
     """to_integer_dorefa_adaround converts `layers` layers and leaves nothing to the plain converters; each converted
     layer meets the bound against its fake-quant layer on the input that layer saw; channels-last equals NCHW."""
@@ -355,7 +328,8 @@ def test_adaround_ptq_resnet18_converts_every_layer():
     tv = pytest.importorskip("torchvision")
     from sparsebit_b200.quantization.tools import CalibrationRunner, trace_quant_model
     torch.manual_seed(0)
-    model = trace_quant_model(_wrap(tv.models.resnet18(num_classes=10), "uniform", "adaround", 8).to(dev()))
+    model = trace_quant_model(wrap_quantized(tv.models.resnet18(num_classes=10), cfg("per-tensor-affine", "feature"),
+                                             cfg("per-channel-symmetric", "weight", qtype="adaround")).to(dev()))
     x = torch.randn(4, 3, 64, 64, device=dev())
     runner = CalibrationRunner(model)
     runner.adaround_kwargs = dict(max_steps=30, batch_size=2, print_freq=0)

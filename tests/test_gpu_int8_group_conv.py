@@ -7,13 +7,13 @@ import torch
 import torch.nn as nn
 
 from gpu_util import dev, t
-from int8_conv_ref import grid_offset
+from gpu_util import no_tf32_autouse  # noqa: F401 -- TF32 off on every test
 from int8_group_conv_ref import truth
+from int8_harness import calibrated, cfg, check_converted, layer_qparams, stored_rows, wrap_quantized
 from oracle import observers as oobs
 from sparsebit_b200 import SparsebitB200Error, ops
-from sparsebit_b200 import config as sbcfg
-from sparsebit_b200.quantization.modules import QConv2d, QConv2dGroupInt8, QConv2dInt8, QLinear, resolve_conv_padding
-from sparsebit_b200.quantization.tools import CalibrationRunner, to_integer_convs, to_integer_group_convs
+from sparsebit_b200.quantization.modules import QConv2d, QConv2dGroupInt8, QConv2dInt8
+from sparsebit_b200.quantization.tools import to_integer_convs, to_integer_group_convs
 
 pytestmark = pytest.mark.gpu
 
@@ -41,27 +41,9 @@ GEOMS = [
 RANGES = [((-128, 127), (-128, 127)), ((0, 255), (-128, 127)), ((0, 15), (-8, 7))]
 
 
-@pytest.fixture(autouse=True)
-def _no_tf32():
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
-
-
-def _weights(w, ws, wz, wqmin, wqmax):
-    c_out = w.shape[0]
-    ws = np.broadcast_to(np.asarray(ws, F32).reshape(-1), (c_out,)).copy()
-    wz = np.broadcast_to(np.asarray(wz, F32).reshape(-1), (c_out,)).copy()
-    w_q, w_sum, w_nan = ops.int8_quantize_rows(t(w.reshape(c_out, -1)), t(ws), t(wz), wqmin, wqmax)
-    w_scale = torch.where(w_nan, torch.full_like(t(ws), float("nan")), t(ws))
-    w_zero = t((np.rint(wz) - grid_offset(wqmin)).astype(np.int32))
-    return w_q, w_sum, w_scale, w_zero
-
-
 def _run(args, groups, bias=None, stride=1, padding=0, dilation=1):
     x, xs, xz, xqmin, xqmax, w, ws, wz, wqmin, wqmax = args
-    wts = _weights(w, ws, wz, wqmin, wqmax)
+    wts = stored_rows(w, ws, wz, wqmin, wqmax)
     return ops.int8_group_conv2d(t(x), t(np.array([xs], F32)), t(np.array([xz], F32)), xqmin, xqmax, *wts, w.shape[2:],
                                  groups, None if bias is None else t(bias), stride, padding, dilation).cpu().numpy()
 
@@ -75,7 +57,7 @@ def _per_group_dense(args, groups, bias=None, stride=1, padding=0, dilation=1):
     outs = []
     for g in range(groups):
         o = slice(g * m_g, (g + 1) * m_g)
-        wts = _weights(np.ascontiguousarray(w[o]), ws[o], wz[o], wqmin, wqmax)
+        wts = stored_rows(np.ascontiguousarray(w[o]), ws[o], wz[o], wqmin, wqmax)
         outs.append(ops.int8_conv2d(t(np.ascontiguousarray(x[:, g * c_g:(g + 1) * c_g])), t(np.array([xs], F32)),
                                     t(np.array([xz], F32)), xqmin, xqmax, *wts, w.shape[2:],
                                     None if bias is None else t(np.ascontiguousarray(bias[o])), stride, padding,
@@ -182,7 +164,7 @@ def test_deterministic_and_graph_replay():
     rng = np.random.default_rng(5)
     args, bias = _minmax_case(rng, 4, c, 14, 14, c_out, groups, kernel, kernel, True, True)
     x, xs, xz, xqmin, xqmax, wt, ws, wz, wqmin, wqmax = args
-    wts = _weights(wt, ws, wz, wqmin, wqmax)
+    wts = stored_rows(wt, ws, wz, wqmin, wqmax)
     xt, s, z, b = t(x), t(np.array([xs], F32)), t(np.array([xz], F32)), t(bias)
 
     def call():
@@ -213,7 +195,7 @@ def test_far_end_past_2_31_elements():
     rng = np.random.default_rng(11)
     wt = rng.standard_normal((c, 1, 3, 3)).astype(F32)
     xs, ws = F32(2.0 ** -5), np.full(c, 2.0 ** -7, F32)
-    wts = _weights(wt, ws, np.zeros(c, F32), -128, 127)
+    wts = stored_rows(wt, ws, np.zeros(c, F32), -128, 127)
     y = ops.int8_group_conv2d(x, t(np.array([xs], F32)), t(np.zeros(1, F32)), -128, 127, *wts, 3, c, None, 1, 1, 1)
     assert y.numel() > 2**31
     tail = y[0, c - 1, h - 9:, w - 200:].cpu().numpy()[None, None]
@@ -245,100 +227,48 @@ def test_argument_errors():
 
 
 # ---------------------------------------------------------------------------------------------- modules and models
-def _cfg(scheme, target):
-    return sbcfg.quantizer_config(scheme, 8, target, layout="NCHW")
-
-
-def _calibrated(model, batches):
-    model = model.to(dev())
-    runner = CalibrationRunner(model, streaming=True, record_inputs=False)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for b in batches:
-            model(b)
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if hasattr(m, "set_quant") and callable(m.set_quant) and getattr(m, "input_quantizer", None) is not None:
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
-def _wrapped(net):
-    def wrap(module):
-        for name, child in list(module.named_children()):
-            if isinstance(child, nn.Conv2d):
-                setattr(module, name, QConv2d(child).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                     _cfg("per-channel-symmetric", "weight")))
-            elif isinstance(child, nn.Linear):
-                setattr(module, name, QLinear(child).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                     _cfg("per-channel-symmetric", "weight")))
-            else:
-                wrap(child)
-
-    wrap(net)
-    return net
-
-
-def _layer_truth(qconv, x):
-    aq, wq = qconv.input_quantizer, qconv.weight_quantizer
-    xs, xz = (v.detach().reshape(-1).cpu().numpy() for v in aq._qparams_preprocess(x))
-    ws, wz = (v.detach().reshape(-1).cpu().numpy() for v in wq._qparams_preprocess(qconv.weight))
-    b = qconv.bias.detach().cpu().numpy() if qconv.bias is not None else None
-    kw = qconv.fwd_kwargs
-    pad = resolve_conv_padding(kw["padding"], qconv.weight.shape[2:], kw["dilation"], kw["stride"])
-    return truth(x.cpu().numpy(), xs[0], xz[0], *aq.qdesc.qrange, qconv.weight.detach().cpu().numpy(), ws, wz,
-                 *wq.qdesc.qrange, kw["groups"], bias=b, stride=kw["stride"], padding=pad, dilation=kw["dilation"])
-
-
-def _check_converted(model, originals, x, names):
-    seen = {}
-    hooks = [model.get_submodule(nm).register_forward_hook(lambda mod, i, o, nm=nm: seen.__setitem__(nm, (i[0], o)))
-             for nm in names]
-    with torch.no_grad():
-        model(x)
-    for h in hooks:
-        h.remove()
-    for nm in names:
-        xin, y = seen[nm]
-        t_, bound = _layer_truth(originals[nm], xin)
-        err = np.abs(y.cpu().numpy() - t_)
-        assert np.all(err <= bound), (nm, float((err / bound).max()))
+def _truth_of(qconv, x):
+    return truth(**layer_qparams(qconv, x), groups=qconv.fwd_kwargs["groups"])
 
 
 def test_mobilenet_v2_converts_all_52_convs_and_meets_the_bound():
     import torchvision
 
     torch.manual_seed(0)
-    qnet = _wrapped(torchvision.models.mobilenet_v2(weights=None).eval())
+    qnet = wrap_quantized(torchvision.models.mobilenet_v2(weights=None).eval(), cfg("per-tensor-affine", "feature"),
+                          cfg("per-channel-symmetric", "weight"))
     batches = [torch.randn(2, 3, 96, 96, device=dev()) for _ in range(2)]
-    qnet = _calibrated(qnet, batches)
+    qnet = calibrated(qnet, batches, streaming=True, record_inputs=False)
     originals = {nm: m for nm, m in qnet.named_modules() if isinstance(m, QConv2d)}
     dense = to_integer_convs(qnet)
     grouped = to_integer_group_convs(qnet)
     assert len(dense) == 35 and len(grouped) == 17 and sorted(dense + grouped) == sorted(originals)
     assert all(isinstance(qnet.get_submodule(nm), QConv2dGroupInt8) for nm in grouped)
     assert all(type(qnet.get_submodule(nm)) is QConv2dInt8 for nm in dense)
-    _check_converted(qnet, originals, batches[0][:1], dense + grouped)
+    check_converted(qnet, originals, [batches[0][:1]], dense + grouped, expected_cls=None, layer_truth=_truth_of,
+                    compare_fake_quant=False)
 
 
 def test_regnet_x_400mf_converts_every_grouped_conv_and_meets_the_bound():
     import torchvision
 
     torch.manual_seed(1)
-    qnet = _wrapped(torchvision.models.regnet_x_400mf(weights=None).eval())
+    qnet = wrap_quantized(torchvision.models.regnet_x_400mf(weights=None).eval(), cfg("per-tensor-affine", "feature"),
+                          cfg("per-channel-symmetric", "weight"))
     batches = [torch.randn(2, 3, 96, 96, device=dev()) for _ in range(2)]
-    qnet = _calibrated(qnet, batches)
+    qnet = calibrated(qnet, batches, streaming=True, record_inputs=False)
     originals = {nm: m for nm, m in qnet.named_modules() if isinstance(m, QConv2d) and m.fwd_kwargs["groups"] > 1}
     grouped = to_integer_group_convs(qnet)
     assert len(grouped) == 22 and grouped == list(originals)
-    _check_converted(qnet, originals, batches[0][:1], grouped)
+    check_converted(qnet, originals, [batches[0][:1]], grouped, expected_cls=QConv2dGroupInt8, layer_truth=_truth_of,
+                    compare_fake_quant=False)
 
 
 def test_module_input_forms():
     torch.manual_seed(2)
-    q = QConv2d(nn.Conv2d(16, 32, 3, padding=1, groups=8)).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                            _cfg("per-channel-symmetric", "weight"))
-    q = _calibrated(q, [torch.randn(4, 16, 12, 12, device=dev())])
+    q = QConv2d(nn.Conv2d(16, 32, 3, padding=1, groups=8)).build_quantizer(cfg("per-tensor-affine", "feature"),
+                                                                            cfg("per-channel-symmetric", "weight"))
+    q = calibrated(q, [torch.randn(4, 16, 12, 12, device=dev())], streaming=True, record_inputs=False)
     conv = QConv2dGroupInt8.from_qconv2d(q)
     assert "groups=8" in repr(conv)
     x = torch.randn(3, 16, 12, 12, device=dev())

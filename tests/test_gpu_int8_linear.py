@@ -14,25 +14,18 @@ import torch
 import torch.nn as nn
 
 from gpu_util import dev, t
-from int8_linear_ref import BOUND, grid_offset, truth
+from gpu_util import no_tf32_autouse  # noqa: F401 -- TF32 off on every test
+from int8_harness import calibrated, cfg, check_converted, layer_qparams, qrange, stored_rows
+from int8_linear_ref import grid_offset, truth
 from oracle import observers as oobs
 from oracle import qdq as oqdq
 from sparsebit_b200 import SparsebitB200Error, ops
-from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import QConv2d, QLinear, QLinearInt8, QReLU
-from sparsebit_b200.quantization.tools import CalibrationRunner, to_integer_linears
+from sparsebit_b200.quantization.tools import to_integer_linears
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
-
-
-@pytest.fixture(autouse=True)
-def _no_tf32():
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
 
 
 # ---------------------------------------------------------------------------------------------- the integer grid
@@ -94,25 +87,11 @@ def test_grid_matches_the_qdq_kernel_values():
 
 
 # ---------------------------------------------------------------------------------------------- the GEMM
-def _weights(w, ws, wz, wqmin, wqmax):
-    n = w.shape[0]
-    ws = np.broadcast_to(np.asarray(ws, F32).reshape(-1), (n,)).copy()
-    wz = np.broadcast_to(np.asarray(wz, F32).reshape(-1), (n,)).copy()
-    w_q, w_sum, w_nan = ops.int8_quantize_rows(t(w), t(ws), t(wz), wqmin, wqmax)
-    w_scale = torch.where(w_nan, torch.full_like(t(ws), float("nan")), t(ws))
-    w_zero = t((np.rint(wz) - grid_offset(wqmin)).astype(np.int32))
-    return w_q, w_sum, w_scale, w_zero
-
-
 def _run(x, xs, xz, xqmin, xqmax, w, ws, wz, wqmin, wqmax, bias=None):
-    w_q, w_sum, w_scale, w_zero = _weights(w, ws, wz, wqmin, wqmax)
+    w_q, w_sum, w_scale, w_zero = stored_rows(w, ws, wz, wqmin, wqmax)
     y = ops.int8_linear(t(x), t(np.array([xs], F32)), t(np.array([xz], F32)), xqmin, xqmax, w_q, w_sum, w_scale, w_zero,
                         None if bias is None else t(bias))
     return y.cpu().numpy().reshape(-1, w.shape[0])
-
-
-def _range(bits, affine):
-    return (0, (1 << bits) - 1) if affine else (-(1 << (bits - 1)), (1 << (bits - 1)) - 1)
 
 
 def _exact_case(rng, m, k, n, xr, wr, zx_at=None, zw_at=None):
@@ -149,11 +128,11 @@ EXACT = [
     (7, 768, 100, (0, 255), (0, 255), "max", "max"),
     (591, 33, 100, (0, 255), (0, 255), "min", "max"),
     (7, 3072, 2304, (0, 255), (-128, 127), "max", None),
-    (7, 768, 100, _range(4, False), _range(4, False), None, None),
-    (7, 768, 100, _range(4, True), _range(4, True), "max", "min"),
-    (7, 768, 100, _range(2, False), _range(2, True), None, "max"),
-    (7, 768, 100, _range(2, True), _range(2, False), "min", None),
-    (1, 33, 8, _range(2, True), _range(4, True), "max", "max"),
+    (7, 768, 100, qrange(4, False), qrange(4, False), None, None),
+    (7, 768, 100, qrange(4, True), qrange(4, True), "max", "min"),
+    (7, 768, 100, qrange(2, False), qrange(2, True), None, "max"),
+    (7, 768, 100, qrange(2, True), qrange(2, False), "min", None),
+    (1, 33, 8, qrange(2, True), qrange(4, True), "max", "max"),
 ]
 
 
@@ -213,7 +192,7 @@ def test_nan_rows_and_inf_inputs():
 def test_deterministic_and_graph_replay():
     rng = np.random.default_rng(12)
     (x, xs, xz, xqmin, xqmax, w, ws, wz, wqmin, wqmax), bias = _minmax_case(rng, 517, 768, 300, True, True)
-    w_q, w_sum, w_scale, w_zero = _weights(w, ws, wz, wqmin, wqmax)
+    w_q, w_sum, w_scale, w_zero = stored_rows(w, ws, wz, wqmin, wqmax)
     xt, xst, xzt, bt = t(x), t(np.array([xs], F32)), t(np.array([xz], F32)), t(bias)
 
     def call():
@@ -247,20 +226,16 @@ def test_k_limit_is_unsupported():
 
 
 # ---------------------------------------------------------------------------------------------- modules
-def _cfg(scheme, target, layout="NCHW", **kw):
-    return sbcfg.quantizer_config(scheme, 8, target, layout=layout, **kw)
-
-
 class CnnHead(nn.Module):
     def __init__(self):
         super().__init__()
-        self.conv = QConv2d(nn.Conv2d(3, 16, 3, stride=2)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                           _cfg("per-channel-symmetric", "weight"))
-        self.relu = QReLU().build_quantizer(_cfg("per-tensor-symmetric", "feature", disable=True))
-        self.fc1 = QLinear(nn.Linear(16 * 7 * 7, 120)).build_quantizer(_cfg("per-tensor-affine", "feature"),
-                                                                        _cfg("per-channel-symmetric", "weight"))
-        self.fc2 = QLinear(nn.Linear(120, 10)).build_quantizer(_cfg("per-tensor-symmetric", "feature"),
-                                                                _cfg("per-tensor-symmetric", "weight"))
+        self.conv = QConv2d(nn.Conv2d(3, 16, 3, stride=2)).build_quantizer(cfg("per-tensor-symmetric", "feature"),
+                                                                           cfg("per-channel-symmetric", "weight"))
+        self.relu = QReLU().build_quantizer(cfg("per-tensor-symmetric", "feature", disable=True))
+        self.fc1 = QLinear(nn.Linear(16 * 7 * 7, 120)).build_quantizer(cfg("per-tensor-affine", "feature"),
+                                                                        cfg("per-channel-symmetric", "weight"))
+        self.fc2 = QLinear(nn.Linear(120, 10)).build_quantizer(cfg("per-tensor-symmetric", "feature"),
+                                                                cfg("per-tensor-symmetric", "weight"))
 
     def forward(self, x):
         x = torch.flatten(self.relu(self.conv(x)), 1)
@@ -272,87 +247,48 @@ class DeitMlp(nn.Module):
 
     def __init__(self):
         super().__init__()
-        a = dict(layout="NLC")
-        self.fc1 = QLinear(nn.Linear(768, 3072)).build_quantizer(_cfg("per-tensor-symmetric", "feature", **a),
-                                                                  _cfg("per-channel-symmetric", "weight"))
-        self.fc2 = QLinear(nn.Linear(3072, 768)).build_quantizer(_cfg("per-tensor-affine", "feature", **a),
-                                                                  _cfg("per-channel-symmetric", "weight"))
-        self.proj = QLinear(nn.Linear(768, 64)).build_quantizer(_cfg("per-channel-symmetric", "feature", **a),
-                                                                 _cfg("per-channel-symmetric", "weight"))
+        self.fc1 = QLinear(nn.Linear(768, 3072)).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC"),
+                                                                  cfg("per-channel-symmetric", "weight"))
+        self.fc2 = QLinear(nn.Linear(3072, 768)).build_quantizer(cfg("per-tensor-affine", "feature", layout="NLC"),
+                                                                  cfg("per-channel-symmetric", "weight"))
+        self.proj = QLinear(nn.Linear(768, 64)).build_quantizer(cfg("per-channel-symmetric", "feature", layout="NLC"),
+                                                                 cfg("per-channel-symmetric", "weight"))
 
     def forward(self, x):
         return self.proj(self.fc2(nn.functional.gelu(self.fc1(x))))
 
 
-def _calibrated(model, batches):
-    model = model.to(dev())
-    runner = CalibrationRunner(model)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for b in batches:
-            model(b)
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if hasattr(m, "set_quant") and callable(m.set_quant) and getattr(m, "input_quantizer", None) is not None:
-            m.set_quant(w_quant=True, a_quant=True)
-    return model
-
-
-def _layer_truth(qlinear, x):
-    aq, wq = qlinear.input_quantizer, qlinear.weight_quantizer
-    xs, xz = (v.detach().reshape(-1).cpu().numpy() for v in aq._qparams_preprocess(x))
-    ws, wz = (v.detach().reshape(-1).cpu().numpy() for v in wq._qparams_preprocess(qlinear.weight))
-    b = qlinear.bias.detach().cpu().numpy() if qlinear.bias is not None else None
-    return truth(x.cpu().numpy(), xs[0], xz[0], *aq.qdesc.qrange, qlinear.weight.detach().cpu().numpy(), ws, wz,
-                 *wq.qdesc.qrange, bias=b)
-
-
-def _check_converted(model, originals, inputs, names):
-    seen = {}
-    hooks = [getattr(model, nm).register_forward_hook(lambda mod, i, o, nm=nm: seen.__setitem__(nm, (i[0], o))) for nm in names]
-    with torch.no_grad():
-        for x in inputs:
-            model(x)
-            for nm in names:
-                xin, y = seen[nm]
-                t_, bound = _layer_truth(originals[nm], xin)
-                y = y.reshape(-1, y.shape[-1]).cpu().numpy()
-                err = np.abs(y - t_)
-                assert np.all(err <= bound), (nm, float((err / bound).max()))
-                ref = originals[nm](xin).reshape(-1, y.shape[-1]).cpu().numpy()  # the fake-quant path: QDQ + F.linear
-                ref_err = np.abs(ref - t_)
-                k = xin.shape[-1]
-                assert np.all(ref_err <= 2.0 ** -22 * k * bound / BOUND), nm
-                print(f"{nm}: int8 max |y - T| = {err.max():.3e}, fake-quant F.linear max |y - T| = {ref_err.max():.3e}")
-    for h in hooks:
-        h.remove()
+def _truth_of(qlinear, x):
+    return truth(**layer_qparams(qlinear, x))
 
 
 def test_cnn_head_converts_and_meets_the_bound():
     torch.manual_seed(0)
     batches = [torch.randn(8, 3, 16, 16, device=dev()) for _ in range(3)]
-    model = _calibrated(CnnHead(), batches)
+    model = calibrated(CnnHead(), batches, streaming=True, record_inputs=None)
     originals = {"fc1": model.fc1, "fc2": model.fc2}
     names = to_integer_linears(model)
     assert names == ["fc1", "fc2"]
     assert isinstance(model.fc1, QLinearInt8) and isinstance(model.fc2, QLinearInt8) and isinstance(model.conv, QConv2d)
-    _check_converted(model, originals, batches[:2], names)
+    check_converted(model, originals, batches[:2], names, expected_cls=QLinearInt8, layer_truth=_truth_of,
+                    compare_fake_quant=True)
 
 
 def test_deit_mlp_converts_and_meets_the_bound():
     torch.manual_seed(1)
     batches = [torch.randn(2, 197, 768, device=dev()) for _ in range(2)]
-    model = _calibrated(DeitMlp(), batches)
+    model = calibrated(DeitMlp(), batches, streaming=True, record_inputs=None)
     originals = {"fc1": model.fc1, "fc2": model.fc2}
     assert to_integer_linears(model) == ["fc1", "fc2"]
     assert isinstance(model.proj, QLinear)  # per-channel activations: not eligible, left alone
-    _check_converted(model, originals, batches[:1], ["fc1", "fc2"])
+    check_converted(model, originals, batches[:1], ["fc1", "fc2"], expected_cls=QLinearInt8, layer_truth=_truth_of,
+                    compare_fake_quant=True)
 
 
 def test_module_input_forms():
     torch.manual_seed(2)
     batches = [torch.randn(4, 197, 768, device=dev())]
-    model = _calibrated(DeitMlp(), batches)
+    model = calibrated(DeitMlp(), batches, streaming=True, record_inputs=None)
     to_integer_linears(model)
     fc1 = model.fc1
     x = batches[0]
@@ -371,7 +307,7 @@ def test_module_input_forms():
 
 def test_weight_nan_row_gives_a_nan_column():
     torch.manual_seed(3)
-    model = _calibrated(CnnHead(), [torch.randn(8, 3, 16, 16, device=dev())])
+    model = calibrated(CnnHead(), [torch.randn(8, 3, 16, 16, device=dev())], streaming=True, record_inputs=None)
     with torch.no_grad():
         model.fc2.weight[4, 7] = float("nan")
     conv = QLinearInt8.from_qlinear(model.fc2)

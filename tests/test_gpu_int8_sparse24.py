@@ -19,13 +19,14 @@ import torch.nn as nn
 
 import int8_sparse24_ref as ref
 from gpu_util import dev, t
-from int8_linear_ref import grid_offset, truth
+from int8_harness import calibrated, cfg, stored_rows
+from int8_linear_ref import truth
 from oracle import observers as oobs
 from sparsebit_b200 import SparsebitB200Error, ops
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import (QLinear, QLinearSparse24Int8, int8_ineligibility,
                                                  int8_sparse24_ineligibility)
-from sparsebit_b200.quantization.tools import CalibrationRunner, to_integer_linears, to_sparse24_integer_linears
+from sparsebit_b200.quantization.tools import to_integer_linears, to_sparse24_integer_linears
 from sparsebit_b200.sparse.modules import SLinear
 
 pytestmark = pytest.mark.gpu
@@ -76,16 +77,6 @@ def test_sparser_type_and_ratio():
 
 
 # ---------------------------------------------------------------------------------------------- pack
-def _stored(w, ws, wz, wqmin, wqmax):
-    n = w.shape[0]
-    ws = np.broadcast_to(np.asarray(ws, F32).reshape(-1), (n,)).copy()
-    wz = np.broadcast_to(np.asarray(wz, F32).reshape(-1), (n,)).copy()
-    w_q, w_sum, w_nan = ops.int8_quantize_rows(t(w), t(ws), t(wz), wqmin, wqmax)
-    w_scale = torch.where(w_nan, torch.full_like(t(ws), float("nan")), t(ws))
-    w_zero = t((np.rint(wz) - grid_offset(wqmin)).astype(np.int32))
-    return w_q, w_sum, w_scale, w_zero
-
-
 def _sparse_weights(rng, n, k, wr, ws, wz, scale=0.45):
     """Weights 2:4 sparse in value (so on the grid), spread over +-scale of the range around 0."""
     wqmin, wqmax = wr
@@ -103,7 +94,7 @@ def test_pack_is_the_restatement(n, k, wr, zero):
     w[1, 5] = np.nan  # a NaN row: packed as zeros
     if n > 3:
         w[3, :4] = (np.array([1, 1, 1, 0], F32) * ws[3] * 3)  # three nonzeros: bad
-    w_q, _, w_scale, w_zero = _stored(w, ws, wz, *wr)
+    w_q, _, w_scale, w_zero = stored_rows(w, ws, wz, *wr)
     vals, meta, dsum, bad = ops.int8_sparse24_pack(w_q, w_zero, w_scale, k)
     ev, em, ed, eb = ref.pack(w_q.cpu().numpy(), w_zero.cpu().numpy(), w_scale.cpu().numpy(), k)
     assert np.array_equal(vals.cpu().numpy(), ev)
@@ -116,7 +107,7 @@ def test_pack_is_the_restatement(n, k, wr, zero):
 def _both(x, xs, xz, xqmin, xqmax, w, ws, wz, wqmin, wqmax, bias=None):
     """(sparse y, dense y) as fp32 [M, N] arrays from the same stored weight."""
     k = w.shape[1]
-    w_q, w_sum, w_scale, w_zero = _stored(w, ws, wz, wqmin, wqmax)
+    w_q, w_sum, w_scale, w_zero = stored_rows(w, ws, wz, wqmin, wqmax)
     vals, meta, dsum, bad = ops.int8_sparse24_pack(w_q, w_zero, w_scale, k)
     assert not bad.any()
     xt, xst, xzt = t(x), t(np.array([xs], F32)), t(np.array([xz], F32))
@@ -201,7 +192,7 @@ def test_meets_the_truth_bound():
 def test_deterministic_and_graph_replay_after_a_larger_call():
     rng = np.random.default_rng(12)
     x, xs, xz, xqmin, xqmax, w, ws, wz, wqmin, wqmax = _case(rng, 33, 768, 300, UNSIGNED, SIGNED, 100, 0, True)
-    w_q, _, w_scale, w_zero = _stored(w, ws, wz, wqmin, wqmax)
+    w_q, _, w_scale, w_zero = stored_rows(w, ws, wz, wqmin, wqmax)
     vals, meta, dsum, _ = ops.int8_sparse24_pack(w_q, w_zero, w_scale, 768)
     xt, xst, xzt = t(x), t(np.array([xs], F32)), t(np.array([xz], F32))
     big = t(rng.standard_normal((4000, 768)).astype(F32))
@@ -240,10 +231,6 @@ def test_k_limit_is_unsupported():
 
 
 # ---------------------------------------------------------------------------------------------- modules
-def _cfg(scheme, target, bit=8, **kw):
-    return sbcfg.quantizer_config(scheme, bit, target, layout="NLC", **kw)
-
-
 class Mlp(nn.Module):
     """Two 2:4-pruned layers (fc1 4-bit per-channel weights, fc2 affine activations) and a dense one."""
 
@@ -272,7 +259,8 @@ class QMlp(nn.Module):
             with torch.no_grad():
                 lin.weight.copy_(src.weight * src.w_mask if isinstance(src, SLinear) else src.weight)
                 lin.bias.copy_(src.bias)
-            setattr(self, name, QLinear(lin).build_quantizer(_cfg(ascheme, "feature"), _cfg(scheme, "weight", bit=bits)))
+            setattr(self, name, QLinear(lin).build_quantizer(cfg(ascheme, "feature", layout="NLC"),
+                                                             cfg(scheme, "weight", bit=bits)))
 
     def forward(self, x):
         return self.head(torch.relu(self.fc2(torch.relu(self.fc1(x)))))
@@ -286,14 +274,7 @@ def test_pruned_model_converts_exactly_its_sparse_layers():
         assert np.array_equal(m.w_mask.cpu().numpy(), ref.mask24(m.weight.detach().cpu().numpy()))
     model = QMlp(mlp)
     batches = [torch.randn(4, 50, 768, device=dev()) for _ in range(2)]
-    runner = CalibrationRunner(model)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for b in batches:
-            model(b)
-    runner.layerwise_calibration(dev())
-    for m in (model.fc1, model.fc2, model.head):
-        m.set_quant(w_quant=True, a_quant=True)
+    calibrated(model, batches, streaming=True, record_inputs=None)
     assert "not 2:4 sparse" in int8_sparse24_ineligibility(model.head)
     assert "row 0, group" in int8_sparse24_ineligibility(model.head)
     dense = copy.deepcopy(model)
@@ -317,7 +298,7 @@ def test_ineligibility_names_the_row_and_group():
     with torch.no_grad():
         lin.weight.mul_(torch.from_numpy(ref.mask24(lin.weight.cpu().numpy())).to(dev()))
         lin.weight[5, 9] = 0.3  # group 2 of row 5 now has three nonzeros
-    q = QLinear(lin).build_quantizer(_cfg("per-tensor-symmetric", "feature"), _cfg("per-channel-symmetric", "weight"))
+    q = QLinear(lin).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC"), cfg("per-channel-symmetric", "weight"))
     q.input_quantizer.update_observer(torch.randn(2, 8, 64, device=dev()))
     q.input_quantizer.calc_qparams()
     q.weight_quantizer.update_observer(q.weight)
@@ -332,7 +313,7 @@ def test_ineligibility_names_the_row_and_group():
     with torch.no_grad():
         lin.weight[5, 9] = 0.0
         lin.weight.abs_()
-    qa = QLinear(lin).build_quantizer(_cfg("per-tensor-symmetric", "feature"), _cfg("per-tensor-affine", "weight"))
+    qa = QLinear(lin).build_quantizer(cfg("per-tensor-symmetric", "feature", layout="NLC"), cfg("per-tensor-affine", "weight"))
     qa.input_quantizer.update_observer(torch.randn(2, 8, 64, device=dev()))
     qa.input_quantizer.calc_qparams()
     qa.weight_quantizer.update_observer(qa.weight)

@@ -17,14 +17,13 @@ import torch
 import torch.nn as nn
 
 import int8_sparse24_ref as ref
-from int8_linear_ref import grid_offset
 from gpu_util import dev, t
+from int8_harness import calibrated, cfg, stored_rows
 from sparsebit_b200 import SparsebitB200Error, ops
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import (QConv2d, QConv2dGroupInt8, QConv2dInt8, QConv2dSparse24Int8,
                                                  int8_conv_ineligibility, int8_sparse24_conv_ineligibility)
-from sparsebit_b200.quantization.tools import (CalibrationRunner, to_integer_convs, to_integer_group_convs,
-                                               to_sparse24_integer_convs)
+from sparsebit_b200.quantization.tools import to_integer_convs, to_integer_group_convs, to_sparse24_integer_convs
 from sparsebit_b200.sparse.modules import SConv2d
 
 pytestmark = pytest.mark.gpu
@@ -37,22 +36,10 @@ def _bits(y):
     return np.asarray(y, F32).view(np.uint32)
 
 
-def _stored(w, ws, wz, wqmin, wqmax):
-    """The rows of weight.reshape(C_out, -1) on the stored grid: (w_q, w_rowsum, w_scale, w_zero)."""
-    rows = w.reshape(w.shape[0], -1)
-    n = rows.shape[0]
-    ws = np.broadcast_to(np.asarray(ws, F32).reshape(-1), (n,)).copy()
-    wz = np.broadcast_to(np.asarray(wz, F32).reshape(-1), (n,)).copy()
-    w_q, w_sum, w_nan = ops.int8_quantize_rows(t(rows), t(ws), t(wz), wqmin, wqmax)
-    w_scale = torch.where(w_nan, torch.full_like(t(ws), float("nan")), t(ws))
-    w_zero = t((np.rint(wz) - grid_offset(wqmin)).astype(np.int32))
-    return w_q, w_sum, w_scale, w_zero
-
-
 def _both(x, xs, xz, xr, w, ws, wz, wr, bias=None, stride=1, padding=0, dilation=1):
     """(sparse y, dense y) as fp32 NCHW arrays from the same stored weight."""
     kernel = w.shape[2:]
-    w_q, w_sum, w_scale, w_zero = _stored(w, ws, wz, *wr)
+    w_q, w_sum, w_scale, w_zero = stored_rows(w, ws, wz, *wr)
     vals, meta, dsum, bad = ops.int8_sparse24_pack(w_q, w_zero, w_scale, w[0].size)
     assert not bad.any()
     xt, xst, xzt = t(x), t(np.array([xs], F32)), t(np.array([xz], F32))
@@ -151,7 +138,7 @@ def test_resnet50_shapes_are_bit_identical(c, hw, c_out, k, stride, padding):
 def test_deterministic_and_graph_replay_after_a_larger_call():
     rng = np.random.default_rng(12)
     x, xs, xz, xr, w, ws, wz, wr = _case(rng, 2, 16, 10, 10, 96, 3, 3, UNSIGNED, SIGNED, 100, 0, True)
-    w_q, _, w_scale, w_zero = _stored(w, ws, wz, *wr)
+    w_q, _, w_scale, w_zero = stored_rows(w, ws, wz, *wr)
     vals, meta, dsum, _ = ops.int8_sparse24_pack(w_q, w_zero, w_scale, w[0].size)
     xt, xst, xzt = t(x), t(np.array([xs], F32)), t(np.array([xz], F32))
     big = t(rng.standard_normal((16, 16, 40, 40)).astype(F32))
@@ -190,10 +177,6 @@ def test_k_limit_is_unsupported():
 
 
 # ---------------------------------------------------------------------------------------------- modules
-def _cfg(scheme, target, bit=8):
-    return sbcfg.quantizer_config(scheme, bit, target, layout="NCHW")
-
-
 class Cnn(nn.Module):
     """An unpruned stem, 2:4-pruned 3x3 and 1x1 convs, a depthwise conv and a dense 1x1."""
 
@@ -230,7 +213,7 @@ class QCnn(nn.Module):
                 conv.weight.copy_(src.weight * src.w_mask if isinstance(src, SConv2d) else src.weight)
                 if src.bias is not None:
                     conv.bias.copy_(src.bias)
-            setattr(self, name, QConv2d(conv).build_quantizer(_cfg(ascheme, "feature"), _cfg(scheme, "weight", bit=bits)))
+            setattr(self, name, QConv2d(conv).build_quantizer(cfg(ascheme, "feature"), cfg(scheme, "weight", bit=bits)))
 
     def forward(self, x):
         return self.head(torch.relu(self.dw(torch.relu(self.c1(torch.relu(self.c3(torch.relu(self.stem(x)))))))))
@@ -243,15 +226,7 @@ def test_pruned_cnn_converts_exactly_its_sparse_convs():
         m.calc_mask()
         assert np.array_equal(m.w_mask.cpu().numpy(), ref.mask24(m.weight.detach().cpu().numpy()))
     model = QCnn(cnn)
-    runner = CalibrationRunner(model)
-    runner.prepare_calibration()
-    with torch.no_grad():
-        for _ in range(2):
-            model(torch.randn(4, 3, 32, 32, device=dev()))
-    runner.layerwise_calibration(dev())
-    for m in model.modules():
-        if isinstance(m, QConv2d):
-            m.set_quant(w_quant=True, a_quant=True)
+    calibrated(model, (torch.randn(4, 3, 32, 32, device=dev()) for _ in range(2)), streaming=True, record_inputs=None)
     assert "not 2:4 sparse" in int8_sparse24_conv_ineligibility(model.stem)
     assert int8_sparse24_conv_ineligibility(model.dw) == int8_conv_ineligibility(model.dw)
     dense = copy.deepcopy(model)
@@ -283,7 +258,7 @@ def test_ineligibility_names_the_row_and_group():
         conv.weight[5, 1, 0, 0] = 0.3  # k = 9 of row 5: group 2 (k = 8 .. 11) now has three nonzeros
         conv.weight[5, 1, 0, 1] = 0.2
         conv.weight[5, 1, 0, 2] = -0.25
-    q = QConv2d(conv).build_quantizer(_cfg("per-tensor-symmetric", "feature"), _cfg("per-channel-symmetric", "weight"))
+    q = QConv2d(conv).build_quantizer(cfg("per-tensor-symmetric", "feature"), cfg("per-channel-symmetric", "weight"))
     q.input_quantizer.update_observer(torch.randn(2, 8, 6, 6, device=dev()))
     q.input_quantizer.calc_qparams()
     q.weight_quantizer.update_observer(q.weight)

@@ -15,6 +15,8 @@ import torch
 import torch.nn.functional as F
 
 from gpu_util import bits_equal, dev, seed_of, t
+# TF32 off on every test: the module-step bounds assume fp32 products and sums in the conv / linear
+from gpu_util import no_tf32_autouse  # noqa: F401
 from oracle import qdq as oqdq
 from qat_ref import GRAD_KEYS, case_geometry, oracle_case, plant_grid_edges, plant_pact_bounds, within_l1
 from sparsebit_b200 import config as sbcfg
@@ -24,15 +26,6 @@ from sparsebit_b200.quantization.modules import QConv2d, QLinear
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
-
-
-@pytest.fixture(autouse=True)
-def no_tf32():
-    """The module-step bounds assume fp32 products and sums in the conv / linear (TF32 would round operands to 10 bits)."""
-    saved = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = saved
 
 
 def _quantizer(qtype, scheme, bit, target, layout, x, alpha=10.0):

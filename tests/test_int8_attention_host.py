@@ -5,8 +5,6 @@ coverage of the branch cases (tests/int8_attention_geometry.py).
 * Every bad argument is rejected on the host before any CUDA call (there is no device here), with its code and the
   message of its check (csrc/int8_attention.cu: sb200_int8_attention and check_dims).
 * The workspace query is a pure, monotone function of (batch, tq, tk, d, dv), O(batch (tq + tk) d + batch dv tk)."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
@@ -14,6 +12,7 @@ import torch.nn as nn
 
 import int8_attention_geometry as geo
 import int8_attention_ref as ref
+from int8_harness import E_INVALID, E_UNSUPPORTED, E_WORKSPACE, buf, refusal, rejector
 from oracle import qdq as oqdq
 from sparsebit_b200 import _lib
 from sparsebit_b200 import config as sbcfg
@@ -25,30 +24,17 @@ from sparsebit_b200.quantization.tools import (CalibrationRunner, to_integer_att
 from sparsebit_b200.quantization.tools.calibration import _is_quant_opr
 from test_gpu_int8_attention_branches import CASES, case_branches
 
-E_INVALID, E_UNSUPPORTED, E_WORKSPACE = -1, -3, -4
 F32 = np.float32
-
-
-def _buf(nbytes=4096):
-    b = ctypes.create_string_buffer(nbytes + 16)
-    return b, (ctypes.addressof(b) + 15) // 16 * 16
 
 
 def test_attention_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     ws_ok = int(lib.sb200_int8_attention_workspace_bytes(3, 5, 7, 64, 32))
     # q k v | q: s z lo hi | k: s z lo hi | p: s z lo hi | v: s z lo hi | has_scale scale out p_q | b tq tk d dv | ws ws_bytes stream
     ok = [p, p, p, p, p, -128, 127, p, p, -128, 127, p, p, 0, 255, p, p, -128, 127, 1, 0.125, p, p, 3, 5, 7, 64, 32, p,
           ws_ok, None]
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert lib.sb200_int8_attention(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-
+    rejected = rejector(lib.sb200_int8_attention, ok)
     for i in (0, 1, 2, 3, 4, 7, 8, 11, 12, 15, 16, 21, 28):  # null pointers (p_q, 22, may be null)
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     for i in range(23, 28):  # check_dims: an empty dimension
@@ -157,13 +143,7 @@ def test_eligible_modules():
     assert m.pv.left.input_quantizer.qdesc.qrange == (0, 255) and m.qk.left.input_quantizer.qdesc.qrange == (-128, 127)
 
 
-def _reason(m):
-    r = int8_attention_ineligibility(m)
-    assert r is not None
-    with pytest.raises(ValueError) as e:
-        QAttentionInt8.from_qattention(m)
-    assert r in str(e.value)
-    return r
+_reason = refusal(int8_attention_ineligibility, QAttentionInt8.from_qattention)
 
 
 @pytest.mark.parametrize("role,side", [("qk", "left"), ("qk", "right"), ("pv", "left"), ("pv", "right")])

@@ -5,27 +5,20 @@ tests/int8_attention_mask_ref.py and the coverage of the masked branch cases.
 * Every bad argument of the masked entry point is rejected on the host before any CUDA call (there is no device here).
 * Its workspace query is a pure function: that of sb200_int8_attention, plus the causal column sums of v; the query of
   sb200_int8_attention keeps its values."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
 import int8_attention_mask_ref as mref
 import int8_attention_ref as ref
+from int8_harness import E_INVALID, E_UNSUPPORTED, E_WORKSPACE, buf, rejector
 from sparsebit_b200 import _lib, ops
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.modules import QAttention
 from sparsebit_b200.quantization.tools import trace_quant_model
 from test_gpu_int8_attention_mask_branches import CASES, case_branches
 
-E_INVALID, E_UNSUPPORTED, E_WORKSPACE = -1, -3, -4
 F32 = np.float32
-
-
-def _buf(nbytes=4096):
-    b = ctypes.create_string_buffer(nbytes + 16)
-    return b, (ctypes.addressof(b) + 15) // 16 * 16
 
 
 # q k v | q: s z lo hi | k: s z lo hi | p: s z lo hi | v: s z lo hi | has_scale scale |
@@ -37,18 +30,10 @@ def _ok_args(p, ws_bytes, causal=1):
 
 def test_masked_entry_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     ws_ok = int(lib.sb200_int8_attention_masked_workspace_bytes(6, 5, 7, 64, 32, 1))
     ok = _ok_args(p, ws_ok)
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert lib.sb200_int8_attention_masked(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-        assert lib.sb200_last_error().startswith(b"sb200_int8_attention_masked")
-
+    rejected = rejector(lib.sb200_int8_attention_masked, ok, prefix=b"sb200_int8_attention_masked")
     for i in (0, 1, 2, 3, 4, 7, 8, 11, 12, 15, 16, 27, 34):  # null pointers (the mask, 21, and p_q, 28, may be null)
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     for i in range(29, 34):

@@ -16,14 +16,14 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from int8_conv_ref import integer_terms, lowered, out_hw, to_nchw, truth
+from int8_harness import (BAD_GEOMS, E_INVALID, E_WORKSPACE, buf, check_geometry_rules, conv_geom, refusal,
+                          rejector)
 from sparsebit_b200 import _lib
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.common import Backend
 from sparsebit_b200.quantization.modules import (QConv2d, QConv2dInt8, QLinear, int8_conv_ineligibility,
                                                  resolve_conv_padding)
 from sparsebit_b200.quantization.tools import to_integer_convs
-
-E_INVALID, E_UNSUPPORTED, E_WORKSPACE = -1, -3, -4
 
 GEOMS = [
     # (n, c, h, w, c_out, kh, kw, stride, padding, dilation)
@@ -110,56 +110,16 @@ def test_padding_that_does_not_resolve():
 
 
 # ---------------------------------------------------------------------------------------------- C-ABI on the host
-def _buf(nbytes=4096):
-    b = ctypes.create_string_buffer(nbytes + 16)
-    return b, (ctypes.addressof(b) + 15) // 16 * 16
-
-
-def _geom(**kw):
-    g = dict(n=2, c=4, h=8, w=8, kh=3, kw=3, stride_h=1, stride_w=1, dilation_h=1, dilation_w=1, pad_top=1, pad_bottom=1,
-             pad_left=1, pad_right=1)
-    g.update(kw)
-    return _lib.Conv2dGeom(**g)
-
-
-BAD_GEOMS = [dict(n=0), dict(c=-1), dict(h=0), dict(w=0), dict(kh=0), dict(kw=-3), dict(stride_h=0), dict(stride_w=-1),
-             dict(dilation_h=0), dict(dilation_w=0), dict(pad_top=-1), dict(pad_right=-2), dict(h=1 << 31)]
-
-
-def _check_geometry_rules(rejected, at):
-    for bad in BAD_GEOMS:
-        rejected(E_INVALID, b"non-positive geometry", **{f"a{at}": ctypes.byref(_geom(**bad))})
-    rejected(E_INVALID, b"empty output", **{f"a{at}": ctypes.byref(_geom(kh=11))})
-    rejected(E_INVALID, b"empty output", **{f"a{at}": ctypes.byref(_geom(kw=5, dilation_w=3))})
-    rejected(E_INVALID, b"too many output pixels", **{f"a{at}": ctypes.byref(_geom(n=1 << 20, h=64, w=64, c=1))})
-    rejected(E_UNSUPPORTED, b"K < 2^17", **{f"a{at}": ctypes.byref(_geom(c=1 << 17, kh=1, kw=1, pad_top=0, pad_bottom=0,
-                                                                          pad_left=0, pad_right=0))})
-    rejected(E_UNSUPPORTED, b"K < 2^17", **{f"a{at}": ctypes.byref(_geom(c=(1 << 17) // 9 + 1))})
-
-
-def _rejector(call, ok):
-    lib = _lib.load()
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert call(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-
-    return rejected
-
-
 def test_im2col_quantize_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
-    g = _geom()
+    keep, p = buf()
+    g = conv_geom()
     # (x, geom, scale, zp, qmin, qmax, q, row_sum, nan_flag, stream)
     ok = [p, ctypes.byref(g), p, p, 0, 255, p, p, p, None]
-    rejected = _rejector(lib.sb200_int8_im2col_quantize, ok)
+    rejected = rejector(lib.sb200_int8_im2col_quantize, ok)
     for i in (0, 1, 2, 3, 6, 7, 8):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
-    _check_geometry_rules(rejected, 1)
+    check_geometry_rules(rejected, 1)
     rejected(E_INVALID, b"wider than 8 bits", a4=-200, a5=100)
     rejected(E_INVALID, b"qmin", a4=5, a5=4)
     rejected(E_INVALID, b"neither signed", a4=-1, a5=200)
@@ -168,18 +128,18 @@ def test_im2col_quantize_rejects_bad_arguments_on_the_host():
 
 def test_conv2d_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
-    g = _geom()
+    keep, p = buf()
+    g = conv_geom()
     ws_ok = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     # (x, geom, xs, xz, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, ws, ws_bytes, stream)
     ok = [p, ctypes.byref(g), p, p, -128, 127, p, p, p, p, None, p, 8, p, ws_ok, None]
-    rejected = _rejector(lib.sb200_int8_conv2d, ok)
+    rejected = rejector(lib.sb200_int8_conv2d, ok)
     for i in (0, 1, 2, 3, 6, 7, 8, 9, 11, 13):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     rejected(E_INVALID, b"empty operand", a12=0)
     rejected(E_INVALID, b"empty operand", a12=-4)
     rejected(E_INVALID, b"too large", a12=1 << 31)
-    _check_geometry_rules(rejected, 1)
+    check_geometry_rules(rejected, 1)
     rejected(E_INVALID, b"wider than 8 bits", a4=0, a5=256)
     rejected(E_INVALID, b"neither signed", a4=-129, a5=0)
     rejected(E_INVALID, b"16-byte aligned", a6=p + 1)
@@ -193,9 +153,9 @@ def test_workspace_query_is_pure():
     lin = lib.sb200_int8_linear_workspace_bytes
     assert q(None) == 0
     for bad in BAD_GEOMS + [dict(kh=11), dict(n=1 << 20, h=64, w=64, c=1)]:
-        assert q(ctypes.byref(_geom(**bad))) == 0
+        assert q(ctypes.byref(conv_geom(**bad))) == 0
     for kw in [{}, dict(stride_h=2, stride_w=2), dict(c=3, kh=7, kw=7, pad_top=3, pad_bottom=3, pad_left=3, pad_right=3)]:
-        g = _geom(**kw)
+        g = conv_geom(**kw)
         first = q(ctypes.byref(g))
         oh = (g.h + g.pad_top + g.pad_bottom - g.dilation_h * (g.kh - 1) - 1) // g.stride_h + 1
         ow = (g.w + g.pad_left + g.pad_right - g.dilation_w * (g.kw - 1) - 1) // g.stride_w + 1
@@ -225,13 +185,7 @@ def test_eligible_convs():
     assert int8_conv_ineligibility(_qconv(kernel_size=4, padding="same", dilation=2)) is None
 
 
-def _reason(q):
-    r = int8_conv_ineligibility(q)
-    assert r is not None
-    with pytest.raises(ValueError) as e:
-        QConv2dInt8.from_qconv2d(q)
-    assert r in str(e.value)
-    return r
+_reason = refusal(int8_conv_ineligibility, QConv2dInt8.from_qconv2d)
 
 
 def test_every_ineligible_conv_gives_its_reason():

@@ -11,7 +11,7 @@ import int8_nhwc_geometry as geo
 import test_gpu_int8_conv_nhwc_branches as suite
 from branch_cases import assert_table_covers, check_reach
 from sparsebit_b200 import SparsebitB200Error, _lib, ops
-from test_int8_conv_host import E_INVALID, E_UNSUPPORTED, E_WORKSPACE, _buf, _check_geometry_rules, _geom, _rejector
+from int8_harness import E_INVALID, E_UNSUPPORTED, E_WORKSPACE, buf, check_geometry_rules, conv_geom, rejector
 
 
 def test_branch_cases_reach_every_branch():
@@ -51,13 +51,13 @@ def test_each_branch_case_reaches_its_branch():
 
 def test_im2col_quantize_nhwc_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
-    g = _geom()
+    keep, p = buf()
+    g = conv_geom()
     ok = [p, ctypes.byref(g), p, p, 0, 255, p, p, p, None]
-    rejected = _rejector(lib.sb200_int8_im2col_quantize_nhwc, ok)
+    rejected = rejector(lib.sb200_int8_im2col_quantize_nhwc, ok)
     for i in (0, 1, 2, 3, 6, 7, 8):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
-    _check_geometry_rules(rejected, 1)
+    check_geometry_rules(rejected, 1)
     rejected(E_INVALID, b"wider than 8 bits", a4=-200, a5=100)
     rejected(E_INVALID, b"qmin", a4=5, a5=4)
     rejected(E_INVALID, b"neither signed", a4=-1, a5=200)
@@ -68,18 +68,18 @@ def test_im2col_quantize_nhwc_rejects_bad_arguments_on_the_host():
 @pytest.mark.parametrize("fn", ["sb200_int8_conv2d_nhwc", "sb200_int8_sparse24_conv2d_nhwc"])
 def test_conv2d_nhwc_rejects_bad_arguments_on_the_host(fn):
     lib = _lib.load()
-    keep, p = _buf()
-    g = _geom()
+    keep, p = buf()
+    g = conv_geom()
     ws_ok = int(lib.sb200_int8_conv2d_workspace_bytes(ctypes.byref(g)))
     # dense: (x, geom, xs, xz, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, ws, ws_bytes, stream)
     # 2:4:   (x, geom, xs, xz, qmin, qmax, vals, meta, dsum, w_scale, bias, out, c_out, ws, ws_bytes, stream)
     ok = [p, ctypes.byref(g), p, p, -128, 127, p, p, p, p, None, p, 8, p, ws_ok, None]
-    rejected = _rejector(getattr(lib, fn), ok)
+    rejected = rejector(getattr(lib, fn), ok)
     for i in (0, 1, 2, 3, 6, 7, 8, 9, 11, 13):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     rejected(E_INVALID, b"empty operand", a12=0)
     rejected(E_INVALID, b"too large", a12=1 << 31)
-    _check_geometry_rules(rejected, 1)
+    check_geometry_rules(rejected, 1)
     rejected(E_INVALID, b"wider than 8 bits", a4=0, a5=256)
     rejected(E_INVALID, b"neither signed", a4=-129, a5=0)
     rejected(E_INVALID, b"16-byte aligned", a6=p + 1)
@@ -92,25 +92,25 @@ def test_conv2d_nhwc_rejects_bad_arguments_on_the_host(fn):
 
 def test_group_conv2d_nhwc_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
-    g = _geom(c=8)
+    keep, p = buf()
+    g = conv_geom(c=8)
     # (x, geom, groups, xs, xz, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, stream)
     ok = [p, ctypes.byref(g), 8, p, p, -128, 127, p, p, p, p, None, p, 8, None]
-    rejected = _rejector(lib.sb200_int8_group_conv2d_nhwc, ok)
+    rejected = rejector(lib.sb200_int8_group_conv2d_nhwc, ok)
     for i in (0, 1, 3, 4, 7, 8, 9, 10, 12):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     rejected(E_INVALID, b"empty operand", a13=0)
     rejected(E_INVALID, b"too large", a13=1 << 31)
     rejected(E_INVALID, b"sb200_int8_conv2d_nhwc", a2=1)
     rejected(E_INVALID, b"groups = 0", a2=0)
-    rejected(E_INVALID, b"empty output", a1=ctypes.byref(_geom(c=8, kh=11)))
-    rejected(E_INVALID, b"non-positive geometry", a1=ctypes.byref(_geom(c=8, stride_h=0)))
-    rejected(E_INVALID, b"too many output pixels", a1=ctypes.byref(_geom(c=8, n=1 << 20, h=64, w=64)))
+    rejected(E_INVALID, b"empty output", a1=ctypes.byref(conv_geom(c=8, kh=11)))
+    rejected(E_INVALID, b"non-positive geometry", a1=ctypes.byref(conv_geom(c=8, stride_h=0)))
+    rejected(E_INVALID, b"too many output pixels", a1=ctypes.byref(conv_geom(c=8, n=1 << 20, h=64, w=64)))
     rejected(E_INVALID, b"does not divide", a2=3)
     rejected(E_INVALID, b"does not divide", a13=12)
     rejected(E_INVALID, b"wider than 8 bits", a5=0, a6=256)
     rejected(E_INVALID, b"neither signed", a5=-129, a6=0)
-    rejected(E_UNSUPPORTED, b"K_g < 2^17", a1=ctypes.byref(_geom(c=2 * ((1 << 17) // 9 + 1))), a2=2, a13=2)
+    rejected(E_UNSUPPORTED, b"K_g < 2^17", a1=ctypes.byref(conv_geom(c=2 * ((1 << 17) // 9 + 1))), a2=2, a13=2)
 
 
 def _nhwc_ops():

@@ -17,11 +17,11 @@ import test_gpu_int8_conv_nhwc_branches as nhwc_suite
 import test_gpu_int8_dorefa as dorefa_suite
 import test_gpu_int8_group_branches as grp_suite
 from branch_cases import assert_table_covers, check_reach
+from int8_harness import E_INVALID, buf, conv_geom, rejector
 from sparsebit_b200 import _lib, config as sbcfg
 from sparsebit_b200.quantization.modules import (ADAROUND_SCALE_RANGE, QConv2d, QLinear, dorefa_adaround_ineligibility,
                                                  int8_conv_ineligibility, int8_group_conv_ineligibility,
                                                  int8_ineligibility)
-from test_int8_conv_host import E_INVALID, _buf, _geom, _rejector
 
 F32 = np.float32
 
@@ -111,11 +111,11 @@ def _nulled(rejected, at):
 
 def test_dorefa_entry_points_reject_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
-    g = _geom()
+    keep, p = buf()
+    g = conv_geom()
     # each: the counterpart's null-pointer check first (x), a bad range, then a null x_absmax with all else valid
     lin = [p, p, p, p, -128, 127, p, p, p, p, None, p, 4, 16, 8, p, 1 << 20, None]
-    rejected = _rejector(lib.sb200_int8_linear_dorefa, lin)
+    rejected = rejector(lib.sb200_int8_linear_dorefa, lin)
     rejected(E_INVALID, b"null pointer", a0=None)
     rejected(E_INVALID, b"empty operand", a12=0)
     rejected(E_INVALID, b"qmin", a4=5, a5=1)
@@ -123,17 +123,17 @@ def test_dorefa_entry_points_reject_on_the_host():
     _nulled(rejected, 3)
     for fn in (lib.sb200_int8_conv2d_dorefa, lib.sb200_int8_conv2d_nhwc_dorefa):
         conv = [p, ctypes.byref(g), p, p, p, -128, 127, p, p, p, p, None, p, 8, p, 1 << 20, None]
-        rejected = _rejector(fn, conv)
+        rejected = rejector(fn, conv)
         rejected(E_INVALID, b"null pointer", a1=None)
         rejected(E_INVALID, b"empty operand", a13=0)
-        rejected(E_INVALID, b"non-positive geometry", a1=ctypes.byref(_geom(n=0)))
+        rejected(E_INVALID, b"non-positive geometry", a1=ctypes.byref(conv_geom(n=0)))
         rejected(E_INVALID, b"qmin", a5=5, a6=1)
         rejected(-4, b"workspace too small", a15=16)
         _nulled(rejected, 4)
     for fn, dense in ((lib.sb200_int8_group_conv2d_dorefa, b"sb200_int8_conv2d"),
                       (lib.sb200_int8_group_conv2d_nhwc_dorefa, b"sb200_int8_conv2d_nhwc")):
         grp = [p, ctypes.byref(g), 2, p, p, p, -128, 127, p, p, p, p, None, p, 8, None]
-        rejected = _rejector(fn, grp)
+        rejected = rejector(fn, grp)
         rejected(E_INVALID, b"null pointer", a0=None)
         rejected(E_INVALID, dense, a2=1)
         rejected(E_INVALID, b"does not divide", a2=3)

@@ -2,6 +2,7 @@
 C-ABI rejection of sb200_int8_group_conv2d (no kernel launched), the conversion rules of QConv2dGroupInt8, and the
 branch coverage of the GPU branch suite."""
 import ctypes
+import functools
 
 import numpy as np
 import pytest
@@ -10,6 +11,7 @@ import torch.nn as nn
 
 import int8_group_geometry as geo
 from int8_group_conv_ref import group_integer_form, truth
+from int8_harness import BAD_GEOMS, E_INVALID, E_UNSUPPORTED, buf, conv_geom, refusal, rejector
 from sparsebit_b200 import _lib
 from sparsebit_b200 import config as sbcfg
 from sparsebit_b200.quantization.common import Backend
@@ -19,7 +21,6 @@ from sparsebit_b200.quantization.modules import QConv2dInt8
 from sparsebit_b200.quantization.tools import to_integer_convs, to_integer_group_convs
 from test_gpu_int8_group_branches import BIG, CASES, case_branches
 
-E_INVALID, E_UNSUPPORTED = -1, -3
 
 GEOMS = [
     # (n, c, h, w, c_out, groups, kernel, stride, padding, dilation)
@@ -51,28 +52,16 @@ def test_truth_equals_the_group_integer_form(geom, xrange, wrange):
 
 
 # ---------------------------------------------------------------------------------------------- C-ABI on the host
-def _geom(**kw):
-    g = dict(n=2, c=8, h=8, w=8, kh=3, kw=3, stride_h=1, stride_w=1, dilation_h=1, dilation_w=1, pad_top=1, pad_bottom=1,
-             pad_left=1, pad_right=1)
-    g.update(kw)
-    return _lib.Conv2dGeom(**g)
+_geom = functools.partial(conv_geom, c=8)
 
 
 def test_group_conv2d_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep = ctypes.create_string_buffer(4096 + 16)
-    p = (ctypes.addressof(keep) + 15) // 16 * 16
+    keep, p = buf()
     g = _geom()
     # (x, geom, groups, xs, xz, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias, out, c_out, stream)
     ok = [p, ctypes.byref(g), 8, p, p, -128, 127, p, p, p, p, None, p, 8, None]
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert lib.sb200_int8_group_conv2d(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-
+    rejected = rejector(lib.sb200_int8_group_conv2d, ok)
     for i in (0, 1, 3, 4, 7, 8, 9, 10, 12):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     rejected(E_INVALID, b"empty operand", a13=0)
@@ -81,8 +70,7 @@ def test_group_conv2d_rejects_bad_arguments_on_the_host():
     rejected(E_INVALID, b"sb200_int8_conv2d", a2=1)
     rejected(E_INVALID, b"groups = 0", a2=0)
     rejected(E_INVALID, b"groups = -2", a2=-2)
-    for bad in [dict(n=0), dict(c=-1), dict(h=0), dict(w=0), dict(kh=0), dict(kw=-3), dict(stride_h=0), dict(stride_w=-1),
-                dict(dilation_h=0), dict(dilation_w=0), dict(pad_top=-1), dict(pad_right=-2), dict(h=1 << 31)]:
+    for bad in BAD_GEOMS:
         rejected(E_INVALID, b"non-positive geometry", a1=ctypes.byref(_geom(**bad)))
     rejected(E_INVALID, b"empty output", a1=ctypes.byref(_geom(kh=11)))
     rejected(E_INVALID, b"too many output pixels", a1=ctypes.byref(_geom(n=1 << 20, h=64, w=64)))
@@ -121,13 +109,7 @@ def test_eligible_group_convs():
     assert int8_group_conv_ineligibility(_qconv(kernel_size=4, padding="same", dilation=2)) is None
 
 
-def _reason(q):
-    r = int8_group_conv_ineligibility(q)
-    assert r is not None
-    with pytest.raises(ValueError) as e:
-        QConv2dGroupInt8.from_qconv2d(q)
-    assert r in str(e.value)
-    return r
+_reason = refusal(int8_group_conv_ineligibility, QConv2dGroupInt8.from_qconv2d)
 
 
 def test_every_ineligible_group_conv_gives_its_reason():

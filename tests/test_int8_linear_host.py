@@ -6,13 +6,12 @@ eligibility rules of QLinearInt8.from_qlinear.
 * Every bad argument is rejected on the host, before any CUDA call (there is no device here), with its code and message.
 * The workspace query is a pure function of (m, k).
 * Every rule of from_qlinear gives its reason, and to_integer_linears leaves those layers alone."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 import torch.nn as nn
 
+from int8_harness import E_INVALID, E_UNSUPPORTED, E_WORKSPACE, buf, refusal, rejector
 from int8_linear_ref import BOUND, integer_terms, truth
 from sparsebit_b200 import _lib
 from sparsebit_b200 import config as sbcfg
@@ -20,9 +19,6 @@ from sparsebit_b200.quantization.common import Backend
 from sparsebit_b200.quantization.modules import (QConv2dSparse24Int8, QLinear, QLinearInt8, QLinearSparse24Int8,
                                                  int8_ineligibility)
 from sparsebit_b200.quantization.tools import to_integer_linears
-
-E_INVALID, E_UNSUPPORTED, E_WORKSPACE = -1, -3, -4
-
 
 def _operands(rng, m, k, n, xrange, wrange, pow2):
     x = (rng.standard_normal((m, k)) * 3).astype(np.float32)
@@ -67,26 +63,13 @@ def test_bound_is_the_stated_one():
     assert BOUND == 2.0 ** -21
 
 
-def _buf(nbytes=4096):
-    b = ctypes.create_string_buffer(nbytes + 16)
-    return b, (ctypes.addressof(b) + 15) // 16 * 16
-
-
 def test_linear_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     ws_ok = int(lib.sb200_int8_linear_workspace_bytes(4, 64))
     # (x, xs, xz, qmin, qmax, w_q, w_rowsum, w_scale, w_zero, bias, out, m, k, n, ws, ws_bytes, stream)
     ok = [p, p, p, -128, 127, p, p, p, p, None, p, 4, 64, 8, p, ws_ok, None]
-    call = lib.sb200_int8_linear
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert call(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-
+    rejected = rejector(lib.sb200_int8_linear, ok)
     for i in (0, 1, 2, 5, 6, 7, 8, 10, 14):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     for i in (11, 12, 13):
@@ -108,18 +91,10 @@ def test_linear_rejects_bad_arguments_on_the_host():
 
 def test_quantize_rows_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     # (x, scale, zp, per_row, qmin, qmax, q, row_sum, nan_flag, rows, k, stream)
     ok = [p, p, p, 0, -128, 127, p, p, p, 4, 64, None]
-    call = lib.sb200_int8_quantize_rows
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert call(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-
+    rejected = rejector(lib.sb200_int8_quantize_rows, ok)
     for i in (0, 1, 2, 6, 7, 8):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     for i in (9, 10):
@@ -157,13 +132,7 @@ def test_eligible_layers():
     assert int8_ineligibility(_qlinear(backend=Backend.TENSORRT)) is None
 
 
-def _reason(q):
-    r = int8_ineligibility(q)
-    assert r is not None
-    with pytest.raises(ValueError) as e:
-        QLinearInt8.from_qlinear(q)
-    assert r in str(e.value)
-    return r
+_reason = refusal(int8_ineligibility, QLinearInt8.from_qlinear)
 
 
 def test_every_ineligible_case_gives_its_reason():

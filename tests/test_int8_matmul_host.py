@@ -7,13 +7,12 @@ eligibility rules of QMatMulInt8.from_qmatmul and what calibration sees of a QMa
 * The workspace query is a pure, monotone function of (batch, m, k, n).
 * Every rule of from_qmatmul gives its reason; to_integer_matmuls leaves those modules, QLinear and QConv2d alone.
 * QMatMul is not a quant operator for CalibrationRunner; its two carriers are, under hooks and under the fx trace."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 import torch.nn as nn
 
+from int8_harness import E_INVALID, E_UNSUPPORTED, E_WORKSPACE, buf, refusal, rejector
 from int8_matmul_ref import BOUND, integer_form, quantize_cols, truth
 from oracle import qdq as oqdq
 from sparsebit_b200 import _lib
@@ -25,7 +24,6 @@ from sparsebit_b200.quantization.tools import (CalibrationRunner, to_integer_con
                                                to_integer_matmuls, trace_quant_model)
 from sparsebit_b200.quantization.tools.calibration import _is_quant_opr
 
-E_INVALID, E_UNSUPPORTED, E_WORKSPACE = -1, -3, -4
 F32 = np.float32
 RANGES = [((-128, 127), (-128, 127)), ((0, 255), (-128, 127)), ((0, 255), (0, 255)), ((-8, 7), (0, 15)), ((0, 3), (-2, 1))]
 
@@ -81,31 +79,13 @@ def test_quantize_cols_reference_layout():
     assert np.array_equal(q[..., :19], np.swapaxes(g, 1, 2)) and np.array_equal(col_sum, g.sum(1))
 
 
-def _buf(nbytes=4096):
-    b = ctypes.create_string_buffer(nbytes + 16)
-    return b, (ctypes.addressof(b) + 15) // 16 * 16
-
-
-def _rejecter(call, ok):
-    lib = _lib.load()
-
-    def rejected(code, text, **changes):
-        args = list(ok)
-        for i, v in changes.items():
-            args[int(i[1:])] = v
-        assert call(*args) == code, changes
-        assert text in lib.sb200_last_error(), (changes, lib.sb200_last_error())
-
-    return rejected
-
-
 def test_matmul_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     ws_ok = int(lib.sb200_int8_matmul_workspace_bytes(3, 4, 64, 8))
     # (a, b, b_k_major, a_scale, a_zp, qmin_a, qmax_a, b_scale, b_zp, qmin_b, qmax_b, out, batch, m, k, n, ws, ws_bytes, stream)
     ok = [p, p, 0, p, p, -128, 127, p, p, 0, 255, p, 3, 4, 64, 8, p, ws_ok, None]
-    rejected = _rejecter(lib.sb200_int8_matmul, ok)
+    rejected = rejector(lib.sb200_int8_matmul, ok)
     for i in (0, 1, 3, 4, 7, 8, 11, 16):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     for i in (12, 13, 14, 15):
@@ -131,10 +111,10 @@ def test_matmul_rejects_bad_arguments_on_the_host():
 
 def test_quantize_cols_rejects_bad_arguments_on_the_host():
     lib = _lib.load()
-    keep, p = _buf()
+    keep, p = buf()
     # (x, scale, zp, qmin, qmax, q, col_sum, nan_flag, batch, k, n, stream)
     ok = [p, p, p, -128, 127, p, p, p, 2, 64, 8, None]
-    rejected = _rejecter(lib.sb200_int8_quantize_cols, ok)
+    rejected = rejector(lib.sb200_int8_quantize_cols, ok)
     for i in (0, 1, 2, 5, 6, 7):
         rejected(E_INVALID, b"null pointer", **{f"a{i}": None})
     for i in (8, 9, 10):
@@ -176,13 +156,7 @@ def test_eligible_modules():
     assert q.left.input_quantizer is not q.right.input_quantizer
 
 
-def _reason(q):
-    r = int8_matmul_ineligibility(q)
-    assert r is not None
-    with pytest.raises(ValueError) as e:
-        QMatMulInt8.from_qmatmul(q)
-    assert r in str(e.value)
-    return r
+_reason = refusal(int8_matmul_ineligibility, QMatMulInt8.from_qmatmul)
 
 
 @pytest.mark.parametrize("side", ["left", "right"])
