@@ -40,6 +40,7 @@ namespace {
 constexpr int kDgCols = 128;        // threads per CTA; the columns n one pass of the CTA reads
 constexpr int kDgUnitK = 32;        // k per CTA (one unit)
 constexpr long long kDgTargetCtas = 1024;  // N is split until the grid has about this many CTAs (~8 per SM)
+constexpr long long kDgMaxGridY = 65535;   // CUDA's limit on gridDim.y
 
 // scales / zeros [N, G] -> sz[g, n] = (s, z): the SIMT kernel reads them along n, coalesced
 __global__ void __launch_bounds__(256) dgrad_sz_kernel(const float* __restrict__ scales, const float* __restrict__ zeros,
@@ -50,70 +51,80 @@ __global__ void __launch_bounds__(256) dgrad_sz_kernel(const float* __restrict__
   sz[i] = make_float2(scales[(size_t)n * G + g], zeros[(size_t)n * G + g]);
 }
 
-// grid (units, M tiles, N slices); partial == nullptr: one slice, the CTA adds into grad_in itself
-template <int BITS, int MT>
-__global__ void __launch_bounds__(kDgCols) gptq_dgrad_simt_kernel(const float* __restrict__ go, const uint32_t* __restrict__ qw,
+// grid (units, M tiles, N slices); partial == nullptr: one slice, the CTA adds into grad_in itself.  gridDim.y is capped
+// at 65535 (kDgMaxGridY), so a CTA walks the M tiles blockIdx.y, blockIdx.y + gridDim.y, ...; each tile is reduced as if
+// it had a CTA of its own.  Only LOOP kernels (M > 262,140, so MT = 4) walk; the others run their one tile with the code
+// and registers they had before the cap (the loop in every kernel cost ~3% at M = 65536, K = 4096, N = 128 on an H100).
+// The loop's bound of three CTAs per SM keeps it at 168 registers without spills; ptxas gives it ~200 without the bound,
+// room for two CTAs of 128 threads per SM.
+template <int BITS, int MT, bool LOOP>
+__global__ void __launch_bounds__(kDgCols, LOOP ? 3 : 0) gptq_dgrad_simt_kernel(const float* __restrict__ go, const uint32_t* __restrict__ qw,
                                                                    float* __restrict__ grad_in, const float2* __restrict__ sz,
                                                                    float* __restrict__ partial, int M, int K, int N, int KW,
                                                                    int group_size, int slice_n) {
   constexpr int kWords = GptqFmt<BITS>::kUnitWords;
   __shared__ float red[kDgUnitK][kDgCols + 1];
   const int tid = threadIdx.x;
-  const int u = blockIdx.x, m0 = blockIdx.y * MT;
+  const int u = blockIdx.x;
   const int n_begin = blockIdx.z * slice_n, n_end = min(N, n_begin + slice_n);
   const int g = (u * kDgUnitK) / group_size;
   const float2* szg = sz + (size_t)g * N;
-  float acc[MT][kDgUnitK], zacc[MT];
-#pragma unroll
-  for (int m = 0; m < MT; ++m) {
-    zacc[m] = 0.f;
-#pragma unroll
-    for (int j = 0; j < kDgUnitK; ++j) acc[m][j] = 0.f;
-  }
-  for (int n = n_begin + tid; n < n_end; n += kDgCols) {
-    uint32_t w[kWords];
-#pragma unroll
-    for (int r = 0; r < kWords; ++r) {
-      const int row = u * kWords + r;
-      w[r] = row < KW ? __ldg(qw + (size_t)row * N + n) : 0u;
-    }
-    const float2 p = __ldg(szg + n);
-    float gs[MT];
+  const int m_tiles = LOOP ? (int)(((long long)M + MT - 1) / MT) : 0;  // M + MT - 1 passes INT_MAX for M near 2^31
+  for (int tile = blockIdx.y; !LOOP || tile < m_tiles; tile += gridDim.y) {  // uniform across the CTA
+    const int m0 = tile * MT;
+    float acc[MT][kDgUnitK], zacc[MT];
 #pragma unroll
     for (int m = 0; m < MT; ++m) {
-      const float gv = (m0 + m < M) ? __ldg(go + (size_t)(m0 + m) * N + n) : 0.f;
-      gs[m] = gv * p.x;
-      zacc[m] = fmaf(gv, p.y, zacc[m]);
+      zacc[m] = 0.f;
+#pragma unroll
+      for (int j = 0; j < kDgUnitK; ++j) acc[m][j] = 0.f;
     }
-    float q[32];
-    decode_unit<BITS>(w, q);
+    for (int n = n_begin + tid; n < n_end; n += kDgCols) {
+      uint32_t w[kWords];
 #pragma unroll
-    for (int m = 0; m < MT; ++m)
+      for (int r = 0; r < kWords; ++r) {
+        const int row = u * kWords + r;
+        w[r] = row < KW ? __ldg(qw + (size_t)row * N + n) : 0u;
+      }
+      const float2 p = __ldg(szg + n);
+      float gs[MT];
 #pragma unroll
-      for (int j = 0; j < kDgUnitK; ++j) acc[m][j] = fmaf(gs[m], q[j], acc[m][j]);
-  }
-  // fixed-order sum over the 128 threads: thread t adds red[t / 4][32 (t % 4) ...] and the 4 quarters meet in shuffles
-  const int jr = tid >> 2, part = tid & 3;
+      for (int m = 0; m < MT; ++m) {
+        const float gv = (m0 + m < M) ? __ldg(go + (size_t)(m0 + m) * N + n) : 0.f;
+        gs[m] = gv * p.x;
+        zacc[m] = fmaf(gv, p.y, zacc[m]);
+      }
+      float q[32];
+      decode_unit<BITS>(w, q);
 #pragma unroll
-  for (int m = 0; m < MT; ++m) {
-    __syncthreads();
+      for (int m = 0; m < MT; ++m)
 #pragma unroll
-    for (int j = 0; j < kDgUnitK; ++j) red[j][tid] = acc[m][j] - zacc[m];
-    __syncthreads();
-    float v = 0.f;
+        for (int j = 0; j < kDgUnitK; ++j) acc[m][j] = fmaf(gs[m], q[j], acc[m][j]);
+    }
+    // fixed-order sum over the 128 threads: thread t adds red[t / 4][32 (t % 4) ...] and the 4 quarters meet in shuffles
+    const int jr = tid >> 2, part = tid & 3;
+#pragma unroll
+    for (int m = 0; m < MT; ++m) {
+      __syncthreads();
+#pragma unroll
+      for (int j = 0; j < kDgUnitK; ++j) red[j][tid] = acc[m][j] - zacc[m];
+      __syncthreads();
+      float v = 0.f;
 #pragma unroll 8
-    for (int i = 0; i < kDgCols / 4; ++i) v += red[jr][part * (kDgCols / 4) + i];
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    const int k = u * kDgUnitK + jr;
-    if (part == 0 && m0 + m < M && k < K) {
-      if (partial) {
-        partial[((size_t)blockIdx.z * M + m0 + m) * K + k] = v;
-      } else {
-        float* o = grad_in + (size_t)(m0 + m) * K + k;
-        *o += v;
+      for (int i = 0; i < kDgCols / 4; ++i) v += red[jr][part * (kDgCols / 4) + i];
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      const int k = u * kDgUnitK + jr;
+      if (part == 0 && m0 + m < M && k < K) {
+        if (partial) {
+          partial[((size_t)blockIdx.z * M + m0 + m) * K + k] = v;
+        } else {
+          float* o = grad_in + (size_t)(m0 + m) * K + k;
+          *o += v;
+        }
       }
     }
+    if (!LOOP) break;
   }
 }
 
@@ -156,14 +167,17 @@ int launch_simt(const float* go, const int32_t* qweight, float* grad_in, const f
   float* partial = p.slices > 1 ? reinterpret_cast<float*>(ws + p.sz_bytes) : nullptr;
   dgrad_sz_kernel<<<(unsigned)(((long long)N * G + 255) / 256), 256, 0, st>>>(scales, zeros, sz, (int)N, G);
   SB_LAUNCHED();
-  const dim3 grid((unsigned)((K + kDgUnitK - 1) / kDgUnitK), (unsigned)((M + p.mt - 1) / p.mt), (unsigned)p.slices);
+  const long long m_tiles = (M + p.mt - 1) / p.mt;
+  const dim3 grid((unsigned)((K + kDgUnitK - 1) / kDgUnitK), (unsigned)(m_tiles < kDgMaxGridY ? m_tiles : kDgMaxGridY),
+                  (unsigned)p.slices);
   const uint32_t* qw = reinterpret_cast<const uint32_t*>(qweight);
-#define SB_GO(MT_)                                                                                                \
-  gptq_dgrad_simt_kernel<BITS, MT_><<<grid, kDgCols, 0, st>>>(go, qw, grad_in, sz, partial, (int)M, (int)K, (int)N, \
-                                                              (int)KW, group_size, p.slice_n)
-  if (p.mt == 1) SB_GO(1);
-  else if (p.mt == 2) SB_GO(2);
-  else SB_GO(4);
+#define SB_GO(MT_, LOOP_)                                                                                         \
+  gptq_dgrad_simt_kernel<BITS, MT_, LOOP_><<<grid, kDgCols, 0, st>>>(go, qw, grad_in, sz, partial, (int)M, (int)K,  \
+                                                                     (int)N, (int)KW, group_size, p.slice_n)
+  if (m_tiles > kDgMaxGridY) SB_GO(4, true);  // M > 4 * 65535: mt = 4
+  else if (p.mt == 1) SB_GO(1, false);
+  else if (p.mt == 2) SB_GO(2, false);
+  else SB_GO(4, false);
 #undef SB_GO
   SB_LAUNCHED();
   if (partial) {

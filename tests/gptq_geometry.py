@@ -33,6 +33,7 @@ DG_TC_MIN_M = 48            # gptq.cu:225 kDgradTcMinM
 DG_COLS = 128               # gptq_dgrad.cu:40 kDgCols
 DG_UNIT_K = 32              # gptq_dgrad.cu:41 kDgUnitK
 DG_TARGET_CTAS = 1024       # gptq_dgrad.cu:42 kDgTargetCtas
+DG_MAX_GRID_Y = 65535       # gptq_dgrad.cu:43 kDgMaxGridY
 DG_STAGES = 5               # gptq_dgrad.cu:179 kDgStages
 DG_CHUNK = 8                # gptq_dgrad.cu:180 kDgChunk
 DG_C_CLAMP = 100            # gptq_dgrad.cu:228
@@ -326,14 +327,20 @@ def f16_branches(m, k, n, kw, gs, state, bias, sm, mode=DEC_DEFAULT_MODE, static
 
 # ----------------------------------------------------------------------------------------------- input gradient
 def dgrad_simt_plan(m, k, n):
-    """simt_plan, gptq_dgrad.cu:135-148 (the launch geometry; the workspace sizes are not restated)."""
+    """simt_plan, gptq_dgrad.cu:143-156, and the grid of launch_simt, :167-169 (the workspace sizes are not restated).
+    grid = (32-k units, M tiles capped at 65535, N slices); m_passes: the M tiles the busiest CTA walks.  The kernel
+    forms its own tile count, ceil(M / MT), in 64 bits (gptq_dgrad.cu:71), so this m_tiles, which Python cannot
+    overflow, is the kernel's for every M < 2^31."""
     mt = 1 if m == 1 else (2 if m == 2 else 4)
-    base = _cdiv(k, DG_UNIT_K) * _cdiv(m, mt)
+    m_tiles = _cdiv(m, mt)
+    base = _cdiv(k, DG_UNIT_K) * m_tiles
     s = _cdiv(DG_TARGET_CTAS, base)
     s_max = _cdiv(n, 4 * DG_COLS)
     s = max(1, min(s, s_max))
     slice_n = _cdiv(_cdiv(n, s), DG_COLS) * DG_COLS
-    return dict(mt=mt, slice_n=slice_n, slices=_cdiv(n, slice_n))
+    slices = _cdiv(n, slice_n)
+    grid = (_cdiv(k, DG_UNIT_K), min(m_tiles, DG_MAX_GRID_Y), slices)
+    return dict(mt=mt, slice_n=slice_n, slices=slices, m_tiles=m_tiles, grid=grid, m_passes=_cdiv(m_tiles, grid[1]))
 
 
 def dgrad_tc_ok(bits, k, n, gs, go_off=0):
@@ -377,8 +384,10 @@ def dgrad_branches(bits, m, k, n, kw, gs, impl, go_off=0):
     b |= {f"dg.simt.b{bits}", f"dg.simt.mt{p['mt']}", "dg.simt.slices" if p["slices"] > 1 else "dg.simt.one_slice"}
     if k % DG_UNIT_K:
         b.add("dg.simt.k_tail")  # gptq_dgrad.cu:109
-    if _cdiv(m, p["mt"]) > 1:
+    if p["m_tiles"] > 1:
         b.add("dg.simt.m_tiles")
+    if p["m_passes"] > 1:
+        b.add("dg.simt.m_loop")  # gptq_dgrad.cu:72: gridDim.y is capped, a CTA walks several M tiles
     return b
 
 

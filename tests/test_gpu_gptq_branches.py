@@ -317,10 +317,15 @@ def test_geometry_matches_documented_launches():
     # the single-launch fp16 path at 4096 x 4096, M = 1: 32 column blocks, 21 wanted, S = 2, 16 slices
     assert geo.dec_plan([(4096, 4096, 512)], 1, DEFAULT_MODE, sm)["slices"] == 16
     # dgrad SIMT plan, 4096 x 4096 at M = 32: mt 4, 128 units x 8 row tiles = 1024 CTAs already, one slice of all N
-    assert geo.dgrad_simt_plan(32, 4096, 4096) == dict(mt=4, slice_n=4096, slices=1)
+    assert geo.dgrad_simt_plan(32, 4096, 4096) == dict(mt=4, slice_n=4096, slices=1, m_tiles=8, grid=(128, 8, 1),
+                                                        m_passes=1)
     # ... M = 40, K = 1000, N = 2512: 32 units x 10 tiles = 320, 4 slices of 640 columns
-    assert geo.dgrad_simt_plan(40, 1000, 2512) == dict(mt=4, slice_n=640, slices=4)
-    assert geo.dgrad_simt_plan(1, 6661, 61) == dict(mt=1, slice_n=128, slices=1)
+    assert geo.dgrad_simt_plan(40, 1000, 2512) == dict(mt=4, slice_n=640, slices=4, m_tiles=10, grid=(32, 10, 4),
+                                                        m_passes=1)
+    assert geo.dgrad_simt_plan(1, 6661, 61) == dict(mt=1, slice_n=128, slices=1, m_tiles=1, grid=(209, 1, 1), m_passes=1)
+    # ... M = 600001: 150001 row tiles, gridDim.y capped at 65535, so some CTAs walk 3 tiles
+    assert geo.dgrad_simt_plan(600001, 64, 256) == dict(mt=4, slice_n=256, slices=1, m_tiles=150001,
+                                                        grid=(2, 65535, 1), m_passes=3)
     # wgmma refusals and the tile whose second feature row is past N
     assert geo.tc_refusal(1004, 256, 1004) == "k8" and geo.tc_refusal(1000, 256, 1000) == "group128"
     assert geo.tc_refusal(512, 256, 128, x_off=1) == "x_misaligned" and geo.tc_refusal(512, 256, 128, qw_off=2) == "qw_misaligned"
