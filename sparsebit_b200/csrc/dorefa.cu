@@ -11,7 +11,9 @@
 // Same IEEE op sequence as the eager chain: libdevice tanhf (what ATen's CUDA tanh calls), a true division by m
 // (`tensor / 0-dim tensor` is a real division in ATen, not a reciprocal multiply: dorefa_norm of common.cuh gives that
 // IEEE quotient), then quant_tensor.py:181-184.
-// Weights are small (<= a few M elements), so these are plain chunked grid-stride kernels like adaround.cu.
+// Plain chunked grid-stride kernels like adaround.cu, with 64-bit element indices throughout: besides weights they serve
+// whole activations, whose max |tanh| the integer-grid layers take on DoReFa inputs, and those pass 2^31 elements
+// (tests/test_gpu_far_end_conv.py runs all three past it, and dorefa_absmax past 2^32).
 #include "common.cuh"
 
 namespace sb200 {
