@@ -697,6 +697,53 @@ int sb200_int8_attention_masked(const float* q, const float* k, const float* v, 
                                 int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* ---- (5h) The attention of (5e) / (5f) over an int8 key/value cache, for generation (sm_90a) ----
+ * New; the reference's GPT-2 (wikitext) concatenates layer_past onto the new key and value at every step.  Here each
+ * key and value is quantized once, when it is appended, into a cache that the caller allocates zeroed.  Per entry e of
+ * `batch` (the flattened leading dimensions), capacity C, L keys stored, dp = round_up(d, 16), Cp = round_up(C, 16):
+ *   k_q [batch, C, dp] s8     row j = the stored grid of key j as sb200_int8_quantize_rows writes it (padding 0)
+ *   k_sum, k_nan [batch, C]   int32 / uint8: that row's sum and NaN flag
+ *   v_t [batch, dv, Cp] s8    v^T, key-major, as sb200_int8_quantize_cols writes it
+ *   v_sum, v_nan [batch, dv]  int32 / uint8: the column sums over the L stored keys; a sticky NaN flag
+ * Every byte at a key position >= L stays 0.  k_q and v_t are 16-byte aligned.  The qparams and ranges of k and v must
+ * be the same at every append and attention call of a cache.
+ *
+ * sb200_int8_kv_append writes k [batch, t, d] and v [batch, t, dv] (fp32 contiguous) at positions [length,
+ * length + t) in one launch and updates v_sum / v_nan.  Checks, before any CUDA call: null pointers, an empty
+ * dimension, a negative length, length + t > capacity, batch capacity >= 2^31, a k_q or v_t not 16-byte aligned and
+ * the range rules are SB200_E_INVALID; capacity >= 2^17, d > 128 or dv > 128 is SB200_E_UNSUPPORTED.
+ *
+ * sb200_int8_attention_cached is sb200_int8_attention_masked (q [batch, tq, d], the four qparams, scale, mask, causal,
+ * out, p_q) with k and v the first `length` keys of the cache.  tq > 16: q is quantized and the fused kernel of (5e)
+ * runs over the cache; out and p_q are bit-identical to sb200_int8_attention_masked on the fp32 keys and values that
+ * were appended.  tq <= 16 (decode): a split-key kernel pair plus a combine (at most four launches with q's
+ * quantization): the scores are bit-identical to sb200_int8_matmul(q, k^T), every p is within the bound of (5e), out is
+ * exactly the integer p @ v of the kernel's own p_q, and the NaN rules are those of (5f).  Only the fp64 summation
+ * order of the softmax denominator differs from the fused kernel, so a p grid value can differ from it by one step
+ * where RN32(1 / l) rounds differently.  Deterministic: the key split depends on the shape only.
+ * Checks: those of (5f) with tk = length (length >= 1), then those of the append on the cache; a too small workspace
+ * is SB200_E_WORKSPACE.
+ * workspace: sb200_int8_attention_cached_workspace_bytes(batch, tq, capacity, length, d, dv, causal) bytes: q's grid,
+ * and with tq <= 16 the fp32 scores [batch, tq, length] and per key split int32 partials (a pure function; 0 for
+ * arguments it rejects). */
+int sb200_int8_kv_append(const float* k, const float* v, const float* k_scale, const float* k_zero_point, int qmin_k,
+                         int qmax_k, const float* v_scale, const float* v_zero_point, int qmin_v, int qmax_v,
+                         int8_t* k_q, int32_t* k_sum, uint8_t* k_nan, int8_t* v_t, int32_t* v_sum, uint8_t* v_nan,
+                         int64_t batch, int64_t capacity, int64_t length, int64_t t, int64_t d, int64_t dv,
+                         void* stream);
+size_t sb200_int8_attention_cached_workspace_bytes(int64_t batch, int64_t tq, int64_t capacity, int64_t length,
+                                                   int64_t d, int64_t dv, int causal);
+int sb200_int8_attention_cached(const float* q, const float* q_scale, const float* q_zero_point, int qmin_q, int qmax_q,
+                                const float* k_scale, const float* k_zero_point, int qmin_k, int qmax_k,
+                                const float* p_scale, const float* p_zero_point, int qmin_p, int qmax_p,
+                                const float* v_scale, const float* v_zero_point, int qmin_v, int qmax_v, int has_scale,
+                                float scale, const float* mask, int64_t mask_stride_outer, int64_t mask_stride_inner,
+                                int64_t mask_inner, int64_t mask_stride_row, int causal, const int8_t* k_q,
+                                const int32_t* k_sum, const uint8_t* k_nan, const int8_t* v_t, const int32_t* v_sum,
+                                const uint8_t* v_nan, int64_t capacity, int64_t length, float* out, int8_t* p_q,
+                                int64_t batch, int64_t tq, int64_t d, int64_t dv, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
 /* ---- (5g) Integer-grid layers with a DoReFa input ------------------------------------------------------------------
  * Replaces the chain of sparsebit/quantization/quantizers/dorefa.py:15-20 (t = tanh(x); x_n = t / max |t|; QDQ(x_n))
  * feeding F.linear / F.conv2d when the layer's input quantizer is DoReFa: the lowering (or the grouped kernel) quantizes

@@ -141,6 +141,13 @@ PROTOTYPES = {
                                             c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_i64, c_i64,
                                             c_i64, c_i64, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp,
                                             c_sz, c_vp]),
+    "sb200_int8_kv_append": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp,
+                                     c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp]),
+    "sb200_int8_attention_cached_workspace_bytes": (c_sz, [c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_int]),
+    "sb200_int8_attention_cached": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_int,
+                                            c_int, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_i64, c_i64, c_i64,
+                                            c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp,
+                                            c_i64, c_i64, c_i64, c_i64, c_vp, c_sz, c_vp]),
     "sb200_gptq4_set_impl": (c_int, [c_int]),
     "sb200_gptq4_set_wait_backoff": (c_int, [c_int]),
     "sb200_gptq4_set_decode": (c_int, [c_int]),

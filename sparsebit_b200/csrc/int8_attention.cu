@@ -34,48 +34,17 @@
 // range adds its exact (g_0 - Z_p) sum (v - Z_v) over the skipped keys.  p_q receives the grid of 0 * RN32(1 / l)
 // at skipped keys, as at a hidden key the kernel visits.  A NaN in k poisons only the rows that see its key; a row
 // without a visible key is NaN.
-#include "int8_grid.cuh"
-#include "tc_common.cuh"
+#include "int8_attention.cuh"
 
 namespace sb200 {
 namespace {
 
-constexpr int kAtRows = 128;                    // query rows per CTA (two consumer warpgroups x 64)
-constexpr int kAtKeys = 128;                    // keys per block: wgmma N of q k^T, K of p v
 constexpr int kAtStages = 4;
 constexpr int kAtThreads = 384;
 constexpr int kAtTile = 128 * 128;              // 16 KB: the q tile, a k block, a v^T block (128 rows x 128 bytes)
 constexpr int kAtStageBytes = 2 * kAtTile;      // k block | v^T block
 constexpr int kAtPBytes = 64 * 128;             // one warpgroup's p tile (64 rows x 128 keys)
-constexpr int kAtMaxDim = 128;                  // d, dv
-constexpr long long kAtMaxTk = 1LL << 17;       // exact s32 sums of p v
 constexpr size_t kAtSmem = 1024 + kAtTile + (size_t)kAtStages * kAtStageBytes + 2 * kAtPBytes + 128;
-
-struct AtParams {
-  const int* q_sum;
-  const uint8_t* q_nan;
-  const int* k_sum;
-  const uint8_t* k_nan;
-  const int* v_sum;
-  const uint8_t* v_nan;
-  const float *q_scale, *q_zero, *k_scale, *k_zero, *p_scale, *p_zero, *v_scale, *v_zero;
-  int q_off, k_off, p_off, v_off;
-  float p_qmin, p_qmax;
-  int has_scale;
-  float scale;
-  float* out;
-  int8_t* p_q;  // [B, Tq, Tkp] or null
-  int Tq, Tk, Tkp, d, dp, dv, vec2;
-};
-
-// The mask of the masked instantiation, a separate kernel argument so that AtParams keeps its layout.  Entry b of the
-// batch reads mask + (b / inner) stride_outer + (b % inner) stride_inner + i stride_row + j (all 64-bit).
-struct AtMask {
-  const float* mask;  // or null
-  long long stride_outer, stride_inner, stride_row;
-  const int* v_pre;  // causal: [B, dv, nkb] running column sums of v^T over the key blocks
-  int inner, causal, batch;
-};
 
 // Key blocks a CTA of rows [m0, m0 + 128) visits: all of them, or under causal those up to the last key its last row
 // sees (0 when no row sees a key).
@@ -83,17 +52,6 @@ __device__ __forceinline__ int at_visible_blocks(int m0, int Tq, int Tk, int nkb
   if (!causal) return nkb;
   const long long last = (long long)min(m0 + kAtRows, Tq) - 1 + Tk - Tq;  // the last key the CTA's last row sees
   return last < 0 ? 0 : min(nkb, (int)(last / kAtKeys) + 1);
-}
-
-// exp(s - m) for fp32 s <= m: the difference is split exactly into hi + lo (TwoSum), expf(hi) is corrected by lo.
-// Differences below -104 underflow to 0 in fp32 anyway and return 0 (also for a masked s = -inf); NaN propagates.
-__device__ __forceinline__ float exp_diff(float s, float m) {
-  const float hi = __fsub_rn(s, m);
-  if (s == -INFINITY || hi < -104.f) return 0.f;
-  const float bb = __fsub_rn(hi, s);
-  const float lo = __fadd_rn(__fsub_rn(s, __fsub_rn(hi, bb)), __fsub_rn(-m, bb));
-  const float e = expf(hi);
-  return __fmaf_rn(e, lo, e);
 }
 
 // acc = the q tile rows of this warpgroup times the 128 keys of a k block, over nk32 steps of 32 d
@@ -110,8 +68,10 @@ __device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;
 
 // One CTA per 128 query rows of one batch entry (row tile fastest; under causal batch fastest, the last row tiles,
 // which visit the most key blocks, first).  Maps: q (dp, Tq, B), k (dp, Tk, B), v^T (Tkp, dv, B), boxes of 128 x 128
-// bytes: rows past Tq / Tk / dv and bytes past dp / Tkp are zero-filled.  kMasked = false ignores mk.
-template <bool kMasked>
+// bytes: rows past Tq / Tk / dv and bytes past dp / Tkp are zero-filled.  kMasked = false ignores mk.  kCache: k_sum /
+// k_nan of entry b start at b ks (a key/value cache), not at b Tk; a template flag, so that the kernels of the
+// concatenated operands keep their code.
+template <bool kMasked, bool kCache>
 __global__ void __launch_bounds__(kAtThreads, 1)
 int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                       const __grid_constant__ CUtensorMap map_v, const __grid_constant__ AtParams a,
@@ -162,7 +122,7 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   reg_inc<232>();
   const int wg = (warp - 4) >> 2, q4 = lane & 3;
   const int rl = 16 * (warp & 3) + (lane >> 2);  // the thread's first row within the warpgroup's 64; the second is +8
-  const size_t qrow0 = (size_t)batch * a.Tq, krow0 = (size_t)batch * a.Tk, vrow0 = (size_t)batch * a.dv;
+  const size_t qrow0 = (size_t)batch * a.Tq, krow0 = (size_t)batch * (kCache ? a.ks : a.Tk), vrow0 = (size_t)batch * a.dv;
   const double sqk = (double)__ldg(a.q_scale) * (double)__ldg(a.k_scale);
   const long long zq = (long long)rintf(__ldg(a.q_zero)) - a.q_off, zk = (long long)rintf(__ldg(a.k_zero)) - a.k_off;
   const long long zv = (long long)rintf(__ldg(a.v_zero)) - a.v_off;
@@ -184,7 +144,7 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
   const float* mrow[2] = {nullptr, nullptr};  // the mask row of each of the thread's rows (none past Tq)
   long long vis[2] = {0, 0};                  // causal: the last key each row sees
   if constexpr (kMasked) {
-    const long long base = (long long)(batch / mk.inner) * mk.stride_outer + (long long)(batch % mk.inner) * mk.stride_inner;
+    const long long base = at_mask_base(mk, batch);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (mk.mask != nullptr && row[h] < a.Tq) mrow[h] = mk.mask + base + (long long)row[h] * mk.stride_row;
@@ -215,12 +175,10 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         float sc = -INFINITY;
         if (key < a.Tk) {
           const long long I = (long long)acc[j + e] + rterm[h] - zq * (long long)__ldg(a.k_sum + krow0 + key);
-          sc = __double2float_rn((double)I * sqk);
-          if (a.has_scale) sc = __fmul_rn(sc, a.scale);
+          sc = at_score(I, sqk, a.has_scale, a.scale);
           if constexpr (kMasked) {
             const bool seen = key <= vis[h];
-            if (!seen) sc = -INFINITY;
-            if (mrow[h] != nullptr) sc = __fadd_rn(sc, __ldg(mrow[h] + key));
+            sc = at_masked(sc, seen, mrow[h], key);
             knr[h] |= seen && __ldg(a.k_nan + krow0 + key) != 0;
           } else {
             if (h == 0) knan |= __ldg(a.k_nan + krow0 + key) != 0;
@@ -248,7 +206,7 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     float m = mx[h];
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-    double lh = l[h] == 0.0 ? 0.0 : l[h] * exp((double)mx[h] - (double)m);
+    double lh = at_rescale(l[h], mx[h], m);
     lh += __shfl_xor_sync(0xffffffffu, lh, 1);
     lh += __shfl_xor_sync(0xffffffffu, lh, 2);
     mx[h] = m;
@@ -288,14 +246,9 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         for (int e = 0; e < 2; ++e) {
           if (key + e >= a.Tk) continue;  // masked keys store 0: with v^T zero there, they add nothing
           const long long I = (long long)acc[4 * c + 2 * h + e] + rterm[h] - kz[e];
-          float sc = __double2float_rn((double)I * sqk);
-          if (a.has_scale) sc = __fmul_rn(sc, a.scale);
-          if constexpr (kMasked) {
-            if (key + e > vis[h]) sc = -INFINITY;
-            if (mrow[h] != nullptr) sc = __fadd_rn(sc, __ldg(mrow[h] + key + e));
-          }
-          const float p = __fmul_rn(exp_diff(sc, mx[h]), inv[h]);
-          const int g = stored_grid(p, pp, a.p_off, pnan[h]);
+          float sc = at_score(I, sqk, a.has_scale, a.scale);
+          if constexpr (kMasked) sc = at_masked(sc, key + e <= vis[h], mrow[h], key + e);
+          const int g = at_p_grid(sc, mx[h], inv[h], pp, a.p_off, pnan[h]);
           psum[h] += g;
           pair |= ((uint32_t)g & 0xFFu) << (8 * e);
         }
@@ -330,7 +283,6 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
 
   // ---- epilogue: I_pv = sum g_p v - Z_v sum g_p - Z_p sum v + Tk Z_p Z_v, out = RN32(fp64(I_pv) s_p s_v)
   const double spv = (double)__ldg(a.p_scale) * (double)__ldg(a.v_scale);
-  const float qnan = __int_as_float(0x7fc00000);
   // the masked kernel over a visited prefix of nvis keys: - Z_p sum v over the prefix, and (g_0 - Z_p) (v - Z_v) for
   // each skipped key, g_0 the grid of p = 0 (the products of the skipped keys vanish when Z_p lies in the range)
   const int nvis = kMasked ? min(nvb * kAtKeys, a.Tk) : a.Tk;
@@ -348,10 +300,11 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     ps += __shfl_xor_sync(0xffffffffu, ps, 2);
     pn |= __shfl_xor_sync(0xffffffffu, pn, 2);
     rp[h] = (long long)nvis * zp * zv - zv * (long long)ps;
-    bad[h] = bad[h] || kbad || pn != 0;
     if constexpr (kMasked) {
       rp[h] -= d0 * (long long)(a.Tk - nvis) * zv;
-      bad[h] = bad[h] || knr[h] || mx[h] == -INFINITY;  // a NaN key the row sees; no visible key
+      bad[h] = at_row_nan(bad[h], knr[h], pn != 0, mx[h] == -INFINITY);  // a NaN key the row sees; no visible key
+    } else {
+      bad[h] = at_row_nan(bad[h], kbad, pn != 0, false);
     }
   }
 #pragma unroll
@@ -379,8 +332,7 @@ int8_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
       float y[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        y[e] = __double2float_rn((double)((long long)o[4 * c + 2 * h + e] + rp[h] - cn[e]) * spv);
-        if (bad[h] || cnan[e]) y[e] = qnan;
+        y[e] = at_out((long long)o[4 * c + 2 * h + e] + rp[h] - cn[e], spv, bad[h] || cnan[e]);
       }
       float* dst = a.out + (qrow0 + row[h]) * (size_t)a.dv + n;
       if (a.vec2) {  // dv is even: the pair is in range and 8-byte aligned
@@ -434,25 +386,14 @@ AtLayout at_layout(long long batch, long long tq, long long tk, long long d, lon
   return w;
 }
 
-// 0 when the dimensions are acceptable, else the SB200 code; sets the message
-int check_dims(const char* fn, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv) {
-  SB_REQUIRE(batch > 0 && tq > 0 && tk > 0 && d > 0 && dv > 0,
-             "%s: empty operand (batch=%lld Tq=%lld Tk=%lld d=%lld dv=%lld)", fn, (long long)batch, (long long)tq,
-             (long long)tk, (long long)d, (long long)dv);
-  if (d > kAtMaxDim || dv > kAtMaxDim || tk >= kAtMaxTk) {
-    set_error("%s: d = %lld, dv = %lld, Tk = %lld; the fused attention supports d <= 128, dv <= 128 and Tk < 2^17",
-              fn, (long long)d, (long long)dv, (long long)tk);
-    return SB200_E_UNSUPPORTED;
-  }
-  SB_REQUIRE((__int128)batch * tq < (1LL << 31) && (__int128)batch * tk < (1LL << 31) &&
-                 (__int128)batch * ((tq + kAtRows - 1) / kAtRows) < (1LL << 31),
-             "%s: dimension too large (batch Tq and batch Tk must be < 2^31)", fn);
+template <bool kMasked, bool kCache>
+int at_run(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v, const AtParams& a,
+           const AtMask& mk, long long ctas, cudaStream_t st) {
+  static std::atomic<int> attr_done[64];
+  SB_CUDA(ensure_dyn_smem(int8_attention_kernel<kMasked, kCache>, (int)kAtSmem, attr_done));
+  int8_attention_kernel<kMasked, kCache><<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a, mk);
+  SB_LAUNCHED();
   return SB200_OK;
-}
-
-// Causal: the running column sums of v^T (int8_attention_vprefix_kernel) after the operands, [batch dv, nkb] int32
-size_t at_vpre_bytes(long long batch, long long tk, long long dv) {
-  return align_up((size_t)(batch * dv) * (size_t)((tk + kAtKeys - 1) / kAtKeys) * 4, 1024);
 }
 
 size_t at_workspace_bytes(int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv, int causal) {
@@ -474,24 +415,11 @@ int attention_run(const char* fn, const float* q, const float* k, const float* v
   SB_REQUIRE(q && k && v && q_scale && q_zero_point && k_scale && k_zero_point && p_scale && p_zero_point && v_scale &&
                  v_zero_point && out && workspace,
              "%s: null pointer argument", fn);
-  if (const int rc = check_dims(fn, batch, tq, tk, d, dv)) return rc;
+  if (const int rc = at_check_dims(fn, batch, tq, tk, d, dv)) return rc;
   const int ranges[4][2] = {{qmin_q, qmax_q}, {qmin_k, qmax_k}, {qmin_p, qmax_p}, {qmin_v, qmax_v}};
-  for (const auto& r : ranges)
-    if (const int rc = check_range(fn, r[0], r[1])) return rc;
-  SB_REQUIRE(!has_scale || (scale == scale && scale - scale == 0.f), "%s: the scale %g is not finite", fn, (double)scale);
-  SB_REQUIRE(p_q == nullptr || aligned16(p_q), "%s: p_q must be 16-byte aligned", fn);
-  SB_REQUIRE(causal == 0 || causal == 1, "%s: causal must be 0 or 1, got %d", fn, causal);
-  if (mask != nullptr) {
-    SB_REQUIRE(mask_stride_outer >= 0 && mask_stride_inner >= 0 && mask_stride_row >= 0,
-               "%s: negative mask stride (outer %lld, inner %lld, row %lld)", fn, (long long)mask_stride_outer,
-               (long long)mask_stride_inner, (long long)mask_stride_row);
-    SB_REQUIRE(mask_inner > 0 && batch % mask_inner == 0, "%s: mask_inner = %lld must be positive and divide batch = %lld",
-               fn, (long long)mask_inner, (long long)batch);
-    SB_REQUIRE((reinterpret_cast<uintptr_t>(mask) & 3u) == 0, "%s: the mask must be 4-byte aligned", fn);
-    const __int128 last = (__int128)(batch / mask_inner - 1) * mask_stride_outer +
-                          (__int128)(mask_inner - 1) * mask_stride_inner + (__int128)(tq - 1) * mask_stride_row + tk - 1;
-    SB_REQUIRE(last < ((__int128)1 << 62), "%s: the mask's offsets exceed 2^62 elements", fn);
-  }
+  if (const int rc = at_check_args(fn, ranges, has_scale, scale, p_q, causal, mask, mask_stride_outer, mask_stride_inner,
+                                   mask_inner, mask_stride_row, batch, tq, tk))
+    return rc;
   if (const int rc = check_workspace(fn, workspace_bytes, at_workspace_bytes(batch, tq, tk, d, dv, causal))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const AtLayout w = at_layout(batch, tq, tk, d, dv);
@@ -522,44 +450,95 @@ int attention_run(const char* fn, const float* q, const float* k, const float* v
                                               reinterpret_cast<int32_t*>(ws + w.v_sum), ws + w.v_nan, batch, tk, dv,
                                               stream))
     return rc;
-  AtMask mk = {mask, mask_stride_outer, mask_stride_inner, mask_stride_row, nullptr, (int)(mask ? mask_inner : 1), causal,
-               (int)batch};
-  if (causal) {
-    int* pre = reinterpret_cast<int*>(ws + w.total);
-    const long long rows = batch * dv;
-    int8_attention_vprefix_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(vq, pre, rows, (int)tkp,
-                                                                              (int)((tk + kAtKeys - 1) / kAtKeys));
-    SB_LAUNCHED();
-    mk.v_pre = pre;
-  }
+  const AtMask mk = {mask, mask_stride_outer, mask_stride_inner, mask_stride_row, nullptr, (int)(mask ? mask_inner : 1),
+                     causal, (int)batch};
   AtParams a;
   a.q_sum = reinterpret_cast<const int*>(ws + w.q_sum), a.q_nan = ws + w.q_nan;
   a.k_sum = reinterpret_cast<const int*>(ws + w.k_sum), a.k_nan = ws + w.k_nan;
   a.v_sum = reinterpret_cast<const int*>(ws + w.v_sum), a.v_nan = ws + w.v_nan;
-  a.q_scale = q_scale, a.q_zero = q_zero_point, a.k_scale = k_scale, a.k_zero = k_zero_point;
-  a.p_scale = p_scale, a.p_zero = p_zero_point, a.v_scale = v_scale, a.v_zero = v_zero_point;
-  a.q_off = grid_offset(qmin_q), a.k_off = grid_offset(qmin_k);
-  a.p_off = grid_offset(qmin_p), a.v_off = grid_offset(qmin_v);
-  a.p_qmin = (float)qmin_p, a.p_qmax = (float)qmax_p;
-  a.has_scale = has_scale != 0, a.scale = has_scale ? scale : 1.f;
+  const float* const qparams[8] = {q_scale, q_zero_point, k_scale, k_zero_point, p_scale, p_zero_point, v_scale,
+                                   v_zero_point};
+  at_set_qparams(a, qparams, ranges, has_scale, scale);
   a.out = out, a.p_q = p_q;
-  a.Tq = (int)tq, a.Tk = (int)tk, a.Tkp = (int)tkp, a.d = (int)d, a.dp = (int)dp, a.dv = (int)dv;
+  a.Tq = (int)tq, a.Tk = (int)tk, a.Tkp = (int)tkp, a.d = (int)d, a.dp = (int)dp, a.dv = (int)dv, a.ks = (int)tk;
   a.vec2 = (dv % 2 == 0) && (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
-  const long long ctas = batch * ((tq + kAtRows - 1) / kAtRows);
-  if (mask == nullptr && !causal) {
-    static std::atomic<int> attr_done[64];
-    SB_CUDA(ensure_dyn_smem(int8_attention_kernel<false>, (int)kAtSmem, attr_done));
-    int8_attention_kernel<false><<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a, mk);
-  } else {
-    static std::atomic<int> attr_done[64];
-    SB_CUDA(ensure_dyn_smem(int8_attention_kernel<true>, (int)kAtSmem, attr_done));
-    int8_attention_kernel<true><<<(unsigned)ctas, kAtThreads, kAtSmem, st>>>(map_q, map_k, map_v, a, mk);
-  }
-  SB_LAUNCHED();
-  return SB200_OK;
+  return at_launch(map_q, map_k, map_v, a, mk, vq, tkp, reinterpret_cast<int*>(ws + w.total), batch, st);
 }
 
 }  // namespace
+
+// ---------------------------------------------------------------------------------- shared through int8_attention.cuh
+int at_check_dims(const char* fn, int64_t batch, int64_t tq, int64_t tk, int64_t d, int64_t dv) {
+  SB_REQUIRE(batch > 0 && tq > 0 && tk > 0 && d > 0 && dv > 0,
+             "%s: empty operand (batch=%lld Tq=%lld Tk=%lld d=%lld dv=%lld)", fn, (long long)batch, (long long)tq,
+             (long long)tk, (long long)d, (long long)dv);
+  if (d > kAtMaxDim || dv > kAtMaxDim || tk >= kAtMaxTk) {
+    set_error("%s: d = %lld, dv = %lld, Tk = %lld; the fused attention supports d <= 128, dv <= 128 and Tk < 2^17",
+              fn, (long long)d, (long long)dv, (long long)tk);
+    return SB200_E_UNSUPPORTED;
+  }
+  SB_REQUIRE((__int128)batch * tq < (1LL << 31) && (__int128)batch * tk < (1LL << 31) &&
+                 (__int128)batch * ((tq + kAtRows - 1) / kAtRows) < (1LL << 31),
+             "%s: dimension too large (batch Tq and batch Tk must be < 2^31)", fn);
+  return SB200_OK;
+}
+
+int at_check_args(const char* fn, const int (&ranges)[4][2], int has_scale, float scale, const int8_t* p_q, int causal,
+                  const float* mask, int64_t mask_stride_outer, int64_t mask_stride_inner, int64_t mask_inner,
+                  int64_t mask_stride_row, int64_t batch, int64_t tq, int64_t tk) {
+  for (const auto& r : ranges)
+    if (const int rc = check_range(fn, r[0], r[1])) return rc;
+  SB_REQUIRE(!has_scale || (scale == scale && scale - scale == 0.f), "%s: the scale %g is not finite", fn, (double)scale);
+  SB_REQUIRE(p_q == nullptr || aligned16(p_q), "%s: p_q must be 16-byte aligned", fn);
+  SB_REQUIRE(causal == 0 || causal == 1, "%s: causal must be 0 or 1, got %d", fn, causal);
+  if (mask != nullptr) {
+    SB_REQUIRE(mask_stride_outer >= 0 && mask_stride_inner >= 0 && mask_stride_row >= 0,
+               "%s: negative mask stride (outer %lld, inner %lld, row %lld)", fn, (long long)mask_stride_outer,
+               (long long)mask_stride_inner, (long long)mask_stride_row);
+    SB_REQUIRE(mask_inner > 0 && batch % mask_inner == 0, "%s: mask_inner = %lld must be positive and divide batch = %lld",
+               fn, (long long)mask_inner, (long long)batch);
+    SB_REQUIRE((reinterpret_cast<uintptr_t>(mask) & 3u) == 0, "%s: the mask must be 4-byte aligned", fn);
+    const __int128 last = (__int128)(batch / mask_inner - 1) * mask_stride_outer +
+                          (__int128)(mask_inner - 1) * mask_stride_inner + (__int128)(tq - 1) * mask_stride_row + tk - 1;
+    SB_REQUIRE(last < ((__int128)1 << 62), "%s: the mask's offsets exceed 2^62 elements", fn);
+  }
+  return SB200_OK;
+}
+
+void at_set_qparams(AtParams& a, const float* const (&qparams)[8], const int (&ranges)[4][2], int has_scale,
+                    float scale) {
+  a.q_scale = qparams[0], a.q_zero = qparams[1], a.k_scale = qparams[2], a.k_zero = qparams[3];
+  a.p_scale = qparams[4], a.p_zero = qparams[5], a.v_scale = qparams[6], a.v_zero = qparams[7];
+  a.q_off = grid_offset(ranges[0][0]), a.k_off = grid_offset(ranges[1][0]);
+  a.p_off = grid_offset(ranges[2][0]), a.v_off = grid_offset(ranges[3][0]);
+  a.p_qmin = (float)ranges[2][0], a.p_qmax = (float)ranges[2][1];
+  a.has_scale = has_scale != 0, a.scale = has_scale ? scale : 1.f;
+}
+
+size_t at_vpre_bytes(long long batch, long long tk, long long dv) {
+  return align_up((size_t)(batch * dv) * (size_t)((tk + kAtKeys - 1) / kAtKeys) * 4, 1024);
+}
+
+int at_launch(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v, const AtParams& a, AtMask mk,
+              const int8_t* vt, long long vt_stride, int* v_pre, long long batch, cudaStream_t st) {
+  if (mk.causal) {
+    const long long rows = batch * a.dv;
+    int8_attention_vprefix_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(vt, v_pre, rows, (int)vt_stride,
+                                                                              (a.Tk + kAtKeys - 1) / kAtKeys);
+    SB_LAUNCHED();
+    mk.v_pre = v_pre;
+  }
+  const long long ctas = batch * ((a.Tq + kAtRows - 1) / kAtRows);
+  const bool masked = mk.mask != nullptr || mk.causal, cache = a.ks != a.Tk;
+  if (!masked && !cache)
+    return at_run<false, false>(map_q, map_k, map_v, a, mk, ctas, st);
+  if (masked && !cache)
+    return at_run<true, false>(map_q, map_k, map_v, a, mk, ctas, st);
+  if (!masked)
+    return at_run<false, true>(map_q, map_k, map_v, a, mk, ctas, st);
+  return at_run<true, true>(map_q, map_k, map_v, a, mk, ctas, st);
+}
+
 }  // namespace sb200
 
 using namespace sb200;

@@ -230,15 +230,16 @@ static inline bool make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const v
              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// `batch` matrices of `rows` x `inner` elements, row_bytes apart, back to back; a box is box_inner x box_rows of one
-// matrix, so rows past the end of a matrix are zero-filled instead of read from the next one
+// `batch` matrices of `rows` x `inner` elements, row_bytes apart, back to back (or matrix_bytes apart when given: a
+// view of the first rows of larger matrices); a box is box_inner x box_rows of one matrix, so rows past the end of a
+// matrix are zero-filled instead of read from the next one
 static inline bool make_map_3d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t rows,
                                uint64_t batch, uint64_t row_bytes, uint32_t box_inner, uint32_t box_rows,
-                               CUtensorMapSwizzle sw) {
+                               CUtensorMapSwizzle sw, uint64_t matrix_bytes = 0) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return false;
   const cuuint64_t dims[3] = {inner, rows, batch};
-  const cuuint64_t strides[2] = {row_bytes, rows * row_bytes};
+  const cuuint64_t strides[2] = {row_bytes, matrix_bytes ? matrix_bytes : rows * row_bytes};
   const cuuint32_t box[3] = {box_inner, box_rows, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   return enc(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,

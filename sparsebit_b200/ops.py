@@ -959,6 +959,41 @@ def attention_mask_strides(shape, strides, lead, tq, tk):
     return (dims[0][1], dims[1][1], dims[1][0], es[-2])
 
 
+def _attention_qparams(fn, *qparams):
+    """The C-ABI arguments of (q, k, p, v) qparams: ``(scale, zero_point, (qmin, qmax))`` each, per-tensor fp32."""
+    qp = []
+    for (s, z, qrange), name in zip(qparams, ("q", "k", "p", "v")):
+        _req(s, f"{name}_scale"), _req(z, f"{name}_zero_point")
+        _check_per_tensor(fn, s, z)
+        qp += [s.data_ptr(), z.data_ptr(), int(qrange[0]), int(qrange[1])]
+    return qp
+
+
+def _attention_mask(fn, attn_mask, causal, device, lead, tq, tk):
+    """(fp32 mask or None, its ``attention_mask_strides`` plan) of an attention call over ``lead + (tq, tk)``; a mask
+    whose broadcast cannot be addressed in place is copied (batch dimensions and keys, a broadcast row kept)."""
+    if causal not in (False, True):
+        raise SparsebitB200Error(f"{fn}: causal must be a bool, got {causal!r}")
+    if attn_mask is None:
+        return None, None
+    mask = attention_mask_check(attn_mask)
+    if mask.device != device:
+        raise SparsebitB200Error(f"{fn}: attn_mask is on {mask.device}, q on {device}")
+    try:
+        plan = attention_mask_strides(mask.shape, mask.stride(), lead, tq, tk)
+    except ValueError as e:
+        raise SparsebitB200Error(f"{fn}: attn_mask: {e}") from None
+    if plan is None:  # materialise the batch dimensions and the keys, keep a broadcast row
+        shape = (1,) * (len(lead) + 2 - mask.dim()) + tuple(mask.shape)
+        mask = mask.reshape(shape).expand(lead + (shape[-2], tk)).contiguous()
+        plan = attention_mask_strides(mask.shape, mask.stride(), lead, tq, tk)
+    return mask, plan
+
+
+def _mask_args(mask, plan):
+    return [mask.data_ptr(), *plan[:3], plan[3]] if mask is not None else [None, 0, 0, 1, 0]
+
+
 def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=None, return_p=False, attn_mask=None,
                    causal=False):
     """``softmax(q @ k^T [* scale] [masked]) @ v`` with q, k, the softmax output p and v each on a per-tensor int8 grid,
@@ -976,11 +1011,7 @@ def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=No
     for x, name in ((q, "q"), (k, "k"), (v, "v")):
         if not isinstance(x, torch.Tensor) or x.dim() < 2:
             raise SparsebitB200Error(f"int8_attention: {name} must be a tensor with at least 2 dimensions")
-    qp = []
-    for (s, z, qrange), name in ((q_qparams, "q"), (k_qparams, "k"), (p_qparams, "p"), (v_qparams, "v")):
-        _req(s, f"{name}_scale"), _req(z, f"{name}_zero_point")
-        _check_per_tensor("int8_attention", s, z)
-        qp += [s.data_ptr(), z.data_ptr(), int(qrange[0]), int(qrange[1])]
+    qp = _attention_qparams("int8_attention", q_qparams, k_qparams, p_qparams, v_qparams)
     lead = tuple(q.shape[:-2])
     if tuple(k.shape[:-2]) != lead or tuple(v.shape[:-2]) != lead:
         raise SparsebitB200Error(f"int8_attention: q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} need equal "
@@ -989,21 +1020,7 @@ def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=No
     if dk != d or tkv != tk:
         raise SparsebitB200Error(f"int8_attention: q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} do not "
                                  "chain (q and k need the same d, k and v the same Tk)")
-    if causal not in (False, True):
-        raise SparsebitB200Error(f"int8_attention: causal must be a bool, got {causal!r}")
-    mask = None
-    if attn_mask is not None:
-        mask = attention_mask_check(attn_mask)
-        if mask.device != q.device:
-            raise SparsebitB200Error(f"int8_attention: attn_mask is on {mask.device}, q on {q.device}")
-        try:
-            plan = attention_mask_strides(mask.shape, mask.stride(), lead, tq, tk)
-        except ValueError as e:
-            raise SparsebitB200Error(f"int8_attention: attn_mask: {e}") from None
-        if plan is None:  # materialise the batch dimensions and the keys, keep a broadcast row
-            shape = (1,) * (len(lead) + 2 - mask.dim()) + tuple(mask.shape)
-            mask = mask.reshape(shape).expand(lead + (shape[-2], tk)).contiguous()
-            plan = attention_mask_strides(mask.shape, mask.stride(), lead, tq, tk)
+    mask, plan = _attention_mask("int8_attention", attn_mask, causal, q.device, lead, tq, tk)
     q, k, v = (x.reshape(-1, *x.shape[-2:]).contiguous() for x in (q, k, v))
     _req(q, "q"), _req(k, "k"), _req(v, "v")
     batch = q.shape[0]
@@ -1018,12 +1035,110 @@ def int8_attention(q, k, v, q_qparams, k_qparams, p_qparams, v_qparams, scale=No
             check(lib.sb200_int8_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), *qp, *scl, *tail, ws.data_ptr(),
                                            ws.numel(), _stream(q)))
     else:
-        mk = [mask.data_ptr(), *plan[:3], plan[3]] if mask is not None else [None, 0, 0, 1, 0]
+        mk = _mask_args(mask, plan)
         ws_bytes = int(lib.sb200_int8_attention_masked_workspace_bytes(batch, tq, tk, d, dv, int(causal)))
         ws = _int8_workspace(q.device, max(ws_bytes, 16))
         with torch.cuda.device(q.device):
             check(lib.sb200_int8_attention_masked(q.data_ptr(), k.data_ptr(), v.data_ptr(), *qp, *scl, *mk, int(causal),
                                                   *tail, ws.data_ptr(), ws.numel(), _stream(q)))
+    return (out, p_q) if return_p else out
+
+
+class Int8KVCache:
+    """An int8 key/value cache of ``int8_attention_cached``: keys and values quantized once, on append, with the
+    qparams of the layer that owns the cache (``QAttentionInt8.new_cache``).  For ``lead`` entries (the leading
+    dimensions of q / k / v), ``capacity`` keys of width ``d`` and values of width ``dv``, zero-initialised:
+
+    * ``k_q`` int8 [*lead, capacity, round_up(d, 16)], ``k_sum`` int32 / ``k_nan`` bool [*lead, capacity]: key j's
+      stored grid, its sum and NaN flag, as ``int8_quantize_rows`` writes them;
+    * ``v_t`` int8 [*lead, dv, round_up(capacity, 16)], ``v_sum`` int32 / ``v_nan`` bool [*lead, dv]: v^T as
+      ``int8_quantize_cols`` writes it, the column sums over the stored keys and a sticky NaN flag.
+
+    ``length`` (a host integer) keys are stored; every byte past them is 0."""
+
+    def __init__(self, layer, lead, capacity, d, dv, device):
+        lead, capacity, d, dv = tuple(int(n) for n in lead), int(capacity), int(d), int(dv)
+        if min(lead + (capacity, d, dv), default=1) <= 0:
+            raise SparsebitB200Error(f"Int8KVCache: lead {lead}, capacity {capacity}, d {d} and dv {dv} must be positive")
+        self.layer, self.lead, self.capacity, self.d, self.dv, self.length = layer, lead, capacity, d, dv, 0
+        z = dict(device=device)
+        self.k_q = torch.zeros(lead + (capacity, int8_padded_k(d)), dtype=torch.int8, **z)
+        self.k_sum = torch.zeros(lead + (capacity,), dtype=torch.int32, **z)
+        self.k_nan = torch.zeros(lead + (capacity,), dtype=torch.bool, **z)
+        self.v_t = torch.zeros(lead + (dv, int8_padded_k(capacity)), dtype=torch.int8, **z)
+        self.v_sum = torch.zeros(lead + (dv,), dtype=torch.int32, **z)
+        self.v_nan = torch.zeros(lead + (dv,), dtype=torch.bool, **z)
+
+    def buffers(self):
+        return (self.k_q, self.k_sum, self.k_nan, self.v_t, self.v_sum, self.v_nan)
+
+    def __repr__(self):
+        return f"Int8KVCache(lead={self.lead}, length={self.length}, capacity={self.capacity}, d={self.d}, dv={self.dv})"
+
+
+def int8_kv_append(cache, k, v, k_qparams, v_qparams):
+    """Quantize ``k`` [*lead, t, d] and ``v`` [*lead, t, dv] (fp32) into ``cache`` at positions [length, length + t)
+    in one launch (sb200_int8_kv_append), then advance ``cache.length``.  ``k_qparams`` / ``v_qparams`` are
+    ``(scale, zero_point, (qmin, qmax))`` and must be the same at every call on a cache."""
+    lib = _lib.load()
+    fn = "int8_kv_append"
+    for x, name in ((k, "k"), (v, "v")):
+        if not isinstance(x, torch.Tensor) or x.dim() < 2:
+            raise SparsebitB200Error(f"{fn}: {name} must be a tensor with at least 2 dimensions")
+    (t, d), (tv, dv) = k.shape[-2:], v.shape[-2:]
+    if tuple(k.shape[:-2]) != cache.lead or tuple(v.shape[:-2]) != cache.lead or tv != t or d != cache.d or dv != cache.dv:
+        raise SparsebitB200Error(f"{fn}: k {tuple(k.shape)} and v {tuple(v.shape)} do not match the cache's lead "
+                                 f"{cache.lead}, d = {cache.d} and dv = {cache.dv}")
+    if cache.length + t > cache.capacity:
+        raise SparsebitB200Error(f"{fn}: {cache.length} + {t} keys overflow the cache's capacity {cache.capacity}")
+    qp = []
+    for (s, z, qrange), name in ((k_qparams, "k"), (v_qparams, "v")):
+        _req(s, f"{name}_scale"), _req(z, f"{name}_zero_point")
+        _check_per_tensor(fn, s, z)
+        qp.append([s.data_ptr(), z.data_ptr(), int(qrange[0]), int(qrange[1])])
+    k, v = (x.reshape(-1, *x.shape[-2:]).contiguous() for x in (k, v))
+    _req(k, "k"), _req(v, "v")
+    if k.device != cache.k_q.device:
+        raise SparsebitB200Error(f"{fn}: k is on {k.device}, the cache on {cache.k_q.device}")
+    with torch.cuda.device(k.device):
+        check(lib.sb200_int8_kv_append(k.data_ptr(), v.data_ptr(), *qp[0], *qp[1], *(b.data_ptr() for b in cache.buffers()),
+                                       k.shape[0], cache.capacity, cache.length, t, d, dv, _stream(k)))
+    cache.length += int(t)
+
+
+def int8_attention_cached(q, cache, q_qparams, k_qparams, p_qparams, v_qparams, scale=None, return_p=False,
+                          attn_mask=None, causal=False):
+    """``int8_attention`` of ``q`` [*lead, Tq, d] over the ``cache.length`` keys and values stored in ``cache``
+    (sb200_int8_attention_cached), with the same arguments, mask broadcasting over [*lead, Tq, length], ``return_p``
+    and workspace.  Tq > 16 runs the fused kernel over the cache: bit-identical to ``int8_attention`` on the
+    concatenated fp32 keys and values.  Tq <= 16 runs the split-key decode kernels: the same scores bit for bit, every p
+    within the bound of the fused kernel, out exact on the returned p grid; a p grid value can differ from the fused
+    kernel's by one step where its fp64 denominator rounds differently."""
+    lib = _lib.load()
+    fn = "int8_attention_cached"
+    if not isinstance(q, torch.Tensor) or q.dim() < 2:
+        raise SparsebitB200Error(f"{fn}: q must be a tensor with at least 2 dimensions")
+    lead, (tq, d) = tuple(q.shape[:-2]), q.shape[-2:]
+    if lead != cache.lead or d != cache.d:
+        raise SparsebitB200Error(f"{fn}: q {tuple(q.shape)} does not match the cache's lead {cache.lead} and d = {cache.d}")
+    tk, dv = cache.length, cache.dv
+    if tk == 0:
+        raise SparsebitB200Error(f"{fn}: the cache is empty")
+    qp = _attention_qparams(fn, q_qparams, k_qparams, p_qparams, v_qparams)
+    mask, plan = _attention_mask(fn, attn_mask, causal, q.device, lead, tq, tk)
+    q = q.reshape(-1, tq, d).contiguous()
+    _req(q, "q")
+    batch = q.shape[0]
+    out = torch.empty(lead + (tq, dv), dtype=torch.float32, device=q.device)
+    p_q = torch.empty(lead + (tq, int8_padded_k(tk)), dtype=torch.int8, device=q.device) if return_p else None
+    scl = [int(scale is not None), float(scale) if scale is not None else 1.0]
+    ws_bytes = int(lib.sb200_int8_attention_cached_workspace_bytes(batch, tq, cache.capacity, tk, d, dv, int(causal)))
+    ws = _int8_workspace(q.device, max(ws_bytes, 16))
+    with torch.cuda.device(q.device):
+        check(lib.sb200_int8_attention_cached(q.data_ptr(), *qp, *scl, *_mask_args(mask, plan), int(causal),
+                                              *(b.data_ptr() for b in cache.buffers()), cache.capacity, tk,
+                                              out.data_ptr(), p_q.data_ptr() if p_q is not None else None, batch, tq,
+                                              d, dv, ws.data_ptr(), ws.numel(), _stream(q)))
     return (out, p_q) if return_p else out
 
 

@@ -844,7 +844,13 @@ class QAttentionInt8(nn.Module):
     scores never reach memory.  Built by ``from_qattention``.  q, k, v have equal leading dimensions; fp16 input is
     up-cast and the output is fp32, as in the fake-quant op.  ``attn_mask`` and ``causal`` are those of
     ``QAttention.forward``, computed in the kernel (``ops.int8_attention``).  There is no backward: QAT keeps
-    ``QAttention``."""
+    ``QAttention``.
+
+    Generation: ``new_cache(lead, capacity, d, dv)`` makes an ``ops.Int8KVCache`` bound to this layer, and
+    ``forward(q, k, v, attn_mask, causal, cache=cache)`` appends the new keys and values k, v to it (quantized once)
+    and attends q to all ``cache.length`` stored keys: ``forward(q, cat(past_k, k), cat(past_v, v), attn_mask,
+    causal)``, bit for bit for Tq > 16; for Tq <= 16 the split-key decode kernels give the same scores and an output
+    exact on their own p grid, which can differ from the fused kernel's by one step (``ops.int8_attention_cached``)."""
 
     ROLES = ("q", "k", "p", "v")
 
@@ -865,11 +871,29 @@ class QAttentionInt8(nn.Module):
         mod.qranges.update(qranges)
         return mod
 
-    def forward(self, q, k, v, attn_mask=None, causal=False):
+    def new_cache(self, lead, capacity, d, dv):
+        """An empty int8 key/value cache of ``capacity`` keys for q / k / v with leading dimensions ``lead``, on this
+        layer's device and bound to this layer (its qparams quantize what is appended)."""
+        return ops.Int8KVCache(self, lead, capacity, d, dv, self.q_scale.device)
+
+    def forward(self, q, k, v, attn_mask=None, causal=False, cache=None):
         _check_inference_only(self, "QAttention", q, k, v)
         qp = [(getattr(self, f"{r}_scale"), getattr(self, f"{r}_zero_point"), self.qranges[r]) for r in self.ROLES]
-        return ops.int8_attention(q.float(), k.float(), v.float(), *qp, scale=self.scale, attn_mask=attn_mask,
-                                  causal=causal)
+        if cache is None:
+            return ops.int8_attention(q.float(), k.float(), v.float(), *qp, scale=self.scale, attn_mask=attn_mask,
+                                      causal=causal)
+        if not isinstance(cache, ops.Int8KVCache) or cache.layer is not self:
+            raise ValueError("QAttentionInt8: the cache was not created by this layer's new_cache")
+        lead = tuple(q.shape[:-2])
+        if (lead != cache.lead or tuple(k.shape[:-2]) != lead or tuple(v.shape[:-2]) != lead or q.shape[-1] != cache.d
+                or k.shape[-1] != cache.d or v.shape[-1] != cache.dv or k.shape[-2] != v.shape[-2]):
+            raise ValueError(f"QAttentionInt8: q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} do not "
+                             f"match the cache's lead {cache.lead}, d = {cache.d} and dv = {cache.dv}")
+        # the mask over the keys after the append is checked first, so that a bad mask leaves the cache untouched
+        ops._attention_mask("QAttentionInt8", attn_mask, causal, q.device, lead, q.shape[-2],
+                            cache.length + k.shape[-2])
+        ops.int8_kv_append(cache, k.float(), v.float(), qp[1], qp[3])
+        return ops.int8_attention_cached(q.float(), cache, *qp, scale=self.scale, attn_mask=attn_mask, causal=causal)
 
     def extra_repr(self):
         return f"scale={self.scale}, " + ", ".join(f"{r}_qrange={list(self.qranges[r])}" for r in self.ROLES)
